@@ -51,8 +51,13 @@ def parse():
     ap.add_argument("--config", default="c2", choices=["c1", "c2", "c3", "c4", "c5"],
                     help="BASELINE.json configuration: c2 (default, the headline line); c1/c3/c4/c5 = the other "
                          "configurations on one GPU (librecommender_b200/bench_configs.py)")
-    ap.add_argument("--epi-warps", type=int, default=0, help="tuning: epilogue warps per TMEM quadrant (2|3)")
+    ap.add_argument("--epi-warps", type=int, default=0,
+                    help="tuning: sweep organisation code, 100 * cluster (1|2) + 10 * MMA groups (1|2) + record stores (3|5)")
     ap.add_argument("--pre-coef", type=float, default=0.0, help="tuning: speculative rank coefficient")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the ids the last timed step returned (device leg and "
+                         "end-to-end leg) as DIR/<name>.npy in float64; above 64 MB in all, a seeded sample of rows "
+                         "(DIR/rows.npy)")
     return ap.parse_args()
 
 
@@ -264,6 +269,8 @@ def main():
         torch.cuda.set_device(local_rank)
         device = torch.device("cuda", local_rank)
     if args.config != "c2":
+        if args.dump_outputs:
+            sys.exit("--dump-outputs is implemented for the default configuration (c2) only")
         if rank != 0 or args.impl != "b200":
             return 0
         from librecommender_b200 import bench_configs
@@ -408,6 +415,8 @@ def main():
     e2e_ms = max_over_ranks(e0.elapsed_time(e1))
     e2e_value = world * args.batch * args.steps / (e2e_ms * 1e-3)
     assert res.shape == (args.batch, args.topk) and res.dtype == np.int64 and (res >= 0).all()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"device_ids": out.cpu().numpy(), "e2e_ids": res})
 
     # ---- parity of one TIMED batch, outside the timed region: fused result vs the exact path ----
     last = batches_d[n_batches - 1]
@@ -430,7 +439,7 @@ def main():
         finish_with_secondary({}, run_secondary, rank, world, device, max_over_ranks, barrier)
         return 0
 
-    # ---- roofline of the dominant kernel (tcgen05 sweep) ----------------------------------
+    # ---- roofline of the dominant kernel (wgmma sweep) ------------------------------------
     peaks = {}
     try:
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
@@ -444,20 +453,12 @@ def main():
         flops = 2.0 * args.dim * args.items * rows_per_launch          # per launch (SURVEY §8d: 2*d*N per user)
         avg_ms = float(np.mean(sweep_ms))
         achieved = flops / (avg_ms * 1e-3) / 1e12
-        peak = float(peaks.get("bf16_tflops_sustained", 1400.0))
-        traffic = None
-        try:
-            tr = json.load(open(os.path.join(ROOT, "profiles", "sweep_traffic.json")))
-            # the capture is of a 16 384-user launch: scale to this run's users per launch (records and item-table
-            # passes both grow linearly with the user tiles)
-            traffic = tr["dram_bytes_per_launch"] * rows_per_launch / float(tr.get("users_per_launch", 16384))
-        except Exception:
-            pass
+        peak = float(peaks.get("bf16_tflops_sustained", 989.0))
         roofline = {"bound": "tensor", "kernel": "b200::tc::sweep_kernel (PRE + guess + MAIN)", "achieved": achieved,
                     "peak": peak, "unit": "TFLOP/s", "frac": achieved / peak,
                     "peak_source": "MEASURED_PEAKS.json bf16_tflops_sustained (of measured; fp16 runs at the bf16 rate)"
-                    if peaks else "fallback 1400 (of fallback)",
-                    "traffic": traffic, "avg_launch_ms": avg_ms, "launches_timed": len(sweep_ms),
+                    if peaks else "H100 SXM data-sheet dense fp16 rate at 700 W (not a measured peak)",
+                    "traffic": None, "avg_launch_ms": avg_ms, "launches_timed": len(sweep_ms),
                     "rows_per_launch": rows_per_launch,
                     "share_of_step": avg_ms * len(sweep_ms) / max(dev_ms, 1e-9) if not distributed else None}
 
@@ -499,6 +500,23 @@ def main():
     }
     finish_with_secondary(line, run_secondary, rank, world, device, max_over_ranks, barrier)
     return 0
+
+
+def dump_outputs(directory, arrays, max_bytes=64 << 20):
+    """Write each [B, ...] array as <directory>/<name>.npy in float64 (ids < 2^31 are exact in float64).
+    When all of them together exceed `max_bytes`, the same fixed, seeded sample of rows is written for
+    every array, and the sampled row numbers go to <directory>/rows.npy."""
+    os.makedirs(directory, exist_ok=True)
+    n_rows = len(next(iter(arrays.values())))
+    row_bytes = sum(8 * int(np.prod(np.shape(a)[1:])) for a in arrays.values())
+    rows = None
+    if n_rows * row_bytes > max_bytes:
+        keep = (max_bytes - 8 * n_rows) // row_bytes
+        rows = np.sort(np.random.default_rng(SEED_Q + 2000).choice(n_rows, size=keep, replace=False))
+        np.save(os.path.join(directory, "rows.npy"), rows.astype(np.float64))
+    for name, a in arrays.items():
+        a = np.asarray(a) if rows is None else np.asarray(a)[rows]
+        np.save(os.path.join(directory, f"{name}.npy"), np.ascontiguousarray(a, dtype=np.float64))
 
 
 def finish_with_secondary(line, run_secondary, rank, world, device, max_over_ranks, barrier):

@@ -1,5 +1,5 @@
 /*
- * b200reco.h — C-ABI of librecommender_b200 (sm_100a only).
+ * b200reco.h — C-ABI of librecommender_b200 (sm_90a only).
  *
  * The reference (massquantity/LibRecommender @ 7463d9d) has no FFI on this path:
  * its seams are Python callables (SURVEY.md §8b).  Each entry point below names
@@ -98,7 +98,7 @@ int b200_recommend_embed(const float* U, int64_t ldu, const int64_t* user_ids, i
                          int32_t K, int64_t* out_ids, float* out_scores, int32_t* row_status,
                          void* workspace, size_t workspace_bytes, void* stream,
                          void* ev_sweep_start /* cudaEvent_t or NULL: recorded on `stream` */,
-                         void* ev_sweep_stop  /* just before / after the tcgen05 sweep kernel */);
+                         void* ev_sweep_stop  /* just before / after the wgmma sweep kernels */);
 
 /* ---- 8e row 2: row-sharded embedding table over NVLink peer memory ------------------------
  * (the reference has ONE table, libreco/layers/embedding.py:16-23; here row r lives on GPU r % G at
@@ -231,9 +231,9 @@ int b200_linear_f32(const float* X, int64_t ldx, int64_t R, const float* Wt, int
                     const float* bias, int32_t din, int32_t dout, int32_t relu, float* Y,
                     int64_t ldy, void* stream);
 
-/* Same contract as b200_linear_f32 on the tcgen05 tensor cores: operands split x = hi + lo into
- * two tf32 values, three kind::tf32 products (hi*hi + lo*hi + hi*lo) in separate main / correction
- * TMEM accumulators promoted to registers every 64 k: fp32-level accuracy, not tf32-level.
+/* Same contract as b200_linear_f32 on the tensor cores (wgmma): operands split x = hi + lo into
+ * two tf32 values, three tf32 products (hi*hi + lo*hi + hi*lo) in separate main / correction
+ * accumulators promoted to fp32 registers every 64 k: fp32-level accuracy, not tf32-level.
  * Requires 16-byte aligned X rows (ldx % 4 == 0).  Wsplit (optional, NULL allowed): the layer's
  * weights pre-split once by b200_linear_tf32x3_split_weights — 2 * dout * split_ld(din) floats —
  * which removes the per-tile weight splitting from the kernel; without it Wt rows must be 16-byte

@@ -1,6 +1,6 @@
-"""librecommender_b200 — B200-native scoring / top-K engine behind LibRecommender's
+"""librecommender_b200 — H100-native scoring / top-K engine behind LibRecommender's
 ``recommend_user`` hot path (see DESIGN.md).  Importing the package loads the
-sm_100a shared library; it raises if the library is missing."""
+sm_90a shared library; it raises if the library is missing."""
 from . import _lib  # noqa: F401  (fail loudly when the CUDA library is absent)
 from .consumed import ConsumedCSR
 from .recommendation import (

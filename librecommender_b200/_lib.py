@@ -15,7 +15,7 @@ LIB_PATH = os.path.join(_PKG_DIR, "libb200reco.so")
 if not os.path.exists(LIB_PATH):
     raise ImportError(
         f"{LIB_PATH} is missing: build it with `python -m librecommender_b200.build` "
-        "(nvcc, sm_100a).  librecommender_b200 has no CPU fallback."
+        "(nvcc, sm_90a).  librecommender_b200 has no CPU fallback."
     )
 
 lib = ctypes.CDLL(LIB_PATH)
@@ -156,5 +156,5 @@ def require_cuda():
     import torch
 
     if not torch.cuda.is_available():
-        raise B200Error("librecommender_b200 needs a CUDA device (sm_100a); there is no CPU fallback")
+        raise B200Error("librecommender_b200 needs a CUDA device (sm_90a); there is no CPU fallback")
     return torch.device("cuda", torch.cuda.current_device())

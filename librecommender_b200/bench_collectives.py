@@ -11,14 +11,14 @@
 * ``row_sharded_lookup``: DeepFM-shaped (K = 16) and DIN-shaped (K' = 64) row gathers from a table
   sharded ``row % N`` — (a) NCCL path (index all-to-all, local gather, row all-to-all), (b) ONE
   kernel that pulls the rows over NVLink from the peer shards (``b200_peer_gather_rows``).
-  ``nvlink_gbs`` = bytes that must cross NVLink into one GPU / time; ``frac`` against the 770 GB/s
-  peer-copy reference of the profiling recipe.
+  ``nvlink_gbs`` = bytes that must cross NVLink into one GPU / time; ``frac`` against the H100 SXM
+  data-sheet NVLink rate per direction (450 GB/s, not a measured figure).
 """
 from __future__ import annotations
 
 import numpy as np
 
-NVLINK_REF_GBS = 770.0   # measured peer copy per direction per GPU on this pool (B200_PROFILING.md)
+NVLINK_REF_GBS = 450.0   # H100 SXM NVLink 4: 900 GB/s per GPU both directions together (data sheet)
 
 
 def _timed(fn, iters, max_over_ranks, barrier):

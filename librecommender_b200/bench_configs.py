@@ -1,11 +1,12 @@
 """``bench.py --config c1|c3|c4|c5``: the other BASELINE.json configurations on ONE GPU, each as a JSON
 line with the contract's keys (``metric`` / ``value`` / ``unit`` / ``roofline`` in HBM GB/s where SURVEY.md
-§8d says HBM-bound / ``clocks`` / ``cpu_baseline``).  Shapes follow SURVEY.md §8d scaled to one GPU
+§8d says HBM-bound / ``clocks`` / ``cpu_baseline``).  Every timed leg runs ``--warmup`` untimed and
+``--steps`` timed calls.  Shapes follow SURVEY.md §8d scaled to one GPU
 (the 8-GPU row-sharded variants are exercised by the ``secondary`` legs of the default config at N > 1):
 
 * ``c3``  DeepFM 100 sparse + 10 dense columns, K = 16, hidden (128, 64, 32): training-step
   interactions/s (gather fwd + MLP + loss + backward scatter + TF-Adam on the device) and predict rows/s;
-  roofline = the K1 gather against the measured copy bandwidth (algorithmic bytes/row of §8d);
+  roofline = the K1 gather against the HBM bandwidth (algorithmic bytes/row of §8d);
 * ``c4``  DIN, T = 50, item features (K' = 64): predict rows/s and all-items recommend users/s;
 * ``c5``  LightGCN 3-layer propagation over a Zipf bipartite graph: nnz/s and algorithmic GB/s (§8d), then
   top-100 serving over the propagated embeddings;
@@ -21,7 +22,7 @@ import time
 import numpy as np
 
 
-def _timeit(fn, iters=10, warm=3):
+def _timeit(fn, iters, warm):
     import torch
 
     for _ in range(warm):
@@ -36,11 +37,14 @@ def _timeit(fn, iters=10, warm=3):
     return e0.elapsed_time(e1) / iters
 
 
-def _peaks(root):
+def _hbm_peak(root):
+    """(GB/s, source): a measured copy bandwidth from MEASURED_PEAKS.json when present, else the H100 SXM
+    data-sheet HBM3 figure."""
     try:
-        return json.load(open(os.path.join(root, "MEASURED_PEAKS.json")))
+        return (float(json.load(open(os.path.join(root, "MEASURED_PEAKS.json")))["hbm_gbs"]),
+                "MEASURED_PEAKS.json hbm_gbs (measured)")
     except Exception:
-        return {}
+        return 3350.0, "H100 SXM data-sheet HBM3 bandwidth (not measured)"
 
 
 def _line(metric, value, unit, steps, warmup, ms, config, roofline, cpu, clocks, extra=None):
@@ -76,37 +80,38 @@ def c3(args, root, sampler):
     pw = torch.empty((R, K), dtype=torch.float32, device="cuda")
     lin = torch.empty(R, dtype=torch.float32, device="cuda")
     sampler.start()
-    ms_g = _timeit(lambda: model._feat_forward(model.spec.layout, users, items, R, 0, concat=concat, pw=pw, lin=lin))
+    ms_g = _timeit(lambda: model._feat_forward(model.spec.layout, users, items, R, 0, concat=concat, pw=pw, lin=lin),
+                   args.steps, args.warmup)
     read = R * ((2 + Fs) * (4 * K + 4) + 4 * Fs + 4 * Fd + 16)          # SURVEY 8d: fwd bytes/row
     alg = read + R * (F * K + K + 1) * 4
     up, ip_ = users[:1 << 18].cpu().numpy(), items[:1 << 18].cpu().numpy()
-    ms_p = _timeit(lambda: model.logits(up, ip_), iters=5)
+    ms_p = _timeit(lambda: model.logits(up, ip_), args.steps, args.warmup)
     # ---- training step (collate + negatives come from the caller in the reference; here labels are given)
     tr = DeepFMTrainer(spec, w, use_bn=True, lr=1e-3)
     B = 8192
     tu, ti = users[:B].contiguous(), items[:B].contiguous()
     labels = torch.as_tensor((rng.random(B) < 1 / 6).astype(np.float32)).cuda()
-    ms_eager = _timeit(lambda: tr.step(tu, ti, labels), iters=20, warm=5)
+    ms_eager = _timeit(lambda: tr.step(tu, ti, labels), args.steps, args.warmup)
     # the same step captured once into a CUDA graph and replayed (launch-bound when issued from Python)
-    ms_t = _timeit(lambda: tr.step_graph(tu, ti, labels), iters=20, warm=5)
+    ms_t = _timeit(lambda: tr.step_graph(tu, ti, labels), args.steps, args.warmup)
     clocks = sampler.stop()
-    peaks = _peaks(root)
-    peak = float(peaks.get("hbm_gbs", 6650.0))
+    peak, peak_source = _hbm_peak(root)
     gbs = alg / (ms_g * 1e-3) / 1e9
     roofline = {"bound": "hbm", "kernel": "b200::feat::feat_forward_* (K1 gather + FM sums + deep-input write)",
                 "achieved": gbs, "peak": peak, "unit": "GB/s", "frac": gbs / peak, "traffic": None,
-                "peak_source": "MEASURED_PEAKS.json hbm_gbs (of measured)" if peaks else "fallback 6650 (of fallback)",
+                "peak_source": peak_source,
                 "avg_launch_ms": ms_g, "algorithmic_bytes_per_row": alg / R}
     config = {"workload": f"C3 DeepFM: {Fs} sparse + {Fd} dense columns, K {K}, hidden (128, 64, 32), "
                           f"{n_users} users x {n_items} items, shared sparse table {spec['sparse_vocab']} rows, "
                           f"batch {B} rows/step, one GPU (tables replicated)",
               "l2": "tables 1.3 GB > L2"}
-    return _line("training-step interactions/sec (DeepFM)", B / (ms_t * 1e-3), "interactions/s", 20, 5, ms_t, config,
+    return _line("training-step interactions/sec (DeepFM)", B / (ms_t * 1e-3), "interactions/s", args.steps, args.warmup, ms_t, config,
                  roofline, None, clocks,
                  {"predict_rows_per_s": (1 << 18) / (ms_p * 1e-3), "gather_rows_per_s": R / (ms_g * 1e-3),
                   "ms_per_step_eager_launches": ms_eager, "step": "CUDA graph replay (step_graph)",
                   "kernels_per_captured_step": int(getattr(tr, "graph_launches_per_step", 0)),
-                  "gpu_launches": int(_lib.launch_count()) + 25 * int(getattr(tr, "graph_launches_per_step", 0))})
+                  "gpu_launches": int(_lib.launch_count())
+                                  + (args.steps + args.warmup) * int(getattr(tr, "graph_launches_per_step", 0))})
 
 
 def c4(args, root, sampler):
@@ -133,22 +138,21 @@ def c4(args, root, sampler):
     users = rng.integers(0, n_users, R)
     items = rng.integers(0, n_items, R)
     sampler.start()
-    ms_p = _timeit(lambda: model.logits(users, items), iters=5)
+    ms_p = _timeit(lambda: model.logits(users, items), args.steps, args.warmup)
     uids = rng.integers(0, n_users, 16)
     model.recommend(uids[:2], 100, True)
-    ms_r = _timeit(lambda: model.recommend(uids, 100, True), iters=3, warm=1)
+    ms_r = _timeit(lambda: model.recommend(uids, 100, True), args.steps, args.warmup)
     clocks = sampler.stop()
     Kp = model.Kp
-    peaks = _peaks(root)
-    peak = float(peaks.get("hbm_gbs", 6650.0))
+    peak, peak_source = _hbm_peak(root)
     alg = R * ((2 + T) * 4 * Kp + 4 * T + 64)                            # SURVEY 8d a7 rows: bytes/row
     gbs = alg / (ms_p * 1e-3) / 1e9
     roofline = {"bound": "hbm", "kernel": "b200::seq::din_attention_kernel + K1 + MLP (predict rows)", "achieved": gbs,
                 "peak": peak, "unit": "GB/s", "frac": gbs / peak, "traffic": None, "avg_launch_ms": ms_p,
-                "peak_source": "MEASURED_PEAKS.json hbm_gbs (of measured)" if peaks else "fallback 6650 (of fallback)"}
+                "peak_source": peak_source}
     config = {"workload": f"C4 DIN: seq_len {T}, {n_users} users x {n_items} items, K {K}, K' {Kp}, "
                           f"hidden (128, 64, 32), one GPU", "l2": "item feature table 25 MB (L2 resident), rows 13 KB"}
-    return _line("DIN predict rows/sec", R / (ms_p * 1e-3), "rows/s", 5, 3, ms_p, config, roofline, None, clocks,
+    return _line("DIN predict rows/sec", R / (ms_p * 1e-3), "rows/s", args.steps, args.warmup, ms_p, config, roofline, None, clocks,
                  {"recommend_users_per_s": len(uids) / (ms_r * 1e-3), "recommend_batch": len(uids),
                   "gpu_launches": int(_lib.launch_count())})
 
@@ -175,25 +179,24 @@ def c5(args, root, sampler):
     E0 = torch.randn(n_users + n_items, d, device=dev, generator=g) * 0.1
     n, nnz = n_users + n_items, graph.nnz
     sampler.start()
-    ms = _timeit(lambda: propagate(graph, E0, layers), iters=5)
+    ms = _timeit(lambda: propagate(graph, E0, layers), args.steps, args.warmup)
     out = propagate(graph, E0, layers)
     scorer = EmbedScorer(out[:n_users], out[n_users:], n_items, csr, n_users=n_users, device=dev)
     uid = torch.randint(0, n_users, (8192,), device=dev, generator=g)
     scorer.recommend_device(uid, 100, True, False)
-    ms_s = _timeit(lambda: scorer.recommend_device(uid, 100, True, False), iters=5)
+    ms_s = _timeit(lambda: scorer.recommend_device(uid, 100, True, False), args.steps, args.warmup)
     clocks = sampler.stop()
     alg = layers * (nnz * (8 + 4 * d) + n * (4 * d + 8)) + layers * n * 4 * d      # SURVEY 8d a10 + layer-mean accumulate
-    peaks = _peaks(root)
-    peak = float(peaks.get("hbm_gbs", 6650.0))
+    peak, peak_source = _hbm_peak(root)
     gbs = alg / (ms * 1e-3) / 1e9
     roofline = {"bound": "hbm", "kernel": "b200::spmm_* (3 layers, layer mean fused)", "achieved": gbs, "peak": peak,
                 "unit": "GB/s", "frac": gbs / peak, "traffic": None, "avg_launch_ms": ms / layers,
                 "note": "algorithmic bytes count every gathered row as if it came from HBM; popular rows are served "
-                        "by the 126 MB L2, so this can read above 1",
-                "peak_source": "MEASURED_PEAKS.json hbm_gbs (of measured)" if peaks else "fallback 6650 (of fallback)"}
+                        "by the 50 MB L2, so this can read above 1",
+                "peak_source": peak_source}
     config = {"workload": f"C5 LightGCN: {layers}-layer propagation, {n_users} x {n_items} bipartite graph, nnz {nnz}, "
                           f"d {d}; then top-100 over {n_items} items for 8192 users", "l2": "E 563 MB + CSR 2.2 GB > L2"}
-    return _line("LightGCN propagation nnz/sec", layers * nnz / (ms * 1e-3), "nnz/s", 5, 3, ms, config, roofline, None, clocks,
+    return _line("LightGCN propagation nnz/sec", layers * nnz / (ms * 1e-3), "nnz/s", args.steps, args.warmup, ms, config, roofline, None, clocks,
                  {"serving_users_per_s": 8192 / (ms_s * 1e-3), "gpu_launches": int(_lib.launch_count())})
 
 
@@ -228,9 +231,12 @@ def c1(args, root, sampler):
     model = FM(spec, w, di.user_consumed)
     users = np.arange(di.n_users)
     sampler.start()
-    model.recommend(users[:64], 7, True)
+    for _ in range(args.warmup):
+        model.recommend(users, 7, True)
+        model.recommend(users, 100, True)
+    torch.cuda.synchronize()
     t0 = time.perf_counter()
-    iters = 5
+    iters = args.steps
     for _ in range(iters):
         model.recommend(users, 7, True)
         model.recommend(users, 100, True)
@@ -239,7 +245,7 @@ def c1(args, root, sampler):
     clocks = sampler.stop()
     config = {"workload": f"C1 FM on sample_movielens_merged ({di.n_users} users x {di.n_items} items, embed 16, 5 sparse "
                           "+ 1 dense columns): recommend_user for ALL users, n_rec 7 and 100 (two calls per step)"}
-    return _line("recommend_user users/sec (all-items top-K, FM)", 2 * di.n_users / (ms * 1e-3), "users/s", iters, 1, ms,
+    return _line("recommend_user users/sec (all-items top-K, FM)", 2 * di.n_users / (ms * 1e-3), "users/s", iters, args.warmup, ms,
                  config, None, None, clocks, {"gpu_launches": int(_lib.launch_count())})
 
 

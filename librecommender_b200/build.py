@@ -1,4 +1,4 @@
-"""Build the sm_100a shared library IN-TREE (``librecommender_b200/libb200reco.so``).
+"""Build the sm_90a shared library IN-TREE (``librecommender_b200/libb200reco.so``).
 
 nvcc cross-compiles without a GPU; the built ``.so`` is git-ignored but travels to
 the GPU box with the repo snapshot.
@@ -15,7 +15,7 @@ CSRC = os.path.join(PKG_DIR, "csrc")
 LIB_PATH = os.path.join(PKG_DIR, "libb200reco.so")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "-shared",
     "--use_fast_math=false",

@@ -1,4 +1,4 @@
-// Shared helpers for the sm_100a kernels of librecommender_b200.
+// Shared helpers for the sm_90a kernels of librecommender_b200.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -29,7 +29,13 @@ int check_cuda(cudaError_t e, const char* what);
 extern unsigned long long g_launch_count;
 inline void count_launch(int n = 1) { g_launch_count += (unsigned long long)n; }
 
-constexpr int kNumSMs = 148;
+// SM count of the current device (0 if it cannot be queried): launch sizing and the fused scorer's plan
+inline int num_sms() {
+  int dev = 0, n = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
+    return 0;
+  return n;
+}
 
 __host__ __device__ inline int64_t ceil_div64(int64_t a, int64_t b) { return (a + b - 1) / b; }
 

@@ -1056,7 +1056,7 @@ extern "C" int b200_feat_forward(const b200_feat_layout* L, const b200_feat_tabl
     const int n_id = ((L->id_mask & 1) ? 1 : 0) + ((L->id_mask & 2) ? 1 : 0);
     const int NS = (n_id + L->n_sparse + L->n_dense + FPW - 1) / FPW;
     if (NS <= 16) {
-      const unsigned blocks = (unsigned)std::min<int64_t>(ceil_div64(R, 8), (int64_t)148 * 2);
+      const unsigned blocks = (unsigned)std::min<int64_t>(ceil_div64(R, 8), (int64_t)std::max(1, num_sms()) * 2);
       cudaStream_t st = (cudaStream_t)stream;
       switch (K4v) {
         case 1: feat_forward_pipe_kernel<1><<<blocks, 256, 0, st>>>(*L, *T, users, items, R, grid_items, row_offset, o, h, NS); break;
@@ -1089,7 +1089,7 @@ extern "C" int b200_feat_forward(const b200_feat_layout* L, const b200_feat_tabl
       if (best_w >= 8) {
         const size_t dyn = best_wpb * per_warp + meta;
         const int64_t blocks_needed = ceil_div64(R, best_wpb);
-        const unsigned blocks = (unsigned)std::min<int64_t>(blocks_needed, (int64_t)148 * best_nb);
+        const unsigned blocks = (unsigned)std::min<int64_t>(blocks_needed, (int64_t)std::max(1, num_sms()) * best_nb);
         cudaStream_t st = (cudaStream_t)stream;
         auto launch = [&](auto kern) -> int {
           B200_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn));
@@ -1112,7 +1112,7 @@ extern "C" int b200_feat_forward(const b200_feat_layout* L, const b200_feat_tabl
   }
   if (group_ok) {
     // field-group kernel: persistent over rows (the per-block metadata staging is paid once per CTA)
-    const unsigned blocks = (unsigned)std::min<int64_t>(ceil_div64(R, 8), (int64_t)148 * 3);
+    const unsigned blocks = (unsigned)std::min<int64_t>(ceil_div64(R, 8), (int64_t)std::max(1, num_sms()) * 3);
     cudaStream_t st = (cudaStream_t)stream;
     switch (K4v) {
       case 1: feat_forward_fieldgroup_kernel<1><<<blocks, 256, 0, st>>>(*L, *T, users, items, R, grid_items, row_offset, o, h); break;

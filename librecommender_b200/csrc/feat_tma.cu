@@ -20,7 +20,7 @@
 // back to the register kernels of feat.cu otherwise.
 #include "common.cuh"
 #include "feat_common.cuh"
-#include "ptx_sm100.cuh"
+#include "ptx_sm90.cuh"
 #include "../../include/b200reco.h"
 
 namespace b200 {
@@ -245,12 +245,8 @@ int launch_feat_forward_tma(const b200_feat_layout* L, const b200_feat_tables* T
   o.ssum = ssum; o.sqsum = sqsum; o.ld_s = ld_s;
   FtHead h; h.lin_kernel = lin_kernel; h.lin_bias = lin_bias; h.bn_scale = bn_scale; h.bn_shift = bn_shift;
   h.pw_kernel = pw_kernel; h.pw_bias = pw_bias;
-  static int sm_count = 0;
-  if (!sm_count) {
-    int dev = 0;
-    B200_CUDA_OK(cudaGetDevice(&dev));
-    B200_CUDA_OK(cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, dev));
-  }
+  const int sm_count = num_sms();
+  B200_REQUIRE(sm_count > 0, "no CUDA device");
   const int ctas_per_sm = smem <= 110 * 1024 ? 2 : 1;
   const int64_t n_batches = (R + RB - 1) / RB;
   const int64_t want = (int64_t)sm_count * ctas_per_sm;

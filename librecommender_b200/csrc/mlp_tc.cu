@@ -1,36 +1,39 @@
-// Dense layer on the 5th-generation tensor cores with fp32-level accuracy: Y = act(X Wt^T + b).
+// Dense layer on the Hopper tensor cores (wgmma) with fp32-level accuracy: Y = act(X Wt^T + b).
 //
 // Replaces tf_dense (reference libreco/layers/dense.py:52-80, BN folded by the caller) for the MLP
 // tails of DeepFM / DIN / YouTubeRanking / TwoTower when the layer is large enough to be
 // compute-bound on the SIMT path (b200_linear_f32).  The reference computes these layers in fp32
 // (TensorFlow MatMul); a plain tf32 or bf16 tensor-core GEMM would miss the 1e-5 parity bar, so
 // the operands are split  x = hi + lo  (hi = top 11 mantissa bits, lo = next 11) and three
-// tcgen05.mma kind::tf32 products are accumulated:  hi*hi + lo*hi + hi*lo  (truncation keeps 10
-// explicit mantissa bits, |lo| < 2^-10 |x|: the dropped lo*lo term is < 2^-20 |x||w| and the two
-// truncated cross terms add < 2^-20 each; tests/test_tf32x3_model_cpu.py).  The tensor core truncates its fp32 accumulator once per MMA (measured: a
-// single accumulator over 48 MMAs drifts by ~2e-6 of sum|x w|), so (a) the dominant hi*hi products
-// and the 2^-11-times smaller cross products go to SEPARATE TMEM accumulators, and (b) both are
-// promoted to registers (round-to-nearest adds) every GC k-chunks = GC*4 MMAs per accumulator.
+// wgmma tf32 products are accumulated:  hi*hi + lo*hi + hi*lo  (truncation keeps 10 explicit
+// mantissa bits, |lo| < 2^-10 |x|: the dropped lo*lo term is < 2^-20 |x||w| and the two truncated
+// cross terms add < 2^-20 each; tests/test_tf32x3_model_cpu.py).  Both hi and lo are written
+// explicitly (hi in place of the loaded tile), so the result does not depend on how the tensor core
+// treats the 13 low mantissa bits of an fp32 container.  The dominant hi*hi products and the
+// 2^-11-times smaller cross products go to SEPARATE wgmma accumulators, and both are promoted to
+// fp32 registers (round-to-nearest adds) every GC k-chunks, so no accumulator runs over many MMAs.
 //
 // One persistent CTA per SM, warp-specialised:
-//   warp 0      TMA producer: X tile [128 x 32 fp32] and Wt tile [n_pad x 32 fp32] per k-chunk
-//   warp 1      MMA issuer (one elected lane)
-//   warps 2-5   splitters: write the `lo` tile next to every landed X tile (the X tile itself is the
-//               `hi` operand); the weight tiles arrive pre-split when the caller made a split copy
-//   warps 6-9   epilogue: TMEM -> registers (+=), then bias / ReLU / store at the end of a row tile
+//   warpgroups 0-1  split the landed tiles into hi / lo, issue the wgmma of rows [64 g, 64 g + 64) of
+//                   the 128-row tile, promote, and run the bias / ReLU / store epilogue
+//   warp 8          TMA producer: X tile [128 x 32 fp32] and Wt tile [n_pad x 32 fp32] per k-chunk
+//                   (the weight tiles arrive pre-split when the caller made a split copy)
+#include <type_traits>
 #include "common.cuh"
-#include "ptx_sm100.cuh"
+#include "ptx_sm90.cuh"
 #include "../../include/b200reco.h"
 
 namespace b200 {
 namespace mlp {
 
-constexpr int TM = 128;          // rows per tile (UMMA M)
+constexpr int TM = 128;          // rows per tile (two wgmma M = 64 warpgroups)
 constexpr int KC = 32;           // fp32 per k-chunk = one 128-byte swizzled row
 constexpr int GC = 2;            // k-chunks per accumulator group (promotion interval = 64 k)
 constexpr int NMAX = 128;        // output columns per CTA (grid.y covers wider layers)
 constexpr int MAXSTAGE = 4;
-constexpr int THREADS = 320;
+constexpr int CONSUMER_THREADS = 256;
+constexpr int THREADS = CONSUMER_THREADS + 128;   // + the producer warpgroup
+constexpr int PRODUCER_REGS = 40, CONSUMER_REGS = 232;
 constexpr int A_BYTES = TM * KC * 4;   // 16 KB
 
 struct Params {
@@ -46,38 +49,18 @@ struct Params {
 };
 
 struct Smem {
-  uint64_t full[MAXSTAGE], split[MAXSTAGE], empty[MAXSTAGE];
-  uint64_t tmem_full[2], tmem_empty[2];
-  uint32_t tmem_base;
-  uint32_t pad_[3];
-  float bias_s[NMAX];      // bias of this CTA's column block (0 past dout / without bias): the epilogue read 128
-                           // separate global words per thread and tile before — 27 % of the kernel's stall samples
+  uint64_t full[MAXSTAGE], empty[MAXSTAGE];
+  float bias_s[NMAX];      // bias of this CTA's column block (0 past dout / without bias)
 };
 
-__host__ __device__ constexpr uint32_t idesc_tf32(int M, int N) {
-  // D = f32 (1 @ bit 4), A = B = tf32 (2 @ bits 7, 10), both K-major, dense
-  return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(da), "l"(db), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
+__device__ __forceinline__ float hi_part(float x) { return __uint_as_float(__float_as_uint(x) & 0xffffe000u); }
 
 // x -> (hi, lo): hi keeps the 10 explicit mantissa bits of tf32, lo = x - hi (exact in fp32).
-// The tensor core reads 32-bit containers and ignores the 13 low mantissa bits (truncation —
-// verified by tests/test_gpu_linear_tc.py: a rounding conversion would show up as a 2^-11 error),
-// so the X tile itself serves as the `hi` operand and only the `lo` tile is written.
-__device__ __forceinline__ float lo_part(float x) {
-  return x - __uint_as_float(__float_as_uint(x) & 0xffffe000u);
-}
-__device__ __forceinline__ float4 lo4(const float4 v) {
-  return make_float4(lo_part(v.x), lo_part(v.y), lo_part(v.z), lo_part(v.w));
+__device__ __forceinline__ void split4(float4* hi, float4* lo) {
+  const float4 v = *hi;
+  const float4 h = make_float4(hi_part(v.x), hi_part(v.y), hi_part(v.z), hi_part(v.w));
+  *hi = h;
+  *lo = make_float4(v.x - h.x, v.y - h.y, v.z - h.z, v.w - h.w);
 }
 
 // weights: explicit hi / lo copies, made once per layer (b200_linear_tf32x3_split_weights)
@@ -87,21 +70,30 @@ __global__ void split_weights_kernel(const float* __restrict__ W, int64_t ldw, i
   if (i >= (int64_t)dout * ld) return;
   const int r = (int)(i / ld), c = (int)(i % ld);
   const float x = c < din ? W[(int64_t)r * ldw + c] : 0.f;
-  const float h = __uint_as_float(__float_as_uint(x) & 0xffffe000u);
+  const float h = hi_part(x);
   out[i] = h;
   out[(int64_t)dout * ld + i] = x - h;
 }
 
-// WSPLIT: tmW / tmWlo address the pre-split weight copies; otherwise the splitters also split the
-// weight tile of every stage (self-contained call, more shared-memory traffic).
-template <bool WSPLIT, bool DOT>
+// D (+)= A B^T for one k8 step at N = NP
+template <int NP>
+__device__ __forceinline__ void mma_tf32(float (&d)[NP / 2], uint64_t da, uint64_t db, bool first) {
+  if constexpr (NP == 32) { if (first) ptx::wgmma_tf32_n32_first(d, da, db); else ptx::wgmma_tf32_n32(d, da, db); }
+  if constexpr (NP == 64) { if (first) ptx::wgmma_tf32_n64_first(d, da, db); else ptx::wgmma_tf32_n64(d, da, db); }
+  if constexpr (NP == 96) { if (first) ptx::wgmma_tf32_n96_first(d, da, db); else ptx::wgmma_tf32_n96(d, da, db); }
+  if constexpr (NP == 128) { if (first) ptx::wgmma_tf32_n128_first(d, da, db); else ptx::wgmma_tf32_n128(d, da, db); }
+}
+
+// WSPLIT: tmW / tmWlo address the pre-split weight copies; otherwise the consumers also split the
+// weight tile of every stage (self-contained call, more shared-memory traffic).  NP = n_pad.
+template <bool WSPLIT, bool DOT, int NP>
 __global__ void __launch_bounds__(THREADS, 1)
 linear_tf32x3_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmW,
                      const __grid_constant__ CUtensorMap tmWlo, const Params p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-  const int b_bytes = p.n_pad * KC * 4;
-  const int stage_bytes = 2 * A_BYTES + 2 * b_bytes;
+  constexpr int b_bytes = NP * KC * 4;
+  constexpr int stage_bytes = 2 * A_BYTES + 2 * b_bytes;
   Smem* ss = (Smem*)(smem + (size_t)p.nstage * stage_bytes);
 
   const int warp = threadIdx.x >> 5;
@@ -113,33 +105,22 @@ linear_tf32x3_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_const
   if (threadIdx.x == 0) {
     for (int s = 0; s < p.nstage; ++s) {
       ptx::mbar_init(&ss->full[s], 1);
-      ptx::mbar_init(&ss->split[s], 4);
-      ptx::mbar_init(&ss->empty[s], 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      ptx::mbar_init(&ss->tmem_full[a], 1);
-      ptx::mbar_init(&ss->tmem_empty[a], 4);
+      ptx::mbar_init(&ss->empty[s], CONSUMER_THREADS / 32);
     }
     ptx::fence_barrier_init();
     ptx::prefetch_tensormap(&tmX);
     ptx::prefetch_tensormap(&tmW);
   }
-  if (warp == 1) {
-    ptx::tmem_alloc(&ss->tmem_base, 4 * NMAX);
-    ptx::tmem_relinquish();
-  }
-  if (threadIdx.x >= 64 && threadIdx.x < 64 + NMAX) {
-    const int c = threadIdx.x - 64;
+  if (threadIdx.x < NMAX) {
+    const int c = threadIdx.x;
     ss->bias_s[c] = (p.bias && col0 + c < p.dout) ? __ldg(p.bias + col0 + c) : 0.f;
   }
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = ss->tmem_base;
 
-  if (warp == 0) {
+  if (threadIdx.x >= CONSUMER_THREADS) {
+    ptx::setmaxnreg_dec<PRODUCER_REGS>();
     // ===================== TMA producer =====================
-    if (lane == 0) {
+    if (threadIdx.x == CONSUMER_THREADS) {
       int stage = 0;
       uint32_t phase = 0;
       for (int tile = blockIdx.x; tile < p.n_tiles; tile += gridDim.x) {
@@ -155,164 +136,107 @@ linear_tf32x3_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_const
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      const uint32_t idesc = idesc_tf32(TM, p.n_pad);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      const uint32_t s_addr = ptx::smem_u32(smem);
-      for (int tile = blockIdx.x; tile < p.n_tiles; tile += gridDim.x) {
-        for (int kc = 0; kc < kc_count; ++kc) {
-          const int gpos = kc % GC;
-          if (gpos == 0) {   // new accumulator group
-            ptx::mbar_wait(&ss->tmem_empty[acc], acc_phase ^ 1);
-            ptx::tc_fence_after();
-          }
-          ptx::mbar_wait(&ss->split[stage], phase);
-          ptx::tc_fence_after();
-          const uint32_t st = s_addr + (uint32_t)(stage * stage_bytes);
-          const uint64_t a_hi = ptx::umma_desc_sw128_kmajor(st);
-          const uint64_t a_lo = ptx::umma_desc_sw128_kmajor(st + A_BYTES);
-          const uint64_t b_hi = ptx::umma_desc_sw128_kmajor(st + 2 * A_BYTES);
-          const uint64_t b_lo = ptx::umma_desc_sw128_kmajor(st + 2 * A_BYTES + b_bytes);
-          const uint32_t d_main = tmem_base + (uint32_t)(acc * 2 * NMAX);   // hi*hi
-          const uint32_t d_corr = d_main + NMAX;                            // lo*hi + hi*lo
+    return;
+  }
+
+  // ===================== consumers: split, MMA, promote, epilogue =====================
+  ptx::setmaxnreg_inc<CONSUMER_REGS>();
+  const int t = threadIdx.x;                 // 0..255
+  const int g = warp >> 2;
+  const int quad = lane >> 2, tq = lane & 3;
+  const int trow0 = 64 * g + 16 * (warp & 3) + quad;   // rows trow0 and trow0 + 8 of the tile
+  const uint32_t s_addr = ptx::smem_u32(smem);
+  int stage = 0;
+  uint32_t phase = 0;
+  float acc_main[NP / 2], acc_corr[NP / 2];
+  for (int tile = blockIdx.x; tile < p.n_tiles; tile += gridDim.x) {
+    float y[NP / 2];
 #pragma unroll
-          for (int k4 = 0; k4 < KC / 8; ++k4) {
-            // 8 tf32 = 32 bytes per MMA inside the 128-byte swizzled row: +2 in the >>4 field
-            const uint64_t o = (uint64_t)(k4 * 2);
-            const uint32_t cont = (uint32_t)((gpos | k4) != 0);
-            umma_tf32(d_main, a_hi + o, b_hi + o, idesc, cont);
-            umma_tf32(d_corr, a_lo + o, b_hi + o, idesc, cont);
-            umma_tf32(d_corr, a_hi + o, b_lo + o, idesc, 1u);
-          }
-          ptx::umma_commit(&ss->empty[stage]);
-          if (++stage == p.nstage) { stage = 0; phase ^= 1; }
-          if (gpos == GC - 1 || kc == kc_count - 1) {
-            ptx::umma_commit(&ss->tmem_full[acc]);
-            acc ^= 1;
-            if (acc == 0) acc_phase ^= 1;
-          }
-        }
+    for (int i = 0; i < NP / 2; ++i) y[i] = 0.f;
+    for (int kc = 0; kc < kc_count; ++kc) {
+      const int gpos = kc % GC;
+      ptx::mbar_wait(&ss->full[stage], phase);
+      uint8_t* st = smem + (size_t)stage * stage_bytes;
+#pragma unroll
+      for (int j = 0; j < A_BYTES / 16 / CONSUMER_THREADS; ++j)
+        split4((float4*)st + t + j * CONSUMER_THREADS, (float4*)(st + A_BYTES) + t + j * CONSUMER_THREADS);
+      if (!WSPLIT)
+        for (int j = t; j < b_bytes / 16; j += CONSUMER_THREADS)
+          split4((float4*)(st + 2 * A_BYTES) + j, (float4*)(st + 2 * A_BYTES + b_bytes) + j);
+      ptx::fence_proxy_async_smem();         // generic-proxy writes -> visible to the tensor core
+      ptx::named_bar_sync(1, CONSUMER_THREADS);
+      ptx::wgmma_fence();
+      const uint32_t sa = s_addr + (uint32_t)(stage * stage_bytes) + (uint32_t)(g * 64 * KC * 4);
+      const uint64_t a_hi = ptx::wgmma_desc_sw128_kmajor(sa);
+      const uint64_t a_lo = ptx::wgmma_desc_sw128_kmajor(sa + A_BYTES);
+      const uint64_t b_hi = ptx::wgmma_desc_sw128_kmajor(s_addr + (uint32_t)(stage * stage_bytes + 2 * A_BYTES));
+      const uint64_t b_lo = ptx::wgmma_desc_sw128_kmajor(s_addr + (uint32_t)(stage * stage_bytes + 2 * A_BYTES + b_bytes));
+#pragma unroll
+      for (int k4 = 0; k4 < KC / 8; ++k4) {
+        // 8 tf32 = 32 bytes per MMA inside the 128-byte swizzled row: +2 in the >>4 field
+        const uint64_t o = (uint64_t)(k4 * 2);
+        const bool first = gpos == 0 && k4 == 0;
+        mma_tf32<NP>(acc_main, a_hi + o, b_hi + o, first);
+        mma_tf32<NP>(acc_corr, a_lo + o, b_hi + o, first);
+        mma_tf32<NP>(acc_corr, a_hi + o, b_lo + o, false);
+      }
+      ptx::wgmma_commit();
+      ptx::wgmma_wait<0>(acc_main);
+      ptx::wgmma_wait<0>(acc_corr);
+      __syncwarp();
+      if (lane == 0) ptx::mbar_arrive(&ss->empty[stage]);
+      if (++stage == p.nstage) { stage = 0; phase ^= 1; }
+      if (gpos == GC - 1 || kc == kc_count - 1) {
+#pragma unroll
+        for (int i = 0; i < NP / 2; ++i) y[i] = (y[i] + acc_corr[i]) + acc_main[i];   // correction first
       }
     }
-  } else if (warp < 6) {
-    // ===================== splitters =====================
-    const int t = threadIdx.x - 64;          // 0..127
-    int stage = 0;
-    uint32_t phase = 0;
-    const int b_vec = b_bytes / 16;          // float4 per B tile
-    for (int tile = blockIdx.x; tile < p.n_tiles; tile += gridDim.x) {
-      for (int kc = 0; kc < kc_count; ++kc) {
-        ptx::mbar_wait(&ss->full[stage], phase);
-        uint8_t* st = smem + (size_t)stage * stage_bytes;
-        float4* ah = (float4*)st;
-        float4* al = (float4*)(st + A_BYTES);
+    // fragment: y[4 j + 2 rs + e] = row trow0 + 8 rs, column 8 j + 2 tq + e
+    const int ncol = min(p.dout - col0, NMAX);
 #pragma unroll
-        for (int j = 0; j < A_BYTES / 16 / 128; ++j) al[t + j * 128] = lo4(ah[t + j * 128]);
-        if (!WSPLIT) {
-          const float4* bh = (const float4*)(st + 2 * A_BYTES);
-          float4* bl = (float4*)(st + 2 * A_BYTES + b_bytes);
-          for (int j = t; j < b_vec; j += 128) bl[j] = lo4(bh[j]);
-        }
-        ptx::fence_proxy_async_smem();       // generic-proxy writes -> visible to the tensor core
-        __syncwarp();
-        if (lane == 0) ptx::mbar_arrive(&ss->split[stage]);
-        if (++stage == p.nstage) { stage = 0; phase ^= 1; }
-      }
-    }
-  } else {
-    // ===================== epilogue =====================
-    const int q = warp & 3;                  // TMEM lane quadrant this warp may read
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    const int n_groups = (kc_count + GC - 1) / GC;
-    for (int tile = blockIdx.x; tile < p.n_tiles; tile += gridDim.x) {
-      float y[NMAX];
-#pragma unroll
-      for (int i = 0; i < NMAX; ++i) y[i] = 0.f;
-      for (int g = 0; g < n_groups; ++g) {
-        ptx::mbar_wait(&ss->tmem_full[acc], acc_phase);
-        ptx::tc_fence_after();
-        const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * 2 * NMAX);
-#pragma unroll
-        for (int c = 0; c < NMAX / 32; ++c) {
-          if (c * 32 < p.n_pad) {
-            uint32_t r[32];
-            ptx::tmem_ld_32x32b_x32(taddr + (uint32_t)(NMAX + c * 32), r);     // correction first
-            ptx::tmem_ld_wait_regs(r);
-#pragma unroll
-            for (int i = 0; i < 32; ++i) y[c * 32 + i] += __uint_as_float(r[i]);
-            ptx::tmem_ld_32x32b_x32(taddr + (uint32_t)(c * 32), r);
-            ptx::tmem_ld_wait_regs(r);
-#pragma unroll
-            for (int i = 0; i < 32; ++i) y[c * 32 + i] += __uint_as_float(r[i]);
-          }
-        }
-        ptx::tc_fence_before();
-        __syncwarp();
-        if (lane == 0) ptx::mbar_arrive(&ss->tmem_empty[acc]);
-        acc ^= 1;
-        if (acc == 0) acc_phase ^= 1;
-      }
-      const int64_t row = (int64_t)tile * TM + q * 32 + lane;
-      if (DOT && row < p.R) {
+    for (int rs = 0; rs < 2; ++rs) {
+      const int64_t row = (int64_t)tile * TM + trow0 + 8 * rs;
+      if (DOT) {
         // fused attention epilogue (DIN all-items): per group of 16 columns ONE output
         //   a[row, (col0 + 16 g) / 16] = sum_j dot_w[j] * sigmoid(y[16 g + j] + bias)
         // the [R, dout] pre-activations (16x the bytes) are never written
-        const int ncol = min(p.dout - col0, NMAX);
-        float w2[16];
-#pragma unroll
-        for (int j = 0; j < 16; ++j) w2[j] = __ldg(p.dot_w + j);
         float* yd = p.Y + row * p.ldy + col0 / 16;
 #pragma unroll
-        for (int g = 0; g < NMAX / 16; ++g) {
-          if (g * 16 < ncol) {
-            float a = 0.f;
+        for (int gg = 0; gg < NP / 16; ++gg) {
+          float a = 0.f;
 #pragma unroll
-            for (int j = 0; j < 16; ++j) {
-              const int c = g * 16 + j;
-              const float v = y[c] + ss->bias_s[c];
-              a = fmaf(w2[j], 1.0f / (1.0f + expf(-v)), a);
+          for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int cj = 8 * h + 2 * tq + e;          // column inside the group of 16
+              const float v = y[4 * (2 * gg + h) + 2 * rs + e] + ss->bias_s[16 * gg + cj];
+              a = fmaf(__ldg(p.dot_w + cj), 1.0f / (1.0f + expf(-v)), a);
             }
-            yd[g] = a;
-          }
+          a += __shfl_xor_sync(0xffffffffu, a, 1);
+          a += __shfl_xor_sync(0xffffffffu, a, 2);
+          if (tq == 0 && gg * 16 < ncol && row < p.R) yd[gg] = a;
         }
-      } else if (!DOT && row < p.R) {
+      } else if (row < p.R) {
         float* yr = p.Y + (int64_t)blockIdx.z * p.split_stride + row * p.ldy + col0;
-        const int ncol = min(p.dout - col0, NMAX);
-        const bool vec = ((p.ldy & 3) == 0) && ((((uintptr_t)p.Y) & 15) == 0);
+        const bool vec = ((p.ldy & 1) == 0) && ((((uintptr_t)p.Y) & 7) == 0);
 #pragma unroll
-        for (int c4 = 0; c4 < NMAX / 4; ++c4) {
-          if (c4 * 4 < ncol) {
-            float o[4];
+        for (int j = 0; j < NP / 8; ++j) {
+          const int c = 8 * j + 2 * tq;
+          float o[2];
 #pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              const int c = c4 * 4 + i;
-              float v = y[c] + ss->bias_s[c];
-              o[i] = p.relu ? fmaxf(v, 0.f) : v;
-            }
-            if (vec && c4 * 4 + 3 < ncol) {
-              *(float4*)(yr + c4 * 4) = make_float4(o[0], o[1], o[2], o[3]);
-            } else {
-#pragma unroll
-              for (int i = 0; i < 4; ++i)
-                if (c4 * 4 + i < ncol) yr[c4 * 4 + i] = o[i];
-            }
+          for (int e = 0; e < 2; ++e) {
+            const float v = y[4 * j + 2 * rs + e] + ss->bias_s[c + e];
+            o[e] = p.relu ? fmaxf(v, 0.f) : v;
+          }
+          if (vec && c + 1 < ncol) {
+            *(float2*)(yr + c) = make_float2(o[0], o[1]);
+          } else {
+            if (c < ncol) yr[c] = o[0];
+            if (c + 1 < ncol) yr[c + 1] = o[1];
           }
         }
       }
     }
-  }
-
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    ptx::tc_fence_after();
-    ptx::tmem_dealloc(tmem_base, 4 * NMAX);
   }
 }
 
@@ -462,28 +386,32 @@ static int launch_linear_tf32x3(const float* X, int64_t ldx, int64_t R, const fl
     tmWlo = tmW;
   }
 
-  static bool attr_set = false;
-  if (!attr_set) {
-    B200_CUDA_OK(cudaFuncSetAttribute(linear_tf32x3_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
-    B200_CUDA_OK(cudaFuncSetAttribute(linear_tf32x3_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
-    B200_CUDA_OK(cudaFuncSetAttribute(linear_tf32x3_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
-    B200_CUDA_OK(cudaFuncSetAttribute(linear_tf32x3_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
-    attr_set = true;
-  }
-  int dev = 0, sms = 148;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  const int sms = num_sms();
+  B200_REQUIRE(sms > 0, "no CUDA device");
   const int gy = (dout + NMAX - 1) / NMAX;
   const int gx = max(1, min(p.n_tiles, sms / (gy * splits)));
   const dim3 grid(gx, gy, splits);
   cudaStream_t st = (cudaStream_t)stream;
-  if (dot_w) {
-    if (Wsplit) linear_tf32x3_kernel<true, true><<<grid, THREADS, smem, st>>>(tmX, tmW, tmWlo, p);
-    else linear_tf32x3_kernel<false, true><<<grid, THREADS, smem, st>>>(tmX, tmW, tmWlo, p);
-  } else {
-    if (Wsplit) linear_tf32x3_kernel<true, false><<<grid, THREADS, smem, st>>>(tmX, tmW, tmWlo, p);
-    else linear_tf32x3_kernel<false, false><<<grid, THREADS, smem, st>>>(tmX, tmW, tmWlo, p);
-  }
+  auto launch = [&](auto kernel) -> int {
+    B200_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
+    kernel<<<grid, THREADS, smem, st>>>(tmX, tmW, tmWlo, p);
+    return 0;
+  };
+  auto by_width = [&](auto wsplit, auto dot) -> int {
+    constexpr bool WS = decltype(wsplit)::value, DT = decltype(dot)::value;
+    switch (p.n_pad) {
+      case 32: return launch(linear_tf32x3_kernel<WS, DT, 32>);
+      case 64: return launch(linear_tf32x3_kernel<WS, DT, 64>);
+      case 96: return launch(linear_tf32x3_kernel<WS, DT, 96>);
+      default: return launch(linear_tf32x3_kernel<WS, DT, 128>);
+    }
+  };
+  using T = std::true_type;
+  using F = std::false_type;
+  int rc;
+  if (dot_w) rc = Wsplit ? by_width(T{}, T{}) : by_width(F{}, T{});
+  else rc = Wsplit ? by_width(T{}, F{}) : by_width(F{}, F{});
+  if (rc) return rc;
   if (splits > 1) {
     const int64_t n = R * (int64_t)dout;
     splitk_reduce_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(workspace, splits, R, dout, bias, relu, Y, ldy);

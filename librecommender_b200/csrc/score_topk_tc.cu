@@ -1,4 +1,4 @@
-// K4 — fused user x all-items scoring + consumed filter + top-K on the 5th-gen tensor cores.
+// K4 — fused user x all-items scoring + consumed filter + top-K on the Hopper tensor cores (wgmma).
 //
 // Replaces recommend_from_embedding + rank_recommendations
 // (libreco/recommendation/recommend.py:57-78, ranking.py:10-78) without ever materialising
@@ -13,10 +13,10 @@
 //                maximum coarse score of each sampled 128-item block (one coalesced store per
 //                tile, no divergence); guess_kernel turns the block maxima into a SPECULATIVE
 //                per-row threshold (the pre_k-th largest block maximum).
-//   sweep<MAIN>  persistent tcgen05 kernel over all item tiles: TMA -> smem (SWIZZLE_128B) ->
-//                tcgen05.mma (fp16 in, fp32 accumulate in TMEM, 128x256 tile, double-buffered
-//                accumulator) -> epilogue warps read TMEM (tcgen05.ld) and keep, per user row,
-//                every item whose COARSE score is >= tau.  tau starts at the speculative value and
+//   sweep<MAIN>  persistent wgmma kernel over all item tiles: TMA -> smem (SWIZZLE_128B, multi-stage
+//                ring, item tiles shared by a 2-CTA cluster through TMA multicast) -> wgmma (fp16 in,
+//                fp32 accumulate in registers, 128x256 tile = two warpgroups x 64 user rows) -> the
+//                same warpgroups keep, per user row, every item whose COARSE score is >= tau.  tau starts at the speculative value and
 //                is only ever raised by a rigorous bound: (k_row-th best coarse score counted so
 //                far in the row's global histogram) - 2*eps.
 //   finalize     per row: exact k_row-th coarse score c_k over the union of the lists; checks that
@@ -42,27 +42,24 @@
 // near-ties) are flagged in row_status and re-run by the caller on the exact materialised path.
 #include <type_traits>
 #include "common.cuh"
-#include "ptx_sm100.cuh"
+#include "ptx_sm90.cuh"
 #include "../../include/b200reco.h"
 #include <cuda_fp16.h>
 
 namespace b200 {
 namespace tc {
 
-constexpr int TM = 128;        // users per tile (UMMA M)
-constexpr int TN = 256;        // items per tile (UMMA N)
+constexpr int TM = 128;        // users per tile (two wgmma M = 64 warpgroups)
+constexpr int TN = 256;        // items per tile (wgmma N)
 constexpr int KBLK = 64;       // fp16 per 128-byte swizzled row
 constexpr int CAPG_MAX = 256;  // candidate GROUP records per (row, list), upper limit (runtime capg <= this)
 constexpr int GW = 8;          // a record = the 8 coarse scores of one 8-column group + its first item id ...
 constexpr int REC = 12;        // ... in 12 words (48 bytes: two 16-byte score halves, the id, padding)
 constexpr int NB = 1024;       // bins of the per-row global coarse-score histogram
-constexpr int STEP = 64;       // accumulator columns per epilogue step (one tcgen05.ld.32x32b.x64)
-constexpr int STEPS_PER_TILE = TN / STEP;   // 4
-// Epilogue organisation: W warps per TMEM lane quadrant (4 quadrants => 4W epilogue warps).  The
-// 64-column steps of every tile are dealt to the W warps of a quadrant (W = 2: two adjacent steps
-// each, W = 4: one step each, W = 3: round-robin over the running step count).  Each warp owns one
-// candidate list per (row, item split): n_lists = W * n_splits.
-constexpr int W_PRE = 2;       // the pre-pass always runs with 2 warps per quadrant (block = 128 columns)
+constexpr int STEP = 64;       // accumulator columns per epilogue vote
+// Every (row, item split) has two candidate lists, one per 128-column half of the item tiles:
+// n_lists = 2 * n_splits.  The pre-pass records one block maximum per row and half (block = 128 items).
+constexpr int W_PRE = 2;
 constexpr int KROW_MAX = 288;  // fast-path limit for k_row = K + c_u
 constexpr int MAX_KB = 4;      // d_pad <= 256
 constexpr int PRE_STRIDE = 16; // the pre-pass visits every 16th item tile of a split
@@ -75,7 +72,12 @@ constexpr int FIN_THREADS = 256;
 // fp16 x fp16 products, both operands rounded to nearest: (1 + 2^-11)^2 - 1 = 2^-10 (1 + 2^-12)
 constexpr float ERR_COEF = 0.00097705f;
 
-__host__ __device__ constexpr int sweep_threads(int W) { return 64 + 128 * W; }
+constexpr int SWEEP_CONSUMER_WARPS = 8;   // two warpgroups: wgmma M = 64 user rows each
+constexpr int WARP_TMA = SWEEP_CONSUMER_WARPS;   // first warp of the producer warpgroup
+// registers are handed out per warpgroup: the producer warpgroup gives most of its share to the two
+// consumer warpgroups (128 accumulator registers per thread plus the epilogue state, no spills)
+constexpr int SWEEP_THREADS = 32 * (SWEEP_CONSUMER_WARPS + 4);
+constexpr int SWEEP_PRODUCER_REGS = 40, SWEEP_CONSUMER_REGS = 232;
 
 struct CatalogHeader {   // first 256 bytes of the catalog buffer (device)
   uint32_t max_norm_bits;  // max_i ||I_i||_2 of the UNSCALED rows (fp32 bits; non-negative so uint order == float order)
@@ -227,12 +229,8 @@ __global__ void prep_users_kernel(const float* __restrict__ U, int64_t ldu,
 struct SweepSmem {
   uint64_t full[8];
   uint64_t empty[8];
-  uint64_t tmem_full[2][2];    // [accumulator stage][column half]
-  uint64_t tmem_empty[2][2];
   uint64_t a_full;
   uint64_t a_empty;
-  uint32_t tmem_base;
-  uint32_t pad_[3];
 };
 
 __device__ __forceinline__ int score_bin(float s, float R, float inv_w) {
@@ -340,11 +338,26 @@ __device__ __forceinline__ float fmax3(float a, float b, float c) { return fmaxf
 // ADJACENT user tiles of the SAME item split in lock step: every item tile is fetched from L2 once
 // per cluster — each CTA loads half of it and the TMA multicasts that half into both CTAs' shared
 // memory — which halves the L2 -> SM traffic of the item table (the pass is L2-bandwidth bound
-// otherwise: 64 user tiles x 128 MB per launch at C2).  NH = MMA groups per item tile (2: two N=128
-// halves with their own accumulator barriers, 1: one N=256 group, the user tile is read from shared
-// memory once per k-step instead of twice).
-template <bool PRE, int W, int EPI, int CL, int NH>
-__global__ void __launch_bounds__(sweep_threads(W), 1)
+// otherwise).  NH = MMA groups per item tile (1: one N=256 wgmma chain; 2: two N=128 chains into
+// separate accumulators, the epilogue of the first runs while the tensor core computes the second).
+// EPI = record stores of a hot 64-column step: 3 divergent per-group branches, 5 predicated stores.
+//
+// Threads: warpgroups 0 and 1 issue the wgmma of user rows [64 g, 64 g + 64) of the tile and run the
+// epilogue on the accumulator registers; one lane of warpgroup 2 is the TMA producer.  In the m64nN fragment, lane
+// (4 quad + tq) of warp w holds rows 16 w + quad and 16 w + quad + 8, columns 8 j + 2 tq + {0, 1}:
+// the 8 columns of a group are spread over the 4 lanes of a quad, which reduce the group maximum
+// with two shuffles and write the 48-byte record together (8 bytes each, the id from lane tq = 0).
+// Lane tq of a quad also owns one (row, list) pair — row quad + 8 (tq >> 1), list tq & 1 — for
+// the warp-wide bookkeeping (compaction votes, list lengths, pre-pass maxima).
+__device__ __forceinline__ int sel22(const int (&c)[2][2], int rs, int j) {
+  return rs ? (j ? c[1][1] : c[1][0]) : (j ? c[0][1] : c[0][0]);
+}
+__device__ __forceinline__ void set22(int (&c)[2][2], int rs, int j, int v) {
+  if (rs) { if (j) c[1][1] = v; else c[1][0] = v; } else { if (j) c[0][1] = v; else c[0][0] = v; }
+}
+
+template <bool PRE, int EPI, int CL, int NH>
+__global__ void __launch_bounds__(SWEEP_THREADS, 1)
 sweep_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
              const __grid_constant__ CUtensorMap tmBh, const SweepParams p) {
   extern __shared__ uint8_t smem_raw[];
@@ -363,41 +376,27 @@ sweep_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
   const int n_units = m_groups * p.n_splits;              // units per cluster-rank
   constexpr int STRIDE = PRE ? PRE_STRIDE : 1;
   constexpr uint16_t CL_MASK = (uint16_t)((1u << CL) - 1u);
-  // Warp roles.  The warp scheduler of an SM sub-partition prefers the HIGHEST warp id among its
-  // ready warps, so the two single-lane roles that feed the tensor core (MMA issuer, TMA producer)
-  // take the two highest warp ids: they are asleep on an mbarrier most of the time and must win the
-  // issue slot the moment they wake up, ahead of the always-busy epilogue warps of their sub-partition.
-  constexpr int WARP_MMA = 4 * W, WARP_TMA = 4 * W + 1;   // epilogue: warps 0 .. 4W-1 (quadrant = warp % 4)
 
   if (threadIdx.x == 0) {
     // a shared-memory stage is written by the multicasts of all CL producers and may be refilled only
-    // when the MMAs of all CL CTAs have read it: `empty` collects one (multicast) commit per CTA
-    for (int s = 0; s < p.nstage; ++s) { ptx::mbar_init(&ss->full[s], 1); ptx::mbar_init(&ss->empty[s], CL); }
-    for (int a = 0; a < 2; ++a)
-      for (int hh = 0; hh < 2; ++hh) {
-        ptx::mbar_init(&ss->tmem_full[a][hh], 1);
-        // one arrival per processed step: 4 lane quadrants x the steps of one MMA group
-        ptx::mbar_init(&ss->tmem_empty[a][hh], 4 * (STEPS_PER_TILE / NH));
-      }
+    // when every consumer warp of all CL CTAs has finished its MMAs on it
+    for (int s = 0; s < p.nstage; ++s) {
+      ptx::mbar_init(&ss->full[s], 1);
+      ptx::mbar_init(&ss->empty[s], SWEEP_CONSUMER_WARPS * CL);
+    }
     ptx::mbar_init(&ss->a_full, 1);
-    ptx::mbar_init(&ss->a_empty, 1);
+    ptx::mbar_init(&ss->a_empty, SWEEP_CONSUMER_WARPS);
     ptx::fence_barrier_init();
     ptx::prefetch_tensormap(&tmA);
     ptx::prefetch_tensormap(&tmB);
   }
-  if (warp == WARP_MMA) {
-    ptx::tmem_alloc(&ss->tmem_base, 512);
-    ptx::tmem_relinquish();
-  }
-  ptx::tc_fence_before();
   __syncthreads();
   if (CL > 1) ptx::cluster_sync_all();     // the peer's barriers exist before anything is multicast to them
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = ss->tmem_base;
 
-  if (warp == WARP_TMA) {
-    // ===================== TMA producer =====================
-    if (lane == 0) {
+  if (warp >= WARP_TMA) {
+    ptx::setmaxnreg_dec<SWEEP_PRODUCER_REGS>();
+    // ===================== TMA producer (one lane of the last warpgroup) =====================
+    if (warp == WARP_TMA && lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
       uint32_t uiter = 0;
@@ -442,322 +441,242 @@ sweep_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
         }
       }
     }
-  } else if (warp == WARP_MMA) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      constexpr uint32_t idesc = ptx::umma_idesc_f16_f32(TM, TN / NH);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      uint32_t uiter = 0;
-      const uint32_t a_addr = ptx::smem_u32(smemA);
-      const uint32_t b_addr = ptx::smem_u32(smemB);
-      for (int unit = cid; unit < n_units; unit += n_clusters, ++uiter) {
-        const int split = unit / m_groups;
-        const int t0 = split * p.tiles_per_split;
-        const int t1 = min(t0 + p.tiles_per_split, p.total_tiles);
-        ptx::mbar_wait_hint(&ss->a_full, uiter & 1, p.hint_ns);
-        for (int t = t0; t < t1; t += STRIDE) {
-          if (p.kb_stages) {
-            // k-block stages (NH == 1): the accumulator of the tile is built block by block, every stage is handed
-            // back as soon as its four MMAs have read it
-            ptx::mbar_wait_hint(&ss->tmem_empty[acc][0], acc_phase ^ 1, p.hint_ns);
-            ptx::tc_fence_after();
-            const uint32_t d_tmem = tmem_base + (uint32_t)(acc * TN);
-            for (int kb = 0; kb < p.KB; ++kb) {
-              ptx::mbar_wait_hint(&ss->full[stage], phase, p.hint_ns);
-              ptx::tc_fence_after();
-              const uint64_t da = ptx::umma_desc_sw128_kmajor(a_addr + (uint32_t)(kb * A_KB_BYTES));
-              const uint64_t db = ptx::umma_desc_sw128_kmajor(b_addr + (uint32_t)(stage * B_KB_BYTES));
-#pragma unroll
-              for (int k4 = 0; k4 < KBLK / 16; ++k4)
-                ptx::umma_f16(d_tmem, da + (uint64_t)(k4 * 2), db + (uint64_t)(k4 * 2), idesc, (uint32_t)((kb | k4) != 0));
-              if (CL == 1) ptx::umma_commit(&ss->empty[stage]);
-              else ptx::umma_commit_multicast(&ss->empty[stage], CL_MASK);
-              if (++stage == p.nstage) { stage = 0; phase ^= 1; }
-            }
-            ptx::umma_commit(&ss->tmem_full[acc][0]);
-            acc ^= 1;
-            if (acc == 0) acc_phase ^= 1;
-            continue;
-          }
-          ptx::mbar_wait_hint(&ss->full[stage], phase, p.hint_ns);
-          // NH MMA groups per item tile, each with its own accumulator full / empty barrier pair, so the
-          // epilogue steps of a group start as soon as that group is done
-#pragma unroll
-          for (int hh = 0; hh < NH; ++hh) {
-            ptx::mbar_wait_hint(&ss->tmem_empty[acc][hh], acc_phase ^ 1, p.hint_ns);
-            ptx::tc_fence_after();
-            const uint32_t d_tmem = tmem_base + (uint32_t)(acc * TN + hh * (TN / NH));
-            for (int kb = 0; kb < p.KB; ++kb) {
-              const uint64_t da = ptx::umma_desc_sw128_kmajor(a_addr + (uint32_t)(kb * A_KB_BYTES));
-              const uint64_t db = ptx::umma_desc_sw128_kmajor(
-                  b_addr + (uint32_t)((stage * p.KB + kb) * B_KB_BYTES + hh * (TN / NH) * KBLK * 2));
-#pragma unroll
-              for (int k4 = 0; k4 < KBLK / 16; ++k4) {
-                // advance 16 fp16 = 32 bytes inside the 128-byte swizzled row: +2 in the >>4 field
-                ptx::umma_f16(d_tmem, da + (uint64_t)(k4 * 2), db + (uint64_t)(k4 * 2), idesc,
-                              (uint32_t)((kb | k4) != 0));
-              }
-            }
-            ptx::umma_commit(&ss->tmem_full[acc][hh]);   // this group is ready for its epilogue steps
-          }
-          // the shared-memory stage is reusable (in every CTA of the cluster) when these MMAs have read it
-          if (CL == 1) ptx::umma_commit(&ss->empty[stage]);
-          else ptx::umma_commit_multicast(&ss->empty[stage], CL_MASK);
-          if (++stage == p.nstage) { stage = 0; phase ^= 1; }
-          acc ^= 1;
-          if (acc == 0) acc_phase ^= 1;
-        }
-        ptx::umma_commit(&ss->a_empty);             // A tile reusable after the unit's last MMA
-      }
-    }
   } else {
-    // ===================== epilogue: 4 TMEM lane quadrants x W warps ==========
-    const int q = warp & 3;                 // TMEM lanes [32q, 32q+32) (hardware: warp id % 4)
-    const int j = warp >> 2;                // warp index inside its quadrant
-    const int trow = q * 32 + lane;         // row inside the tile
-    uint32_t tc = 0;                        // running tile count of this CTA (accumulator stage / phase)
+    ptx::setmaxnreg_inc<SWEEP_CONSUMER_REGS>();
+    // ===================== MMA + epilogue: 2 warpgroups x 64 user rows ==========
+    constexpr int NC = TN / NH;             // accumulator columns per MMA group
+    const int g = warp >> 2;
+    const int quad = lane >> 2, tq = lane & 3;
+    const int my_rs = tq >> 1, my_j = tq & 1;          // the (row, list) pair this lane reports
+    const int trow0 = 64 * g + 16 * (warp & 3) + quad;   // rows trow0 and trow0 + 8 of the tile
     const float pinf = __int_as_float(0x7f800000);
     const float ninf = __int_as_float(0xff800000);
-    for (int unit = cid; unit < n_units; unit += n_clusters) {
+    const uint32_t a_addr = ptx::smem_u32(smemA) + (uint32_t)(g * 64 * KBLK * 2);
+    const uint32_t b_addr = ptx::smem_u32(smemB);
+    float acc[NH][NC / 2];
+    int stage = 0;
+    uint32_t phase = 0;
+
+    // hand a stage back: one arrival per consumer warp on the stage's barrier in every CTA of the cluster
+    auto release = [&]() {
+      __syncwarp();
+      if (lane == 0) {
+        if (CL == 1) ptx::mbar_arrive(&ss->empty[stage]);
+        else
+#pragma unroll
+          for (int c = 0; c < CL; ++c) ptx::mbar_arrive_cluster(&ss->empty[stage], (uint32_t)c);
+      }
+      if (++stage == p.nstage) { stage = 0; phase ^= 1; }
+    };
+    // the four k16 MMAs of one 64-wide k-block; the first k-block of a tile starts the accumulator
+    auto mma_kblock = [&](float (&d)[NC / 2], uint64_t da, uint64_t db, bool first) {
+      if (first) {
+        if (NH == 1) ptx::wgmma_f16_n256_first(*reinterpret_cast<float(*)[128]>(&d[0]), da, db);
+        else ptx::wgmma_f16_n128_first(*reinterpret_cast<float(*)[64]>(&d[0]), da, db);
+      }
+#pragma unroll
+      for (int k4 = first ? 1 : 0; k4 < KBLK / 16; ++k4) {
+        // advance 16 fp16 = 32 bytes inside the 128-byte swizzled row: +2 in the >>4 field
+        if (NH == 1) ptx::wgmma_f16_n256(*reinterpret_cast<float(*)[128]>(&d[0]), da + 2 * k4, db + 2 * k4);
+        else ptx::wgmma_f16_n128(*reinterpret_cast<float(*)[64]>(&d[0]), da + 2 * k4, db + 2 * k4);
+      }
+    };
+    // MMAs of column group hh of the item tile in the current (whole-tile) stage
+    auto issue_group = [&](float (&d)[NC / 2], int hh) {
+      const uint32_t b_hh = b_addr + (uint32_t)(stage * p.KB * B_KB_BYTES + hh * NC * KBLK * 2);
+      mma_kblock(d, ptx::wgmma_desc_sw128_kmajor(a_addr), ptx::wgmma_desc_sw128_kmajor(b_hh), true);
+#pragma unroll 1
+      for (int kb = 1; kb < p.KB; ++kb)
+        mma_kblock(d, ptx::wgmma_desc_sw128_kmajor(a_addr + (uint32_t)(kb * A_KB_BYTES)),
+                   ptx::wgmma_desc_sw128_kmajor(b_hh + (uint32_t)(kb * B_KB_BYTES)), false);
+      ptx::wgmma_commit();
+    };
+    // every MMA group of one item tile; `epi(acc_group, column offset)` runs as soon as its group is done
+    auto tile_mma = [&](auto&& epi) {
+      if (NH == 1 && p.kb_stages) {
+        // k-block stages: the accumulator of the tile is built block by block, every stage is handed back
+        // as soon as its MMAs are complete
+        auto kblock_stage = [&](int kb, bool first) {
+          ptx::mbar_wait_hint(&ss->full[stage], phase, p.hint_ns);
+          ptx::wgmma_fence();
+          mma_kblock(acc[0], ptx::wgmma_desc_sw128_kmajor(a_addr + (uint32_t)(kb * A_KB_BYTES)),
+                     ptx::wgmma_desc_sw128_kmajor(b_addr + (uint32_t)(stage * B_KB_BYTES)), first);
+          ptx::wgmma_commit();
+          ptx::wgmma_wait<0>(acc[0]);
+          release();
+        };
+        kblock_stage(0, true);
+#pragma unroll 1
+        for (int kb = 1; kb < p.KB; ++kb) kblock_stage(kb, false);
+        epi(acc[0], std::integral_constant<int, 0>{});
+        return;
+      }
+      ptx::mbar_wait_hint(&ss->full[stage], phase, p.hint_ns);
+      ptx::wgmma_fence();
+#pragma unroll
+      for (int hh = 0; hh < NH; ++hh) issue_group(acc[hh], hh);
+      if (NH == 2) {
+        ptx::wgmma_wait<1>(acc[0]);
+        epi(acc[0], std::integral_constant<int, 0>{});
+        ptx::wgmma_wait<0>(acc[NH - 1]);
+        release();
+        epi(acc[NH - 1], std::integral_constant<int, NC>{});
+      } else {
+        ptx::wgmma_wait<0>(acc[0]);
+        release();
+        epi(acc[0], std::integral_constant<int, 0>{});
+      }
+    };
+
+    uint32_t uiter = 0;
+    for (int unit = cid; unit < n_units; unit += n_clusters, ++uiter) {
       const int split = unit / m_groups, m = (unit % m_groups) * CL + crank;
       const int t0 = split * p.tiles_per_split;
       const int t1 = min(t0 + p.tiles_per_split, p.total_tiles);
-      const int grow = m * TM + trow;
-      const int list_id = split * W + j;
+      const int grow0 = m * TM + trow0;                 // global rows grow0 (rs = 0) and grow0 + 8 (rs = 1)
+      const int list_base = split * 2;                  // list j = column half j of the tile
+      ptx::mbar_wait_hint(&ss->a_full, uiter & 1, p.hint_ns);
 
       if (PRE) {
-        // ---- pre-pass: per sampled tile the maximum coarse score of this warp's 128 columns ----
-        float* bm = p.blockmax + (int64_t)list_id * p.n_pre_tiles * p.B_pad + grow;
+        // ---- pre-pass: per sampled tile the maximum coarse score of each row and 128-column half ----
+        float* bm = p.blockmax + (int64_t)(list_base + my_j) * p.n_pre_tiles * p.B_pad + grow0 + 8 * my_rs;
         int ti = 0;
-        for (int t = t0; t < t1; t += STRIDE, ++ti, ++tc) {
-          const int acc = (int)(tc & 1u);
-          const uint32_t acc_phase = (tc >> 1) & 1u;
-          constexpr int PH = NH == 2 ? 1 : 0;    // W_PRE == 2: warp j <-> column half j (group j when NH == 2)
-          ptx::mbar_wait_hint(&ss->tmem_full[acc][j * PH], acc_phase, p.hint_ns);
-          ptx::tc_fence_after();
-          const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * TN + j * (TN / 2));
-          float tm = ninf;
-#pragma unroll 1
-          for (int ch = 0; ch < (TN / 2) / STEP; ++ch) {
-            uint32_t r[STEP];
-            ptx::tmem_ld_32x32b_x64(taddr + (uint32_t)(ch * STEP), r);
-            ptx::tmem_ld_wait_regs64(r);
-            float g[STEP / 8];
+        for (int t = t0; t < t1; t += STRIDE, ++ti) {
+          float mx[2][2] = {{ninf, ninf}, {ninf, ninf}};
+          tile_mma([&](auto& d, auto c0) {
+            constexpr int COL0 = decltype(c0)::value;
 #pragma unroll
-            for (int gq = 0; gq < STEP / 8; ++gq) {
-              const float a0 = fmax3(__uint_as_float(r[gq * 8 + 0]), __uint_as_float(r[gq * 8 + 1]), __uint_as_float(r[gq * 8 + 2]));
-              const float a1 = fmax3(__uint_as_float(r[gq * 8 + 3]), __uint_as_float(r[gq * 8 + 4]), __uint_as_float(r[gq * 8 + 5]));
-              g[gq] = fmax3(a0, a1, fmaxf(__uint_as_float(r[gq * 8 + 6]), __uint_as_float(r[gq * 8 + 7])));
+            for (int jj = 0; jj < NC / 8; ++jj) {
+              const int j = (COL0 + 8 * jj) >= TN / 2;
+#pragma unroll
+              for (int rs = 0; rs < 2; ++rs) {
+                const float v = fmaxf(d[4 * jj + 2 * rs], d[4 * jj + 2 * rs + 1]);
+                if (j) mx[rs][1] = fmaxf(mx[rs][1], v); else mx[rs][0] = fmaxf(mx[rs][0], v);
+              }
             }
-            tm = fmaxf(tm, fmax3(fmax3(g[0], g[1], g[2]), fmax3(g[3], g[4], g[5]), fmaxf(g[6], g[7])));
-            ptx::tc_fence_before();
-            __syncwarp();
-            if (lane == 0) ptx::mbar_arrive(&ss->tmem_empty[acc][j * PH]);
-          }
+          });
+#pragma unroll
+          for (int rs = 0; rs < 2; ++rs)
+#pragma unroll
+            for (int j = 0; j < 2; ++j) {
+              mx[rs][j] = fmaxf(mx[rs][j], __shfl_xor_sync(0xffffffffu, mx[rs][j], 1));
+              mx[rs][j] = fmaxf(mx[rs][j], __shfl_xor_sync(0xffffffffu, mx[rs][j], 2));
+            }
+          float tm = my_rs ? (my_j ? mx[1][1] : mx[1][0]) : (my_j ? mx[0][1] : mx[0][0]);
           // tiles that contain zero-padded item rows would bias the estimate: drop them
           if ((int64_t)(t + 1) * TN > p.N) tm = ninf;
           bm[(int64_t)ti * p.B_pad] = tm;
         }
         for (; ti < p.n_pre_tiles; ++ti) bm[(int64_t)ti * p.B_pad] = ninf;   // short last split
-        continue;
-      }
+      } else {
+        // ---- main pass ----
+        float tau[2];
+        int cnt[2][2] = {{0, 0}, {0, 0}}, n_counted[2][2] = {{0, 0}, {0, 0}};
+        float* lp[2][2];
+        const int64_t cap_words = (int64_t)p.capg * REC;
+#pragma unroll
+        for (int rs = 0; rs < 2; ++rs) {
+          const int grow = grow0 + 8 * rs;
+          tau[rs] = p.meta[grow].active ? ninf : pinf;
+          if (tau[rs] == ninf) {  // speculative start value (guess_kernel) / bounds published by other lists
+            const uint32_t gk = __ldcg(p.row_tau_key + grow);
+            if (gk != 0u) tau[rs] = key_to_float(gk);
+          }
+          if (p.ablate >= 1) tau[rs] = pinf;   // diagnostics: nothing is ever collected (cold path only)
+#pragma unroll
+          for (int j = 0; j < 2; ++j) lp[rs][j] = p.cand_r + ((int64_t)(list_base + j) * p.B_pad + grow) * cap_words;
+        }
 
-      // ---- main pass ----
-      const RowMeta meta = p.meta[grow];
-      const int64_t list0 = (int64_t)list_id * p.B_pad + (m * TM + q * 32);  // lane 0's slot
-      float* my_r = p.cand_r + (list0 + lane) * (int64_t)(p.capg * REC);
-      bool active = meta.active != 0;
-      float tau = active ? ninf : pinf;
-      int cnt = 0, n_counted = 0;
-      if (active) {  // speculative start value (guess_kernel) / bounds published by other lists
-        const uint32_t gk = __ldcg(p.row_tau_key + grow);
-        if (gk != 0u) tau = key_to_float(gk);
-      }
-      if (p.ablate >= 1) tau = pinf;   // diagnostics: nothing is ever collected (cold path only)
-
-      // compaction of the lists flagged in `need` (warp-uniform mask)
-      auto compact_flagged = [&](uint32_t need) {
-        while (need) {
-          const int src = __ffs(need) - 1;
-          need &= need - 1;
-          const int s_cnt = __shfl_sync(0xffffffffu, cnt, src);
-          const int s_cntd = __shfl_sync(0xffffffffu, n_counted, src);
-          const int s_k = __shfl_sync(0xffffffffu, meta.k_row, src);
-          const float s_e = __shfl_sync(0xffffffffu, meta.eps2, src);
-          const float s_R = __shfl_sync(0xffffffffu, meta.R, src);
-          const float s_tau = __shfl_sync(0xffffffffu, tau, src);
-          float new_tau;
-          const int w = compact_row(p.cand_r + (list0 + src) * (int64_t)(p.capg * REC), s_cnt, s_cntd, s_k, s_e, s_R,
-                                    s_tau, p.ghist + (int64_t)(m * TM + q * 32 + src) * NB, lane, (int32_t)p.N,
-                                    &new_tau);
-          if (lane == src) {
-            cnt = w;
-            n_counted = w;
-            // also pick up what other lists of this row published meanwhile
-            tau = fmaxf(new_tau, key_to_float(max(__ldcg(p.row_tau_key + grow), 1u)));
-            atomicMax(p.row_tau_key + grow, float_to_key(new_tau));
-            if (w > p.capg - 32) {  // too many near-ties to bound: hand the row to the exact path
-              active = false;
-              tau = pinf;
-              cnt = 0;
-              n_counted = 0;
-              p.row_status[grow] = 1;
+        // Zero-padded item rows of the last tile (ids >= N, coarse score exactly 0) may be collected when
+        // tau <= 0; compact_row and finalize_kernel ignore ids >= N, so the sweep needs no tail code.
+        for (int t = t0; t < t1; ++t) {
+          const int c_before = cnt[0][0] + cnt[0][1] + cnt[1][0] + cnt[1][1];
+          tile_mma([&](auto& d, auto c0) {
+            constexpr int COL0 = decltype(c0)::value;
+#pragma unroll
+            for (int s = 0; s < NC / STEP; ++s) {
+              // one warp vote per 64-column step: a cold step (the common case) costs its max tree only
+              float m0 = ninf, m1 = ninf;
+#pragma unroll
+              for (int jj = 8 * s; jj < 8 * s + 8; ++jj) {
+                m0 = fmax3(m0, d[4 * jj + 0], d[4 * jj + 1]);
+                m1 = fmax3(m1, d[4 * jj + 2], d[4 * jj + 3]);
+              }
+              if (!__any_sync(0xffffffffu, m0 >= tau[0] || m1 >= tau[1])) continue;
+#pragma unroll
+              for (int jj = 8 * s; jj < 8 * s + 8; ++jj) {
+                const int col = COL0 + 8 * jj;
+                const int j = col >= TN / 2;
+                const int32_t idv = t * TN + col;
+#pragma unroll
+                for (int rs = 0; rs < 2; ++rs) {
+                  const float v0 = d[4 * jj + 2 * rs], v1 = d[4 * jj + 2 * rs + 1];
+                  float gm = fmaxf(v0, v1);
+                  gm = fmaxf(gm, __shfl_xor_sync(0xffffffffu, gm, 1));
+                  gm = fmaxf(gm, __shfl_xor_sync(0xffffffffu, gm, 2));
+                  int& c = j ? cnt[rs][1] : cnt[rs][0];
+                  float* dst = (j ? lp[rs][1] : lp[rs][0]) + (size_t)c * REC;
+                  if (EPI == 5) {
+                    asm volatile(
+                        "{\n\t.reg .pred p, q;\n\t"
+                        "setp.ge.f32 p, %0, %1;\n\t"
+                        "setp.eq.and.u32 q, %6, 0, p;\n\t"
+                        "@p st.global.v2.f32 [%2], {%3, %4};\n\t"
+                        "@q st.global.b32 [%5], %7;\n\t}"
+                        ::"f"(gm), "f"(tau[rs]), "l"(dst + 2 * tq), "f"(v0), "f"(v1), "l"(dst + 8), "r"(tq), "r"(idv)
+                        : "memory");
+                    c += (gm >= tau[rs]) ? 1 : 0;
+                  } else if (gm >= tau[rs]) {
+                    *reinterpret_cast<float2*>(dst + 2 * tq) = make_float2(v0, v1);
+                    if (tq == 0) reinterpret_cast<int32_t*>(dst)[8] = idv;
+                    ++c;
+                  }
+                }
+              }
+            }
+          });
+          // one overflow / compaction check per TILE (a tile adds at most 16 records to a list)
+          if (!__any_sync(0xffffffffu, cnt[0][0] + cnt[0][1] + cnt[1][0] + cnt[1][1] != c_before)) continue;
+          const int mc = sel22(cnt, my_rs, my_j), mn = sel22(n_counted, my_rs, my_j);
+          uint32_t need = __ballot_sync(0xffffffffu, (mc - mn > p.trig) || (mc > p.capg - 24));
+          while (need) {
+            const int src = __ffs(need) - 1;
+            need &= need - 1;
+            const int s_cnt = __shfl_sync(0xffffffffu, mc, src);
+            const int s_cntd = __shfl_sync(0xffffffffu, mn, src);
+            const float s_tau = __shfl_sync(0xffffffffu, my_rs ? tau[1] : tau[0], src);
+            const int sq = src >> 2, srs = (src >> 1) & 1, sj = src & 1;
+            const int sgrow = m * TM + 64 * g + 16 * (warp & 3) + sq + 8 * srs;
+            const RowMeta sm = p.meta[sgrow];
+            float new_tau;
+            const int w = compact_row(p.cand_r + ((int64_t)(list_base + sj) * p.B_pad + sgrow) * cap_words, s_cnt, s_cntd,
+                                      sm.k_row, sm.eps2, sm.R, s_tau, p.ghist + (int64_t)sgrow * NB, lane, (int32_t)p.N,
+                                      &new_tau);
+            if (quad == sq) {
+              set22(cnt, srs, sj, w);
+              set22(n_counted, srs, sj, w);
+              // also pick up what other lists of this row published meanwhile
+              float nt = fmaxf(new_tau, key_to_float(max(__ldcg(p.row_tau_key + sgrow), 1u)));
+              if (lane == src) atomicMax(p.row_tau_key + sgrow, float_to_key(new_tau));
+              if (w > p.capg - 32) {  // too many near-ties to bound: hand the row to the exact path
+                nt = pinf;
+                set22(cnt, srs, sj, 0);
+                set22(n_counted, srs, sj, 0);
+                if (lane == src) p.row_status[sgrow] = 1;
+              }
+              if (srs) tau[1] = nt; else tau[0] = nt;
             }
           }
         }
-      };
-
-      // Zero-padded item rows of the last tile (ids >= N, coarse score exactly 0) may be collected when
-      // tau <= 0; compact_row and finalize_kernel ignore ids >= N, so the sweep needs no tail code.
-      // Every warp owns two adjacent 64-column steps of every tile (W = 2).
-      for (int t = t0; t < t1; ++t, ++tc) {
-        const int acc = (int)(tc & 1u);
-        const uint32_t acc_phase = (tc >> 1) & 1u;
-        const int cnt0 = cnt;
-        if (NH == 1) {   // one MMA group per tile: one wait, the accumulator goes back after the second read
-          ptx::mbar_wait_hint(&ss->tmem_full[acc][0], acc_phase, p.hint_ns);
-          ptx::tc_fence_after();
-        }
-        if (EPI == 6) {
-          // variant 6 (NH == 1): the warp's 128 columns as FOUR 32-column reads, double-buffered — the next read is
-          // issued right after the wait for the current one, so its tensor-memory latency runs under the max tree /
-          // group tests of the current 32 columns (tcgen05.wait::ld waits for ALL outstanding loads of the thread,
-          // hence issue-after-wait rather than two loads in flight).  Same 64 registers of read data as variant 3.
-          const uint32_t tb = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * TN + 2 * j * STEP);
-          const int nb = t * TN + 2 * j * STEP;
-          auto process32 = [&](const uint32_t (&r)[32], const int n_base) {
-#pragma unroll
-            for (int gq = 0; gq < 4; ++gq) {
-              const float a0 = fmax3(__uint_as_float(r[gq * 8 + 0]), __uint_as_float(r[gq * 8 + 1]), __uint_as_float(r[gq * 8 + 2]));
-              const float a1 = fmax3(__uint_as_float(r[gq * 8 + 3]), __uint_as_float(r[gq * 8 + 4]), __uint_as_float(r[gq * 8 + 5]));
-              const float gm = fmax3(a0, a1, fmaxf(__uint_as_float(r[gq * 8 + 6]), __uint_as_float(r[gq * 8 + 7])));
-              if (gm >= tau) {
-                float4* dst = reinterpret_cast<float4*>(my_r + (size_t)cnt * REC);
-                dst[0] = make_float4(__uint_as_float(r[gq * 8 + 0]), __uint_as_float(r[gq * 8 + 1]),
-                                     __uint_as_float(r[gq * 8 + 2]), __uint_as_float(r[gq * 8 + 3]));
-                dst[1] = make_float4(__uint_as_float(r[gq * 8 + 4]), __uint_as_float(r[gq * 8 + 5]),
-                                     __uint_as_float(r[gq * 8 + 6]), __uint_as_float(r[gq * 8 + 7]));
-                reinterpret_cast<int32_t*>(dst)[8] = n_base + gq * 8;
-                ++cnt;
-              }
-            }
-          };
-          uint32_t ra[32], rb[32];
-          ptx::tmem_ld_32x32b_x32(tb, ra);
-          ptx::tmem_ld_wait_regs(ra);
-          ptx::tmem_ld_32x32b_x32(tb + 32, rb);
-          process32(ra, nb);
-          __syncwarp();
-          ptx::tmem_ld_wait_regs(rb);
-          ptx::tmem_ld_32x32b_x32(tb + 64, ra);
-          process32(rb, nb + 32);
-          __syncwarp();
-          ptx::tmem_ld_wait_regs(ra);
-          ptx::tmem_ld_32x32b_x32(tb + 96, rb);
-          process32(ra, nb + 64);
-          __syncwarp();
-          ptx::tmem_ld_wait_regs(rb);
-          ptx::tc_fence_before();              // all four reads of this warp are done: the accumulator may be reused
-          __syncwarp();
-          if (lane == 0) ptx::mbar_arrive_cnt(&ss->tmem_empty[acc][0], 2);
-          process32(rb, nb + 96);
-        } else
-#pragma unroll
-        for (int i = 0; i < 2; ++i) {
-          const int s = 2 * j + i;
-          if (NH == 2 && i == 0) {   // group j of the tile belongs to warp j alone
-            ptx::mbar_wait_hint(&ss->tmem_full[acc][j], acc_phase, p.hint_ns);
-            ptx::tc_fence_after();
-          }
-          const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * TN + s * STEP);
-          const int n_base = t * TN + s * STEP;
-          if (EPI == 9) {   // DIAGNOSTIC instantiation: the epilogue only hands the accumulator back (no read)
-            if (i == 1) {
-              ptx::tc_fence_before();
-              __syncwarp();
-              if (lane == 0) ptx::mbar_arrive_cnt(&ss->tmem_empty[acc][NH == 2 ? j : 0], 2);
-            }
-            continue;
-          }
-          uint32_t r[STEP];
-          ptx::tmem_ld_32x32b_x64(taddr, r);
-          ptx::tmem_ld_wait_regs64(r);
-          if (i == 1) {   // both reads of this warp are done: the MMA issuer may reuse the accumulator
-            ptx::tc_fence_before();
-            __syncwarp();
-            if (lane == 0) ptx::mbar_arrive_cnt(&ss->tmem_empty[acc][NH == 2 ? j : 0], 2);
-          }
-          if (EPI == 8) {   // DIAGNOSTIC instantiation: tensor-memory read only (xor keeps the load alive)
-            uint32_t x = 0;
-#pragma unroll
-            for (int c = 0; c < STEP; ++c) x ^= r[c];
-            if (x == 0x7fc00001u) my_r[0] = __uint_as_float(x);
-            continue;
-          }
-          float g[STEP / 8];
-#pragma unroll
-          for (int gq = 0; gq < STEP / 8; ++gq) {
-            const float a0 = fmax3(__uint_as_float(r[gq * 8 + 0]), __uint_as_float(r[gq * 8 + 1]), __uint_as_float(r[gq * 8 + 2]));
-            const float a1 = fmax3(__uint_as_float(r[gq * 8 + 3]), __uint_as_float(r[gq * 8 + 4]), __uint_as_float(r[gq * 8 + 5]));
-            g[gq] = fmax3(a0, a1, fmaxf(__uint_as_float(r[gq * 8 + 6]), __uint_as_float(r[gq * 8 + 7])));
-          }
-          if (EPI == 5) {
-            // ONE warp vote per 64-column step on its maximum (cold step: max tree + 7 instructions); a hot
-            // step writes every 8-column group that reaches tau in its lane as ONE 48-byte record (8 coarse
-            // scores + the first item id) with PREDICATED stores — no branches: lanes / groups without a hit
-            // issue the stores with a false predicate.  finalize_kernel sorts out which of the 8 scores count.
-            const float mm = fmax3(fmax3(g[0], g[1], g[2]), fmax3(g[3], g[4], g[5]), fmaxf(g[6], g[7]));
-            if (__any_sync(0xffffffffu, mm >= tau)) {
-#pragma unroll
-              for (int gq = 0; gq < STEP / 8; ++gq) {
-                float* dst = my_r + (size_t)cnt * REC;
-                const int32_t idv = n_base + gq * 8;
-                asm volatile(
-                    "{\n\t.reg .pred p;\n\t"
-                    "setp.ge.f32 p, %0, %1;\n\t"
-                    "@p st.global.v4.b32 [%2], {%3, %4, %5, %6};\n\t"
-                    "@p st.global.v4.b32 [%2+16], {%7, %8, %9, %10};\n\t"
-                    "@p st.global.b32 [%2+32], %11;\n\t}"
-                    ::"f"(g[gq]), "f"(tau), "l"(dst), "r"(r[gq * 8 + 0]), "r"(r[gq * 8 + 1]), "r"(r[gq * 8 + 2]),
-                    "r"(r[gq * 8 + 3]), "r"(r[gq * 8 + 4]), "r"(r[gq * 8 + 5]), "r"(r[gq * 8 + 6]),
-                    "r"(r[gq * 8 + 7]), "r"(idv)
-                    : "memory");
-                cnt += (g[gq] >= tau) ? 1 : 0;
-              }
-            }
-          } else {
-            // variant 3: group tests as divergent per-lane branches straight from the compare
-#pragma unroll
-            for (int gq = 0; gq < STEP / 8; ++gq) {
-              if (g[gq] >= tau) {
-                float4* dst = reinterpret_cast<float4*>(my_r + (size_t)cnt * REC);
-                dst[0] = make_float4(__uint_as_float(r[gq * 8 + 0]), __uint_as_float(r[gq * 8 + 1]),
-                                     __uint_as_float(r[gq * 8 + 2]), __uint_as_float(r[gq * 8 + 3]));
-                dst[1] = make_float4(__uint_as_float(r[gq * 8 + 4]), __uint_as_float(r[gq * 8 + 5]),
-                                     __uint_as_float(r[gq * 8 + 6]), __uint_as_float(r[gq * 8 + 7]));
-                reinterpret_cast<int32_t*>(dst)[8] = n_base + gq * 8;
-                ++cnt;
-              }
-            }
-          }
-        }
-        // one overflow / compaction check per TILE (a tile adds at most 16 records to a list)
-        if (EPI != 8 && EPI != 9)
-          if (__any_sync(0xffffffffu, cnt != cnt0))
-            compact_flagged(__ballot_sync(0xffffffffu, (cnt - n_counted > p.trig) || (cnt > p.capg - 24)));
+        p.cand_cnt[(int64_t)(list_base + my_j) * p.B_pad + grow0 + 8 * my_rs] = sel22(cnt, my_rs, my_j);
       }
-      p.cand_cnt[list0 + lane] = cnt;
+      // the user tile is reusable once every consumer warp's last MMA of the unit is complete
+      __syncwarp();
+      if (lane == 0) ptx::mbar_arrive(&ss->a_empty);
     }
   }
   __syncthreads();
   if (CL > 1) ptx::cluster_sync_all();     // no CTA leaves while a peer may still multicast to it
-  if (warp == WARP_MMA) {
-    ptx::tc_fence_after();
-    ptx::tmem_dealloc(tmem_base, 512);
-  }
 }
 
 // ------------------------------------------------------------------------------------------
@@ -1218,9 +1137,9 @@ static inline size_t al256(size_t x) { return (x + 255) & ~(size_t)255; }
 
 
 // ---- tuning knobs (defaults compiled in; b200_recommend_embed_tune overrides them per process) ----
-static int g_epi = 3;              // epilogue variant of the main pass: 3 divergent group tests (measured best), 5 step vote + predicated stores
+static int g_epi = 5;              // record stores of a hot epilogue step: 5 predicated stores (measured best on H100), 3 divergent group tests
 static int g_cluster = 2;          // 2 = pairs of user tiles share every item tile through TMA multicast, 1 = off
-static int g_nh = 1;               // MMA groups per item tile (1 x N=256; 2 x N=128 re-reads the user tile: ~2x slower)
+static int g_nh = 1;               // MMA groups per item tile (1 x N=256; 2 x N=128, epilogue of the first overlaps the second)
 static int g_ablate = 0;           // b200_recommend_embed_debug
 static int g_hint_ns = 20000;      // suspend-time hint of the mbarrier waits in the sweep kernels
 static int g_pre_margin = 12;      // additive part of the speculative rank: pre_k = margin + coef * f * k_row sampled block maxima
@@ -1255,10 +1174,12 @@ static int make_plan(int64_t B, int64_t N, int d, Plan* pl) {
   const int ovh = 12;
   long best = -1;
   int bestS = 1;
-  const int maxS = pl->total_tiles < 2 * kNumSMs ? pl->total_tiles : 2 * kNumSMs;
+  const int sms = num_sms();
+  B200_REQUIRE(sms > 0, "no CUDA device");
+  const int maxS = pl->total_tiles < 2 * sms ? pl->total_tiles : 2 * sms;
   for (int S = 1; S <= maxS; ++S) {
     const long units = (long)pl->m_tiles * S;
-    const long waves = (units + kNumSMs - 1) / kNumSMs;
+    const long waves = (units + sms - 1) / sms;
     const long tps = (pl->total_tiles + S - 1) / S;
     const long cost = waves * (tps + ovh);
     if (best < 0 || cost < best) { best = cost; bestS = S; }
@@ -1308,19 +1229,19 @@ static int make_plan(int64_t B, int64_t N, int d, Plan* pl) {
   return 0;
 }
 
-template <bool PRE, int W, int EPI, int CL, int NH>
+template <bool PRE, int EPI, int CL, int NH>
 static int launch_sweep(int grid, const Plan& pl, cudaStream_t stream, const CUtensorMap& tmA,
                         const CUtensorMap& tmB, const CUtensorMap& tmBh, const SweepParams& sp) {
   static bool attr_set = false;
   if (!attr_set) {
-    B200_CUDA_OK(cudaFuncSetAttribute(sweep_kernel<PRE, W, EPI, CL, NH>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    B200_CUDA_OK(cudaFuncSetAttribute(sweep_kernel<PRE, EPI, CL, NH>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                       227 * 1024));
     attr_set = true;
   }
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
   cfg.gridDim = dim3((unsigned)grid, 1, 1);
-  cfg.blockDim = dim3((unsigned)sweep_threads(W), 1, 1);
+  cfg.blockDim = dim3((unsigned)SWEEP_THREADS, 1, 1);
   cfg.dynamicSmemBytes = pl.smem_bytes;
   cfg.stream = stream;
   cudaLaunchAttribute at[1];
@@ -1328,35 +1249,33 @@ static int launch_sweep(int grid, const Plan& pl, cudaStream_t stream, const CUt
   at[0].val.clusterDim.x = CL; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
   cfg.attrs = at;
   cfg.numAttrs = 1;
-  B200_CUDA_OK(cudaLaunchKernelEx(&cfg, sweep_kernel<PRE, W, EPI, CL, NH>, tmA, tmB, tmBh, sp));
+  B200_CUDA_OK(cudaLaunchKernelEx(&cfg, sweep_kernel<PRE, EPI, CL, NH>, tmA, tmB, tmBh, sp));
   count_launch();
   return 0;
 }
 
-// organisation = (epilogue warps per quadrant W, epilogue variant, cluster size CL, MMA groups NH); the
-// instantiated combinations are the default (W 2, variant 3, CL 2, NH 1) and its A/B neighbours
+// organisation = (record stores EPI, cluster size CL, MMA groups NH); the default is (5, 2, 1)
 static int launch_pre_dispatch(int grid, const Plan& pl, cudaStream_t stream, const CUtensorMap& tmA,
                                const CUtensorMap& tmB, const CUtensorMap& tmBh, const SweepParams& sp) {
-  // the pre-pass has one epilogue (2 warps per quadrant, block maxima only)
+  // the pre-pass stores no records: one epilogue
   if (pl.CL == 2) {
-    if (pl.NH == 1) return launch_sweep<true, 2, 3, 2, 1>(grid, pl, stream, tmA, tmB, tmBh, sp);
-    return launch_sweep<true, 2, 3, 2, 2>(grid, pl, stream, tmA, tmB, tmBh, sp);
+    if (pl.NH == 1) return launch_sweep<true, 3, 2, 1>(grid, pl, stream, tmA, tmB, tmBh, sp);
+    return launch_sweep<true, 3, 2, 2>(grid, pl, stream, tmA, tmB, tmBh, sp);
   }
-  if (pl.NH == 1) return launch_sweep<true, 2, 3, 1, 1>(grid, pl, stream, tmA, tmB, tmBh, sp);
-  return launch_sweep<true, 2, 3, 1, 2>(grid, pl, stream, tmA, tmB, tmBh, sp);
+  if (pl.NH == 1) return launch_sweep<true, 3, 1, 1>(grid, pl, stream, tmA, tmB, tmBh, sp);
+  return launch_sweep<true, 3, 1, 2>(grid, pl, stream, tmA, tmB, tmBh, sp);
 }
 
 static int launch_main_dispatch(int grid, const Plan& pl, int epi, cudaStream_t stream, const CUtensorMap& tmA,
                                 const CUtensorMap& tmB, const CUtensorMap& tmBh, const SweepParams& sp) {
-#define B200_SWEEP(E_, C_, N_) return launch_sweep<false, 2, E_, C_, N_>(grid, pl, stream, tmA, tmB, tmBh, sp)
-  // default: variant 3 (divergent per-lane group tests), one N=256 MMA group per tile, clusters of 2;
-  // the other instantiations are A/B points and diagnostics
-  if (epi == 8) { if (pl.NH == 2) B200_SWEEP(8, 1, 2); B200_SWEEP(8, 1, 1); }
-  if (epi == 9) { if (pl.NH == 2) B200_SWEEP(9, 1, 2); B200_SWEEP(9, 1, 1); }
-  if (pl.NH == 2) { if (pl.CL == 2) B200_SWEEP(3, 2, 2); B200_SWEEP(3, 1, 2); }
-  if (epi == 5) { if (pl.CL == 2) B200_SWEEP(5, 2, 1); B200_SWEEP(5, 1, 1); }
-  if (epi == 6) { if (pl.CL == 2) B200_SWEEP(6, 2, 1); B200_SWEEP(6, 1, 1); }
-  if (pl.CL == 2) B200_SWEEP(3, 2, 1);
+#define B200_SWEEP(E_, C_, N_) return launch_sweep<false, E_, C_, N_>(grid, pl, stream, tmA, tmB, tmBh, sp)
+  if (epi == 5) {
+    if (pl.CL == 2) { if (pl.NH == 2) B200_SWEEP(5, 2, 2); B200_SWEEP(5, 2, 1); }
+    if (pl.NH == 2) B200_SWEEP(5, 1, 2);
+    B200_SWEEP(5, 1, 1);
+  }
+  if (pl.CL == 2) { if (pl.NH == 2) B200_SWEEP(3, 2, 2); B200_SWEEP(3, 2, 1); }
+  if (pl.NH == 2) B200_SWEEP(3, 1, 2);
   B200_SWEEP(3, 1, 1);
 #undef B200_SWEEP
 }
@@ -1404,9 +1323,8 @@ extern "C" int b200_recommend_embed_tune(int32_t epilogue_warps_per_quadrant, fl
   if (epilogue_warps_per_quadrant != 0) {   // organisation code: 100 * cluster size + 10 * MMA groups per tile + epilogue variant
     const int code = epilogue_warps_per_quadrant % 1000;
     const int cl = (code / 100) % 10, nh = (code / 10) % 10, epi = code % 10;
-    B200_REQUIRE((cl == 1 || cl == 2) && (nh == 1 || nh == 2) &&
-                     (epi == 3 || epi == 5 || (epi == 6 && nh == 1) || ((epi == 8 || epi == 9) && cl == 1)),
-                 "b200_recommend_embed_tune: code = 100 * cluster (1|2) + 10 * MMA groups (1|2) + epilogue (3|5|6; 6 needs one MMA group)");
+    B200_REQUIRE((cl == 1 || cl == 2) && (nh == 1 || nh == 2) && (epi == 3 || epi == 5),
+                 "b200_recommend_embed_tune: code = 100 * cluster (1|2) + 10 * MMA groups (1|2) + record stores (3|5)");
     g_cluster = cl; g_nh = nh; g_epi = epi;
   }
   if (pre_rank_coef != 0.f) {
@@ -1498,12 +1416,7 @@ extern "C" int b200_recommend_embed(const float* U, int64_t ldu, const int64_t* 
   sp.row_status = status; sp.ghist = ghist; sp.cand_r = cand_r; sp.cand_cnt = cnt;
   sp.blockmax = bm; sp.ablate = g_ablate; sp.hint_ns = (uint32_t)g_hint_ns;
   const int n_units = pl.m_tiles * pl.n_splits;
-  static int sm_count = 0;
-  if (!sm_count) {
-    int dev = 0;
-    B200_CUDA_OK(cudaGetDevice(&dev));
-    B200_CUDA_OK(cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, dev));
-  }
+  const int sm_count = num_sms();
   int grid = n_units < sm_count ? n_units : sm_count;
   grid -= grid % pl.CL;                                    // whole clusters
 

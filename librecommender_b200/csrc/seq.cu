@@ -808,7 +808,7 @@ extern "C" int b200_din_attention_hoisted(const float* Z, int64_t ldz, int64_t N
   const bool z_ok = Z && (ldz % 4 == 0) && ((reinterpret_cast<uintptr_t>(Z) & 15) == 0);
   if (len >= 1 && len <= 64 && z_ok && (size_t)len * Kp * 4 <= 48 * 1024 && N >= 1024) {
     const size_t smem = (size_t)len * Kp * 4;
-    const unsigned blocks = (unsigned)std::min<int64_t>(ceil_div64(N, 8), (int64_t)148 * 8);
+    const unsigned blocks = (unsigned)std::min<int64_t>(ceil_div64(N, 8), (int64_t)std::max(1, num_sms()) * 8);
     cudaStream_t st = (cudaStream_t)stream;
     switch ((Kp + 31) / 32) {
       case 1: din_attention_hoisted_v2_kernel<1><<<blocks, 256, smem, st>>>(Z, ldz, N, G, ldg, Kp, seq, len, k2, b2, out, ld_out); break;
@@ -836,7 +836,7 @@ extern "C" int b200_din_attention_from_logits(const float* A, int64_t lda, int64
   if (N == 0) return 0;
   const size_t smem = (size_t)len * Kp * 4;
   B200_REQUIRE(smem <= 48 * 1024, "b200_din_attention_from_logits: keys do not fit shared memory");
-  const unsigned blocks = (unsigned)std::min<int64_t>(ceil_div64(N, 8), (int64_t)148 * 8);
+  const unsigned blocks = (unsigned)std::min<int64_t>(ceil_div64(N, 8), (int64_t)std::max(1, num_sms()) * 8);
   din_attention_from_logits_kernel<<<blocks, 256, smem, (cudaStream_t)stream>>>(A, lda, N, G, ldg, Kp, seq, len, b2, out,
                                                                                ld_out);
   B200_CUDA_OK(cudaGetLastError());
@@ -857,7 +857,7 @@ extern "C" int b200_din_attention_backward(const float* G, int64_t ldg, int32_t 
   if (R == 0) return 0;
   AttW w{k1, b1, k2, b2};
   const size_t smem = ((size_t)4 * Kp * HID + (size_t)4 * BWD_T * HID + (size_t)8 * BWD_T) * 4;
-  const unsigned blocks = (unsigned)std::min<int64_t>(ceil_div64(R, 4), (int64_t)148 * 4);
+  const unsigned blocks = (unsigned)std::min<int64_t>(ceil_div64(R, 4), (int64_t)std::max(1, num_sms()) * 4);
   cudaStream_t st = (cudaStream_t)stream;
   auto launch = [&](auto kern) -> int {
     B200_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -927,7 +927,7 @@ extern "C" int b200_din_attention(const float* G, int64_t ldg, int32_t Kp, const
                      ((reinterpret_cast<uintptr_t>(k1) & 15) == 0);
   if (v2_ok) {
     const size_t smem = (size_t)4 * Kp * HID * 4;
-    const unsigned blocks = (unsigned)std::min<int64_t>(ceil_div64(R, 4), (int64_t)148 * 16);
+    const unsigned blocks = (unsigned)std::min<int64_t>(ceil_div64(R, 4), (int64_t)std::max(1, num_sms()) * 16);
     cudaStream_t st = (cudaStream_t)stream;
     switch ((Kp + 31) / 32) {
       case 1: din_attention_v2_kernel<1><<<blocks, 128, smem, st>>>(G, ldg, Kp, items, seqs, ld_seq, lens, T, users, R, grid_items, row_offset, w, out, ld_out); break;

@@ -62,7 +62,7 @@ def _dev(x, device, dtype):
 
 
 # Dense-layer kernel selection: "auto" sends layers that are compute-bound on the SIMT kernel
-# (din >= TC_MIN_DIN, enough rows to fill the SMs) to the tcgen05 3xTF32 kernel; both are this
+# (din >= TC_MIN_DIN, enough rows to fill the SMs) to the wgmma 3xTF32 kernel; both are this
 # library's own CUDA kernels and both meet the 1e-5 bar.  "f32" / "tf32x3" force one (tests).
 LINEAR_IMPL = "auto"
 TC_MIN_DIN = 64
@@ -112,7 +112,8 @@ def linear(x, Wt, b, relu, cache_split=True):
     if use_tc and aligned and w_ok and not cache_split and din >= TC_LONG_K:
         # few output tiles, long reduction: split the reduction over enough CTAs to fill the SMs
         tiles = -(-R // 128) * -(-dout // 128)
-        splits = max(1, min(16, 148 // tiles, din // 256))
+        sms = torch.cuda.get_device_properties(x.device).multi_processor_count
+        splits = max(1, min(16, sms // tiles, din // 256))
         if splits > 1:
             part = torch.empty(splits * R * dout, dtype=torch.float32, device=x.device)
             _lib.check(_lib.lib.b200_linear_tf32x3_splitk(_lib.ptr(x), x.stride(0), R, _lib.ptr(Wt), Wt.stride(0), bp, din,
@@ -929,7 +930,7 @@ class DIN(_SeqModelBase):
 
     def score_all_items(self, user_ids_d):
         """din.py:165-250 over (this user) x (every item).  Per user: the attention's Dense(16) becomes
-        one GEMM [N, K'] x [K', 16 len] on the library GEMM kernel (tcgen05 3xTF32 for large N), a warp
+        one GEMM [N, K'] x [K', 16 len] on the library GEMM kernel (wgmma 3xTF32 for large N), a warp
         per item finishes sigmoid / Dense(1) / softmax / weighted key sum, the first MLP layer splits
         into user / item / attention parts and the pair kernel runs the small layers."""
         torch = self._torch

@@ -284,7 +284,7 @@ class RowShardedTable:
 
 
 # ------------------------------------------------------------------------------------------------
-# Row-sharded table over NVLink PEER MEMORY (the B200 path of SURVEY.md §8e row 2).  Every rank's
+# Row-sharded table over NVLink PEER MEMORY (SURVEY.md §8e row 2).  Every rank's
 # shard lives in symmetric memory (torch.distributed._symmetric_memory: CUDA VMM allocations
 # mapped into every process of the node), so one CUDA kernel per direction does the gather AND
 # the exchange (`b200_peer_gather_rows` / `b200_peer_scatter_add_rows`): no bucketing by owner, no

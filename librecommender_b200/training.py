@@ -230,7 +230,7 @@ class DeepFMTrainer(_GraphedStep):
     ``dense_nn`` in training mode (``libreco/layers/dense.py:12-49``: BN(input) -> [Dense -> ReLU ->
     BN] x (L-1) -> Dense, no dropout = the reference's default), mean sigmoid CE, TF-Adam.
 
-    The Dense layers run on the library's own GEMM kernels (``feat_models.linear``: tcgen05 3xTF32 or
+    The Dense layers run on the library's own GEMM kernels (``feat_models.linear``: wgmma 3xTF32 or
     exact-fma SIMT) — forward ``Y = X Wt^T + b``, backward ``dX = dY Wt`` and ``dWt = dY^T X`` are the
     same kernel on transposed operands.  ``weights`` uses the inference layout of
     ``feat_models.DeepFM`` / ``oracle.tf_models.make_deepfm_weights``."""

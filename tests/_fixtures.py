@@ -21,3 +21,26 @@ def load_multi_sparse_spec():
     spec["n_sparse"] = len(spec["user_sparse_col_index"]) + len(spec["item_sparse_col_index"])
     spec["n_dense"] = len(spec["user_dense_col_index"]) + len(spec["item_dense_col_index"])
     return g, spec
+
+
+# seeded inputs of the randomized comparisons with the reference; golden/live_reference.npz holds the
+# reference's answers for them (golden/gen_live_reference.py)
+
+def rank_cases():
+    rng = np.random.default_rng(5)
+    for _ in range(20):
+        B, N = int(rng.integers(1, 6)), int(rng.integers(5, 400))
+        K = int(rng.integers(1, N + 1))
+        preds = rng.standard_normal((B, N)).astype(np.float32)
+        consumed = {u: rng.choice(N, size=int(rng.integers(0, N)), replace=False).tolist() for u in range(B)}
+        consumed = {u: v for u, v in consumed.items() if v}
+        yield list(range(B)), preds, K, N, consumed
+
+
+def sampling_cases():
+    gen = np.random.default_rng(9)
+    for trial in range(5):
+        n_items = int(gen.integers(20, 3000))
+        pos = gen.integers(0, n_items, size=int(gen.integers(1, 500)))
+        num_neg = int(gen.integers(1, 6))
+        yield trial, n_items, pos, num_neg

@@ -13,7 +13,7 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, ROOT)
 
-PEAK = 6572.2
+PEAK = 3350.0   # H100 SXM data-sheet HBM3 GB/s, used unless MEASURED_PEAKS.json gives a measured copy rate
 try:
     PEAK = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"]
 except Exception:
@@ -203,10 +203,10 @@ def bench_topk_and_sampler():
 
 
 def bench_linear():
-    """Dense layer: exact-fma SIMT kernel vs the tcgen05 3xTF32 kernel (fp32-level accuracy)."""
+    """Dense layer: exact-fma SIMT kernel vs the wgmma 3xTF32 kernel (fp32-level accuracy)."""
     from librecommender_b200 import _lib
 
-    tc_peak = 1368.6
+    tc_peak = 989.0   # H100 SXM data-sheet dense BF16 TFLOP/s unless MEASURED_PEAKS.json gives a measured rate
     try:
         tc_peak = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["bf16_tflops"]
     except Exception:

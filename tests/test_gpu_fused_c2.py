@@ -121,11 +121,11 @@ def test_wide_embedding_ragged_catalogue_and_scale():
     _check(sc, U, I, csr, users, K, n_oracle=96, min_ok_frac=0.97)
 
 
-@pytest.mark.parametrize("code", [113, 215, 223, 125, 216, 116])
+@pytest.mark.parametrize("code", [113, 215, 223, 125, 115, 225, 213, 123])
 def test_kernel_organisation_variants(code):
-    """The tuning variants of the sweep give the same answers as the default (code 213: cluster of 2 with
-    TMA multicast, one N=256 MMA group per tile, divergent per-lane group tests): no cluster (1xx), two
-    N=128 MMA groups per tile (x2x), step vote + predicated record stores (xx5)."""
+    """The tuning variants of the sweep give the same answers as the default (code 215: cluster of 2 with
+    TMA multicast, one N=256 MMA group per tile, predicated record stores): no cluster (1xx), two
+    N=128 MMA groups per tile (x2x), divergent per-group record stores (xx3)."""
     from librecommender_b200 import _lib
     from librecommender_b200.engine import EmbedScorer
 
@@ -140,4 +140,4 @@ def test_kernel_organisation_variants(code):
         assert plan["use_pre"] == 1 and plan["cluster_x10_plus_mma_groups"] == code // 10, plan
         _check(sc, U, I, csr, users, K, n_oracle=64, min_ok_frac=0.97)
     finally:
-        _lib.check(_lib.lib.b200_recommend_embed_tune(213, 0.0))
+        _lib.check(_lib.lib.b200_recommend_embed_tune(215, 0.0))

@@ -1,4 +1,4 @@
-"""GPU parity of the tcgen05 3xTF32 dense layer (b200_linear_tf32x3) against an fp64 restatement
+"""GPU parity of the wgmma 3xTF32 dense layer (b200_linear_tf32x3) against an fp64 restatement
 of tf_dense (reference libreco/layers/dense.py:52-80) and against the exact-fma SIMT kernel
 (b200_linear_f32).  Tolerance: 2e-6 * sum_k |x_k w_k| — an fp32 sequential sum is itself only
 good to ~sqrt(din) * 6e-8 of that quantity, and north_star's 1e-5 relative bar on the scores is

@@ -8,7 +8,6 @@ import numpy as np
 import pytest
 
 from oracle import ranking as orc
-from oracle.ref_loader import reference_available
 
 
 def _dict_from_csr(indptr, idx):
@@ -73,25 +72,15 @@ def test_embed_matches_reference_golden(path):
         assert (got == g[key]).mean() > 0.999
 
 
-@pytest.mark.skipif(not reference_available(), reason="reference tree not present (GPU box)")
 def test_oracle_vs_live_reference_random():
-    from oracle.ref_loader import load_reference
+    """The reference's rank_recommendations on seeded random inputs (answers stored in
+    golden/live_reference.npz by golden/gen_live_reference.py)."""
+    from _fixtures import rank_cases
 
-    load_reference()
-    from libreco.recommendation import rank_recommendations as ref_rank
-
-    rng = np.random.default_rng(5)
-    for trial in range(20):
-        B, N = int(rng.integers(1, 6)), int(rng.integers(5, 400))
-        K = int(rng.integers(1, N + 1))
-        preds = rng.standard_normal((B, N)).astype(np.float32)
-        consumed = {u: rng.choice(N, size=int(rng.integers(0, N)), replace=False).tolist()
-                    for u in range(B)}
-        consumed = {u: v for u, v in consumed.items() if v}
-        uids = list(range(B))
-        ref = ref_rank("ranking", uids, preds, K, N, consumed, True, False, False)
+    g = np.load(os.path.join(os.path.dirname(__file__), "golden", "live_reference.npz"))
+    for i, (uids, preds, K, N, consumed) in enumerate(rank_cases()):
         got = orc.rank_recommendations("ranking", uids, preds, K, N, consumed, True)
-        np.testing.assert_array_equal(ref, got)
+        np.testing.assert_array_equal(g[f"rank_{i}"], got)
 
 
 def test_assign_oov_and_predict():

@@ -5,10 +5,8 @@ import os
 import random
 
 import numpy as np
-import pytest
 
 from oracle import sampling as osm
-from oracle.ref_loader import reference_available
 
 GOLD = os.path.join(os.path.dirname(__file__), "golden", "sampling.npz")
 
@@ -44,22 +42,16 @@ def test_parity_mode_bit_exact_against_reference_golden():
         osm.check_reference_invariants(got, g["users"], g["items_pos"], num_neg, n_items, consumed)
 
 
-@pytest.mark.skipif(not reference_available(), reason="reference tree not present (GPU box)")
 def test_parity_mode_vs_live_reference():
-    from oracle.ref_loader import load_reference
-
-    load_reference()
-    from libreco.sampling import negatives as ref
+    """The reference's negatives_from_random on seeded random inputs (answers stored in
+    golden/live_reference.npz by golden/gen_live_reference.py)."""
+    from _fixtures import sampling_cases
     from librecommender_b200 import sampling as S
 
-    gen = np.random.default_rng(9)
-    for trial in range(5):
-        n_items = int(gen.integers(20, 3000))
-        pos = gen.integers(0, n_items, size=int(gen.integers(1, 500)))
-        num_neg = int(gen.integers(1, 6))
-        a = ref.negatives_from_random(np.random.default_rng(trial), n_items, pos, num_neg)
+    g = np.load(os.path.join(os.path.dirname(__file__), "golden", "live_reference.npz"))
+    for i, (trial, n_items, pos, num_neg) in enumerate(sampling_cases()):
         b = S.negatives_from_random(np.random.default_rng(trial), n_items, pos, num_neg)
-        np.testing.assert_array_equal(a, b)
+        np.testing.assert_array_equal(g[f"neg_{i}"], b)
 
 
 def test_probs_from_frequency_and_philox_known_answer():

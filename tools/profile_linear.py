@@ -1,4 +1,4 @@
-"""Driver for ncu captures of the tcgen05 3xTF32 dense layer (csrc/mlp_tc.cu).
+"""Driver for ncu captures of the wgmma 3xTF32 dense layer (csrc/mlp_tc.cu).
     ncu --set full --clock-control none --import-source on -k regex:linear_tf32x3 -s 2 -c 1 \
         -o gpurun_out/prof_linear python tools/profile_linear.py
 """
