@@ -474,6 +474,30 @@ int b200_interacted_seqs(const int64_t* indptr, const int32_t* idx, int64_t n_us
                          const int64_t* rand_pos, uint64_t seed, uint64_t step, int32_t* seqs,
                          int32_t* lens, void* stream);
 
+/* ---- AutoInt inference (libreco/algorithms/autoint.py:146-168, layers/attention.py:67-138) -------
+ * X [F, K] = the pair's field embeddings [user, item, sparse.., dense..] (the b200_feat_forward concat).
+ * For each layer l (D = num_heads * hd_l; weights packed per layer as Wq [K, D], Wk [K, D], Wv [K, D],
+ * Wo [D, K], row-major, columns head-major h * hd + j as _split_heads lays them out):
+ *   Q = X Wq, K = X Wk, V = X Wv;  O_h = softmax_rows(Q_h K_h^T / sqrt(hd_l)) V_h;  Y = concat_h(O_h) Wo;
+ *   X = X + Y (use_residual) or X = Y.
+ * logit = <flatten(X), w_out [F*K]> + b_out.  Wv is the EFFECTIVE value map (the TF < 2.10 graph applies its
+ * value Dense to the projected keys, attention.py:104-106: Wv = Wk Wv').  Every dot product is one fmaf chain
+ * over an ascending index, the softmax is max, expf(x - max), an ascending sum, then a division, so both
+ * entry points give bit-identical logits for the same pair.
+ * Supported: 2 <= F <= 130, 1 <= K <= 64, 1 <= n_layers <= 4, num_heads * hd_l <= 64; anything else
+ * returns -2 before launching.  head_dims_host: HOST array [n_layers].
+ * b200_autoint_rows: out[r] for X = rows of the materialised concat X [R, ldx].
+ * b200_autoint_grid: scores[b * ld_scores + n] for every b < B, n < N; field f of pair (b, n) reads
+ *   Xu[b, s*K..] with s = field_map[f] when field_map[f] >= 0, else Xi[n, s*K..] with s = -1 - field_map[f]
+ *   (field_map: device int32 [F]); the [B*N, F*K] concat is never built. */
+int b200_autoint_rows(const float* X, int64_t ldx, int64_t R, int32_t F, int32_t K, int32_t num_heads,
+                      int32_t n_layers, const int32_t* head_dims_host, const float* weights, const float* w_out,
+                      float b_out, int32_t use_residual, float* out, void* stream);
+int b200_autoint_grid(const float* Xu, int64_t ldu, int64_t B, const float* Xi, int64_t ldi, int64_t N,
+                      const int32_t* field_map, int32_t F, int32_t K, int32_t num_heads, int32_t n_layers,
+                      const int32_t* head_dims_host, const float* weights, const float* w_out, float b_out,
+                      int32_t use_residual, float* scores, int64_t ld_scores, void* stream);
+
 /* ---- a14: predict_from_embedding (libreco/prediction/predict.py:36-40) -----------------
  * out[r] = sum_k U[users[r],k] * I[items[r],k]; mode 0: raw, 1: expit (ranking),
  * 2: clip to [lo, hi] (rating) — normalize_prediction (:18-23). */

@@ -113,6 +113,10 @@ SIGNATURES = {
     "b200_interacted_seqs": (c_int, [_P, _P, c_int64, _P, _P, c_int64, c_int32, c_int32, _P, c_uint64, c_uint64,
                                      _P, _P, _P]),
     "b200_gather_dot": (c_int, [_P, c_int64, _P, _P, c_int64, _P, c_int64, c_int32, c_int32, c_float, c_float, _P, _P]),
+    "b200_autoint_rows": (c_int, [_P, c_int64, c_int64, c_int32, c_int32, c_int32, c_int32, _P, _P, _P, c_float, c_int32,
+                                  _P, _P]),
+    "b200_autoint_grid": (c_int, [_P, c_int64, c_int64, _P, c_int64, c_int64, _P, c_int32, c_int32, c_int32, c_int32, _P,
+                                  _P, _P, c_float, c_int32, _P, c_int64, _P]),
 }
 
 for _name, (_res, _args) in SIGNATURES.items():

@@ -676,6 +676,122 @@ class DeepFM(_FeatModelBase):
         return max(1, (1 << 30) // (self.F * self.K * 4))
 
 
+AUTOINT_MAX_K = 64          # the shapes b200_autoint_rows / _grid accept (include/b200reco.h)
+AUTOINT_MAX_D = 64
+AUTOINT_MAX_LAYERS = 4
+AUTOINT_MAX_F = 130
+
+
+class AutoInt(_FeatModelBase):
+    """libreco/algorithms/autoint.py:146-168 (inference): the field embeddings [user, item, sparse.., dense..]
+    stacked into X [F, K], ``L`` layers of multi-head self-attention across the fields (layers/attention.py:67-138,
+    optional residual), then Dense(1) on the flattened block.  No linear tables, and no BN or dropout in the
+    inference graph even though the reference accepts ``use_bn``.
+
+    Weights (besides the embedding tables): ``autoint_layers`` = [{wq, wk, wv [K, D], wo [D, K]}] per layer with
+    head-major columns and ``wv`` the effective value map, ``num_heads``, ``use_residual``, ``out_kernel [F*K]``,
+    ``out_bias`` — :func:`weights_io.autoint_weights` makes them from either TensorFlow graph's variables.
+
+    Every (user, item) pair is a chain of small attentions that nothing outside the pair can be hoisted from, so
+    ``_forward`` runs ``b200_autoint_rows`` on the K1 concat and all-items scoring runs ``b200_autoint_grid`` on a
+    per-model item-side block and a per-call user-side block; both give bit-identical logits."""
+
+    needs_linear = False
+
+    def __init__(self, spec, weights, user_consumed=None, task="ranking", device=None):
+        super().__init__(spec, weights, user_consumed, task, device)
+        torch = self._torch
+        K, F = self.K, self.F
+        H = int(weights["num_heads"])
+        layers = list(weights["autoint_layers"])
+        if K > AUTOINT_MAX_K:
+            raise ValueError(f"AutoInt: embed size {K} > {AUTOINT_MAX_K} is not supported")
+        if F > AUTOINT_MAX_F:
+            raise ValueError(f"AutoInt: {F} fields > {AUTOINT_MAX_F} (2 ids + 128 features) is not supported")
+        if not 1 <= len(layers) <= AUTOINT_MAX_LAYERS:
+            raise ValueError(f"AutoInt: {len(layers)} attention layers, supported 1..{AUTOINT_MAX_LAYERS}")
+        if H < 1:
+            raise ValueError(f"AutoInt: num_heads {H} < 1")
+        hds, packed = [], []
+        for i, lw in enumerate(layers):
+            wq, wk, wv, wo = (np.asarray(lw[k], dtype=np.float32) for k in ("wq", "wk", "wv", "wo"))
+            D = wq.shape[1]
+            if D % H or D > AUTOINT_MAX_D:
+                raise ValueError(f"AutoInt layer {i}: width {D} must be num_heads ({H}) x head size and <= "
+                                 f"{AUTOINT_MAX_D}")
+            if wq.shape != (K, D) or wk.shape != (K, D) or wv.shape != (K, D) or wo.shape != (D, K):
+                raise ValueError(f"AutoInt layer {i}: shapes wq {wq.shape} wk {wk.shape} wv {wv.shape} wo {wo.shape}, "
+                                 f"expected [{K}, {D}] x 3 and [{D}, {K}]")
+            hds.append(D // H)
+            packed += [wq.reshape(-1), wk.reshape(-1), wv.reshape(-1), wo.reshape(-1)]
+        out_kernel = np.asarray(weights["out_kernel"], dtype=np.float32).reshape(-1)
+        if out_kernel.size != F * K:
+            raise ValueError(f"AutoInt: out_kernel has {out_kernel.size} entries, expected F*K = {F}*{K}")
+        self.num_heads, self.head_dims = H, hds
+        self.use_residual = bool(weights.get("use_residual", True))
+        self._hd_host = np.asarray(hds, dtype=np.int32)
+        self.w_layers = _dev(np.concatenate(packed), self.device, torch.float32)
+        self.out_kernel = _dev(out_kernel, self.device, torch.float32)
+        self.out_bias = float(np.asarray(weights["out_bias"]).reshape(-1)[0])
+
+    def _head(self):
+        return (self.F, self.K, self.num_heads, len(self.head_dims), _lib.ptr(self._hd_host), _lib.ptr(self.w_layers),
+                _lib.ptr(self.out_kernel), self.out_bias, int(self.use_residual))
+
+    def _forward(self, layout, users_d, items_d, R, grid_items):
+        torch = self._torch
+        out = torch.empty(R, dtype=torch.float32, device=self.device)
+        step = self.max_grid_rows()
+        for r0 in range(0, R, step):                  # bound the materialised [rows, F*K] concat
+            r1 = min(R, r0 + step)
+            n = r1 - r0
+            concat = torch.empty((n, self.F * self.K), dtype=torch.float32, device=self.device)
+            if grid_items > 0:
+                self._feat_forward(layout, users_d, None, n, grid_items, concat=concat, row_offset=r0)
+            else:
+                self._feat_forward(layout, users_d[r0:r1], items_d[r0:r1], n, 0, concat=concat)
+            _lib.check(_lib.lib.b200_autoint_rows(_lib.ptr(concat), concat.stride(0), n, *self._head(),
+                                                  _lib.ptr(out[r0:r1]), _lib.current_stream()))
+        return out
+
+    def _side_block(self, which, ids_d):
+        """[n, F_side*K] field embeddings of ONE side, in the side's field order of :meth:`_side`."""
+        L, pos = self._side(which)
+        n = int(ids_d.numel())
+        x = self._torch.empty((n, len(pos) * self.K), dtype=self._torch.float32, device=self.device)
+        self._feat_forward(L, ids_d, ids_d, n, 0, concat=x)
+        return x
+
+    def _field_map(self):
+        """int32 [F]: global field f comes from user-side slot m (m >= 0) or item-side slot -1 - m."""
+        if "_fmap" not in self.__dict__:
+            m = np.zeros(self.F, dtype=np.int32)
+            for j, f in enumerate(self._side("user")[1]):
+                m[f] = j
+            for j, f in enumerate(self._side("item")[1]):
+                m[f] = -1 - j
+            self._fmap = _dev(m, self.device, self._torch.int32)
+        return self._fmap
+
+    def score_all_items(self, user_ids_d):
+        """All L layers per (user, item) pair in one kernel: the item-side block once per model (rebuilt after
+        ``assign_oov``), the user-side block once per call; the [b*N, F*K] concat is never built."""
+        torch = self._torch
+        if "_item_side" not in self.__dict__:
+            self._item_side = self._side_block("item", torch.arange(self.n_items, device=self.device))
+        Xi = self._item_side
+        Xu = self._side_block("user", user_ids_d)
+        b, N = int(user_ids_d.numel()), self.n_items
+        scores = torch.empty((b, N), dtype=torch.float32, device=self.device)
+        _lib.check(_lib.lib.b200_autoint_grid(_lib.ptr(Xu), Xu.stride(0), b, _lib.ptr(Xi), Xi.stride(0), N,
+                                              _lib.ptr(self._field_map()), *self._head(), _lib.ptr(scores),
+                                              scores.stride(0), _lib.current_stream()))
+        return scores
+
+    def max_grid_rows(self):
+        return max(1, (1 << 30) // (self.F * self.K * 4))
+
+
 def wide_deep_weights(user_wide, item_wide, sparse_wide, dense_wide, wide_kernel, wide_bias, user_deep, item_deep,
                       sparse_deep, dense_deep, mlp, deep_kernel, deep_bias):
     """WideDeep (``libreco/algorithms/wide_deep.py:150-262``, SURVEY 8f-4) on the DeepFM engine: the wide term

@@ -163,3 +163,34 @@ def make_two_tower_weights(rng, spec, K, hidden=(64, 32), use_bn=True):
     w["user_dense_cols"] = list(spec["user_dense_col_index"])
     w["item_dense_cols"] = list(spec["item_dense_col_index"])
     return w
+
+
+def make_autoint_weights(rng, spec, K, att_embed_size=(8, 8, 8), num_heads=2, use_residual=True, version="keras",
+                         combiner="sqrtn"):
+    """AutoInt variables in the raw shapes of the graph TensorFlow `version` builds (layers/attention.py:67-138):
+    "keras" (>= 2.10) query / key / value [K, H, hd] and attention_output [H, hd, K]; "legacy" q, k [K, D],
+    v [D, D] (applied to the projected keys) and out [D, K].  ``weights_io.autoint_weights`` turns them into
+    the engine's dict.  F counts a multi-sparse group as one field unless ``combiner == "normal"``."""
+    from .weights_io import autoint_head_dims, autoint_scheme
+
+    scheme = autoint_scheme(version)
+    w = make_embeddings(rng, spec, K, linear=False)
+    n_sparse = spec["n_sparse"]
+    info = spec.get("multi_sparse_combine_info")
+    if info is not None and combiner != "normal":
+        n_sparse = int(info["field_offset"][0]) + len(info["field_offset"])
+    F = 2 + n_sparse + spec["n_dense"]
+    H = int(num_heads)
+    mha = []
+    for hd in autoint_head_dims(att_embed_size):
+        D = H * hd
+        if scheme == "keras":
+            mha.append(dict(query=_glorot(rng, (K, D)).reshape(K, H, hd), key=_glorot(rng, (K, D)).reshape(K, H, hd),
+                            value=_glorot(rng, (K, D)).reshape(K, H, hd),
+                            attention_output=_glorot(rng, (D, K)).reshape(H, hd, K)))
+        else:
+            mha.append(dict(query=_glorot(rng, (K, D)), key=_glorot(rng, (K, D)), value=_glorot(rng, (D, D)),
+                            output=_glorot(rng, (D, K))))
+    w.update(autoint_scheme=scheme, autoint_mha=mha, num_heads=H, use_residual=bool(use_residual),
+             out_kernel=_glorot(rng, (F * K, 1)), out_bias=np.float32(0.02).reshape(1))
+    return w

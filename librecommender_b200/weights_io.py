@@ -90,7 +90,8 @@ def load_default_recs(path, model_name):
 # ``tf.variable_scope`` — ``dense_nn`` opens ``<name>`` (default "mlp") and names its Dense layers
 # ``<name>_layer<i>`` (layers/dense.py:28-33).  The creation order per model is read off the graph
 # builders: fm.py:152-171, deepfm.py:158-174, din.py:205-218 (+ the "attention" dense_nn,
-# layers/attention.py:47-53), youtube_ranking.py:208-217, two_tower.py:400-409.  No TensorFlow exists in
+# layers/attention.py:47-53), youtube_ranking.py:208-217, two_tower.py:400-409, autoint.py:160-168 (+
+# multi_head_attention, layers/attention.py:67-138, whose graph depends on the TensorFlow version).  No TensorFlow exists in
 # this environment, so this table is RESTATED from TensorFlow's documented uniquifying rule and is
 # unverified against a real checkpoint; ``resolve_tf_names`` therefore checks every expected name AND
 # shape against the file and reports exactly what is missing instead of guessing.
@@ -108,9 +109,55 @@ def _mlp_names(scope, n_layers, use_bn):
     return names
 
 
-def default_tf_names(model_name, n_hidden, use_bn, use_tf_attention=False):
+def _dense_name(i):
+    return "dense" if i == 0 else f"dense_{i}"
+
+
+def autoint_head_dims(att_embed_size):
+    """``attention_config`` (libreco/tfops/configs.py:6-17): head size per attention layer; None / 0 -> (8, 8, 8),
+    an int -> one layer."""
+    if not att_embed_size:
+        return [8, 8, 8]
+    if isinstance(att_embed_size, (int, np.integer)):
+        return [int(att_embed_size)]
+    if isinstance(att_embed_size, (list, tuple)):
+        return [int(v) for v in att_embed_size]
+    raise ValueError("att_embed_size must be int or list")
+
+
+def autoint_scheme(version):
+    """Which graph ``multi_head_attention`` (layers/attention.py:67-138) built: "keras" for TensorFlow >= 2.10
+    (``tf.keras.layers.MultiHeadAttention``), "legacy" before.  Takes a scheme name or a TF version string."""
+    if version in AUTOINT_SCHEMES:
+        return version
+    parts = [int(p) for p in str(version).split(".")[:2] if p.isdigit()]
+    return "keras" if tuple(parts + [0, 0][len(parts):]) >= (2, 10) else "legacy"
+
+
+AUTOINT_SCHEMES = ("keras", "legacy")
+
+
+def default_tf_names(model_name, n_hidden, use_bn, use_tf_attention=False, n_layers=None, scheme="keras"):
     """{engine weight key: TF variable name (or nested dict / list of names)} for the auto-named
-    variables of `model_name` in {"FM", "DeepFM", "DIN", "YouTubeRanking", "TwoTower"}."""
+    variables of `model_name` in {"FM", "DeepFM", "DIN", "YouTubeRanking", "TwoTower", "AutoInt"}.
+
+    AutoInt (autoint.py:160-168, one ``multi_head_attention`` per layer, then ``tf_dense(1)``) has two schemes:
+    "keras" (TF >= 2.10): ``multi_head_attention[_i]/{query,key,value,attention_output}/kernel:0`` and the head
+    ``dense/{kernel,bias}:0``; "legacy": four bias-free ``tf_dense`` per layer created as q, k, v, out, so layer l
+    owns ``dense_{4l}`` .. ``dense_{4l+3}`` and the head is ``dense_{4L}``.  Returned under ``autoint_mha``
+    (per-layer {query, key, value, attention_output | output}), ``out_kernel``, ``out_bias``."""
+    if model_name == "AutoInt":
+        if scheme == "keras":
+            mha = [{k: f"multi_head_attention{'' if i == 0 else f'_{i}'}/{k}/kernel:0"
+                    for k in ("query", "key", "value", "attention_output")} for i in range(n_layers)]
+            head = _dense_name(0)
+        elif scheme == "legacy":
+            mha = [{k: f"{_dense_name(4 * i + j)}/kernel:0" for j, k in enumerate(("query", "key", "value", "output"))}
+                   for i in range(n_layers)]
+            head = _dense_name(4 * n_layers)
+        else:
+            raise ValueError(f"unknown AutoInt naming scheme `{scheme}`")
+        return {"autoint_mha": mha, "out_kernel": f"{head}/kernel:0", "out_bias": f"{head}/bias:0"}
     if model_name == "FM":
         out = {"lin_kernel": "dense/kernel:0", "lin_bias": "dense/bias:0",
                "pw_kernel": "dense_1/kernel:0", "pw_bias": "dense_1/bias:0"}
@@ -134,30 +181,97 @@ def default_tf_names(model_name, n_hidden, use_bn, use_tf_attention=False):
     raise ValueError(f"no TensorFlow name table for model `{model_name}`")
 
 
-def resolve_tf_names(npz, names):
+def resolve_tf_names(npz, names, shapes=None):
     """Read the (possibly nested) name table out of `npz`; a missing variable raises a ``KeyError`` that
-    lists the expected name and the names the file does contain."""
-    def take(n):
+    lists the expected name and the names the file does contain.  With `shapes` (the same nesting, a shape
+    tuple per name, ``None`` entries match any size) a variable of another shape raises the same way."""
+    def have():
+        return sorted(f"{k} {tuple(np.shape(npz[k]))}" for k in npz.files if not k.startswith("embedding/"))
+
+    def take(n, shp):
         if isinstance(n, dict):
-            return {k: take(v) for k, v in n.items()}
+            return {k: take(v, shp[k] if shp is not None else None) for k, v in n.items()}
         if isinstance(n, list):
-            return [take(v) for v in n]
+            return [take(v, shp[i] if shp is not None else None) for i, v in enumerate(n)]
         if n not in npz:
-            have = sorted(k for k in npz.files if not k.startswith("embedding/"))
-            raise KeyError(f"TF variable `{n}` not in the file; non-embedding variables present: {have}")
-        return np.asarray(npz[n])
-    return take(names)
+            raise KeyError(f"TF variable `{n}` not in the file; non-embedding variables present: {have()}")
+        a = np.asarray(npz[n])
+        if shp is not None and (a.ndim != len(shp) or any(e is not None and e != d for e, d in zip(shp, a.shape))):
+            raise KeyError(f"TF variable `{n}` has shape {a.shape}, expected {tuple(shp)}; non-embedding variables "
+                           f"present: {have()}")
+        return a
+    return take(names, shapes)
 
 
-def load_reference_tf_model(path, model_name, arch, n_hidden, use_bn, use_tf_attention=False, extra_names=None):
+def autoint_tf_shapes(scheme, K, num_heads, head_dims):
+    """Expected shapes for :func:`default_tf_names` ("AutoInt"): keras ``query/key/value [K, H, hd]``,
+    ``attention_output [H, hd, K]``; legacy ``q, k [K, D]``, ``v [D, D]`` (applied to the projected keys),
+    ``out [D, K]``; the head ``[F*K, 1]`` (F is not known here) and ``[1]``."""
+    H = num_heads
+    if scheme == "keras":
+        mha = [dict(query=(K, H, hd), key=(K, H, hd), value=(K, H, hd), attention_output=(H, hd, K)) for hd in head_dims]
+    else:
+        mha = [dict(query=(K, H * hd), key=(K, H * hd), value=(H * hd, H * hd), output=(H * hd, K)) for hd in head_dims]
+    return {"autoint_mha": mha, "out_kernel": (None, 1), "out_bias": (1,)}
+
+
+def autoint_layers(mha, scheme):
+    """Per-layer variables of either graph -> the engine's ``autoint_layers`` [{wq, wk, wv [K, D], wo [D, K]}],
+    columns head-major (h * hd + j, the order ``_split_heads`` reshapes into).  keras: the [K, H, hd] / [H, hd, K]
+    kernels flattened.  legacy: ``values = tf_dense(D)(keys)`` acts on the PROJECTED keys (attention.py:104-106),
+    so V = (X Wk) Wv' and the effective value map is Wk Wv', multiplied in float64 and then cast."""
+    out = []
+    for lw in mha:
+        if scheme == "keras":
+            K, H, hd = np.shape(lw["query"])
+            flat = lambda a: np.asarray(a, dtype=np.float32).reshape(K, H * hd)      # noqa: E731
+            out.append(dict(wq=flat(lw["query"]), wk=flat(lw["key"]), wv=flat(lw["value"]),
+                            wo=np.asarray(lw["attention_output"], dtype=np.float32).reshape(H * hd, K)))
+        elif scheme == "legacy":
+            wk = np.asarray(lw["key"], dtype=np.float32)
+            wv = (wk.astype(np.float64) @ np.asarray(lw["value"], dtype=np.float64)).astype(np.float32)
+            out.append(dict(wq=np.asarray(lw["query"], dtype=np.float32), wk=wk, wv=wv,
+                            wo=np.asarray(lw["output"], dtype=np.float32)))
+        else:
+            raise ValueError(f"unknown AutoInt naming scheme `{scheme}`")
+    return out
+
+
+def autoint_weights(raw):
+    """Engine weight dict for :class:`feat_models.AutoInt` from the raw variables of either graph: ``raw`` holds
+    the embedding tables, ``autoint_scheme``, ``autoint_mha`` (per layer, as :func:`default_tf_names` names them),
+    ``num_heads``, ``use_residual``, ``out_kernel`` and ``out_bias``; other entries pass through."""
+    w = {k: v for k, v in raw.items() if k not in ("autoint_mha", "autoint_scheme")}
+    w["autoint_layers"] = autoint_layers(raw["autoint_mha"], raw["autoint_scheme"])
+    w["out_kernel"] = np.asarray(raw["out_kernel"], dtype=np.float32).reshape(-1)
+    w["out_bias"] = np.float32(np.asarray(raw["out_bias"]).reshape(-1)[0])
+    return w
+
+
+def load_reference_tf_model(path, model_name, arch, n_hidden, use_bn, use_tf_attention=False, extra_names=None,
+                            num_heads=2, att_embed_size=(8, 8, 8), use_residual=True):
     """Engine weight dict of a model saved by the reference (``save_tf_variables``,
     utils/save_load.py:70-98) WITHOUT a hand-written name map: the embedding-scope variables by their
     fixed names, the heads / MLPs / batch-norms through :func:`default_tf_names` (override single entries
-    with `extra_names`)."""
+    with `extra_names`).  AutoInt takes its own constructor arguments ``num_heads``, ``att_embed_size`` and
+    ``use_residual``; its naming scheme (keras or legacy) is read off the names in the file, and every name
+    and shape is checked."""
     from .feat_models import from_tf_variables
 
     npz = np.load(os.path.join(path, f"{model_name}_tf_variables.npz"))
     w = from_tf_variables(npz)
+    if arch == "AutoInt":
+        hds = autoint_head_dims(att_embed_size)
+        scheme = "keras" if "multi_head_attention/query/kernel:0" in npz.files else "legacy"
+        names = default_tf_names(arch, n_hidden, use_bn, n_layers=len(hds), scheme=scheme)
+        names.update(extra_names or {})
+        K = int(np.shape(npz[EMBEDDING_SCOPE["user_embeds"]])[1])
+        raw = resolve_tf_names(npz, names, autoint_tf_shapes(scheme, K, int(num_heads), hds))
+        if raw["out_kernel"].shape[0] % K or raw["out_kernel"].shape[0] < 2 * K:
+            raise KeyError(f"TF variable `{names['out_kernel']}` has shape {raw['out_kernel'].shape}, expected "
+                           f"[F*{K}, 1]")
+        w.update(raw, autoint_scheme=scheme, num_heads=int(num_heads), use_residual=bool(use_residual))
+        return autoint_weights(w)
     names = default_tf_names(arch, n_hidden, use_bn, use_tf_attention)
     names.update(extra_names or {})
     w.update(resolve_tf_names(npz, names))
