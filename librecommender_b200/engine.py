@@ -60,6 +60,26 @@ def _as_device_f32(x, device):
     return t.contiguous()
 
 
+def masked_topk(owner, scores, user_ids_d, n_rec, filter_consumed, out_ids, out_scores):
+    """Consumed filter + top-``n_rec`` of the device fp32 score rows ``scores`` [b, ld] (clobbered by the mask) of
+    the users ``user_ids_d`` into ``out_ids`` / ``out_scores`` (nullable).  ``owner`` holds the catalogue size
+    ``n_items`` and the consumed CSR (``csr`` with its device arrays ``indptr_d``, ``idx_d``)."""
+    import torch
+
+    b, ld = scores.shape[0], scores.stride(0)
+    N = owner.n_items
+    stream = _lib.current_stream()
+    if filter_consumed and owner.csr.nnz > 0:
+        _lib.check(_lib.lib.b200_mask_consumed(
+            _lib.ptr(scores), ld, _lib.ptr(user_ids_d), b, N, n_rec,
+            _lib.ptr(owner.indptr_d), _lib.ptr(owner.idx_d), owner.csr.n_users, stream))
+    nbytes = ctypes.c_size_t(0)
+    _lib.check(_lib.lib.b200_topk_rows_workspace_bytes(b, N, n_rec, ctypes.byref(nbytes)))
+    ws = torch.empty(nbytes.value, dtype=torch.uint8, device=scores.device)
+    _lib.check(_lib.lib.b200_topk_rows(
+        _lib.ptr(scores), ld, b, N, n_rec, _lib.ptr(out_ids), _lib.ptr(out_scores), _lib.ptr(ws), nbytes.value, stream))
+
+
 class EmbedScorer:
     """Score-all-items + consumed filter + top-K for embedding models (a1 + a2)."""
 
@@ -104,21 +124,7 @@ class EmbedScorer:
     # ------------------------------------------------------------------------------------
     def topk_scores_inplace(self, scores, user_ids_d, n_rec, filter_consumed, out_ids, out_scores):
         """scores: device fp32 [b, ld] (clobbered by the mask)."""
-        torch = self._torch
-        b, ld = scores.shape[0], scores.stride(0)
-        N = self.n_items
-        stream = _lib.current_stream()
-        if filter_consumed and self.csr.nnz > 0:
-            _lib.check(_lib.lib.b200_mask_consumed(
-                _lib.ptr(scores), ld, _lib.ptr(user_ids_d), b, N, n_rec,
-                _lib.ptr(self.indptr_d), _lib.ptr(self.idx_d), self.csr.n_users, stream))
-        nbytes = ctypes.c_size_t(0)
-        _lib.check(_lib.lib.b200_topk_rows_workspace_bytes(b, N, n_rec, ctypes.byref(nbytes)))
-        ws = torch.empty(nbytes.value, dtype=torch.uint8, device=self.device)
-        _lib.check(_lib.lib.b200_topk_rows(
-            _lib.ptr(scores), ld, b, N, n_rec, _lib.ptr(out_ids),
-            _lib.ptr(out_scores) if out_scores is not None else None,
-            _lib.ptr(ws), nbytes.value, stream))
+        masked_topk(self, scores, user_ids_d, n_rec, filter_consumed, out_ids, out_scores)
 
     def recommend_exact(self, user_ids_d, n_rec, filter_consumed=True, return_scores=False):
         """Exact fp32 path: materialise score row-batches, mask, radix top-K."""

@@ -20,6 +20,7 @@ import numpy as np
 
 from . import _lib
 from .consumed import ConsumedCSR, as_csr
+from .engine import masked_topk
 
 MAX_FIELDS = 128
 BN_EPS = 1e-3
@@ -59,6 +60,46 @@ def _dev(x, device, dtype):
     if isinstance(x, torch.Tensor):
         return x.to(device=device, dtype=dtype).contiguous()
     return torch.as_tensor(np.ascontiguousarray(x)).to(device=device, dtype=dtype).contiguous()
+
+
+def tables_struct(tensors):
+    """FeatTablesStruct over the device tables in the dict ``tensors`` (missing or None: NULL)."""
+    T = FeatTablesStruct()
+    for name, _ in FeatTablesStruct._fields_:
+        t = tensors.get(name)
+        setattr(T, name, t.data_ptr() if t is not None else None)
+    return T
+
+
+def _ld(t):
+    return t.stride(0) if t is not None else 0
+
+
+def feat_forward(layout, tables, users, items, R, *, grid_items=0, row_offset=0, concat=None, pw=None, lin=None,
+                 fm_out=None, lin_kernel=None, lin_bias=0.0, head=None, ssum=None, sqsum=None):
+    """K1, ``b200_feat_forward``: gathers the field embeddings of R (user, item) rows — explicit ``users`` /
+    ``items``, or rows ``row_offset`` .. of the implicit grid of every user with items 0..``grid_items``-1 — into whichever outputs are given: the concat [R, F*K], the FM pairwise block ``pw``
+    [R, K], the linear term ``lin`` (``lin_kernel``, ``lin_bias``), FM's whole output ``fm_out`` (``head``: BN
+    scale / shift, pw kernel / bias) and the field sums ``ssum`` / ``sqsum`` [R, K]."""
+    head = head or {}
+    _lib.check(_lib.lib.b200_feat_forward(
+        ctypes.byref(layout), ctypes.byref(tables), _lib.ptr(users), _lib.ptr(items), R, grid_items, row_offset,
+        _lib.ptr(concat), _ld(concat), _lib.ptr(pw), _ld(pw), _lib.ptr(lin), _lib.ptr(fm_out), _lib.ptr(lin_kernel),
+        float(lin_bias), _lib.ptr(head.get("bn_scale")), _lib.ptr(head.get("bn_shift")),
+        _lib.ptr(head.get("pw_kernel")), float(head.get("pw_bias", 0.0)), _lib.ptr(ssum), _lib.ptr(sqsum), _ld(ssum),
+        _lib.current_stream()))
+
+
+def feat_backward(layout, tables, users, items, R, grads, *, dpw=None, S=None, dconcat=None, dlogit=None,
+                  lin_kernel=None):
+    """Backward of :func:`feat_forward` (``b200_feat_backward``): the field gradients of the FM block (``dpw``,
+    ``S``), of the concat (``dconcat``) and of the linear term (``dlogit``, ``lin_kernel``) scatter-ADDED into the
+    buffers of ``grads`` named like the tables (and ``lin_kernel``); absent names are skipped."""
+    _lib.check(_lib.lib.b200_feat_backward(
+        ctypes.byref(layout), ctypes.byref(tables), _lib.ptr(users), _lib.ptr(items), R, _lib.ptr(dpw), _ld(dpw),
+        _lib.ptr(S), _ld(S), _lib.ptr(dconcat), _ld(dconcat), _lib.ptr(dlogit), _lib.ptr(lin_kernel),
+        *[_lib.ptr(grads.get(name)) for name, _ in FeatTablesStruct._fields_], _lib.ptr(grads.get("lin_kernel")),
+        _lib.current_stream()))
 
 
 # Dense-layer kernel selection: "auto" sends layers that are compute-bound on the SIMT kernel
@@ -295,6 +336,28 @@ class FeatSpec:
         self.layout = L
         self.item_sparse_cols, self.item_dense_cols = icol, idc
         self.user_sparse_cols, self.user_dense_cols = ucol, udc
+        self._sides = {}
+
+    def side(self, which, with_id=True):
+        """(layout restricted to the fields of one side, ``which`` = "user" or "item", and their positions in the
+        global field order [user, item, sparse.., dense..]), built once.  ``with_id=False`` leaves out the side's
+        id field."""
+        key = (which, with_id)
+        if key not in self._sides:
+            s = 0 if which == "user" else 1
+            scols = self.user_sparse_cols if s == 0 else self.item_sparse_cols
+            dcols = self.user_dense_cols if s == 0 else self.item_dense_cols
+            L = FeatLayoutStruct.from_buffer_copy(self.layout)
+            L.id_mask = (1 << s) if with_id else 0
+            L.n_sparse, L.n_dense = len(scols), len(dcols)
+            for f in range(len(scols)):
+                L.sparse_side[f], L.sparse_col[f] = s, f
+            for f in range(len(dcols)):
+                L.dense_side[f], L.dense_col[f] = s, f
+                L.dense_embed_row[f] = dcols[f]
+            pos = ([s] if with_id else []) + [2 + c for c in scols] + [2 + self.n_sparse + c for c in dcols]
+            self._sides[key] = (L, pos)
+        return self._sides[key]
 
     def with_rows(self, sparse_rows, dense_rows):
         """Layout copy that reads explicit per-row features (predict with given feature rows)."""
@@ -325,13 +388,8 @@ class _FeatModelBase:
         self.n_users, self.n_items = self.spec.n_users, self.spec.n_items
         self.F = 2 + self.spec.n_sparse + self.spec.n_dense
         f32 = torch.float32
-        self.t = {k: _dev(weights.get(k), self.device, f32) for k in
-                  ("user_embeds", "item_embeds", "sparse_embeds", "dense_embeds",
-                   "user_linear", "item_linear", "sparse_linear", "dense_linear")}
-        T = FeatTablesStruct()
-        for k, v in self.t.items():
-            setattr(T, k, v.data_ptr() if v is not None else None)
-        self.tables = T
+        self.t = {k: _dev(weights.get(k), self.device, f32) for k, _ in FeatTablesStruct._fields_}
+        self.tables = tables_struct(self.t)
         if self.needs_linear:
             self.lin_kernel = _dev(np.asarray(weights["lin_kernel"]).reshape(-1), self.device, f32)
             self.lin_bias = float(np.asarray(weights["lin_bias"]).reshape(-1)[0])
@@ -340,46 +398,106 @@ class _FeatModelBase:
         self.csr = as_csr(csr, self.n_users)
         self.indptr_d, self.idx_d = self.csr.device(self.device)
 
-    # -- to be provided by subclasses ---------------------------------------------------------
-    def _forward(self, layout, users_d, items_d, R, grid_items):
+    # -- row forward: chunks of materialised rows -------------------------------------------------
+    def _row_width(self):
+        """Floats per row of the input a chunk of ``_forward`` materialises: the F field embeddings."""
+        return self.F * self.K
+
+    def _chunk_logits(self, layout, users_d, items_d, n, grid_items, row_offset, x, out):
+        """Logits ``out`` [n] of one chunk of rows; ``x`` [n, _row_width()] is free for the chunk's input."""
         raise NotImplementedError
 
+    def _forward(self, layout, users_d, items_d, R, grid_items):
+        torch = self._torch
+        out = torch.empty(R, dtype=torch.float32, device=self.device)
+        step = self.max_grid_rows()
+        for r0 in range(0, R, step):                  # bound the materialised [rows, width] input
+            r1 = min(R, r0 + step)
+            n = r1 - r0
+            x = torch.empty((n, self._row_width()), dtype=torch.float32, device=self.device)
+            if grid_items > 0:
+                self._chunk_logits(layout, users_d, None, n, grid_items, r0, x, out[r0:r1])
+            else:
+                self._chunk_logits(layout, users_d[r0:r1], items_d[r0:r1], n, 0, 0, x, out[r0:r1])
+        return out
+
     # -- hoisted all-items scoring: one-sided partial sums (SURVEY.md §7.2-4) -----------------------
-    def _side(self, which):
-        """(layout restricted to the fields of one side, their positions in the global field order)."""
-        cache = self.__dict__.setdefault("_side_cache", {})
-        if which not in cache:
-            sp = self.spec
-            L = FeatLayoutStruct.from_buffer_copy(sp.layout)
-            L.id_mask = 1 if which == "user" else 2
-            scols = sp.user_sparse_cols if which == "user" else sp.item_sparse_cols
-            dcols = sp.user_dense_cols if which == "user" else sp.item_dense_cols
-            L.n_sparse, L.n_dense = len(scols), len(dcols)
-            for f in range(len(scols)):
-                L.sparse_side[f], L.sparse_col[f] = (0 if which == "user" else 1), f
-            for f in range(len(dcols)):
-                L.dense_side[f], L.dense_col[f] = (0 if which == "user" else 1), f
-                L.dense_embed_row[f] = dcols[f]
-            pos = [0 if which == "user" else 1] + [2 + c for c in scols] + [2 + sp.n_sparse + c for c in dcols]
-            cache[which] = (L, pos)
-        return cache[which]
+    def _side_concat(self, which, ids_d, want_concat=True, extra=0, **outs):
+        """[n, F_side*K + extra] field embeddings of ONE side for the given ids, in the order of
+        :meth:`FeatSpec.side` (``extra`` columns left for the caller); ``outs``: further outputs of the same
+        gather."""
+        L, pos = self.spec.side(which)
+        n = int(ids_d.numel())
+        x = None
+        if want_concat:
+            x = self._torch.empty((n, len(pos) * self.K + extra), dtype=self._torch.float32, device=self.device)
+        self._feat_forward(L, ids_d, ids_d, n, 0, concat=x, **outs)
+        return x
 
     def _side_partials(self, which, ids_d, want_concat):
         """S = sum_f e, Q = sum_f e^2, linear partial (no bias) and optionally the concatenated
         embeddings of ONE side for the given ids."""
         torch = self._torch
-        L, pos = self._side(which)
         n = int(ids_d.numel())
         S = torch.empty((n, self.K), dtype=torch.float32, device=self.device)
         Q = torch.empty((n, self.K), dtype=torch.float32, device=self.device)
         lin = torch.empty(n, dtype=torch.float32, device=self.device)
-        concat = torch.empty((n, len(pos) * self.K), dtype=torch.float32, device=self.device) if want_concat else None
         lk = self.__dict__.setdefault("_side_lin", {})
         if which not in lk:
+            pos = self.spec.side(which)[1]
             lk[which] = self.lin_kernel[torch.as_tensor(pos, device=self.device)].contiguous()
-        self._feat_forward(L, ids_d, ids_d, n, 0, concat=concat, lin=lin, ssum=S, sqsum=Q,
-                           lin_kernel=lk[which], lin_bias=0.0)
+        concat = self._side_concat(which, ids_d, want_concat, lin=lin, ssum=S, sqsum=Q, lin_kernel=lk[which],
+                                   lin_bias=0.0)
         return S, Q, lin, concat
+
+    # -- hoisted all-items scoring of the MLP models (DeepFM, YouTubeRanking, DIN) -------------------
+    def _hoistable(self):
+        """The pair kernel takes the MLP's small layers: 2 or 3 Dense layers of at most 256, 64, 32 units."""
+        dims = [w.shape[0] for w, _, _ in self.mlp]
+        n = len(dims)
+        return self.K <= 64 and n in (2, 3) and dims[0] <= 256 and dims[1] <= 64 and (n == 2 or dims[2] <= 32)
+
+    def _first_layer_partial(self, which, x, with_bias, extra_groups=()):
+        """x [n, F_side*K (+ K per extra group)] times the first MLP layer's columns of ONE side's fields (BN
+        folded), then those of ``extra_groups`` (K-blocks after the F fields); the layer bias when ``with_bias``."""
+        cache = self.__dict__.setdefault("_w1_side", {})
+        if which not in cache:
+            torch = self._torch
+            groups = list(self.spec.side(which)[1]) + list(extra_groups)
+            cols = torch.cat([torch.arange(g * self.K, (g + 1) * self.K, device=self.device) for g in groups])
+            cache[which] = self.mlp[0][0][:, cols].contiguous()          # Wt [H1, F_side*K]
+        return linear(x, cache[which], self.mlp[0][1] if with_bias else None, False)
+
+    def _pair_scores(self, Pu, Pi, scores, fm=None):
+        """``b200_deepfm_pair_scores``: scores [b, N] of every (user b, item n) pair from the first-layer partials
+        Pu [b, H1] and Pi [N, H1] through the MLP's small layers and the output kernel.  ``fm`` = (Su, Qu, lu, Si,
+        Qi, li): DeepFM's FM block and linear term; without it (the sequence models) those inputs are zero blocks
+        and their output weights zero."""
+        torch = self._torch
+        K = self.K
+        b, N = int(Pu.shape[0]), int(Pi.shape[0])
+        if "_tail" not in self.__dict__:
+            three = len(self.mlp) == 3
+            self._tail = (self.mlp[1][0].t().contiguous(), self.mlp[2][0].t().contiguous() if three else None)
+        W2, W3 = self._tail
+        three = W3 is not None
+        if fm is not None:
+            w_out, lin_bias = self.out_kernel, self.lin_bias
+        else:
+            if "_w_out" not in self.__dict__:
+                self._w_out = torch.cat([torch.zeros(1 + K, dtype=torch.float32, device=self.device),
+                                         self.out_kernel]).contiguous()
+                self._zeros_i = torch.zeros((self.n_items, K + 1), dtype=torch.float32, device=self.device)
+            if self.__dict__.get("_zeros_u") is None or self._zeros_u.shape[0] < b:
+                self._zeros_u = torch.zeros((b, K + 1), dtype=torch.float32, device=self.device)
+            zu, zi = self._zeros_u, self._zeros_i
+            fm, w_out, lin_bias = (zu, zu, zu, zi, zi, zi), self._w_out, 0.0
+        Su, Qu, lu, Si, Qi, li = fm
+        _lib.check(_lib.lib.b200_deepfm_pair_scores(
+            _lib.ptr(Su), _lib.ptr(Qu), _lib.ptr(lu), _lib.ptr(Pu), b, _lib.ptr(Si), _lib.ptr(Qi), _lib.ptr(li),
+            _lib.ptr(Pi), N, K, Pu.shape[1], W2.shape[1], W3.shape[1] if three else 0, lin_bias, _lib.ptr(W2),
+            _lib.ptr(self.mlp[1][1]), _lib.ptr(W3), _lib.ptr(self.mlp[2][1]) if three else None, _lib.ptr(w_out),
+            self.out_bias, _lib.ptr(scores), scores.stride(0), _lib.current_stream()))
 
     # -- public ------------------------------------------------------------------------------------
     def logits(self, users, items, sparse_rows=None, dense_rows=None):
@@ -418,21 +536,15 @@ class _FeatModelBase:
             rows_per_chunk = max(1, min(B, (1 << 28) // max(self.n_items, 1)))
         out_ids = torch.empty((B, n_rec), dtype=torch.int64, device=self.device)
         out_sc = torch.empty((B, n_rec), dtype=torch.float32, device=self.device)
-        lib, stream = _lib.lib, _lib.current_stream()
         for r0 in range(0, B, rows_per_chunk):
             u = uid[r0:r0 + rows_per_chunk]
             b = u.numel()
             scores = self.score_all_items(u).contiguous()
-            if filter_consumed and self.csr.nnz > 0:
-                _lib.check(lib.b200_mask_consumed(_lib.ptr(scores), scores.stride(0), _lib.ptr(u), b,
-                                                  self.n_items, n_rec, _lib.ptr(self.indptr_d),
-                                                  _lib.ptr(self.idx_d), self.csr.n_users, stream))
-            nbytes = ctypes.c_size_t(0)
-            _lib.check(lib.b200_topk_rows_workspace_bytes(b, self.n_items, n_rec, ctypes.byref(nbytes)))
-            ws = torch.empty(nbytes.value, dtype=torch.uint8, device=self.device)
-            _lib.check(lib.b200_topk_rows(_lib.ptr(scores), scores.stride(0), b, self.n_items, n_rec,
-                                          _lib.ptr(out_ids[r0:r0 + b]), _lib.ptr(out_sc[r0:r0 + b]),
-                                          _lib.ptr(ws), nbytes.value, stream))
+            masked_topk(self, scores, u, n_rec, filter_consumed, out_ids[r0:r0 + b], out_sc[r0:r0 + b])
+        return self._recs_to_host(out_ids, out_sc, return_scores)
+
+    def _recs_to_host(self, out_ids, out_sc, return_scores):
+        """Top-K ids (and scores, sigmoid for ranking) of ``recommend`` / ``recommend_dynamic`` on the host."""
         ids = out_ids.cpu().numpy()
         if return_scores:
             sc = out_sc.cpu().numpy()
@@ -487,22 +599,10 @@ class _FeatModelBase:
             if restore is not None:
                 self.seqs[u], self.lens[u] = restore
         del keep
-        lib, stream = _lib.lib, _lib.current_stream()
-        if filter_consumed and self.csr.nnz > 0:
-            _lib.check(lib.b200_mask_consumed(_lib.ptr(scores), scores.stride(0), _lib.ptr(uid), 1, N, n_rec,
-                                              _lib.ptr(self.indptr_d), _lib.ptr(self.idx_d), self.csr.n_users, stream))
         out_ids = torch.empty((1, n_rec), dtype=torch.int64, device=self.device)
         out_sc = torch.empty((1, n_rec), dtype=torch.float32, device=self.device)
-        nbytes = ctypes.c_size_t(0)
-        _lib.check(lib.b200_topk_rows_workspace_bytes(1, N, n_rec, ctypes.byref(nbytes)))
-        ws = torch.empty(nbytes.value, dtype=torch.uint8, device=self.device)
-        _lib.check(lib.b200_topk_rows(_lib.ptr(scores), scores.stride(0), 1, N, n_rec, _lib.ptr(out_ids),
-                                      _lib.ptr(out_sc), _lib.ptr(ws), nbytes.value, stream))
-        ids = out_ids.cpu().numpy()
-        if return_scores:
-            sc = out_sc.cpu().numpy()
-            return ids, (1.0 / (1.0 + np.exp(-sc)) if self.task == "ranking" else sc)
-        return ids
+        masked_topk(self, scores, uid, n_rec, filter_consumed, out_ids, out_sc)
+        return self._recs_to_host(out_ids, out_sc, return_scores)
 
     def assign_oov(self, sparse_oov=None):
         """``assign_tf_variables_oov`` (``bases/tf_base.py:310-353``) on the device tables, in place."""
@@ -532,17 +632,12 @@ class _FeatModelBase:
     # -- helpers -----------------------------------------------------------------------------------
     def _feat_forward(self, layout, users_d, items_d, R, grid_items, concat=None, pw=None, lin=None,
                       fm_out=None, head=None, row_offset=0, ssum=None, sqsum=None, lin_kernel=None, lin_bias=None):
-        head = head or {}
-        lk = lin_kernel if lin_kernel is not None else (self.lin_kernel if self.needs_linear else None)
-        lb = lin_bias if lin_bias is not None else (self.lin_bias if self.needs_linear else 0.0)
-        _lib.check(_lib.lib.b200_feat_forward(
-            ctypes.byref(layout), ctypes.byref(self.tables), _lib.ptr(users_d), _lib.ptr(items_d), R,
-            grid_items, row_offset, _lib.ptr(concat), concat.stride(0) if concat is not None else 0,
-            _lib.ptr(pw), pw.stride(0) if pw is not None else 0, _lib.ptr(lin), _lib.ptr(fm_out),
-            _lib.ptr(lk), float(lb),
-            _lib.ptr(head.get("bn_scale")), _lib.ptr(head.get("bn_shift")), _lib.ptr(head.get("pw_kernel")),
-            float(head.get("pw_bias", 0.0)), _lib.ptr(ssum), _lib.ptr(sqsum),
-            ssum.stride(0) if ssum is not None else 0, _lib.current_stream()))
+        if self.needs_linear:         # the model's linear term unless the caller passes its own
+            lin_kernel = self.lin_kernel if lin_kernel is None else lin_kernel
+            lin_bias = self.lin_bias if lin_bias is None else lin_bias
+        feat_forward(layout, self.tables, users_d, items_d, R, grid_items=grid_items, row_offset=row_offset,
+                     concat=concat, pw=pw, lin=lin, fm_out=fm_out, lin_kernel=lin_kernel,
+                     lin_bias=0.0 if lin_bias is None else lin_bias, head=head, ssum=ssum, sqsum=sqsum)
 
     def _mlp(self, x, layers):
         torch = self._torch
@@ -607,43 +702,15 @@ class DeepFM(_FeatModelBase):
         self.out_kernel = _dev(np.asarray(weights["out_kernel"]).reshape(-1), self.device, torch.float32)
         self.out_bias = float(np.asarray(weights["out_bias"]).reshape(-1)[0])
 
-    def _forward(self, layout, users_d, items_d, R, grid_items):
-        torch = self._torch
-        out = torch.empty(R, dtype=torch.float32, device=self.device)
-        step = self.max_grid_rows()
-        for r0 in range(0, R, step):                  # bound the [rows, F*K] deep input
-            r1 = min(R, r0 + step)
-            n = r1 - r0
-            concat = torch.empty((n, self.F * self.K), dtype=torch.float32, device=self.device)
-            pw = torch.empty((n, self.K), dtype=torch.float32, device=self.device)
-            lin = torch.empty(n, dtype=torch.float32, device=self.device)
-            if grid_items > 0:
-                self._feat_forward(layout, users_d, None, n, grid_items, concat=concat, pw=pw, lin=lin,
-                                   row_offset=r0)
-            else:
-                self._feat_forward(layout, users_d[r0:r1], items_d[r0:r1], n, 0, concat=concat, pw=pw, lin=lin)
-            deep = self._mlp(concat, self.mlp)
-            lin2 = lin.view(n, 1)
-            _lib.check(_lib.lib.b200_concat_dense(
-                _lib.ptr(lin2), 1, 1, _lib.ptr(pw), pw.stride(0), self.K, _lib.ptr(deep), deep.stride(0),
-                self.hidden_last, _lib.ptr(self.out_kernel), self.out_bias, n, _lib.ptr(out[r0:r1]),
-                _lib.current_stream()))
-        return out
-
-    def _hoistable(self):
-        n = len(self.mlp)
-        dims = [w.shape[0] for w, _, _ in self.mlp]
-        return self.K <= 64 and n in (2, 3) and dims[0] <= 256 and dims[1] <= 64 and (n == 2 or dims[2] <= 32)
-
-    def _first_layer_partial(self, which, concat, with_bias):
-        torch = self._torch
-        cache = self.__dict__.setdefault("_w1_side", {})
-        if which not in cache:
-            _, pos = self._side(which)
-            cols = torch.cat([torch.arange(g * self.K, (g + 1) * self.K, device=self.device) for g in pos])
-            cache[which] = self.mlp[0][0][:, cols].contiguous()          # Wt [H1, F_side*K], BN already folded
-        Wt = cache[which]
-        return linear(concat, Wt, self.mlp[0][1] if with_bias else None, False)
+    def _chunk_logits(self, layout, users_d, items_d, n, grid_items, row_offset, x, out):
+        pw = self._torch.empty((n, self.K), dtype=self._torch.float32, device=self.device)
+        lin = self._torch.empty(n, dtype=self._torch.float32, device=self.device)
+        self._feat_forward(layout, users_d, items_d, n, grid_items, concat=x, pw=pw, lin=lin, row_offset=row_offset)
+        deep = self._mlp(x, self.mlp)
+        lin2 = lin.view(n, 1)
+        _lib.check(_lib.lib.b200_concat_dense(
+            _lib.ptr(lin2), 1, 1, _lib.ptr(pw), pw.stride(0), self.K, _lib.ptr(deep), deep.stride(0),
+            self.hidden_last, _lib.ptr(self.out_kernel), self.out_bias, n, _lib.ptr(out), _lib.current_stream()))
 
     def score_all_items(self, user_ids_d):
         """Hoisted: first-layer partial products per side, only the small layers per (user, item)."""
@@ -657,23 +724,13 @@ class DeepFM(_FeatModelBase):
         Si, Qi, li, Pi = self._item_side
         Su, Qu, lu, cu = self._side_partials("user", user_ids_d, True)
         Pu = self._first_layer_partial("user", cu, True)
-        W2t, b2, _ = self.mlp[1]
-        three = len(self.mlp) == 3
-        if "_tail" not in self.__dict__:
-            self._tail = (W2t.t().contiguous(), self.mlp[2][0].t().contiguous() if three else None)
-        W2, W3 = self._tail
-        b = int(user_ids_d.numel())
-        scores = torch.empty((b, self.n_items), dtype=torch.float32, device=self.device)
-        _lib.check(_lib.lib.b200_deepfm_pair_scores(
-            _lib.ptr(Su), _lib.ptr(Qu), _lib.ptr(lu), _lib.ptr(Pu), b, _lib.ptr(Si), _lib.ptr(Qi), _lib.ptr(li),
-            _lib.ptr(Pi), self.n_items, self.K, Pu.shape[1], W2.shape[1], W3.shape[1] if three else 0,
-            self.lin_bias, _lib.ptr(W2), _lib.ptr(b2), _lib.ptr(W3), _lib.ptr(self.mlp[2][1]) if three else None,
-            _lib.ptr(self.out_kernel), self.out_bias, _lib.ptr(scores), scores.stride(0), _lib.current_stream()))
+        scores = torch.empty((int(user_ids_d.numel()), self.n_items), dtype=torch.float32, device=self.device)
+        self._pair_scores(Pu, Pi, scores, fm=(Su, Qu, lu, Si, Qi, li))
         return scores
 
     def max_grid_rows(self):
         # deep input bytes per row = F*K*4; keep a chunk under ~1 GiB
-        return max(1, (1 << 30) // (self.F * self.K * 4))
+        return max(1, (1 << 30) // (self._row_width() * 4))
 
 
 AUTOINT_MAX_K = 64          # the shapes b200_autoint_rows / _grid accept (include/b200reco.h)
@@ -738,37 +795,18 @@ class AutoInt(_FeatModelBase):
         return (self.F, self.K, self.num_heads, len(self.head_dims), _lib.ptr(self._hd_host), _lib.ptr(self.w_layers),
                 _lib.ptr(self.out_kernel), self.out_bias, int(self.use_residual))
 
-    def _forward(self, layout, users_d, items_d, R, grid_items):
-        torch = self._torch
-        out = torch.empty(R, dtype=torch.float32, device=self.device)
-        step = self.max_grid_rows()
-        for r0 in range(0, R, step):                  # bound the materialised [rows, F*K] concat
-            r1 = min(R, r0 + step)
-            n = r1 - r0
-            concat = torch.empty((n, self.F * self.K), dtype=torch.float32, device=self.device)
-            if grid_items > 0:
-                self._feat_forward(layout, users_d, None, n, grid_items, concat=concat, row_offset=r0)
-            else:
-                self._feat_forward(layout, users_d[r0:r1], items_d[r0:r1], n, 0, concat=concat)
-            _lib.check(_lib.lib.b200_autoint_rows(_lib.ptr(concat), concat.stride(0), n, *self._head(),
-                                                  _lib.ptr(out[r0:r1]), _lib.current_stream()))
-        return out
-
-    def _side_block(self, which, ids_d):
-        """[n, F_side*K] field embeddings of ONE side, in the side's field order of :meth:`_side`."""
-        L, pos = self._side(which)
-        n = int(ids_d.numel())
-        x = self._torch.empty((n, len(pos) * self.K), dtype=self._torch.float32, device=self.device)
-        self._feat_forward(L, ids_d, ids_d, n, 0, concat=x)
-        return x
+    def _chunk_logits(self, layout, users_d, items_d, n, grid_items, row_offset, x, out):
+        self._feat_forward(layout, users_d, items_d, n, grid_items, concat=x, row_offset=row_offset)
+        _lib.check(_lib.lib.b200_autoint_rows(_lib.ptr(x), x.stride(0), n, *self._head(), _lib.ptr(out),
+                                              _lib.current_stream()))
 
     def _field_map(self):
         """int32 [F]: global field f comes from user-side slot m (m >= 0) or item-side slot -1 - m."""
         if "_fmap" not in self.__dict__:
             m = np.zeros(self.F, dtype=np.int32)
-            for j, f in enumerate(self._side("user")[1]):
+            for j, f in enumerate(self.spec.side("user")[1]):
                 m[f] = j
-            for j, f in enumerate(self._side("item")[1]):
+            for j, f in enumerate(self.spec.side("item")[1]):
                 m[f] = -1 - j
             self._fmap = _dev(m, self.device, self._torch.int32)
         return self._fmap
@@ -778,9 +816,9 @@ class AutoInt(_FeatModelBase):
         ``assign_oov``), the user-side block once per call; the [b*N, F*K] concat is never built."""
         torch = self._torch
         if "_item_side" not in self.__dict__:
-            self._item_side = self._side_block("item", torch.arange(self.n_items, device=self.device))
+            self._item_side = self._side_concat("item", torch.arange(self.n_items, device=self.device))
         Xi = self._item_side
-        Xu = self._side_block("user", user_ids_d)
+        Xu = self._side_concat("user", user_ids_d)
         b, N = int(user_ids_d.numel()), self.n_items
         scores = torch.empty((b, N), dtype=torch.float32, device=self.device)
         _lib.check(_lib.lib.b200_autoint_grid(_lib.ptr(Xu), Xu.stride(0), b, _lib.ptr(Xi), Xi.stride(0), N,
@@ -789,7 +827,7 @@ class AutoInt(_FeatModelBase):
         return scores
 
     def max_grid_rows(self):
-        return max(1, (1 << 30) // (self.F * self.K * 4))
+        return max(1, (1 << 30) // (self._row_width() * 4))
 
 
 def wide_deep_weights(user_wide, item_wide, sparse_wide, dense_wide, wide_kernel, wide_bias, user_deep, item_deep,
@@ -886,32 +924,22 @@ class _SeqModelBase(_FeatModelBase):
         self.out_bias = float(np.asarray(weights["out_bias"]).reshape(-1)[0])
         self.extra = 0          # width of the sequence block appended to the concatenated row
 
-    def _seq_block(self, layout, users_d, items_d, n, grid_items, row_offset, out_view):
+    def _seq_block(self, users_d, items_d, n, grid_items, row_offset, out_view):
         raise NotImplementedError
 
-    def _forward(self, layout, users_d, items_d, R, grid_items):
-        torch = self._torch
-        out = torch.empty(R, dtype=torch.float32, device=self.device)
-        width = self.F * self.K + self.extra
-        step = max(1, (1 << 30) // (width * 4))
-        for r0 in range(0, R, step):
-            r1 = min(R, r0 + step)
-            n = r1 - r0
-            x = torch.empty((n, width), dtype=torch.float32, device=self.device)
-            if grid_items > 0:
-                self._feat_forward(layout, users_d, None, n, grid_items, concat=x, row_offset=r0)
-                self._seq_block(users_d, None, n, grid_items, r0, x[:, self.F * self.K:])
-            else:
-                self._feat_forward(layout, users_d[r0:r1], items_d[r0:r1], n, 0, concat=x)
-                self._seq_block(users_d[r0:r1], items_d[r0:r1], n, 0, 0, x[:, self.F * self.K:])
-            h = self._mlp(x, self.mlp)
-            _lib.check(_lib.lib.b200_concat_dense(
-                _lib.ptr(h), h.stride(0), h.shape[1], None, 0, 0, None, 0, 0, _lib.ptr(self.out_kernel),
-                self.out_bias, n, _lib.ptr(out[r0:r1]), _lib.current_stream()))
-        return out
+    def _row_width(self):
+        return self.F * self.K + self.extra
+
+    def _chunk_logits(self, layout, users_d, items_d, n, grid_items, row_offset, x, out):
+        self._feat_forward(layout, users_d, items_d, n, grid_items, concat=x, row_offset=row_offset)
+        self._seq_block(users_d, items_d, n, grid_items, row_offset, x[:, self.F * self.K:])
+        h = self._mlp(x, self.mlp)
+        _lib.check(_lib.lib.b200_concat_dense(
+            _lib.ptr(h), h.stride(0), h.shape[1], None, 0, 0, None, 0, 0, _lib.ptr(self.out_kernel),
+            self.out_bias, n, _lib.ptr(out), _lib.current_stream()))
 
     def max_grid_rows(self):
-        return max(1, (1 << 30) // ((self.F * self.K + self.extra) * 4))
+        return max(1, (1 << 30) // (self._row_width() * 4))
 
 
 class YouTubeRanking(_SeqModelBase):
@@ -927,29 +955,6 @@ class YouTubeRanking(_SeqModelBase):
         self.mlp = self._upload_mlp(permute_mlp_input(weights["mlp"], perm))
 
     # ---- hoisted all-items scoring (SURVEY.md §7.2-4): everything user-only or item-only once ----
-    def _hoistable(self):
-        dims = [w.shape[0] for w, _, _ in self.mlp]
-        n = len(dims)
-        return self.K <= 64 and n in (2, 3) and dims[0] <= 256 and dims[1] <= 64 and (n == 2 or dims[2] <= 32)
-
-    def _side_input(self, which, ids_d):
-        """Concatenated field embeddings of ONE side for the given ids (+ the pooled history for users)
-        and the matching columns of the first MLP layer."""
-        torch = self._torch
-        L, pos = self._side(which)
-        n = int(ids_d.numel())
-        width = len(pos) * self.K + (self.K if which == "user" else 0)
-        x = torch.empty((n, width), dtype=torch.float32, device=self.device)
-        self._feat_forward(L, ids_d, ids_d, n, 0, concat=x)
-        if which == "user":
-            self._seq_block(ids_d, ids_d, n, 0, 0, x[:, len(pos) * self.K:])
-        cache = self.__dict__.setdefault("_w1_side", {})
-        if which not in cache:
-            groups = list(pos) + ([self.F] if which == "user" else [])     # pooled block sits after the F fields
-            cols = torch.cat([torch.arange(g * self.K, (g + 1) * self.K, device=self.device) for g in groups])
-            cache[which] = self.mlp[0][0][:, cols].contiguous()
-        return x, cache[which]
-
     def score_all_items(self, user_ids_d):
         """youtube_ranking.py:199-218 over the implicit (user, item) grid: the first Dense layer splits
         into a user part (id, user features, pooled history) and an item part, computed once per user /
@@ -959,27 +964,13 @@ class YouTubeRanking(_SeqModelBase):
         if not self._hoistable():
             return super().score_all_items(user_ids_d)
         if "_item_part" not in self.__dict__:
-            xi, Wi = self._side_input("item", torch.arange(self.n_items, device=self.device))
-            self._item_part = linear(xi, Wi, None, False)
-            three = len(self.mlp) == 3
-            self._tail = (self.mlp[1][0].t().contiguous(), self.mlp[2][0].t().contiguous() if three else None)
-            self._w_out = torch.cat([torch.zeros(1 + self.K, dtype=torch.float32, device=self.device),
-                                     self.out_kernel]).contiguous()
-            self._zeros_i = torch.zeros((self.n_items, self.K + 1), dtype=torch.float32, device=self.device)
-        xu, Wu = self._side_input("user", user_ids_d)
-        Pu = linear(xu, Wu, self.mlp[0][1], False)
-        Pi = self._item_part
-        W2, W3 = self._tail
-        three = W3 is not None
-        b = int(user_ids_d.numel())
-        zu = torch.zeros((b, self.K + 1), dtype=torch.float32, device=self.device)
-        zi = self._zeros_i
-        scores = torch.empty((b, self.n_items), dtype=torch.float32, device=self.device)
-        _lib.check(_lib.lib.b200_deepfm_pair_scores(
-            _lib.ptr(zu), _lib.ptr(zu), _lib.ptr(zu), _lib.ptr(Pu), b, _lib.ptr(zi), _lib.ptr(zi), _lib.ptr(zi),
-            _lib.ptr(Pi), self.n_items, self.K, Pu.shape[1], W2.shape[1], W3.shape[1] if three else 0, 0.0,
-            _lib.ptr(W2), _lib.ptr(self.mlp[1][1]), _lib.ptr(W3), _lib.ptr(self.mlp[2][1]) if three else None,
-            _lib.ptr(self._w_out), self.out_bias, _lib.ptr(scores), scores.stride(0), _lib.current_stream()))
+            xi = self._side_concat("item", torch.arange(self.n_items, device=self.device))
+            self._item_part = self._first_layer_partial("item", xi, False)
+        xu = self._side_concat("user", user_ids_d, extra=self.K)
+        self._seq_block(user_ids_d, user_ids_d, xu.shape[0], 0, 0, xu[:, xu.shape[1] - self.K:])
+        Pu = self._first_layer_partial("user", xu, True, [self.F])     # the pooled block sits after the F fields
+        scores = torch.empty((int(user_ids_d.numel()), self.n_items), dtype=torch.float32, device=self.device)
+        self._pair_scores(Pu, self._item_part, scores)
         return scores
 
     def _seq_block(self, users_d, items_d, n, grid_items, row_offset, out_view):
@@ -1027,22 +1018,7 @@ class DIN(_SeqModelBase):
 
     # ---- hoisted all-items scoring (SURVEY.md 8d "a7 DIN all-items") ---------------------------------
     def _hoistable(self):
-        dims = [w.shape[0] for w, _, _ in self.mlp]
-        n = len(dims)
-        return (self.K <= 64 and n in (2, 3) and dims[0] <= 256 and dims[1] <= 64 and (n == 2 or dims[2] <= 32)
-                and self.Kp % 4 == 0 and not self.use_tf_attention)
-
-    def _side_concat(self, which, ids_d):
-        torch = self._torch
-        L, pos = self._side(which)
-        n = int(ids_d.numel())
-        x = torch.empty((n, len(pos) * self.K), dtype=torch.float32, device=self.device)
-        self._feat_forward(L, ids_d, ids_d, n, 0, concat=x)
-        cache = self.__dict__.setdefault("_w1_side", {})
-        if which not in cache:
-            cols = torch.cat([torch.arange(g * self.K, (g + 1) * self.K, device=self.device) for g in pos])
-            cache[which] = self.mlp[0][0][:, cols].contiguous()
-        return x, cache[which]
+        return super()._hoistable() and self.Kp % 4 == 0 and not self.use_tf_attention
 
     def score_all_items(self, user_ids_d):
         """din.py:165-250 over (this user) x (every item).  Per user: the attention's Dense(16) becomes
@@ -1054,21 +1030,13 @@ class DIN(_SeqModelBase):
             return super().score_all_items(user_ids_d)
         N, Kp, FK = self.n_items, self.Kp, self.F * self.K
         if "_item_part" not in self.__dict__:
-            xi, Wi = self._side_concat("item", torch.arange(N, device=self.device))
-            self._item_part = linear(xi, Wi, None, False)
+            xi = self._side_concat("item", torch.arange(N, device=self.device))
+            self._item_part = self._first_layer_partial("item", xi, False)
             self._w_att = self.mlp[0][0][:, FK:FK + Kp].contiguous()           # [H1, K']
-            three = len(self.mlp) == 3
-            self._tail = (self.mlp[1][0].t().contiguous(), self.mlp[2][0].t().contiguous() if three else None)
-            self._w_out = torch.cat([torch.zeros(1 + self.K, dtype=torch.float32, device=self.device),
-                                     self.out_kernel]).contiguous()
-            self._zeros_i = torch.zeros((N, self.K + 1), dtype=torch.float32, device=self.device)
-        W2, W3 = self._tail
-        three = W3 is not None
         b = int(user_ids_d.numel())
-        xu, Wu = self._side_concat("user", user_ids_d)
-        Pu_all = linear(xu, Wu, self.mlp[0][1], False)                           # [b, H1] incl. bias
+        xu = self._side_concat("user", user_ids_d)
+        Pu_all = self._first_layer_partial("user", xu, True)                     # [b, H1] incl. bias
         scores = torch.empty((b, N), dtype=torch.float32, device=self.device)
-        zu = torch.zeros((1, self.K + 1), dtype=torch.float32, device=self.device)
         lens_h = self.lens[user_ids_d].clamp(0, self.T).cpu().numpy()            # one small D2H per call
         Gn = self.G[:N]
         att = torch.empty((N, Kp), dtype=torch.float32, device=self.device)
@@ -1102,13 +1070,7 @@ class DIN(_SeqModelBase):
                     _lib.ptr(Z), Z.stride(0) if Z is not None else 0, N, _lib.ptr(self.G), self.G.stride(0), Kp,
                     _lib.ptr(seq), ln, _lib.ptr(self.att["k2"]), self.att["b2"], _lib.ptr(att), att.stride(0), st))
             Pi = self._item_part + linear(att, self._w_att, None, False)         # [N, H1]
-            Pu = Pu_all[r:r + 1]
-            _lib.check(lib.b200_deepfm_pair_scores(
-                _lib.ptr(zu), _lib.ptr(zu), _lib.ptr(zu), _lib.ptr(Pu), 1, _lib.ptr(self._zeros_i),
-                _lib.ptr(self._zeros_i), _lib.ptr(self._zeros_i), _lib.ptr(Pi), N, self.K, Pu.shape[1], W2.shape[1],
-                W3.shape[1] if three else 0, 0.0, _lib.ptr(W2), _lib.ptr(self.mlp[1][1]), _lib.ptr(W3),
-                _lib.ptr(self.mlp[2][1]) if three else None, _lib.ptr(self._w_out), self.out_bias,
-                _lib.ptr(scores[r]), scores.stride(0), st))
+            self._pair_scores(Pu_all[r:r + 1], Pi, scores[r:r + 1])
         return scores
 
     def _seq_block(self, users_d, items_d, n, grid_items, row_offset, out_view):
@@ -1138,37 +1100,17 @@ class TwoTower:
         f32 = torch.float32
         self.t = {k: _dev(weights.get(k), self.device, f32) for k in
                   ("user_embeds", "item_embeds", "sparse_embeds", "dense_embeds")}
-        T = FeatTablesStruct()
-        for k, v in self.t.items():
-            setattr(T, k, v.data_ptr() if v is not None else None)
-        self.tables = T
-        self.layouts, self.mlps, self.widths = {}, {}, {}
-        for which, mask in (("user", 1), ("item", 2)):
-            L = FeatLayoutStruct.from_buffer_copy(self.base.layout)
-            L.id_mask = mask
-            scols = self.base.user_sparse_cols if which == "user" else self.base.item_sparse_cols
-            dcols = self.base.user_dense_cols if which == "user" else self.base.item_dense_cols
-            L.n_sparse, L.n_dense = len(scols), len(dcols)
-            for f in range(len(scols)):
-                L.sparse_side[f], L.sparse_col[f] = (0 if which == "user" else 1), f
-            for f in range(len(dcols)):
-                L.dense_side[f], L.dense_col[f] = (0 if which == "user" else 1), f
-                L.dense_embed_row[f] = dcols[f]
-            self.layouts[which] = L
-            self.widths[which] = (1 + len(scols) + len(dcols)) * K
-            self.mlps[which] = [(_dev(Wt, self.device, f32), _dev(b, self.device, f32), relu)
-                                for Wt, b, relu in fold_mlp(weights[f"{which}_tower"])]
+        self.tables = tables_struct(self.t)
+        self.mlps = {which: [(_dev(Wt, self.device, f32), _dev(b, self.device, f32), relu)
+                             for Wt, b, relu in fold_mlp(weights[f"{which}_tower"])] for which in ("user", "item")}
 
     def tower(self, which, ids):
         torch = self._torch
         ids_d = torch.as_tensor(np.asarray(ids, dtype=np.int64)).to(self.device)
         n = ids_d.numel()
-        x = torch.empty((n, self.widths[which]), dtype=torch.float32, device=self.device)
-        L = self.layouts[which]
-        _lib.check(_lib.lib.b200_feat_forward(
-            ctypes.byref(L), ctypes.byref(self.tables), _lib.ptr(ids_d), _lib.ptr(ids_d), n, 0, 0,
-            _lib.ptr(x), x.stride(0), None, 0, None, None, None, 0.0, None, None, None, 0.0,
-            None, None, 0, _lib.current_stream()))
+        L, pos = self.base.side(which)
+        x = torch.empty((n, len(pos) * self.K), dtype=torch.float32, device=self.device)
+        feat_forward(L, self.tables, ids_d, ids_d, n, concat=x)
         for Wt, b, relu in self.mlps[which]:
             x = linear(x, Wt, b, relu)
         if self.norm_embed:
@@ -1211,20 +1153,7 @@ class YouTubeRetrieval:
         self.item_embeds = _dev(weights["item_embeds"], self.device, f32)            # [n_items, H]
         self.item_biases = _dev(np.asarray(weights["item_biases"]).reshape(-1), self.device, f32)
         self.t = {k: _dev(weights.get(k), self.device, f32) for k in ("sparse_embeds", "dense_embeds")}
-        T = FeatTablesStruct()
-        for k, v in self.t.items():
-            setattr(T, k, v.data_ptr() if v is not None else None)
-        self.tables = T
-        L = FeatLayoutStruct.from_buffer_copy(self.base.layout)
-        L.id_mask = 0                                      # no id-embedding field: the pooled sequence takes its place
-        scols, dcols = self.base.user_sparse_cols, self.base.user_dense_cols
-        L.n_sparse, L.n_dense = len(scols), len(dcols)
-        for f in range(len(scols)):
-            L.sparse_side[f], L.sparse_col[f] = 0, f
-        for f in range(len(dcols)):
-            L.dense_side[f], L.dense_col[f] = 0, f
-            L.dense_embed_row[f] = dcols[f]
-        self.layout, self.n_feat = L, len(scols) + len(dcols)
+        self.tables = tables_struct(self.t)
         self.seqs = _dev(recent_seqs, self.device, torch.int32)
         self.lens = _dev(recent_seq_lens, self.device, torch.int32)
         self.mlp = [(_dev(Wt, self.device, f32), _dev(b, self.device, f32), relu) for Wt, b, relu in fold_mlp(weights["mlp"])]
@@ -1234,18 +1163,15 @@ class YouTubeRetrieval:
         torch = self._torch
         ids_d = torch.as_tensor(np.asarray(ids, dtype=np.int64)).to(self.device)
         n, K = int(ids_d.numel()), self.K
-        x = torch.empty((n, (1 + self.n_feat) * K), dtype=torch.float32, device=self.device)
+        L, pos = self.base.side("user", with_id=False)      # no id-embedding field: the pooled sequence takes its place
+        x = torch.empty((n, (1 + len(pos)) * K), dtype=torch.float32, device=self.device)
         pooled = x[:, :K]
         _lib.check(_lib.lib.b200_seq_pool(
             _lib.ptr(self.seq_embeds), self.seq_embeds.stride(0), K, self.n_items, _lib.ptr(self.seqs),
             self.seqs.stride(0), _lib.ptr(self.lens), self.seqs.shape[1], _lib.ptr(ids_d), n, 0, 0, _lib.ptr(pooled),
             x.stride(0), _lib.current_stream()))
-        if self.n_feat:
-            feat = x[:, K:]
-            _lib.check(_lib.lib.b200_feat_forward(
-                ctypes.byref(self.layout), ctypes.byref(self.tables), _lib.ptr(ids_d), _lib.ptr(ids_d), n, 0, 0,
-                _lib.ptr(feat), x.stride(0), None, 0, None, None, None, 0.0, None, None, None, 0.0,
-                None, None, 0, _lib.current_stream()))
+        if pos:
+            feat_forward(L, self.tables, ids_d, ids_d, n, concat=x[:, K:])
         for Wt, b, relu in self.mlp:
             x = linear(x, Wt, b, relu)
         if self.norm_embed:

@@ -15,12 +15,10 @@ variable moves, i.e. a dense Adam step with a zero-filled gradient.  torch: memo
 """
 from __future__ import annotations
 
-import ctypes
-
 import numpy as np
 
 from . import _lib
-from .feat_models import FeatSpec, FeatTablesStruct, _dev
+from .feat_models import FeatSpec, _dev, feat_backward, feat_forward, linear, permute_mlp_input, tables_struct
 
 BN_EPS = 1e-3          # tf.layers.batch_normalization defaults
 BN_MOMENTUM = 0.99
@@ -44,56 +42,109 @@ def set_regularisation(tr, reg=None, lr_decay=False, decay_steps=0, decay_rate=0
     return tr
 
 
-def _adam_update(tr):
-    """TF-Adam over every variable of trainer ``tr`` with the step counter and the bias-corrected step size ON THE
-    DEVICE (``b200_adam_begin_step`` / ``b200_adam_dense_dev``): the same launches work eagerly and inside a
-    captured CUDA graph."""
-    torch = tr._torch
-    if getattr(tr, "_step_dev", None) is None:
-        tr._step_dev = torch.full((1,), int(tr.t), dtype=torch.int64, device=tr.device)
-        tr._lr_t = torch.zeros(1, dtype=torch.float32, device=tr.device)
-    lib, st = _lib.lib, _lib.current_stream()
-    reg = float(getattr(tr, "reg", 0.0) or 0.0)
-    if reg > 0.0:                 # L2 on the embedding / linear tables only (the variables built with regularizer=reg)
-        for k in _REG_VARS:
-            if k in tr.params:
-                _lib.check(lib.b200_axpy(_lib.ptr(tr.grads[k]), _lib.ptr(tr.params[k]), 2.0 * reg, tr.params[k].numel(), st))
-    decay_steps = int(getattr(tr, "decay_steps", 0) or 0)
-    _lib.check(lib.b200_adam_begin_step(_lib.ptr(tr._step_dev), tr.lr, BETA1, BETA2,
-                                        float(getattr(tr, "decay_rate", 0.96)), decay_steps, _lib.ptr(tr._lr_t), st))
-    for k, v in tr.params.items():
-        _lib.check(lib.b200_adam_dense_dev(_lib.ptr(v), _lib.ptr(tr.m[k]), _lib.ptr(tr.v[k]), _lib.ptr(tr.grads[k]),
-                                           v.numel(), _lib.ptr(tr._lr_t), BETA1, BETA2, tr.epsilon, st))
-    tr.t += 1
-
-
 def _weight_grad(dy, x):
     """dWt [dout, din] = dY^T X on the library's dense kernel.  The kernel tiles the OUTPUT rows over the SMs, so
     the product is taken in the orientation with more output rows (din > dout: (X^T dY)^T) — the reduction runs
     over the batch either way."""
-    from .feat_models import linear
-
     dyt, xt = dy.t().contiguous(), x.t().contiguous()
     if xt.shape[0] > dyt.shape[0]:
         return linear(xt, dyt, None, False, cache_split=False).t()
     return linear(dyt, xt, None, False, cache_split=False)
 
 
-class _GraphedStep:
-    """``step_graph(*device tensors)``: the trainer's ``step`` captured ONCE per input shape into a CUDA graph and
-    replayed — a step is ~100 small launches (gather, BN, dense layers, reductions, one Adam launch per variable),
-    launch-bound when issued one by one from Python.  Inputs are copied into static buffers; the returned loss
-    is a static device scalar, valid until the next replay.  Semantics are those of ``step``."""
+class _Trainer:
+    """What every trainer of this module shares: the feature spec, device and embed size; the variables (cloned
+    device copies of ``weights``), their gradient buffers and Adam slots; the tables struct the gather reads; the
+    loss workspace; TF-Adam and ``step_graph``.  A subclass adds its own variables in ``_init_params``.
+
+    ``linear_tables``: the model's linear (wide) tables are variables too (FM, DeepFM)."""
+
+    linear_tables = False
+
+    def __init__(self, spec, weights, use_bn, lr, epsilon, device):
+        import torch
+
+        self._torch = torch
+        K = int(weights["user_embeds"].shape[1])
+        self.spec = spec if isinstance(spec, FeatSpec) else FeatSpec(spec, K, device)
+        self.device, self.K = self.spec.device, K
+        self.F = 2 + self.spec.n_sparse + self.spec.n_dense
+        self.n_items = self.spec.n_items
+        self.use_bn, self.lr, self.epsilon, self.t = bool(use_bn), float(lr), float(epsilon), 0
+        self.moving = {}
+        names = _TABLES if self.linear_tables else _TABLES[:4]
+        self.params = {k: self._var(weights[k]) for k in names if weights.get(k) is not None}
+        self._init_params(weights)
+        p = self.params
+        self.grads = {k: torch.zeros_like(v) for k, v in p.items()}
+        self.m = {k: torch.zeros_like(v) for k, v in p.items()}
+        self.v = {k: torch.zeros_like(v) for k, v in p.items()}
+        self.tables = tables_struct(p)
+        self._lws = torch.empty(int(_lib.lib.b200_loss_workspace_bytes()), dtype=torch.uint8, device=self.device)
+
+    def _init_params(self, weights):
+        raise NotImplementedError
+
+    def _var(self, x, shape=None):
+        """Trainable device copy of ``x`` (reshaped to ``shape`` first when given)."""
+        if shape is not None:
+            x = np.asarray(x).reshape(shape)
+        return _dev(x, self.device, self._torch.float32).clone()
+
+    def _export_tables(self):
+        return {k: self.params[k].cpu().numpy() for k in _TABLES if k in self.params}
+
+    def _loss(self, logit, labels_d):
+        """Mean sigmoid cross entropy: (device loss, d loss / d logit)."""
+        torch = self._torch
+        R = int(logit.numel())
+        loss = torch.empty((), dtype=torch.float32, device=self.device)
+        dlogit = torch.empty(R, dtype=torch.float32, device=self.device)
+        _lib.check(_lib.lib.b200_pointwise_loss(_lib.ptr(logit), _lib.ptr(labels_d), R, 0, 0.25, 2.0, _lib.ptr(loss),
+                                                _lib.ptr(dlogit), _lib.ptr(self._lws), self._lws.numel(),
+                                                _lib.current_stream()))
+        return loss, dlogit
+
+    def _device_counters(self):
+        """The Adam step counter and step size live on the device (allocated outside any graph capture)."""
+        if getattr(self, "_step_dev", None) is None:
+            torch = self._torch
+            self._step_dev = torch.full((1,), int(self.t), dtype=torch.int64, device=self.device)
+            self._lr_t = torch.zeros(1, dtype=torch.float32, device=self.device)
+
+    def _adam_update(self):
+        """TF-Adam over every variable with the step counter and the bias-corrected step size ON THE DEVICE
+        (``b200_adam_begin_step`` / ``b200_adam_dense_dev``): the same launches work eagerly and inside a captured
+        CUDA graph."""
+        self._device_counters()
+        lib, st = _lib.lib, _lib.current_stream()
+        reg = float(getattr(self, "reg", 0.0) or 0.0)
+        if reg > 0.0:             # L2 on the embedding / linear tables only (the variables built with regularizer=reg)
+            for k in _REG_VARS:
+                if k in self.params:
+                    _lib.check(lib.b200_axpy(_lib.ptr(self.grads[k]), _lib.ptr(self.params[k]), 2.0 * reg,
+                                             self.params[k].numel(), st))
+        decay_steps = int(getattr(self, "decay_steps", 0) or 0)
+        _lib.check(lib.b200_adam_begin_step(_lib.ptr(self._step_dev), self.lr, BETA1, BETA2,
+                                            float(getattr(self, "decay_rate", 0.96)), decay_steps, _lib.ptr(self._lr_t),
+                                            st))
+        for k, v in self.params.items():
+            _lib.check(lib.b200_adam_dense_dev(_lib.ptr(v), _lib.ptr(self.m[k]), _lib.ptr(self.v[k]),
+                                               _lib.ptr(self.grads[k]), v.numel(), _lib.ptr(self._lr_t), BETA1, BETA2,
+                                               self.epsilon, st))
+        self.t += 1
 
     def step_graph(self, *inputs):
+        """``step`` captured ONCE per input shape into a CUDA graph and replayed — a step is ~100 small launches
+        (gather, BN, dense layers, reductions, one Adam launch per variable), launch-bound when issued one by one
+        from Python.  Inputs are copied into static buffers; the returned loss is a static device scalar, valid
+        until the next replay.  Semantics are those of ``step``."""
         torch = self._torch
         graphs = self.__dict__.setdefault("_graphs", {})
         key = tuple(None if x is None else (tuple(x.shape), x.dtype) for x in inputs)
         ent = graphs.get(key)
         if ent is None:
-            if getattr(self, "_step_dev", None) is None:          # allocate the device counters outside the capture
-                self._step_dev = torch.full((1,), int(self.t), dtype=torch.int64, device=self.device)
-                self._lr_t = torch.zeros(1, dtype=torch.float32, device=self.device)
+            self._device_counters()
             static = [None if x is None else x.detach().clone() for x in inputs]
             graph = torch.cuda.CUDAGraph()
             launches0 = int(_lib.lib.b200_launch_count())
@@ -110,41 +161,30 @@ class _GraphedStep:
         return ent[2]
 
 
-class FMTrainer(_GraphedStep):
+class FMTrainer(_Trainer):
     """Owns the FM variables of ``fm.py`` (scope "embedding" tables + the two Dense(1) heads + BN),
     their Adam slots and gradient buffers.  ``weights`` uses the inference layout of
     ``feat_models.FM`` / ``oracle.tf_models.make_fm_weights``."""
 
-    def __init__(self, spec, weights, use_bn=True, lr=1e-3, epsilon=1e-5, device=None):
-        import torch
+    linear_tables = True
 
-        self._torch = torch
-        K = int(weights["user_embeds"].shape[1])
-        self.spec = spec if isinstance(spec, FeatSpec) else FeatSpec(spec, K, device)
-        self.device, self.K = self.spec.device, K
-        self.use_bn, self.lr, self.epsilon, self.t = bool(use_bn), float(lr), float(epsilon), 0
-        f32 = torch.float32
-        p = {k: _dev(weights[k], self.device, f32).clone() for k in _TABLES if weights.get(k) is not None}
-        p["lin_kernel"] = _dev(np.asarray(weights["lin_kernel"]).reshape(-1), self.device, f32).clone()
-        p["lin_bias"] = _dev(np.asarray(weights["lin_bias"]).reshape(1), self.device, f32).clone()
-        p["pw_kernel"] = _dev(np.asarray(weights["pw_kernel"]).reshape(-1), self.device, f32).clone()
-        p["pw_bias"] = _dev(np.asarray(weights["pw_bias"]).reshape(1), self.device, f32).clone()
+    def __init__(self, spec, weights, use_bn=True, lr=1e-3, epsilon=1e-5, device=None):
+        super().__init__(spec, weights, use_bn, lr, epsilon, device)
+        self._buf = {}
+
+    def _init_params(self, weights):
+        p, K = self.params, self.K
+        p["lin_kernel"] = self._var(weights["lin_kernel"], -1)
+        p["lin_bias"] = self._var(weights["lin_bias"], 1)
+        p["pw_kernel"] = self._var(weights["pw_kernel"], -1)
+        p["pw_bias"] = self._var(weights["pw_bias"], 1)
         if self.use_bn:
             bn = weights.get("fm_bn")
             one, zero = np.ones(K, np.float32), np.zeros(K, np.float32)
-            p["bn_gamma"] = _dev(bn["gamma"] if bn else one, self.device, f32).clone()
-            p["bn_beta"] = _dev(bn["beta"] if bn else zero, self.device, f32).clone()
-            self.moving_mean = _dev(bn["mean"] if bn else zero, self.device, f32).clone()
-            self.moving_var = _dev(bn["var"] if bn else one, self.device, f32).clone()
-        self.params = p
-        self.grads = {k: torch.zeros_like(v) for k, v in p.items()}
-        self.m = {k: torch.zeros_like(v) for k, v in p.items()}
-        self.v = {k: torch.zeros_like(v) for k, v in p.items()}
-        T = FeatTablesStruct()
-        for k in _TABLES:
-            setattr(T, k, p[k].data_ptr() if k in p else None)
-        self.tables = T
-        self._buf = {}
+            p["bn_gamma"] = self._var(bn["gamma"] if bn else one)
+            p["bn_beta"] = self._var(bn["beta"] if bn else zero)
+            self.moving_mean = self._var(bn["mean"] if bn else zero)
+            self.moving_var = self._var(bn["var"] if bn else one)
 
     def _buffers(self, R):
         torch = self._torch
@@ -158,8 +198,7 @@ class FMTrainer(_GraphedStep):
                 z=torch.empty(R, dtype=f32, device=dev), logit=torch.empty(R, dtype=f32, device=dev),
                 dlogit=torch.empty(R, dtype=f32, device=dev), loss=torch.empty((), dtype=f32, device=dev),
                 mean=torch.empty(K, dtype=f32, device=dev), var=torch.empty(K, dtype=f32, device=dev),
-                ws=torch.empty(nb, dtype=torch.uint8, device=dev),
-                lws=torch.empty(int(_lib.lib.b200_loss_workspace_bytes()), dtype=torch.uint8, device=dev))
+                ws=torch.empty(nb, dtype=torch.uint8, device=dev), lws=self._lws)
         return self._buf
 
     def forward(self, users_d, items_d):
@@ -167,11 +206,8 @@ class FMTrainer(_GraphedStep):
         lib, st, p, K = _lib.lib, _lib.current_stream(), self.params, self.K
         R = int(users_d.numel())
         b = self._buffers(R)
-        L = self.spec.layout
-        _lib.check(lib.b200_feat_forward(
-            ctypes.byref(L), ctypes.byref(self.tables), _lib.ptr(users_d), _lib.ptr(items_d), R, 0, 0,
-            None, 0, _lib.ptr(b["pw"]), K, _lib.ptr(b["lin"]), None, _lib.ptr(p["lin_kernel"]), 0.0,
-            None, None, None, 0.0, _lib.ptr(b["S"]), _lib.ptr(b["Q"]), K, st))
+        feat_forward(self.spec.layout, self.tables, users_d, items_d, R, pw=b["pw"], lin=b["lin"],
+                     lin_kernel=p["lin_kernel"], ssum=b["S"], sqsum=b["Q"])
         y = b["pw"]
         if self.use_bn:
             _lib.check(lib.b200_bn_train_forward(
@@ -204,19 +240,15 @@ class FMTrainer(_GraphedStep):
             _lib.ptr(p["pw_kernel"]), _lib.ptr(b["dpw"]), K, _lib.ptr(g["pw_kernel"]), _lib.ptr(g["pw_bias"]),
             _lib.ptr(g["bn_gamma"]) if bn else None, _lib.ptr(g["bn_beta"]) if bn else None,
             _lib.ptr(g["lin_bias"]), _lib.ptr(b["ws"]), b["ws"].numel(), st))
-        gp = lambda k: _lib.ptr(g[k]) if k in g else None      # noqa: E731
-        _lib.check(lib.b200_feat_backward(
-            ctypes.byref(self.spec.layout), ctypes.byref(self.tables), _lib.ptr(users_d), _lib.ptr(items_d), R,
-            _lib.ptr(b["dpw"]), K, _lib.ptr(b["S"]), K, None, 0, _lib.ptr(b["dlogit"]), _lib.ptr(p["lin_kernel"]),
-            gp("user_embeds"), gp("item_embeds"), gp("sparse_embeds"), gp("dense_embeds"), gp("user_linear"),
-            gp("item_linear"), gp("sparse_linear"), gp("dense_linear"), gp("lin_kernel"), st))
-        _adam_update(self)
+        feat_backward(self.spec.layout, self.tables, users_d, items_d, R, g, dpw=b["dpw"], S=b["S"],
+                      dlogit=b["dlogit"], lin_kernel=p["lin_kernel"])
+        self._adam_update()
         return b["loss"]
 
     def export_weights(self):
         """Inference weight dict (feat_models.FM layout) with the BN moving statistics."""
         p = self.params
-        w = {k: p[k].cpu().numpy() for k in _TABLES if k in p}
+        w = self._export_tables()
         w.update(lin_kernel=p["lin_kernel"].cpu().numpy(), lin_bias=np.float32(p["lin_bias"].cpu().numpy()[0]),
                  pw_kernel=p["pw_kernel"].cpu().numpy(), pw_bias=np.float32(p["pw_bias"].cpu().numpy()[0]))
         if self.use_bn:
@@ -225,233 +257,25 @@ class FMTrainer(_GraphedStep):
         return w
 
 
-class DeepFMTrainer(_GraphedStep):
-    """DeepFM training step on the device: ``libreco/algorithms/deepfm.py:143-175`` with
-    ``dense_nn`` in training mode (``libreco/layers/dense.py:12-49``: BN(input) -> [Dense -> ReLU ->
-    BN] x (L-1) -> Dense, no dropout = the reference's default), mean sigmoid CE, TF-Adam.
-
-    The Dense layers run on the library's own GEMM kernels (``feat_models.linear``: wgmma 3xTF32 or
-    exact-fma SIMT) — forward ``Y = X Wt^T + b``, backward ``dX = dY Wt`` and ``dWt = dY^T X`` are the
-    same kernel on transposed operands.  ``weights`` uses the inference layout of
-    ``feat_models.DeepFM`` / ``oracle.tf_models.make_deepfm_weights``."""
-
-    def __init__(self, spec, weights, use_bn=True, lr=1e-3, epsilon=1e-5, device=None):
-        import torch
-
-        self._torch = torch
-        K = int(weights["user_embeds"].shape[1])
-        self.spec = spec if isinstance(spec, FeatSpec) else FeatSpec(spec, K, device)
-        self.device, self.K = self.spec.device, K
-        self.F = 2 + self.spec.n_sparse + self.spec.n_dense
-        self.use_bn, self.lr, self.epsilon, self.t = bool(use_bn), float(lr), float(epsilon), 0
-        f32 = torch.float32
-        p = {k: _dev(weights[k], self.device, f32).clone() for k in _TABLES if weights.get(k) is not None}
-        for k in ("lin_kernel", "out_kernel"):
-            p[k] = _dev(np.asarray(weights[k]).reshape(-1), self.device, f32).clone()
-        for k in ("lin_bias", "out_bias"):
-            p[k] = _dev(np.asarray(weights[k]).reshape(1), self.device, f32).clone()
-        mlp = weights["mlp"]
-        self.n_layers = len(mlp["kernels"])
-        for i in range(self.n_layers):       # trainable layout = transposed kernel [dout, din] (what the GEMM reads)
-            p[f"Wt{i}"] = _dev(np.ascontiguousarray(np.asarray(mlp["kernels"][i]).T), self.device, f32).clone()
-            p[f"b{i}"] = _dev(mlp["biases"][i], self.device, f32).clone()
-        self.moving = {}
-        if self.use_bn:
-            bns = [mlp.get("bn_in")] + list(mlp.get("bns") or [])
-            for j, bn in enumerate(bns):
-                p[f"bn{j}_gamma"] = _dev(bn["gamma"], self.device, f32).clone()
-                p[f"bn{j}_beta"] = _dev(bn["beta"], self.device, f32).clone()
-                self.moving[j] = (_dev(bn["mean"], self.device, f32).clone(), _dev(bn["var"], self.device, f32).clone())
-        self.H = int(p[f"Wt{self.n_layers - 1}"].shape[0])
-        self.params = p
-        self.grads = {k: torch.zeros_like(v) for k, v in p.items()}
-        self.m = {k: torch.zeros_like(v) for k, v in p.items()}
-        self.v = {k: torch.zeros_like(v) for k, v in p.items()}
-        T = FeatTablesStruct()
-        for k in _TABLES:
-            setattr(T, k, p[k].data_ptr() if k in p else None)
-        self.tables = T
-        self._lws = torch.empty(int(_lib.lib.b200_loss_workspace_bytes()), dtype=torch.uint8, device=self.device)
-
-    # ---- small wrappers ---------------------------------------------------------------------------
-    def _bn_forward(self, x, j):
-        torch = self._torch
-        p = self.params
-        R, C = x.shape
-        y = torch.empty_like(x)
-        mean = torch.empty(C, dtype=torch.float32, device=self.device)
-        var = torch.empty(C, dtype=torch.float32, device=self.device)
-        mm, mv = self.moving[j]
-        _lib.check(_lib.lib.b200_bn_train_forward(
-            _lib.ptr(x), x.stride(0), R, C, _lib.ptr(p[f"bn{j}_gamma"]), _lib.ptr(p[f"bn{j}_beta"]), BN_EPS,
-            BN_MOMENTUM, _lib.ptr(y), y.stride(0), _lib.ptr(mean), _lib.ptr(var), _lib.ptr(mm), _lib.ptr(mv),
-            _lib.current_stream()))
-        return y, (mean, var)
-
-    def _bn_backward(self, dy, x, stats, j, relu_mask):
-        torch = self._torch
-        p, g = self.params, self.grads
-        R, C = x.shape
-        dx = torch.empty_like(x)
-        ws = torch.empty(C * 2, dtype=torch.float64, device=self.device)
-        _lib.check(_lib.lib.b200_bn_train_backward(
-            _lib.ptr(dy), dy.stride(0), _lib.ptr(x), x.stride(0), R, C, _lib.ptr(stats[0]), _lib.ptr(stats[1]),
-            _lib.ptr(p[f"bn{j}_gamma"]), BN_EPS, 1 if relu_mask else 0, _lib.ptr(dx), dx.stride(0),
-            _lib.ptr(g[f"bn{j}_gamma"]), _lib.ptr(g[f"bn{j}_beta"]), _lib.ptr(ws), ws.numel() * 8,
-            _lib.current_stream()))
-        return dx
-
-    def _col_reduce(self, X, out, wrow=None):
-        _lib.check(_lib.lib.b200_col_reduce(_lib.ptr(X), X.stride(0) if X.dim() == 2 else 1, X.shape[0],
-                                            X.shape[1] if X.dim() == 2 else 1, _lib.ptr(wrow), None, 0,
-                                            _lib.ptr(out), _lib.current_stream()))
-
-    # ---- forward / step ---------------------------------------------------------------------------
-    def forward(self, users_d, items_d):
-        from .feat_models import linear
-
-        torch = self._torch
-        lib, st, p, K = _lib.lib, _lib.current_stream(), self.params, self.K
-        R = int(users_d.numel())
-        f32, dev = torch.float32, self.device
-        c = dict(R=R, concat=torch.empty((R, self.F * K), dtype=f32, device=dev),
-                 pw=torch.empty((R, K), dtype=f32, device=dev), lin=torch.empty(R, dtype=f32, device=dev),
-                 S=torch.empty((R, K), dtype=f32, device=dev), Q=torch.empty((R, K), dtype=f32, device=dev))
-        _lib.check(lib.b200_feat_forward(
-            ctypes.byref(self.spec.layout), ctypes.byref(self.tables), _lib.ptr(users_d), _lib.ptr(items_d), R, 0, 0,
-            _lib.ptr(c["concat"]), c["concat"].stride(0), _lib.ptr(c["pw"]), K, _lib.ptr(c["lin"]), None,
-            _lib.ptr(p["lin_kernel"]), 0.0, None, None, None, 0.0, _lib.ptr(c["S"]), _lib.ptr(c["Q"]), K, st))
-        a = c["concat"]
-        c["bn_stats"], c["dense_in"], c["relu_out"] = {}, [], []
-        if self.use_bn:
-            a, c["bn_stats"][0] = self._bn_forward(a, 0)
-        for i in range(self.n_layers):
-            last = i == self.n_layers - 1
-            c["dense_in"].append(a)
-            a = linear(a, p[f"Wt{i}"], p[f"b{i}"], not last, cache_split=False)     # weights change every step
-            if not last:
-                c["relu_out"].append(a)
-                if self.use_bn:
-                    a, c["bn_stats"][i + 1] = self._bn_forward(a, i + 1)
-        c["deep"] = a
-        c["logit"] = torch.empty(R, dtype=f32, device=dev)
-        _lib.check(lib.b200_deepfm_head_forward(
-            _lib.ptr(c["lin"]), _lib.ptr(p["lin_bias"]), _lib.ptr(c["pw"]), K, K, _lib.ptr(a), a.stride(0), self.H,
-            _lib.ptr(p["out_kernel"]), _lib.ptr(p["out_bias"]), R, _lib.ptr(c["logit"]), st))
-        self._cache = c
-        return c["logit"]
-
-    def backward(self, labels_d):
-        """Loss + every gradient buffer filled (before the optimiser); returns the device loss."""
-        from .feat_models import linear
-
-        torch = self._torch
-        lib, st, p, g, K, H = _lib.lib, _lib.current_stream(), self.params, self.grads, self.K, self.H
-        c = self._cache
-        R, f32, dev = c["R"], torch.float32, self.device
-        loss = torch.empty((), dtype=f32, device=dev)
-        dlogit = torch.empty(R, dtype=f32, device=dev)
-        _lib.check(lib.b200_pointwise_loss(_lib.ptr(c["logit"]), _lib.ptr(labels_d), R, 0, 0.25, 2.0, _lib.ptr(loss),
-                                           _lib.ptr(dlogit), _lib.ptr(self._lws), self._lws.numel(), st))
-        dlin = torch.empty(R, dtype=f32, device=dev)
-        dpw = torch.empty((R, K), dtype=f32, device=dev)
-        da = torch.empty((R, H), dtype=f32, device=dev)
-        _lib.check(lib.b200_deepfm_head_backward(_lib.ptr(dlogit), _lib.ptr(p["out_kernel"]), K, H, R, _lib.ptr(dlin),
-                                                 _lib.ptr(dpw), K, _lib.ptr(da), H, st))
-        # out_kernel = [w_lin | w_pw (K) | w_deep (H)]: weighted column sums with the row weights dlogit
-        gk = g["out_kernel"]
-        lin_full = c["lin"] + p["lin_bias"]                      # elementwise add of a device scalar (plumbing)
-        self._col_reduce(lin_full.view(R, 1), gk[0:1], dlogit)
-        self._col_reduce(c["pw"], gk[1:1 + K], dlogit)
-        self._col_reduce(c["deep"], gk[1 + K:], dlogit)
-        self._col_reduce(dlogit.view(R, 1), g["out_bias"])
-        self._col_reduce(dlin.view(R, 1), g["lin_bias"])
-        # ---- dense_nn backward
-        for i in range(self.n_layers - 1, -1, -1):
-            if i != self.n_layers - 1:
-                r_out = c["relu_out"][i]
-                if self.use_bn:
-                    da = self._bn_backward(da, r_out, c["bn_stats"][i + 1], i + 1, True)
-                else:
-                    dh = torch.empty_like(da)
-                    _lib.check(lib.b200_relu_backward(_lib.ptr(da), _lib.ptr(r_out), da.numel(), _lib.ptr(dh), st))
-                    da = dh
-            x = c["dense_in"][i]
-            da = da.contiguous()
-            # dWt [dout, din] = dY^T X ; db = column sums of dY ; dX = dY Wt
-            g[f"Wt{i}"] += _weight_grad(da, x)
-            self._col_reduce(da, g[f"b{i}"])
-            da = linear(da, p[f"Wt{i}"].t().contiguous(), None, False, cache_split=False)
-        dconcat = self._bn_backward(da, c["concat"], c["bn_stats"][0], 0, False) if self.use_bn else da
-        gp = lambda k: _lib.ptr(g[k]) if k in g else None      # noqa: E731
-        _lib.check(lib.b200_feat_backward(
-            ctypes.byref(self.spec.layout), ctypes.byref(self.tables), _lib.ptr(c["users"]), _lib.ptr(c["items"]), R,
-            _lib.ptr(dpw), K, _lib.ptr(c["S"]), K, _lib.ptr(dconcat), dconcat.stride(0), _lib.ptr(dlin),
-            _lib.ptr(p["lin_kernel"]), gp("user_embeds"), gp("item_embeds"), gp("sparse_embeds"), gp("dense_embeds"),
-            gp("user_linear"), gp("item_linear"), gp("sparse_linear"), gp("dense_linear"), gp("lin_kernel"), st))
-        return loss
-
-    def step(self, users_d, items_d, labels_d):
-        torch = self._torch
-        users_d = users_d.to(torch.int64).contiguous()
-        items_d = items_d.to(torch.int64).contiguous()
-        labels_d = labels_d.to(torch.float32).contiguous()
-        self.forward(users_d, items_d)
-        self._cache["users"], self._cache["items"] = users_d, items_d
-        loss = self.backward(labels_d)
-        _adam_update(self)
-        self._cache = None
-        return loss
-
-    def export_weights(self):
-        p = self.params
-        w = {k: p[k].cpu().numpy() for k in _TABLES if k in p}
-        w.update(lin_kernel=p["lin_kernel"].cpu().numpy(), lin_bias=np.float32(p["lin_bias"].cpu().numpy()[0]),
-                 out_kernel=p["out_kernel"].cpu().numpy(), out_bias=np.float32(p["out_bias"].cpu().numpy()[0]))
-        n = self.n_layers
-        mlp = dict(kernels=[p[f"Wt{i}"].t().contiguous().cpu().numpy() for i in range(n)],
-                   biases=[p[f"b{i}"].cpu().numpy() for i in range(n)])
-        if self.use_bn:
-            def bn(j):
-                return dict(gamma=p[f"bn{j}_gamma"].cpu().numpy(), beta=p[f"bn{j}_beta"].cpu().numpy(),
-                            mean=self.moving[j][0].cpu().numpy(), var=self.moving[j][1].cpu().numpy())
-            mlp["bn_in"] = bn(0)
-            mlp["bns"] = [bn(i + 1) for i in range(n - 1)]
-        w["mlp"] = mlp
-        return w
-
-
-class _StackTrainer(_GraphedStep):
+class _StackTrainer(_Trainer):
     """Shared pieces of the trainers built on ``dense_nn`` stacks (``libreco/layers/dense.py:12-49``, training mode):
-    parameters ``{prefix}Wt{i}`` [dout, din], ``{prefix}b{i}``, ``{prefix}bn{j}_gamma|beta`` (+ moving statistics),
-    forward / backward of one stack on the library kernels, TF-Adam over every variable."""
+    parameters ``{prefix}Wt{i}`` [dout, din], ``{prefix}b{i}``, ``{prefix}bn{j}_gamma|beta`` (+ moving statistics
+    ``moving[f"{prefix}bn{j}"]``), forward / backward of one stack on the library kernels."""
 
-    def _init_stack(self, prefix, mlp, p):
-        torch = self._torch
-        f32 = torch.float32
+    def _init_stack(self, prefix, mlp):
+        """Adds one stack's variables (trainable layout = transposed kernel [dout, din], what the GEMM reads);
+        returns its number of Dense layers."""
+        p = self.params
         n = len(mlp["kernels"])
         for i in range(n):
-            p[f"{prefix}Wt{i}"] = _dev(np.ascontiguousarray(np.asarray(mlp["kernels"][i]).T), self.device, f32).clone()
-            p[f"{prefix}b{i}"] = _dev(mlp["biases"][i], self.device, f32).clone()
+            p[f"{prefix}Wt{i}"] = self._var(np.ascontiguousarray(np.asarray(mlp["kernels"][i]).T))
+            p[f"{prefix}b{i}"] = self._var(mlp["biases"][i])
         if self.use_bn:
             for j, bn in enumerate([mlp.get("bn_in")] + list(mlp.get("bns") or [])):
-                p[f"{prefix}bn{j}_gamma"] = _dev(bn["gamma"], self.device, f32).clone()
-                p[f"{prefix}bn{j}_beta"] = _dev(bn["beta"], self.device, f32).clone()
-                self.moving[f"{prefix}bn{j}"] = (_dev(bn["mean"], self.device, f32).clone(),
-                                                 _dev(bn["var"], self.device, f32).clone())
+                p[f"{prefix}bn{j}_gamma"] = self._var(bn["gamma"])
+                p[f"{prefix}bn{j}_beta"] = self._var(bn["beta"])
+                self.moving[f"{prefix}bn{j}"] = (self._var(bn["mean"]), self._var(bn["var"]))
         return n
-
-    def _finish_init(self, p):
-        torch = self._torch
-        self.params = p
-        self.grads = {k: torch.zeros_like(v) for k, v in p.items()}
-        self.m = {k: torch.zeros_like(v) for k, v in p.items()}
-        self.v = {k: torch.zeros_like(v) for k, v in p.items()}
-        T = FeatTablesStruct()
-        for k in ("user_embeds", "item_embeds", "sparse_embeds", "dense_embeds"):
-            setattr(T, k, p[k].data_ptr() if k in p else None)
-        self.tables = T
-        self._lws = torch.empty(int(_lib.lib.b200_loss_workspace_bytes()), dtype=torch.uint8, device=self.device)
 
     def _bn_forward(self, x, name):
         torch = self._torch
@@ -487,8 +311,6 @@ class _StackTrainer(_GraphedStep):
 
     def _stack_forward(self, prefix, n_layers, x):
         """BN(input) -> [Dense -> ReLU -> BN] x (L-1) -> Dense with batch statistics; returns (out, cache)."""
-        from .feat_models import linear
-
         p = self.params
         c = dict(concat=x, bn_stats={}, dense_in=[], relu_out=[])
         a = x
@@ -497,7 +319,7 @@ class _StackTrainer(_GraphedStep):
         for i in range(n_layers):
             last = i == n_layers - 1
             c["dense_in"].append(a)
-            a = linear(a, p[f"{prefix}Wt{i}"], p[f"{prefix}b{i}"], not last, cache_split=False)
+            a = linear(a, p[f"{prefix}Wt{i}"], p[f"{prefix}b{i}"], not last, cache_split=False)  # weights change every step
             if not last:
                 c["relu_out"].append(a)
                 if self.use_bn:
@@ -506,8 +328,6 @@ class _StackTrainer(_GraphedStep):
 
     def _stack_backward(self, prefix, n_layers, c, da):
         """Gradients of the stack's variables ADDED into ``self.grads``; returns d loss / d input."""
-        from .feat_models import linear
-
         torch = self._torch
         lib, st, p, g = _lib.lib, _lib.current_stream(), self.params, self.grads
         da = da.contiguous()
@@ -522,13 +342,11 @@ class _StackTrainer(_GraphedStep):
                     da = dh
             x = c["dense_in"][i]
             da = da.contiguous()
+            # dWt [dout, din] = dY^T X ; db = column sums of dY ; dX = dY Wt
             g[f"{prefix}Wt{i}"] += _weight_grad(da, x)
             self._col_sum(da, g[f"{prefix}b{i}"])
             da = linear(da, p[f"{prefix}Wt{i}"].t().contiguous(), None, False, cache_split=False)
         return self._bn_backward(da, c["concat"], c["bn_stats"][0], f"{prefix}bn0", False) if self.use_bn else da
-
-    def _adam_all(self):
-        _adam_update(self)
 
     def _export_stack(self, prefix, n):
         p = self.params
@@ -542,6 +360,95 @@ class _StackTrainer(_GraphedStep):
             mlp["bn_in"] = bn(0)
             mlp["bns"] = [bn(i + 1) for i in range(n - 1)]
         return mlp
+
+
+class DeepFMTrainer(_StackTrainer):
+    """DeepFM training step on the device: ``libreco/algorithms/deepfm.py:143-175`` with
+    ``dense_nn`` in training mode (``libreco/layers/dense.py:12-49``: BN(input) -> [Dense -> ReLU ->
+    BN] x (L-1) -> Dense, no dropout = the reference's default), mean sigmoid CE, TF-Adam.
+
+    The Dense layers run on the library's own GEMM kernels (``feat_models.linear``: wgmma 3xTF32 or
+    exact-fma SIMT) — forward ``Y = X Wt^T + b``, backward ``dX = dY Wt`` and ``dWt = dY^T X`` are the
+    same kernel on transposed operands.  ``weights`` uses the inference layout of
+    ``feat_models.DeepFM`` / ``oracle.tf_models.make_deepfm_weights``."""
+
+    linear_tables = True
+
+    def __init__(self, spec, weights, use_bn=True, lr=1e-3, epsilon=1e-5, device=None):
+        super().__init__(spec, weights, use_bn, lr, epsilon, device)
+
+    def _init_params(self, weights):
+        p = self.params
+        for k in ("lin_kernel", "out_kernel"):
+            p[k] = self._var(weights[k], -1)
+        for k in ("lin_bias", "out_bias"):
+            p[k] = self._var(weights[k], 1)
+        self.n_layers = self._init_stack("", weights["mlp"])
+        self.H = int(p[f"Wt{self.n_layers - 1}"].shape[0])
+
+    def forward(self, users_d, items_d):
+        torch = self._torch
+        p, K = self.params, self.K
+        R = int(users_d.numel())
+        f32, dev = torch.float32, self.device
+        concat = torch.empty((R, self.F * K), dtype=f32, device=dev)
+        pw, lin = torch.empty((R, K), dtype=f32, device=dev), torch.empty(R, dtype=f32, device=dev)
+        S, Q = torch.empty((R, K), dtype=f32, device=dev), torch.empty((R, K), dtype=f32, device=dev)
+        feat_forward(self.spec.layout, self.tables, users_d, items_d, R, concat=concat, pw=pw, lin=lin,
+                     lin_kernel=p["lin_kernel"], ssum=S, sqsum=Q)
+        a, c = self._stack_forward("", self.n_layers, concat)
+        logit = torch.empty(R, dtype=f32, device=dev)
+        _lib.check(_lib.lib.b200_deepfm_head_forward(
+            _lib.ptr(lin), _lib.ptr(p["lin_bias"]), _lib.ptr(pw), K, K, _lib.ptr(a), a.stride(0), self.H,
+            _lib.ptr(p["out_kernel"]), _lib.ptr(p["out_bias"]), R, _lib.ptr(logit), _lib.current_stream()))
+        c.update(R=R, users=users_d, items=items_d, pw=pw, lin=lin, S=S, deep=a, logit=logit)
+        self._cache = c
+        return logit
+
+    def backward(self, labels_d):
+        """Loss + every gradient buffer filled (before the optimiser); returns the device loss."""
+        torch = self._torch
+        p, g, K, H = self.params, self.grads, self.K, self.H
+        c = self._cache
+        R, f32, dev = c["R"], torch.float32, self.device
+        loss, dlogit = self._loss(c["logit"], labels_d)
+        dlin = torch.empty(R, dtype=f32, device=dev)
+        dpw = torch.empty((R, K), dtype=f32, device=dev)
+        da = torch.empty((R, H), dtype=f32, device=dev)
+        _lib.check(_lib.lib.b200_deepfm_head_backward(_lib.ptr(dlogit), _lib.ptr(p["out_kernel"]), K, H, R,
+                                                      _lib.ptr(dlin), _lib.ptr(dpw), K, _lib.ptr(da), H,
+                                                      _lib.current_stream()))
+        # out_kernel = [w_lin | w_pw (K) | w_deep (H)]: weighted column sums with the row weights dlogit
+        gk = g["out_kernel"]
+        lin_full = c["lin"] + p["lin_bias"]                      # elementwise add of a device scalar (plumbing)
+        self._col_sum(lin_full.view(R, 1), gk[0:1], dlogit)
+        self._col_sum(c["pw"], gk[1:1 + K], dlogit)
+        self._col_sum(c["deep"], gk[1 + K:], dlogit)
+        self._col_sum(dlogit.view(R, 1), g["out_bias"])
+        self._col_sum(dlin.view(R, 1), g["lin_bias"])
+        dconcat = self._stack_backward("", self.n_layers, c, da)
+        feat_backward(self.spec.layout, self.tables, c["users"], c["items"], R, g, dpw=dpw, S=c["S"], dconcat=dconcat,
+                      dlogit=dlin, lin_kernel=p["lin_kernel"])
+        return loss
+
+    def step(self, users_d, items_d, labels_d):
+        torch = self._torch
+        users_d = users_d.to(torch.int64).contiguous()
+        items_d = items_d.to(torch.int64).contiguous()
+        labels_d = labels_d.to(torch.float32).contiguous()
+        self.forward(users_d, items_d)
+        loss = self.backward(labels_d)
+        self._adam_update()
+        self._cache = None
+        return loss
+
+    def export_weights(self):
+        p = self.params
+        w = self._export_tables()
+        w.update(lin_kernel=p["lin_kernel"].cpu().numpy(), lin_bias=np.float32(p["lin_bias"].cpu().numpy()[0]),
+                 out_kernel=p["out_kernel"].cpu().numpy(), out_bias=np.float32(p["out_bias"].cpu().numpy()[0]))
+        w["mlp"] = self._export_stack("", self.n_layers)
+        return w
 
 
 class TwoTowerTrainer(_StackTrainer):
@@ -558,51 +465,24 @@ class TwoTowerTrainer(_StackTrainer):
     ``weights``: layout of ``feat_models.TwoTower`` / ``synthetic.make_two_tower_weights``.  ``temperature``
     must be positive (the learned-temperature variant, ``temperature <= 0``, is not built)."""
 
-    _T = ("user_embeds", "item_embeds", "sparse_embeds", "dense_embeds")
-
     def __init__(self, spec, weights, use_bn=True, norm_embed=False, temperature=1.0, remove_accidental_hits=False,
                  lr=1e-3, epsilon=1e-5, device=None):
-        import torch
-
-        from .feat_models import FeatLayoutStruct
-
         if temperature <= 0:
             raise ValueError("learned temperature (temperature <= 0) is not supported")
-        self._torch = torch
-        K = int(weights["user_embeds"].shape[1])
-        self.spec = spec if isinstance(spec, FeatSpec) else FeatSpec(spec, K, device)
-        self.device, self.K = self.spec.device, K
-        self.use_bn, self.norm_embed = bool(use_bn), bool(norm_embed)
+        self.norm_embed = bool(norm_embed)
         self.temperature, self.remove_hits = float(temperature), bool(remove_accidental_hits)
-        self.lr, self.epsilon, self.t = float(lr), float(epsilon), 0
-        f32 = torch.float32
-        p = {k: _dev(weights[k], self.device, f32).clone() for k in self._T if weights.get(k) is not None}
-        self.moving, self.n_layers, self.layouts, self.widths = {}, {}, {}, {}
-        for which, mask in (("user", 1), ("item", 2)):
-            self.n_layers[which] = self._init_stack(f"{which}_", weights[f"{which}_tower"], p)
-            L = FeatLayoutStruct.from_buffer_copy(self.spec.layout)
-            L.id_mask = mask
-            scols = self.spec.user_sparse_cols if which == "user" else self.spec.item_sparse_cols
-            dcols = self.spec.user_dense_cols if which == "user" else self.spec.item_dense_cols
-            L.n_sparse, L.n_dense = len(scols), len(dcols)
-            for f in range(len(scols)):
-                L.sparse_side[f], L.sparse_col[f] = (0 if which == "user" else 1), f
-            for f in range(len(dcols)):
-                L.dense_side[f], L.dense_col[f] = (0 if which == "user" else 1), f
-                L.dense_embed_row[f] = dcols[f]
-            self.layouts[which] = L
-            self.widths[which] = (1 + len(scols) + len(dcols)) * K
-        self._finish_init(p)
+        super().__init__(spec, weights, use_bn, lr, epsilon, device)
+
+    def _init_params(self, weights):
+        self.n_layers = {which: self._init_stack(f"{which}_", weights[f"{which}_tower"]) for which in ("user", "item")}
 
     # ---- one tower ----------------------------------------------------------------------------------
     def tower_forward(self, which, ids_d):
         torch = self._torch
         n = int(ids_d.numel())
-        x = torch.empty((n, self.widths[which]), dtype=torch.float32, device=self.device)
-        _lib.check(_lib.lib.b200_feat_forward(
-            ctypes.byref(self.layouts[which]), ctypes.byref(self.tables), _lib.ptr(ids_d), _lib.ptr(ids_d), n, 0, 0,
-            _lib.ptr(x), x.stride(0), None, 0, None, None, None, 0.0, None, None, None, 0.0,
-            None, None, 0, _lib.current_stream()))
+        L, pos = self.spec.side(which)
+        x = torch.empty((n, len(pos) * self.K), dtype=torch.float32, device=self.device)
+        feat_forward(L, self.tables, ids_d, ids_d, n, concat=x)
         a, c = self._stack_forward(f"{which}_", self.n_layers[which], x)
         c["ids"] = ids_d
         if self.norm_embed:
@@ -613,29 +493,21 @@ class TwoTowerTrainer(_StackTrainer):
         return c
 
     def tower_backward(self, which, c, da):
-        lib, st, g = _lib.lib, _lib.current_stream(), self.grads
         n = int(c["ids"].numel())
         da = da.contiguous()
         if self.norm_embed:
             x = c["pre_norm"]
-            _lib.check(lib.b200_l2_normalize_backward(_lib.ptr(x), x.stride(0), _lib.ptr(da), da.stride(0), n,
-                                                      x.shape[1], _lib.ptr(da), da.stride(0), st))
+            _lib.check(_lib.lib.b200_l2_normalize_backward(_lib.ptr(x), x.stride(0), _lib.ptr(da), da.stride(0), n,
+                                                           x.shape[1], _lib.ptr(da), da.stride(0),
+                                                           _lib.current_stream()))
         dconcat = self._stack_backward(f"{which}_", self.n_layers[which], c, da)
-        gp = lambda k: _lib.ptr(g[k]) if k in g else None      # noqa: E731
-        _lib.check(lib.b200_feat_backward(
-            ctypes.byref(self.layouts[which]), ctypes.byref(self.tables), _lib.ptr(c["ids"]), _lib.ptr(c["ids"]), n,
-            None, 0, None, 0, _lib.ptr(dconcat), dconcat.stride(0), None, None,
-            gp("user_embeds"), gp("item_embeds"), gp("sparse_embeds"), gp("dense_embeds"), None, None, None, None,
-            None, st))
+        feat_backward(self.spec.side(which)[0], self.tables, c["ids"], c["ids"], n, self.grads, dconcat=dconcat)
 
     # ---- loss / step --------------------------------------------------------------------------------
     def forward_backward(self, users_d, items_d, correction_d=None):
         """Loss (device scalar) with every gradient buffer filled.  ``correction_d``: item_corrections[items]
         of the batch (``two_tower.py:425-435``, ``tf_feed_dicts.py:121-122``) or None (use_correction=False)."""
-        from .feat_models import linear
-
         torch = self._torch
-        lib, st = _lib.lib, _lib.current_stream()
         cu = self.tower_forward("user", users_d)
         ci = self.tower_forward("item", items_d)
         U, V = cu["out"], ci["out"]
@@ -643,9 +515,9 @@ class TwoTowerTrainer(_StackTrainer):
         S = linear(U, V, None, False, cache_split=False)          # [B, B] = U V^T
         loss = torch.empty((), dtype=torch.float32, device=self.device)
         corr = correction_d.to(torch.float32).contiguous() if correction_d is not None else None
-        _lib.check(lib.b200_softmax_inbatch_loss(_lib.ptr(S), S.stride(0), B, self.temperature, _lib.ptr(corr),
-                                                 _lib.ptr(items_d) if self.remove_hits else None, 1, _lib.ptr(loss),
-                                                 _lib.ptr(self._lws), self._lws.numel(), st))
+        _lib.check(_lib.lib.b200_softmax_inbatch_loss(_lib.ptr(S), S.stride(0), B, self.temperature, _lib.ptr(corr),
+                                                      _lib.ptr(items_d) if self.remove_hits else None, 1, _lib.ptr(loss),
+                                                      _lib.ptr(self._lws), self._lws.numel(), _lib.current_stream()))
         dU = linear(S, V.t().contiguous(), None, False, cache_split=False)
         dV = linear(S.t().contiguous(), U.t().contiguous(), None, False, cache_split=False)
         self.tower_backward("user", cu, dU)
@@ -658,13 +530,12 @@ class TwoTowerTrainer(_StackTrainer):
         users_d = users_d.to(torch.int64).contiguous()
         items_d = items_d.to(torch.int64).contiguous()
         loss = self.forward_backward(users_d, items_d, correction_d)
-        self._adam_all()
+        self._adam_update()
         self._last = None
         return loss
 
     def export_weights(self):
-        p = self.params
-        w = {k: p[k].cpu().numpy() for k in self._T if k in p}
+        w = self._export_tables()
         for which in ("user", "item"):
             w[f"{which}_tower"] = self._export_stack(f"{which}_", self.n_layers[which])
         w["user_dense_cols"] = list(self.spec.user_dense_cols)
@@ -672,11 +543,69 @@ class TwoTowerTrainer(_StackTrainer):
         return w
 
 
-class YouTubeRankingTrainer(_StackTrainer):
+class _SeqTrainer(_StackTrainer):
+    """YouTubeRanking and DIN: the F field blocks and a sequence block -> one ``dense_nn`` stack -> Dense(1), mean
+    sigmoid CE, TF-Adam.  The batch carries one behaviour sequence per ROW (``seqs`` [R, T] padded with ``n_items``,
+    ``lens`` [R]; ``libreco/batch/sequence.py:75-91``).  A subclass fills the sequence block of the stack input
+    (``forward``) and sends its gradient back (``backward``)."""
+
+    def __init__(self, spec, weights, use_bn=True, lr=1e-3, epsilon=1e-5, device=None):
+        super().__init__(spec, weights, use_bn, lr, epsilon, device)
+
+    def _init_params(self, weights):
+        self.n_layers = self._init_stack("", weights["mlp"])
+        self.params["out_kernel"] = self._var(weights["out_kernel"], -1)
+        self.params["out_bias"] = self._var(weights["out_bias"], 1)
+
+    def _head_forward(self, x, **cache):
+        """Stack + Dense(1) on the filled input ``x``; caches what the backward needs and returns the logits."""
+        torch = self._torch
+        p = self.params
+        R = int(x.shape[0])
+        h, c = self._stack_forward("", self.n_layers, x)
+        logit = torch.empty(R, dtype=torch.float32, device=self.device)
+        _lib.check(_lib.lib.b200_concat_dense(_lib.ptr(h), h.stride(0), h.shape[1], None, 0, 0, None, 0, 0,
+                                              _lib.ptr(p["out_kernel"]), 0.0, R, _lib.ptr(logit), _lib.current_stream()))
+        logit += p["out_bias"]                      # device scalar add (the bias is a trainable variable)
+        c.update(R=R, h=h, logit=logit, **cache)
+        self._cache = c
+        return logit
+
+    def _head_backward(self, labels_d):
+        """Loss, the gradients of the head, the stack and the field tables; returns (loss, d loss / d input)."""
+        p, g, c = self.params, self.grads, self._cache
+        R = c["R"]
+        loss, dlogit = self._loss(c["logit"], labels_d)
+        self._col_sum(c["h"], g["out_kernel"], dlogit)
+        self._col_sum(dlogit, g["out_bias"])
+        # d h = dlogit (x) out_kernel: the Dense(1) transposed, on the library's dense kernel (din = 1)
+        da = linear(dlogit.view(R, 1), p["out_kernel"].view(-1, 1), None, False, cache_split=False)
+        dx = self._stack_backward("", self.n_layers, c, da)
+        feat_backward(self.spec.layout, self.tables, c["users"], c["items"], R, g, dconcat=dx)
+        return loss, dx
+
+    def step(self, users_d, items_d, seqs_d, lens_d, labels_d):
+        torch = self._torch
+        self.forward(users_d.to(torch.int64).contiguous(), items_d.to(torch.int64).contiguous(),
+                     seqs_d.to(torch.int32).contiguous(), lens_d.to(torch.int32).contiguous())
+        loss = self.backward(labels_d.to(torch.float32).contiguous())
+        self._adam_update()
+        self._cache = None
+        return loss
+
+    def export_weights(self):
+        p = self.params
+        w = self._export_tables()
+        w["mlp"] = self._export_stack("", self.n_layers)
+        w["out_kernel"] = p["out_kernel"].cpu().numpy()
+        w["out_bias"] = np.float32(p["out_bias"].cpu().numpy()[0])
+        return w
+
+
+class YouTubeRankingTrainer(_SeqTrainer):
     """YouTubeRanking training step on the device: ``libreco/algorithms/youtube_ranking.py:167-218`` in training
     mode (concat(user, item, pooled behaviour sequence, sparse, dense) -> ``dense_nn`` -> Dense(1)), mean sigmoid
-    CE, TF-Adam.  The batch carries one behaviour sequence per ROW (``seqs`` [R, T] padded with ``n_items``,
-    ``lens`` [R]; ``libreco/batch/sequence.py:75-91``).
+    CE, TF-Adam.
 
         K1 gather (b200_feat_forward) + b200_seq_pool -> stack forward -> b200_concat_dense -> b200_pointwise_loss
         -> stack backward -> b200_feat_backward (field gradients) + b200_seq_pool_backward (sequence gradient into
@@ -685,110 +614,50 @@ class YouTubeRankingTrainer(_StackTrainer):
     Internally the pooled block sits AFTER the F field blocks (the inference engine's layout); the first kernel and
     the input batch-norm are permuted on the way in and out (``feat_models.permute_mlp_input``)."""
 
-    _T = ("user_embeds", "item_embeds", "sparse_embeds", "dense_embeds")
-
-    def __init__(self, spec, weights, use_bn=True, lr=1e-3, epsilon=1e-5, device=None):
-        import torch
-
-        from .feat_models import permute_mlp_input
-
-        self._torch = torch
-        K = int(weights["user_embeds"].shape[1])
-        self.spec = spec if isinstance(spec, FeatSpec) else FeatSpec(spec, K, device)
-        self.device, self.K = self.spec.device, K
-        self.F = 2 + self.spec.n_sparse + self.spec.n_dense
-        self.n_items = self.spec.n_items
-        self.use_bn, self.lr, self.epsilon, self.t = bool(use_bn), float(lr), float(epsilon), 0
-        f32 = torch.float32
-        F = self.F
+    def _init_params(self, weights):
+        K, F = self.K, self.F
         self.perm = np.concatenate([np.arange(0, 2 * K), np.arange(3 * K, (F + 1) * K), np.arange(2 * K, 3 * K)])
-        p = {k: _dev(weights[k], self.device, f32).clone() for k in self._T if weights.get(k) is not None}
-        self.moving = {}
-        self.n_layers = self._init_stack("", permute_mlp_input(weights["mlp"], self.perm), p)
-        p["out_kernel"] = _dev(np.asarray(weights["out_kernel"]).reshape(-1), self.device, f32).clone()
-        p["out_bias"] = _dev(np.asarray(weights["out_bias"]).reshape(1), self.device, f32).clone()
-        self._finish_init(p)
+        super()._init_params(dict(weights, mlp=permute_mlp_input(weights["mlp"], self.perm)))
 
     def forward(self, users_d, items_d, seqs_d, lens_d):
         torch = self._torch
-        lib, st, p, K, F = _lib.lib, _lib.current_stream(), self.params, self.K, self.F
+        K, F = self.K, self.F
         R = int(users_d.numel())
         x = torch.empty((R, (F + 1) * K), dtype=torch.float32, device=self.device)
-        _lib.check(lib.b200_feat_forward(
-            ctypes.byref(self.spec.layout), ctypes.byref(self.tables), _lib.ptr(users_d), _lib.ptr(items_d), R, 0, 0,
-            _lib.ptr(x), x.stride(0), None, 0, None, None, None, 0.0, None, None, None, 0.0, None, None, 0, st))
+        feat_forward(self.spec.layout, self.tables, users_d, items_d, R, concat=x)
         rows = torch.arange(R, dtype=torch.int64, device=self.device)
         pooled = x[:, F * K:]
-        E = p["item_embeds"]
-        _lib.check(lib.b200_seq_pool(_lib.ptr(E), E.stride(0), K, self.n_items, _lib.ptr(seqs_d), seqs_d.stride(0),
-                                     _lib.ptr(lens_d), seqs_d.shape[1], _lib.ptr(rows), R, 0, 0, _lib.ptr(pooled),
-                                     pooled.stride(0), st))
-        h, c = self._stack_forward("", self.n_layers, x)
-        logit = torch.empty(R, dtype=torch.float32, device=self.device)
-        _lib.check(lib.b200_concat_dense(_lib.ptr(h), h.stride(0), h.shape[1], None, 0, 0, None, 0, 0,
-                                         _lib.ptr(p["out_kernel"]), 0.0, R, _lib.ptr(logit), st))
-        logit += p["out_bias"]                      # device scalar add (the bias is a trainable variable)
-        c.update(R=R, users=users_d, items=items_d, seqs=seqs_d, lens=lens_d, rows=rows, h=h, logit=logit)
-        self._cache = c
-        return logit
+        E = self.params["item_embeds"]
+        _lib.check(_lib.lib.b200_seq_pool(_lib.ptr(E), E.stride(0), K, self.n_items, _lib.ptr(seqs_d), seqs_d.stride(0),
+                                          _lib.ptr(lens_d), seqs_d.shape[1], _lib.ptr(rows), R, 0, 0, _lib.ptr(pooled),
+                                          pooled.stride(0), _lib.current_stream()))
+        return self._head_forward(x, users=users_d, items=items_d, seqs=seqs_d, lens=lens_d, rows=rows)
 
     def backward(self, labels_d):
-        from .feat_models import linear
-
-        torch = self._torch
-        lib, st, p, g, K, F = _lib.lib, _lib.current_stream(), self.params, self.grads, self.K, self.F
+        K, F = self.K, self.F
         c = self._cache
-        R = c["R"]
-        loss = torch.empty((), dtype=torch.float32, device=self.device)
-        dlogit = torch.empty(R, dtype=torch.float32, device=self.device)
-        _lib.check(lib.b200_pointwise_loss(_lib.ptr(c["logit"]), _lib.ptr(labels_d), R, 0, 0.25, 2.0, _lib.ptr(loss),
-                                           _lib.ptr(dlogit), _lib.ptr(self._lws), self._lws.numel(), st))
-        self._col_sum(c["h"], g["out_kernel"], dlogit)
-        self._col_sum(dlogit, g["out_bias"])
-        # d h = dlogit (x) out_kernel: the Dense(1) transposed, on the library's dense kernel (din = 1)
-        da = linear(dlogit.view(R, 1), p["out_kernel"].view(-1, 1), None, False, cache_split=False)
-        dx = self._stack_backward("", self.n_layers, c, da)
-        gp = lambda k: _lib.ptr(g[k]) if k in g else None      # noqa: E731
-        _lib.check(lib.b200_feat_backward(
-            ctypes.byref(self.spec.layout), ctypes.byref(self.tables), _lib.ptr(c["users"]), _lib.ptr(c["items"]), R,
-            None, 0, None, 0, _lib.ptr(dx), dx.stride(0), None, None,
-            gp("user_embeds"), gp("item_embeds"), gp("sparse_embeds"), gp("dense_embeds"), None, None, None, None,
-            None, st))
+        loss, dx = self._head_backward(labels_d)
         dpool = dx[:, F * K:]
-        ge = g["item_embeds"]
-        _lib.check(lib.b200_seq_pool_backward(_lib.ptr(dpool), dpool.stride(0), K, self.n_items, _lib.ptr(c["seqs"]),
-                                              c["seqs"].stride(0), _lib.ptr(c["lens"]), c["seqs"].shape[1],
-                                              _lib.ptr(c["rows"]), R, _lib.ptr(ge), ge.stride(0), st))
-        return loss
-
-    def step(self, users_d, items_d, seqs_d, lens_d, labels_d):
-        torch = self._torch
-        self.forward(users_d.to(torch.int64).contiguous(), items_d.to(torch.int64).contiguous(),
-                     seqs_d.to(torch.int32).contiguous(), lens_d.to(torch.int32).contiguous())
-        loss = self.backward(labels_d.to(torch.float32).contiguous())
-        self._adam_all()
-        self._cache = None
+        ge = self.grads["item_embeds"]
+        _lib.check(_lib.lib.b200_seq_pool_backward(_lib.ptr(dpool), dpool.stride(0), K, self.n_items,
+                                                   _lib.ptr(c["seqs"]), c["seqs"].stride(0), _lib.ptr(c["lens"]),
+                                                   c["seqs"].shape[1], _lib.ptr(c["rows"]), c["R"], _lib.ptr(ge),
+                                                   ge.stride(0), _lib.current_stream()))
         return loss
 
     def export_weights(self):
-        p = self.params
-        w = {k: p[k].cpu().numpy() for k in self._T if k in p}
-        mlp = self._export_stack("", self.n_layers)
+        w = super().export_weights()
         inv = np.argsort(self.perm)
-        mlp["kernels"][0] = mlp["kernels"][0][inv]
+        w["mlp"]["kernels"][0] = w["mlp"]["kernels"][0][inv]
         if self.use_bn:
-            mlp["bn_in"] = {k: v[inv] for k, v in mlp["bn_in"].items()}
-        w["mlp"] = mlp
-        w["out_kernel"] = p["out_kernel"].cpu().numpy()
-        w["out_bias"] = np.float32(p["out_bias"].cpu().numpy()[0])
+            w["mlp"]["bn_in"] = {k: v[inv] for k, v in w["mlp"]["bn_in"].items()}
         return w
 
 
-class DINTrainer(_StackTrainer):
+class DINTrainer(_SeqTrainer):
     """DIN training step on the device: ``libreco/algorithms/din.py:165-250`` in training mode (paper attention,
     ``libreco/layers/attention.py:28-64``; concat(user, item, sparse, dense, attention output) -> ``dense_nn`` ->
-    Dense(1)), mean sigmoid CE, TF-Adam.  One behaviour sequence per ROW (``seqs`` [R, T] padded with ``n_items``,
-    ``lens`` [R] >= 1, T <= 64).
+    Dense(1)), mean sigmoid CE, TF-Adam.  One behaviour sequence per ROW (``lens`` [R] >= 1, T <= 64).
 
         item feature table G = [item emb | its sparse embs | value x dense embs] rebuilt from the CURRENT tables
         (b200_gather_rows per item sparse field) -> K1 gather + b200_din_attention -> stack forward ->
@@ -798,36 +667,21 @@ class DINTrainer(_StackTrainer):
         b200_col_reduce) -> b200_adam_dense_dev
     """
 
-    _T = ("user_embeds", "item_embeds", "sparse_embeds", "dense_embeds")
-
-    def __init__(self, spec, weights, use_bn=True, lr=1e-3, epsilon=1e-5, device=None):
-        import torch
-
-        self._torch = torch
-        K = int(weights["user_embeds"].shape[1])
-        self.spec = spec if isinstance(spec, FeatSpec) else FeatSpec(spec, K, device)
-        self.device, self.K = self.spec.device, K
-        self.F = 2 + self.spec.n_sparse + self.spec.n_dense
-        self.n_items = self.spec.n_items
-        self.use_bn, self.lr, self.epsilon, self.t = bool(use_bn), float(lr), float(epsilon), 0
-        f32 = torch.float32
-        p = {k: _dev(weights[k], self.device, f32).clone() for k in self._T if weights.get(k) is not None}
-        self.moving = {}
-        self.n_layers = self._init_stack("", weights["mlp"], p)
-        p["out_kernel"] = _dev(np.asarray(weights["out_kernel"]).reshape(-1), self.device, f32).clone()
-        p["out_bias"] = _dev(np.asarray(weights["out_bias"]).reshape(1), self.device, f32).clone()
+    def _init_params(self, weights):
+        torch = self._torch
+        super()._init_params(weights)
+        p = self.params
         att = weights["attention"]
-        p["att_k1"] = _dev(att["k1"], self.device, f32).clone()
-        p["att_b1"] = _dev(att["b1"], self.device, f32).clone()
-        p["att_k2"] = _dev(np.asarray(att["k2"]).reshape(-1), self.device, f32).clone()
-        p["att_b2"] = _dev(np.asarray(att["b2"]).reshape(1), self.device, f32).clone()
+        p["att_k1"] = self._var(att["k1"])
+        p["att_b1"] = self._var(att["b1"])
+        p["att_k2"] = self._var(att["k2"], -1)
+        p["att_b2"] = self._var(att["b2"], 1)
         self._b2_host = float(np.asarray(att["b2"]).reshape(-1)[0])      # Dense(1) bias enters the kernels by value
         sp = self.spec
         self._is = [sp.is_[:, j].to(torch.int64).contiguous() for j in range(sp.is_.shape[1])] if sp.is_ is not None else []
         self._id = [sp.id_[:, j].contiguous() for j in range(sp.id_.shape[1])] if sp.id_ is not None else []
         self._id_cols = list(sp.item_dense_cols)
-        self.Kp = K * (1 + len(self._is) + len(self._id))
-        self._finish_init(p)
+        self.Kp = self.K * (1 + len(self._is) + len(self._id))
 
     def _build_G(self):
         torch = self._torch
@@ -848,53 +702,29 @@ class DINTrainer(_StackTrainer):
 
     def forward(self, users_d, items_d, seqs_d, lens_d):
         torch = self._torch
-        lib, st, p, K, F, Kp = _lib.lib, _lib.current_stream(), self.params, self.K, self.F, self.Kp
+        p, K, F, Kp = self.params, self.K, self.F, self.Kp
         R = int(users_d.numel())
         T = int(seqs_d.shape[1])
         G = self._build_G()
         x = torch.empty((R, F * K + Kp), dtype=torch.float32, device=self.device)
-        _lib.check(lib.b200_feat_forward(
-            ctypes.byref(self.spec.layout), ctypes.byref(self.tables), _lib.ptr(users_d), _lib.ptr(items_d), R, 0, 0,
-            _lib.ptr(x), x.stride(0), None, 0, None, None, None, 0.0, None, None, None, 0.0, None, None, 0, st))
+        feat_forward(self.spec.layout, self.tables, users_d, items_d, R, concat=x)
         rows = torch.arange(R, dtype=torch.int64, device=self.device)
         att_out = x[:, F * K:]
         # the Dense(1) bias shifts every logit of a row alike: the softmax ignores it, its gradient is exactly 0 and
         # TF-Adam never moves it — the initial value is passed by value, no device read
         b2 = self._b2_host
-        _lib.check(lib.b200_din_attention(
+        _lib.check(_lib.lib.b200_din_attention(
             _lib.ptr(G), G.stride(0), Kp, _lib.ptr(items_d), _lib.ptr(seqs_d), seqs_d.stride(0), _lib.ptr(lens_d), T,
             _lib.ptr(rows), R, 0, 0, _lib.ptr(p["att_k1"]), _lib.ptr(p["att_b1"]), _lib.ptr(p["att_k2"]), b2,
-            _lib.ptr(att_out), att_out.stride(0), st))
-        h, c = self._stack_forward("", self.n_layers, x)
-        logit = torch.empty(R, dtype=torch.float32, device=self.device)
-        _lib.check(lib.b200_concat_dense(_lib.ptr(h), h.stride(0), h.shape[1], None, 0, 0, None, 0, 0,
-                                         _lib.ptr(p["out_kernel"]), 0.0, R, _lib.ptr(logit), st))
-        logit += p["out_bias"]
-        c.update(R=R, T=T, users=users_d, items=items_d, seqs=seqs_d, lens=lens_d, rows=rows, h=h, logit=logit, G=G, b2=b2)
-        self._cache = c
-        return logit
+            _lib.ptr(att_out), att_out.stride(0), _lib.current_stream()))
+        return self._head_forward(x, T=T, users=users_d, items=items_d, seqs=seqs_d, lens=lens_d, rows=rows, G=G, b2=b2)
 
     def backward(self, labels_d):
-        from .feat_models import linear
-
         torch = self._torch
         lib, st, p, g, K, F, Kp = _lib.lib, _lib.current_stream(), self.params, self.grads, self.K, self.F, self.Kp
         c = self._cache
         R = c["R"]
-        loss = torch.empty((), dtype=torch.float32, device=self.device)
-        dlogit = torch.empty(R, dtype=torch.float32, device=self.device)
-        _lib.check(lib.b200_pointwise_loss(_lib.ptr(c["logit"]), _lib.ptr(labels_d), R, 0, 0.25, 2.0, _lib.ptr(loss),
-                                           _lib.ptr(dlogit), _lib.ptr(self._lws), self._lws.numel(), st))
-        self._col_sum(c["h"], g["out_kernel"], dlogit)
-        self._col_sum(dlogit, g["out_bias"])
-        da = linear(dlogit.view(R, 1), p["out_kernel"].view(-1, 1), None, False, cache_split=False)
-        dx = self._stack_backward("", self.n_layers, c, da)
-        gp = lambda k: _lib.ptr(g[k]) if k in g else None      # noqa: E731
-        _lib.check(lib.b200_feat_backward(
-            ctypes.byref(self.spec.layout), ctypes.byref(self.tables), _lib.ptr(c["users"]), _lib.ptr(c["items"]), R,
-            None, 0, None, 0, _lib.ptr(dx), dx.stride(0), None, None,
-            gp("user_embeds"), gp("item_embeds"), gp("sparse_embeds"), gp("dense_embeds"), None, None, None, None,
-            None, st))
+        loss, dx = self._head_backward(labels_d)
         # ---- attention backward: gradient of the item feature table + the attention weights
         G = c["G"]
         n = self.n_items + 1
@@ -920,21 +750,9 @@ class DINTrainer(_StackTrainer):
             off += K
         return loss
 
-    def step(self, users_d, items_d, seqs_d, lens_d, labels_d):
-        torch = self._torch
-        self.forward(users_d.to(torch.int64).contiguous(), items_d.to(torch.int64).contiguous(),
-                     seqs_d.to(torch.int32).contiguous(), lens_d.to(torch.int32).contiguous())
-        loss = self.backward(labels_d.to(torch.float32).contiguous())
-        _adam_update(self)
-        self._cache = None
-        return loss
-
     def export_weights(self):
         p = self.params
-        w = {k: p[k].cpu().numpy() for k in self._T if k in p}
-        w["mlp"] = self._export_stack("", self.n_layers)
-        w["out_kernel"] = p["out_kernel"].cpu().numpy()
-        w["out_bias"] = np.float32(p["out_bias"].cpu().numpy()[0])
+        w = super().export_weights()
         w["attention"] = dict(k1=p["att_k1"].cpu().numpy(), b1=p["att_b1"].cpu().numpy(), k2=p["att_k2"].cpu().numpy(),
                               b2=np.float32(p["att_b2"].cpu().numpy()[0]))
         return w

@@ -83,9 +83,10 @@ def test_training_steps_match_oracle(use_bn):
                 err = np.abs(got - ref).max()
                 assert err <= 2e-2 * lr + 1e-6, (k, err)       # first Adam step moves every touched weight by ~lr
     if use_bn:
-        for j, (mm, mv) in tr.moving.items():
-            np.testing.assert_allclose(mm.cpu().numpy(), st["moving"][f"bn{j}"][0], rtol=2e-3, atol=2e-4)
-            np.testing.assert_allclose(mv.cpu().numpy(), st["moving"][f"bn{j}"][1], rtol=2e-3, atol=2e-4)
+        assert sorted(tr.moving) == sorted(st["moving"])
+        for name, (mm, mv) in tr.moving.items():
+            np.testing.assert_allclose(mm.cpu().numpy(), st["moving"][name][0], rtol=2e-3, atol=2e-4)
+            np.testing.assert_allclose(mv.cpu().numpy(), st["moving"][name][1], rtol=2e-3, atol=2e-4)
     users, items, _ = batches[0]
     got = DeepFM(spec, tr.export_weights()).logits(users, items).cpu().numpy()
     sparse, dense = tm.row_features(spec, users, items)
