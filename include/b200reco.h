@@ -498,6 +498,24 @@ int b200_autoint_grid(const float* Xu, int64_t ldu, int64_t B, const float* Xi, 
                       const int32_t* head_dims_host, const float* weights, const float* w_out, float b_out,
                       int32_t use_residual, float* scores, int64_t ld_scores, void* stream);
 
+/* ---- AutoInt training: the attention core of one layer (layers/attention.py:67-125) ----------------
+ * Q, K, V, O: [R*F, ld] row-major, row r*F + f = field f of batch row r, columns head-major (h * hd + j).
+ * Per (row r, head h):  S = scale * Q_h K_h^T [F, F],  P = softmax_rows(S),  O_h = P V_h,
+ * lse[(r * H + h) * F + f] = log sum_g exp(S_fg)  (float [R, H, F]).  P itself is never stored.
+ * The backward recomputes P from Q, K and lse and WRITES (does not add)
+ *   dV_h = P^T dO_h,  dS = P o (dO_h V_h^T - rowsum(dO_h o O_h)),  dQ_h = scale dS K_h,  dK_h = scale dS^T Q_h
+ * into dQ, dK, dV [R*F, ldg].  One warp owns one (row, head) and accumulates on chip: no atomics, and two
+ * identical calls give identical bits.
+ * Supported: 2 <= F <= 130, num_heads >= 1, head_dim >= 1, num_heads * head_dim <= 64, every stride >= that
+ * product, a finite scale; anything else returns -2 before launching. */
+int b200_autoint_attention_forward(const float* Q, int64_t ldq, const float* K, int64_t ldk, const float* V,
+                                   int64_t ldv, int64_t R, int32_t F, int32_t num_heads, int32_t head_dim,
+                                   float scale, float* O, int64_t ldo, float* lse, void* stream);
+int b200_autoint_attention_backward(const float* Q, int64_t ldq, const float* K, int64_t ldk, const float* V,
+                                    int64_t ldv, const float* O, int64_t ldo, const float* lse, const float* dO,
+                                    int64_t lddo, int64_t R, int32_t F, int32_t num_heads, int32_t head_dim,
+                                    float scale, float* dQ, float* dK, float* dV, int64_t ldg, void* stream);
+
 /* ---- a14: predict_from_embedding (libreco/prediction/predict.py:36-40) -----------------
  * out[r] = sum_k U[users[r],k] * I[items[r],k]; mode 0: raw, 1: expit (ranking),
  * 2: clip to [lo, hi] (rating) — normalize_prediction (:18-23). */

@@ -117,6 +117,10 @@ SIGNATURES = {
                                   _P, _P]),
     "b200_autoint_grid": (c_int, [_P, c_int64, c_int64, _P, c_int64, c_int64, _P, c_int32, c_int32, c_int32, c_int32, _P,
                                   _P, _P, c_float, c_int32, _P, c_int64, _P]),
+    "b200_autoint_attention_forward": (c_int, [_P, c_int64, _P, c_int64, _P, c_int64, c_int64, c_int32, c_int32,
+                                               c_int32, c_float, _P, c_int64, _P, _P]),
+    "b200_autoint_attention_backward": (c_int, [_P, c_int64, _P, c_int64, _P, c_int64, _P, c_int64, _P, _P, c_int64,
+                                                c_int64, c_int32, c_int32, c_int32, c_float, _P, _P, _P, c_int64, _P]),
 }
 
 for _name, (_res, _args) in SIGNATURES.items():

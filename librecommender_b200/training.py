@@ -105,6 +105,33 @@ class _Trainer:
                                                 _lib.current_stream()))
         return loss, dlogit
 
+    def _col_sum(self, X, out, wrow=None):
+        X2 = X if X.dim() == 2 else X.view(-1, 1)
+        _lib.check(_lib.lib.b200_col_reduce(_lib.ptr(X2), X2.stride(0), X2.shape[0], X2.shape[1], _lib.ptr(wrow), None, 0,
+                                            _lib.ptr(out), _lib.current_stream()))
+
+    def _dense1_forward(self, h):
+        """Logits of the Dense(1) head (variables ``out_kernel`` [C], ``out_bias`` [1]) on ``h`` [R, C]."""
+        torch = self._torch
+        p = self.params
+        R = int(h.shape[0])
+        logit = torch.empty(R, dtype=torch.float32, device=self.device)
+        _lib.check(_lib.lib.b200_concat_dense(_lib.ptr(h), h.stride(0), h.shape[1], None, 0, 0, None, 0, 0,
+                                              _lib.ptr(p["out_kernel"]), 0.0, R, _lib.ptr(logit), _lib.current_stream()))
+        logit += p["out_bias"]                      # device scalar add (the bias is a trainable variable)
+        return logit
+
+    def _dense1_backward(self, h, logit, labels_d):
+        """Loss and the Dense(1) head's gradients (written into ``grads``); returns (loss, d loss / d h)."""
+        p, g = self.params, self.grads
+        R = int(h.shape[0])
+        loss, dlogit = self._loss(logit, labels_d)
+        self._col_sum(h, g["out_kernel"], dlogit)
+        self._col_sum(dlogit, g["out_bias"])
+        # d h = dlogit (x) out_kernel: the Dense(1) transposed, on the library's dense kernel (din = 1)
+        dh = linear(dlogit.view(R, 1), p["out_kernel"].view(-1, 1), None, False, cache_split=False)
+        return loss, dh
+
     def _device_counters(self):
         """The Adam step counter and step size live on the device (allocated outside any graph capture)."""
         if getattr(self, "_step_dev", None) is None:
@@ -303,11 +330,6 @@ class _StackTrainer(_Trainer):
             _lib.ptr(g[f"{name}_gamma"]), _lib.ptr(g[f"{name}_beta"]), _lib.ptr(ws), ws.numel() * 8,
             _lib.current_stream()))
         return dx
-
-    def _col_sum(self, X, out, wrow=None):
-        X2 = X if X.dim() == 2 else X.view(-1, 1)
-        _lib.check(_lib.lib.b200_col_reduce(_lib.ptr(X2), X2.stride(0), X2.shape[0], X2.shape[1], _lib.ptr(wrow), None, 0,
-                                            _lib.ptr(out), _lib.current_stream()))
 
     def _stack_forward(self, prefix, n_layers, x):
         """BN(input) -> [Dense -> ReLU -> BN] x (L-1) -> Dense with batch statistics; returns (out, cache)."""
@@ -559,27 +581,18 @@ class _SeqTrainer(_StackTrainer):
 
     def _head_forward(self, x, **cache):
         """Stack + Dense(1) on the filled input ``x``; caches what the backward needs and returns the logits."""
-        torch = self._torch
-        p = self.params
         R = int(x.shape[0])
         h, c = self._stack_forward("", self.n_layers, x)
-        logit = torch.empty(R, dtype=torch.float32, device=self.device)
-        _lib.check(_lib.lib.b200_concat_dense(_lib.ptr(h), h.stride(0), h.shape[1], None, 0, 0, None, 0, 0,
-                                              _lib.ptr(p["out_kernel"]), 0.0, R, _lib.ptr(logit), _lib.current_stream()))
-        logit += p["out_bias"]                      # device scalar add (the bias is a trainable variable)
+        logit = self._dense1_forward(h)
         c.update(R=R, h=h, logit=logit, **cache)
         self._cache = c
         return logit
 
     def _head_backward(self, labels_d):
         """Loss, the gradients of the head, the stack and the field tables; returns (loss, d loss / d input)."""
-        p, g, c = self.params, self.grads, self._cache
+        g, c = self.grads, self._cache
         R = c["R"]
-        loss, dlogit = self._loss(c["logit"], labels_d)
-        self._col_sum(c["h"], g["out_kernel"], dlogit)
-        self._col_sum(dlogit, g["out_bias"])
-        # d h = dlogit (x) out_kernel: the Dense(1) transposed, on the library's dense kernel (din = 1)
-        da = linear(dlogit.view(R, 1), p["out_kernel"].view(-1, 1), None, False, cache_split=False)
+        loss, da = self._dense1_backward(c["h"], c["logit"], labels_d)
         dx = self._stack_backward("", self.n_layers, c, da)
         feat_backward(self.spec.layout, self.tables, c["users"], c["items"], R, g, dconcat=dx)
         return loss, dx
@@ -755,4 +768,173 @@ class DINTrainer(_SeqTrainer):
         w = super().export_weights()
         w["attention"] = dict(k1=p["att_k1"].cpu().numpy(), b1=p["att_b1"].cpu().numpy(), k2=p["att_k2"].cpu().numpy(),
                               b2=np.float32(p["att_b2"].cpu().numpy()[0]))
+        return w
+
+
+class AutoIntTrainer(_Trainer):
+    """AutoInt training step on the device: ``libreco/algorithms/autoint.py:146-168`` in training mode (the fields
+    [user, item, sparse.., dense..] stacked into X [F, K], L layers of ``multi_head_attention(X, X)``
+    (``libreco/layers/attention.py:67-125``, optionally ``X + mha(X)``), Flatten, Dense(1)), mean sigmoid CE,
+    TF-Adam.  The graph has no BN and no dropout; ``reg`` applies to the embedding tables only.
+
+        K1 gather (b200_feat_forward, X as [R*F, K]) -> per layer: Q, K, V projections over R*F rows
+        (b200_linear_*) -> b200_autoint_attention_forward -> output projection (b200_linear_*) -> residual add
+        (b200_axpy) -> b200_concat_dense -> b200_pointwise_loss -> the reverse, with
+        b200_autoint_attention_backward for the attention core and the dense kernels for every projection's input
+        and weight gradient -> b200_feat_backward (scatter into the tables) -> b200_adam_dense_dev
+
+    ``weights``: the RAW variables of either graph, as ``synthetic.make_autoint_weights`` makes them (the tables,
+    ``autoint_scheme``, ``autoint_mha``, ``num_heads``, ``use_residual``, ``out_kernel``, ``out_bias``).  Each
+    scheme trains its own variables: keras ``query`` / ``key`` / ``value`` [K, H, hd] (held as [K, D]) and
+    ``attention_output`` [H, hd, K] (held as [D, K]); legacy ``query`` / ``key`` [K, D], ``value`` [D, D]
+    applied to the projected keys (V = (X Wk) Wv', so Wk is trained through both of its paths) and ``output``
+    [D, K].  ``export_weights`` returns the same raw layout and scheme.
+
+    Multi-sparse fields must use the combiner "normal" (every member its own field): the pooling backward is not
+    built.  Shapes outside the attention kernels' envelope (F <= 130, K <= 64, H * hd <= 64, 1..4 layers) raise
+    ``ValueError`` before anything is launched."""
+
+    def __init__(self, spec, weights, lr=1e-3, epsilon=1e-5, device=None):
+        from .feat_models import _spec_get
+
+        g = _spec_get(spec) if not isinstance(spec, FeatSpec) else (lambda k, d=None: d)
+        if g("multi_sparse_combine_info") is not None and weights.get("multi_sparse_combiner", "sqrtn") != "normal":
+            raise ValueError("AutoIntTrainer: multi-sparse fields need the combiner \"normal\"; the pooling backward "
+                             "is not built")
+        super().__init__(spec, weights, False, lr, epsilon, device)
+
+    def _init_params(self, weights):
+        from .feat_models import AUTOINT_MAX_D, AUTOINT_MAX_F, AUTOINT_MAX_K, AUTOINT_MAX_LAYERS
+        from .weights_io import AUTOINT_SCHEMES
+
+        p, K, F = self.params, self.K, self.F
+        self.scheme = weights["autoint_scheme"]
+        H = self.H = int(weights["num_heads"])
+        self.use_residual = bool(weights.get("use_residual", True))
+        self._combiner = weights.get("multi_sparse_combiner")
+        mha = list(weights["autoint_mha"])
+        if self.scheme not in AUTOINT_SCHEMES:
+            raise ValueError(f"AutoIntTrainer: unknown naming scheme `{self.scheme}`")
+        if K > AUTOINT_MAX_K or F > AUTOINT_MAX_F or not 1 <= len(mha) <= AUTOINT_MAX_LAYERS or H < 1:
+            raise ValueError(f"AutoIntTrainer: K {K}, F {F}, {len(mha)} layers, {H} heads outside K <= "
+                             f"{AUTOINT_MAX_K}, F <= {AUTOINT_MAX_F}, 1..{AUTOINT_MAX_LAYERS} layers, heads >= 1")
+        self.names = ("query", "key", "value", "attention_output" if self.scheme == "keras" else "output")
+        self.head_dims = []
+        for l, lw in enumerate(mha):
+            q = np.asarray(lw["query"])
+            D = int(np.prod(q.shape[1:]))
+            hd = D // H
+            if self.scheme == "keras":
+                want = [(K, H, hd), (K, H, hd), (K, H, hd), (H, hd, K)]
+                views = [(K, D), (K, D), (K, D), (D, K)]
+            else:
+                want = views = [(K, D), (K, D), (D, D), (D, K)]
+            got = [tuple(np.shape(lw[n])) for n in self.names]
+            if D % H or not 1 <= D <= AUTOINT_MAX_D or got != [tuple(s) for s in want]:
+                raise ValueError(f"AutoIntTrainer layer {l}: shapes {got} with {H} heads, expected {want} and "
+                                 f"num_heads x head size <= {AUTOINT_MAX_D}")
+            for n, shp in zip(self.names, views):
+                p[f"mha{l}_{n}"] = self._var(lw[n], shp)
+            self.head_dims.append(hd)
+        if np.size(weights["out_kernel"]) != F * K:
+            raise ValueError(f"AutoIntTrainer: out_kernel has {np.size(weights['out_kernel'])} entries, expected "
+                             f"F*K = {F}*{K}")
+        p["out_kernel"] = self._var(weights["out_kernel"], -1)
+        p["out_bias"] = self._var(weights["out_bias"], 1)
+
+    def _axpy(self, y, x):
+        """y += x (same shapes, contiguous) on the library's kernel."""
+        _lib.check(_lib.lib.b200_axpy(_lib.ptr(y), _lib.ptr(x), 1.0, y.numel(), _lib.current_stream()))
+
+    def forward(self, users_d, items_d):
+        """Training-mode logits of the batch; caches what the backward needs."""
+        torch = self._torch
+        p, K, F, H = self.params, self.K, self.F, self.H
+        R = int(users_d.numel())
+        f32, dev = torch.float32, self.device
+        x = torch.empty((R, F * K), dtype=f32, device=dev)
+        feat_forward(self.spec.layout, self.tables, users_d, items_d, R, concat=x)
+        X = x.view(R * F, K)
+        layers = []
+        for l, hd in enumerate(self.head_dims):
+            wq, wk, wv, wo = (p[f"mha{l}_{n}"] for n in self.names)
+            D = H * hd
+            q = linear(X, wq.t().contiguous(), None, False, cache_split=False)
+            k = linear(X, wk.t().contiguous(), None, False, cache_split=False)
+            v = linear(k if self.scheme == "legacy" else X, wv.t().contiguous(), None, False, cache_split=False)
+            o = torch.empty((R * F, D), dtype=f32, device=dev)
+            lse = torch.empty(R * H * F, dtype=f32, device=dev)
+            _lib.check(_lib.lib.b200_autoint_attention_forward(
+                _lib.ptr(q), q.stride(0), _lib.ptr(k), k.stride(0), _lib.ptr(v), v.stride(0), R, F, H, hd,
+                float(1.0 / np.sqrt(hd)), _lib.ptr(o), o.stride(0), _lib.ptr(lse), _lib.current_stream()))
+            y = linear(o, wo.t().contiguous(), None, False, cache_split=False)
+            if self.use_residual:
+                self._axpy(y, X)
+            layers.append(dict(x=X, q=q, k=k, v=v, o=o, lse=lse))
+            X = y
+        h = X.view(R, F * K)
+        logit = self._dense1_forward(h)
+        self._cache = dict(R=R, users=users_d, items=items_d, layers=layers, h=h, logit=logit)
+        return logit
+
+    def backward(self, labels_d):
+        """Loss + every gradient buffer filled (before the optimiser); returns the device loss."""
+        torch = self._torch
+        p, g, K, F, H = self.params, self.grads, self.K, self.F, self.H
+        c = self._cache
+        R = c["R"]
+        loss, dh = self._dense1_backward(c["h"], c["logit"], labels_d)
+        dX = dh.view(R * F, K)
+        for l in range(len(self.head_dims) - 1, -1, -1):
+            hd, a = self.head_dims[l], c["layers"][l]
+            nq, nk, nv, no = (f"mha{l}_{n}" for n in self.names)
+            D = H * hd
+            dY = dX
+            g[no] += _weight_grad(dY, a["o"]).t()                     # dWo = O^T dY
+            dO = linear(dY, p[no], None, False, cache_split=False)     # dO = dY Wo^T
+            dq, dk, dv = (torch.empty((R * F, D), dtype=torch.float32, device=self.device) for _ in range(3))
+            _lib.check(_lib.lib.b200_autoint_attention_backward(
+                _lib.ptr(a["q"]), a["q"].stride(0), _lib.ptr(a["k"]), a["k"].stride(0), _lib.ptr(a["v"]),
+                a["v"].stride(0), _lib.ptr(a["o"]), a["o"].stride(0), _lib.ptr(a["lse"]), _lib.ptr(dO), dO.stride(0),
+                R, F, H, hd, float(1.0 / np.sqrt(hd)), _lib.ptr(dq), _lib.ptr(dk), _lib.ptr(dv), D,
+                _lib.current_stream()))
+            if self.scheme == "legacy":                                # V = Kproj Wv': Wk gets the V path too
+                g[nv] += _weight_grad(dv, a["k"]).t()                 # dWv' = Kproj^T dV
+                self._axpy(dk, linear(dv, p[nv], None, False, cache_split=False))
+            g[nq] += _weight_grad(dq, a["x"]).t()
+            g[nk] += _weight_grad(dk, a["x"]).t()
+            dXn = linear(dq, p[nq], None, False, cache_split=False)
+            self._axpy(dXn, linear(dk, p[nk], None, False, cache_split=False))
+            if self.scheme == "keras":
+                g[nv] += _weight_grad(dv, a["x"]).t()
+                self._axpy(dXn, linear(dv, p[nv], None, False, cache_split=False))
+            if self.use_residual:
+                self._axpy(dXn, dY)
+            dX = dXn
+        feat_backward(self.spec.layout, self.tables, c["users"], c["items"], R, g, dconcat=dX.view(R, F * K))
+        return loss
+
+    def step(self, users_d, items_d, labels_d):
+        """One optimisation step on (users, items, labels) device tensors; returns the device loss."""
+        torch = self._torch
+        self.forward(users_d.to(torch.int64).contiguous(), items_d.to(torch.int64).contiguous())
+        loss = self.backward(labels_d.to(torch.float32).contiguous())
+        self._adam_update()
+        self._cache = None
+        return loss
+
+    def export_weights(self):
+        """The raw variables in the scheme they came in (``weights_io.autoint_weights`` makes the inference dict)."""
+        p, K, H = self.params, self.K, self.H
+        w = self._export_tables()
+        mha = []
+        for l, hd in enumerate(self.head_dims):
+            lw = {n: p[f"mha{l}_{n}"].cpu().numpy() for n in self.names}
+            if self.scheme == "keras":
+                lw = {n: a.reshape((H, hd, K) if n == "attention_output" else (K, H, hd)) for n, a in lw.items()}
+            mha.append(lw)
+        w.update(autoint_scheme=self.scheme, autoint_mha=mha, num_heads=H, use_residual=self.use_residual,
+                 out_kernel=p["out_kernel"].cpu().numpy().reshape(-1, 1), out_bias=p["out_bias"].cpu().numpy().reshape(1))
+        if self._combiner is not None:
+            w["multi_sparse_combiner"] = self._combiner
         return w

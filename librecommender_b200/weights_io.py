@@ -248,6 +248,22 @@ def autoint_weights(raw):
     return w
 
 
+def autoint_tf_variables(raw):
+    """Raw AutoInt variables of either graph (the layout :func:`autoint_weights` takes, e.g.
+    ``training.AutoIntTrainer.export_weights()``) -> ``{TF variable name: array}`` named by
+    :func:`default_tf_names` for the raw dict's scheme: what ``save_tf_variables`` writes as
+    ``<name>_tf_variables.npz``, and the inverse of ``load_reference_tf_model(..., "AutoInt")``."""
+    mha = raw["autoint_mha"]
+    names = default_tf_names("AutoInt", None, False, n_layers=len(mha), scheme=raw["autoint_scheme"])
+    out = to_tf_variables({k: raw[k] for k in EMBEDDING_SCOPE if k in raw})
+    for lw, ln in zip(mha, names["autoint_mha"]):
+        for k, n in ln.items():
+            out[n] = np.asarray(lw[k], dtype=np.float32)
+    out[names["out_kernel"]] = np.asarray(raw["out_kernel"], dtype=np.float32).reshape(-1, 1)
+    out[names["out_bias"]] = np.asarray(raw["out_bias"], dtype=np.float32).reshape(1)
+    return out
+
+
 def load_reference_tf_model(path, model_name, arch, n_hidden, use_bn, use_tf_attention=False, extra_names=None,
                             num_heads=2, att_embed_size=(8, 8, 8), use_residual=True):
     """Engine weight dict of a model saved by the reference (``save_tf_variables``,
