@@ -371,6 +371,23 @@ int b200_softmax_inbatch_loss(float* S, int64_t lds, int32_t B, float temperatur
                               const int64_t* item_ids, int32_t write_grad, float* loss_out, void* workspace,
                               size_t workspace_bytes, void* stream);
 
+/* Sampled-class losses of YouTubeRetrieval training (tf.nn.sampled_softmax_loss / tf.nn.nce_loss, reference
+ * libreco/training/tf_trainer.py:162-235; TensorFlow's _compute_sampled_logits with remove_accidental_hits=True and
+ * subtract_log_q=True).  logits [B, ld] holds U W_s^T (the S sampled classes) on entry, true_dot[B] = <u_r, w_label>.
+ *   z0 = true_dot[r] + bias[label] - log E(label),  z_s = logits[r, s] + bias[id_s] - log E(id_s),
+ * E = TensorFlow's expected count in float: p S if *num_tries == S, else -expm1(num_tries log1p(-p)), with p = 1/n_items
+ * (sampler_kind 0, uniform) or log((c+2)/(c+1)) / log1p(n_items) (1, log-uniform).  A sampled id equal to the row's
+ * label is an accidental hit and contributes exactly nothing.  loss_kind 0: softmax CE over [z0, z_s..] with the
+ * label in column 0; 1 (NCE): sigmoid CE(z0, 1) + sum_s sigmoid CE(z_s, 0).  *loss_out = mean over the B rows
+ * (device scalar; deterministic two-stage reduction); logits is overwritten with d loss / d z_s and dtrue[r] =
+ * d loss / d z0.  num_tries: device scalar (b200_unique_candidates).  1 <= S <= min(n_items, 65536), ld >= S;
+ * workspace >= b200_sampled_class_loss_workspace_bytes(B, S). */
+size_t b200_sampled_class_loss_workspace_bytes(int32_t B, int32_t S);
+int b200_sampled_class_loss(int32_t loss_kind, float* logits, int64_t ld, int32_t B, int32_t S, const float* true_dot,
+                            const int64_t* labels, const int64_t* sampled, const float* bias, int32_t sampler_kind,
+                            int64_t n_items, const int64_t* num_tries, float* loss_out, float* dtrue, void* workspace,
+                            size_t workspace_bytes, void* stream);
+
 /* out[r] = bias + <[a[r,:na], b[r,:nb], c[r,:nc]], w>: Dense(1) on a concatenation
  * (deepfm.py:172-173; the final Dense(1) of DIN / YouTubeRanking). */
 int b200_concat_dense(const float* a, int64_t lda, int32_t na, const float* b, int64_t ldb, int32_t nb,
@@ -463,6 +480,21 @@ int b200_sample_negatives(const int64_t* users, const int64_t* items_pos, int64_
                           uint64_t seed, uint64_t step, const int64_t* indptr,
                           const int32_t* idx_sorted, int64_t n_users, const float* cdf, int64_t* out,
                           void* stream);
+
+/* Unique candidate sampler of the sampled-class losses: TensorFlow's uniform_candidate_sampler (kind 0) /
+ * log_uniform_candidate_sampler (kind 1) with unique=True.  Draws with replacement and keeps first occurrences
+ * until it holds num_sampled = S distinct ids: out[0..S) = those ids in draw order, *num_tries (device int64) =
+ * the number of draws taken.  Draw j = Philox4x32-10(seed, step, j) with step = *step_dev (a DEVICE counter, e.g.
+ * the Adam step of b200_adam_begin_step, so a captured CUDA graph draws fresh candidates on every replay);
+ * uniform: the bounded 64-bit draw of b200_sample_negatives; log-uniform: (int64)exp(u log1p(n_items)) - 1, then
+ * % n_items, u = 53 random bits in [0, 1).  The result equals the sequential process over that draw stream.  One
+ * launch, no host round trip.  workspace: b200_unique_candidates_workspace_bytes(n_items) bytes, filled with 0xFF
+ * before the FIRST call; every call leaves it that way again (O(S) work).  Envelope: 1 <= n_items < 2^31,
+ * 1 <= S <= min(n_items, 65536); anything else returns -2 before launching. */
+#define B200_UNIQUE_MAX_SAMPLED 65536
+size_t b200_unique_candidates_workspace_bytes(int64_t n_items);
+int b200_unique_candidates(int32_t kind, int64_t n_items, int32_t num_sampled, uint64_t seed, const int64_t* step_dev,
+                           void* workspace, size_t workspace_bytes, int64_t* out, int64_t* num_tries, void* stream);
 
 /* a11: per-sample behaviour sequences at collate time (libreco/batch/sequence.py:33-71, mode
  * "recent"; called from batch/collators.py:207-222).  consumed CSR in ARRIVAL order.  position =

@@ -86,6 +86,11 @@ SIGNATURES = {
     "b200_pairwise_loss": (c_int, [_P, c_int64, _P, c_int64, c_int32, c_float, c_float, c_float, c_int32, _P, _P, _P,
                                    _P, c_size_t, _P]),
     "b200_softmax_inbatch_loss": (c_int, [_P, c_int64, c_int32, c_float, _P, _P, c_int32, _P, _P, c_size_t, _P]),
+    "b200_sampled_class_loss_workspace_bytes": (c_size_t, [c_int32, c_int32]),
+    "b200_sampled_class_loss": (c_int, [c_int32, _P, c_int64, c_int32, c_int32, _P, _P, _P, _P, c_int32, c_int64, _P,
+                                        _P, _P, _P, c_size_t, _P]),
+    "b200_unique_candidates_workspace_bytes": (c_size_t, [c_int64]),
+    "b200_unique_candidates": (c_int, [c_int32, c_int64, c_int32, c_uint64, _P, _P, c_size_t, _P, _P, _P]),
     "b200_concat_dense": (c_int, [_P, c_int64, c_int32, _P, c_int64, c_int32, _P, c_int64, c_int32, _P, c_float,
                                   c_int64, _P, _P]),
     "b200_l2_normalize_rows": (c_int, [_P, c_int64, c_int64, c_int32, _P]),

@@ -6,6 +6,8 @@
 //   pairwise : torchops/loss.py:22-60 (bpr_loss, max_margin_loss, pairwise_bce_loss,
 //              pairwise_focal_loss), tfops/loss.py:61-64 (max-margin of the TF two-tower models)
 //   in-batch softmax: tfops/loss.py:67-71 + TwoTower.adjust_logits (algorithms/two_tower.py:458-479)
+//   sampled softmax / NCE over sampled classes: training/tf_trainer.py:162-245 (YouTubeRetrieval;
+//              tf.nn.sampled_softmax_loss / nce_loss with TensorFlow's expected counts)
 #include "common.cuh"
 #include "../../include/b200reco.h"
 
@@ -181,6 +183,86 @@ softmax_rows_kernel(float* __restrict__ S, int64_t lds, int B, float inv_temp, c
   block_sum_store(acc, partial);
 }
 
+// ---- sampled-class losses of YouTubeRetrieval (tf.nn.sampled_softmax_loss / tf.nn.nce_loss through
+// _compute_sampled_logits, remove_accidental_hits=True, subtract_log_q=True) -----------------------------------
+// TensorFlow's ExpectedCountHelper (range_sampler.cc) in float: p S when every draw was distinct, else
+// -expm1(num_tries log1p(-p)); p = 1 / n_items (uniform, the sampler's float inv_range) or
+// log((c + 2) / (c + 1)) / log1p(n_items) (log-uniform, double, then float).
+__device__ __forceinline__ float expected_count(int sampler_kind, int64_t c, int64_t n_items, int S, int64_t tries) {
+  const float p = sampler_kind == 0 ? (float)(1.0 / (double)n_items)
+                                    : (float)(log((c + 2.0) / (c + 1.0)) / log1p((double)n_items));
+  if (tries == (int64_t)S) return p * (float)S;
+  return -expm1f((float)tries * log1pf(-p));
+}
+
+// adj[i] = bias[id] - log E(id) for the S sampled ids, then the B labels
+__global__ void __launch_bounds__(THREADS)
+sampled_adjust_kernel(const int64_t* __restrict__ sampled, int S, const int64_t* __restrict__ labels, int B,
+                      const float* __restrict__ bias, int sampler_kind, int64_t n_items,
+                      const int64_t* __restrict__ num_tries, float* __restrict__ adj) {
+  const int i = blockIdx.x * THREADS + threadIdx.x;
+  if (i >= S + B) return;
+  const int64_t id = i < S ? sampled[i] : labels[i - S];
+  adj[i] = bias[id] - logf(expected_count(sampler_kind, id, n_items, S, *num_tries));
+}
+
+// One warp per row r: z0 = true_dot[r] + adj[S + r] (the label, column 0), z_s = L[r, s] + adj[s]; a sampled id
+// equal to the row's label is an accidental hit (TensorFlow adds -FLT_MAX: it contributes exactly nothing, so it
+// is skipped here and its gradient is 0).  kind 0 softmax CE over [z0, z_s] (online max / sum per lane, merged in
+// a fixed shuffle tree), kind 1 NCE: sigmoid CE(z0, 1) + sum_s sigmoid CE(z_s, 0).  L is overwritten with
+// d(mean loss) / d z_s, dtrue[r] = d(mean loss) / d z0.
+__global__ void __launch_bounds__(THREADS)
+sampled_rows_kernel(float* __restrict__ L, int64_t ldl, int B, int S, int kind, const float* __restrict__ true_dot,
+                    const int64_t* __restrict__ labels, const int64_t* __restrict__ sampled,
+                    const float* __restrict__ adj, float inv_B, float* __restrict__ dtrue,
+                    double* __restrict__ partial) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wpb = THREADS / 32;
+  float acc = 0.f;
+  for (int r = blockIdx.x * wpb + warp; r < B; r += gridDim.x * wpb) {
+    float* row = L + (int64_t)r * ldl;
+    const int64_t lab = labels[r];
+    const float z0 = true_dot[r] + adj[S + r];
+    float loss, d0;
+    if (kind == 0) {
+      float m = z0, s = 0.f;
+      for (int c = lane; c < S; c += 32) {
+        if (sampled[c] == lab) continue;
+        const float z = row[c] + adj[c];
+        if (z > m) { s = s * expf(m - z) + 1.f; m = z; }
+        else s += expf(z - m);
+      }
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) {
+        const float m2 = __shfl_xor_sync(0xffffffffu, m, o), s2 = __shfl_xor_sync(0xffffffffu, s, o);
+        const float mm = fmaxf(m, m2);
+        s = s * expf(m - mm) + s2 * expf(m2 - mm);
+        m = mm;
+      }
+      const float lse = m + logf(s + expf(z0 - m));
+      loss = lse - z0;
+      d0 = (expf(z0 - lse) - 1.f) * inv_B;
+      for (int c = lane; c < S; c += 32)
+        row[c] = sampled[c] == lab ? 0.f : expf(row[c] + adj[c] - lse) * inv_B;
+    } else {
+      float ls = 0.f;
+      for (int c = lane; c < S; c += 32) {
+        if (sampled[c] == lab) { row[c] = 0.f; continue; }
+        const float z = row[c] + adj[c];
+        ls += bce(z, 0.f);
+        row[c] = sigmoidf(z) * inv_B;
+      }
+      loss = warp_sum(ls) + bce(z0, 1.f);
+      d0 = (sigmoidf(z0) - 1.f) * inv_B;
+    }
+    if (lane == 0) {
+      acc += loss;
+      dtrue[r] = d0;
+    }
+  }
+  block_sum_store(acc, partial);
+}
+
 static inline int grid_for(int64_t n) {
   int64_t b = (n + THREADS - 1) / THREADS;
   if (b < 1) b = 1;
@@ -259,5 +341,40 @@ extern "C" int b200_softmax_inbatch_loss(float* S, int64_t lds, int32_t B, float
   final_sum_kernel<<<1, 256, 0, st>>>((const double*)workspace, g, 1.0 / (double)B, loss_out);
   B200_CUDA_OK(cudaGetLastError());
   count_launch(2);
+  return 0;
+}
+
+extern "C" size_t b200_sampled_class_loss_workspace_bytes(int32_t B, int32_t S) {
+  return b200_loss_workspace_bytes() + (size_t)(B > 0 ? B : 0) * 4 + (size_t)(S > 0 ? S : 0) * 4;
+}
+
+extern "C" int b200_sampled_class_loss(int32_t loss_kind, float* logits, int64_t ld, int32_t B, int32_t S,
+                                       const float* true_dot, const int64_t* labels, const int64_t* sampled,
+                                       const float* bias, int32_t sampler_kind, int64_t n_items,
+                                       const int64_t* num_tries, float* loss_out, float* dtrue, void* workspace,
+                                       size_t workspace_bytes, void* stream) {
+  B200_REQUIRE(loss_kind == 0 || loss_kind == 1, "b200_sampled_class_loss: loss kind must be 0 (softmax) or 1 (nce)");
+  B200_REQUIRE(sampler_kind == 0 || sampler_kind == 1,
+               "b200_sampled_class_loss: sampler kind must be 0 (uniform) or 1 (log-uniform)");
+  B200_REQUIRE(B >= 1 && S >= 1 && S <= B200_UNIQUE_MAX_SAMPLED && ld >= S && n_items >= S,
+               "b200_sampled_class_loss: bad shape B %d, S %d, ld %lld, n_items %lld", B, S, (long long)ld,
+               (long long)n_items);
+  B200_REQUIRE(logits && true_dot && labels && sampled && bias && num_tries && loss_out && dtrue,
+               "b200_sampled_class_loss: null pointer");
+  B200_REQUIRE(workspace && workspace_bytes >= b200_sampled_class_loss_workspace_bytes(B, S),
+               "b200_sampled_class_loss: workspace too small");
+  cudaStream_t st = (cudaStream_t)stream;
+  double* partial = (double*)workspace;
+  float* adj = (float*)((char*)workspace + b200_loss_workspace_bytes());
+  sampled_adjust_kernel<<<(unsigned)ceil_div64((int64_t)S + B, THREADS), THREADS, 0, st>>>(
+      sampled, S, labels, B, bias, sampler_kind, n_items, num_tries, adj);
+  const int wpb = THREADS / 32;
+  int g = (B + wpb - 1) / wpb;
+  if (g > MAX_BLOCKS) g = MAX_BLOCKS;
+  sampled_rows_kernel<<<g, THREADS, 0, st>>>(logits, ld, B, S, loss_kind, true_dot, labels, sampled, adj,
+                                             1.f / (float)B, dtrue, partial);
+  final_sum_kernel<<<1, 256, 0, st>>>(partial, g, 1.0 / (double)B, loss_out);
+  B200_CUDA_OK(cudaGetLastError());
+  count_launch(3);
   return 0;
 }

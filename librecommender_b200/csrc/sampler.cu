@@ -17,6 +17,8 @@
 //   mode 2 "popular"    (negatives.py:34-43): inverse-CDF draw from p ~ freq^0.75 (cdf given),
 //                        one re-draw when equal to the positive.
 // Layout: negatives of positive j are out[j*num_neg : (j+1)*num_neg] (collators.py:231-232).
+// Also here: the per-sample history windows (b200_interacted_seqs) and the unique candidate sampler of the
+// sampled-class losses (b200_unique_candidates, training/tf_trainer.py:162-245).
 #include "common.cuh"
 #include "../../include/b200reco.h"
 
@@ -163,10 +165,102 @@ __global__ void interacted_seqs_kernel(const int64_t* __restrict__ indptr, const
   if (lane == 0) lens[j] = pos == 0 ? 1 : (int32_t)count;
 }
 
+// ---- unique candidate sampler of the sampled-class losses (YouTubeRetrieval training): TensorFlow's
+// uniform_candidate_sampler / log_uniform_candidate_sampler with unique=True (range_sampler.cc SampleBatch...):
+// draws with replacement, keeps the FIRST occurrence of every id until S distinct ids are held, num_tries = the
+// number of draws taken.  Draw j is Philox(seed, step, j); the result is that sequential process over the draw
+// stream.  One CTA: a round draws j = base .. base + blockDim - 1, every draw claims its id in owner[] with
+// atomicMin(j) (the lowest draw index of the round wins a tie, an id owned by an earlier round keeps its owner),
+// a draw is fresh iff it owns its id, and a block scan over the fresh flags gives the output ranks in draw order.
+// owner[] (one uint32 per item, 0xFFFFFFFF = free) is left free again by walking the S kept ids and the last
+// round's draws after the stop: O(S) per call, never O(n_items).
+constexpr int UNIQ_THREADS = 1024;
+constexpr uint32_t UNIQ_FREE = 0xFFFFFFFFu;
+constexpr uint32_t UNIQ_MAX_DRAWS = 1u << 31;
+
+__device__ __forceinline__ int64_t candidate(int kind, int64_t n_items, double log_range, uint64_t seed,
+                                             uint64_t step, uint32_t j) {
+  U4 c;
+  c.x = j; c.y = 0u; c.z = 0xca7du; c.w = (uint32_t)step;
+  const U4 r = philox4x32_10(c, (uint32_t)seed, (uint32_t)(seed >> 32) ^ (uint32_t)(step >> 32));
+  if (kind == 0) return bounded(r.x, r.y, n_items);
+  // LogUniformSampler::Sample: (int64)exp(u * log1p(range)) - 1, then % range; u = 53 random bits in [0, 1)
+  const double u = (double)((((uint64_t)r.z << 32) | r.w) >> 11) * 0x1.0p-53;
+  const int64_t v = (int64_t)exp(u * log_range) - 1;
+  return v % n_items;
+}
+
+__global__ void __launch_bounds__(UNIQ_THREADS)
+unique_candidates_kernel(int kind, int64_t n_items, int S, uint64_t seed, const int64_t* __restrict__ step_dev,
+                         uint32_t* __restrict__ owner, int64_t* __restrict__ out, int64_t* __restrict__ num_tries) {
+  __shared__ int warp_cnt[UNIQ_THREADS / 32];
+  __shared__ uint32_t s_stop;
+  const uint64_t step = (uint64_t)*step_dev;
+  const double log_range = log1p((double)n_items);
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  int have = 0;                      // ids kept before the current round (block-uniform)
+  uint32_t stop, j;
+  int64_t id;
+  if (tid == 0) s_stop = 0u;
+  for (uint32_t base = 0;; base += UNIQ_THREADS) {
+    j = base + tid;
+    id = candidate(kind, n_items, log_range, seed, step, j);
+    atomicMin(owner + id, j);
+    __syncthreads();
+    const bool fresh = __ldcg(owner + id) == j;          // L2 read: the atomics bypass L1
+    const unsigned m = __ballot_sync(0xffffffffu, fresh);
+    if (lane == 0) warp_cnt[warp] = __popc(m);
+    __syncthreads();
+    int before = 0, total = 0;
+    for (int w = 0; w < UNIQ_THREADS / 32; ++w) {
+      const int c = warp_cnt[w];
+      total += c;
+      before += w < warp ? c : 0;
+    }
+    const int rank = have + before + __popc(m & ((1u << lane) - 1u));
+    if (fresh && rank < S) out[rank] = id;
+    if (fresh && rank == S - 1) s_stop = j + 1u;
+    const bool last = have + total >= S || base + UNIQ_THREADS >= UNIQ_MAX_DRAWS;
+    have = min(have + total, S);
+    __syncthreads();
+    if (last) {
+      stop = s_stop ? s_stop : base + UNIQ_THREADS;
+      break;
+    }
+  }
+  if (tid == 0) *num_tries = (int64_t)stop;
+  // free the owner slots again: draws of the last round after the stop, then every kept id
+  if (j >= stop) owner[id] = UNIQ_FREE;
+  for (int i = tid; i < have; i += UNIQ_THREADS) owner[out[i]] = UNIQ_FREE;
+}
+
 }  // namespace sampler
 }  // namespace b200
 
 using namespace b200;
+
+extern "C" size_t b200_unique_candidates_workspace_bytes(int64_t n_items) {
+  return n_items > 0 ? (size_t)n_items * sizeof(uint32_t) : 0;
+}
+
+extern "C" int b200_unique_candidates(int32_t kind, int64_t n_items, int32_t num_sampled, uint64_t seed,
+                                      const int64_t* step_dev, void* workspace, size_t workspace_bytes, int64_t* out,
+                                      int64_t* num_tries, void* stream) {
+  B200_REQUIRE(kind == 0 || kind == 1, "b200_unique_candidates: kind must be 0 (uniform) or 1 (log-uniform)");
+  B200_REQUIRE(n_items >= 1 && n_items < ((int64_t)1 << 31), "b200_unique_candidates: n_items %lld outside [1, 2^31)",
+               (long long)n_items);
+  B200_REQUIRE(num_sampled >= 1 && num_sampled <= B200_UNIQUE_MAX_SAMPLED && num_sampled <= n_items,
+               "b200_unique_candidates: num_sampled %d outside [1, min(n_items, %d)]", num_sampled,
+               B200_UNIQUE_MAX_SAMPLED);
+  B200_REQUIRE(step_dev && out && num_tries && workspace, "b200_unique_candidates: null pointer");
+  B200_REQUIRE(workspace_bytes >= b200_unique_candidates_workspace_bytes(n_items),
+               "b200_unique_candidates: workspace too small");
+  sampler::unique_candidates_kernel<<<1, sampler::UNIQ_THREADS, 0, (cudaStream_t)stream>>>(
+      kind, n_items, num_sampled, seed, step_dev, (uint32_t*)workspace, out, num_tries);
+  count_launch();
+  B200_CUDA_OK(cudaGetLastError());
+  return 0;
+}
 
 extern "C" int b200_interacted_seqs(const int64_t* indptr, const int32_t* idx, int64_t n_users,
                                     const int64_t* users, const int64_t* items, int64_t n,

@@ -57,15 +57,18 @@ class _Trainer:
     device copies of ``weights``), their gradient buffers and Adam slots; the tables struct the gather reads; the
     loss workspace; TF-Adam and ``step_graph``.  A subclass adds its own variables in ``_init_params``.
 
-    ``linear_tables``: the model's linear (wide) tables are variables too (FM, DeepFM)."""
+    ``linear_tables``: the model's linear (wide) tables are variables too (FM, DeepFM).  ``embed_table``: the
+    variable whose width is the embed size K.  ``reg_vars``: the variables ``reg`` applies to."""
 
     linear_tables = False
+    embed_table = "user_embeds"
+    reg_vars = _REG_VARS
 
     def __init__(self, spec, weights, use_bn, lr, epsilon, device):
         import torch
 
         self._torch = torch
-        K = int(weights["user_embeds"].shape[1])
+        K = int(weights[self.embed_table].shape[1])
         self.spec = spec if isinstance(spec, FeatSpec) else FeatSpec(spec, K, device)
         self.device, self.K = self.spec.device, K
         self.F = 2 + self.spec.n_sparse + self.spec.n_dense
@@ -147,7 +150,7 @@ class _Trainer:
         lib, st = _lib.lib, _lib.current_stream()
         reg = float(getattr(self, "reg", 0.0) or 0.0)
         if reg > 0.0:             # L2 on the embedding / linear tables only (the variables built with regularizer=reg)
-            for k in _REG_VARS:
+            for k in self.reg_vars:
                 if k in self.params:
                     _lib.check(lib.b200_axpy(_lib.ptr(self.grads[k]), _lib.ptr(self.params[k]), 2.0 * reg,
                                              self.params[k].numel(), st))
@@ -935,6 +938,198 @@ class AutoIntTrainer(_Trainer):
             mha.append(lw)
         w.update(autoint_scheme=self.scheme, autoint_mha=mha, num_heads=H, use_residual=self.use_residual,
                  out_kernel=p["out_kernel"].cpu().numpy().reshape(-1, 1), out_bias=p["out_bias"].cpu().numpy().reshape(1))
+        if self._combiner is not None:
+            w["multi_sparse_combiner"] = self._combiner
+        return w
+
+
+UNIQUE_MAX_SAMPLED = 65536      # B200_UNIQUE_MAX_SAMPLED: the candidate sampler's envelope
+RETRIEVAL_LOSSES = {"sampled_softmax": 0, "nce": 1}
+
+
+class YouTubeRetrievalTrainer(_StackTrainer):
+    """YouTubeRetrieval training step on the device: ``libreco/algorithms/youtube_retrieval.py:169-260`` in training
+    mode (user vector = ``dense_nn(concat(sqrtn-pooled history over seq_embeds_var, user sparse embeddings, user dense
+    value x embedding))``) and ``YoutubeRetrievalTrainer._build_train_ops`` (``libreco/training/tf_trainer.py:162-245``):
+    S = ``num_sampled_per_batch`` (or ``batch_size``) distinct candidates from TensorFlow's unique uniform /
+    log-uniform sampler, ``tf.nn.sampled_softmax_loss`` or ``tf.nn.nce_loss`` over ``item_embeds_var`` /
+    ``item_bias_var`` with accidental hits removed and log Q subtracted, mean over the batch, optional L2 ``reg``
+    on all five tables, TF-Adam.
+
+        b200_unique_candidates (ids [S] + num_tries, both on the device; the draw stream is keyed by the device
+        Adam step) -> b200_seq_pool + K1 over the user-side fields (no id field) -> stack forward ->
+        [b200_l2_normalize_rows] -> b200_gather_rows (sampled and label rows) -> logits U W_s^T (b200_linear_*) and
+        true logits (b200_gather_dot) -> b200_sampled_class_loss (logits become d loss / d logits) ->
+        dU = dL W_s + dtrue W_label, dW_s = dL^T U (b200_linear_*) -> [b200_l2_normalize_backward] ->
+        b200_scatter_add_rows (sampled rows, label rows, biases; labels repeat) + b200_col_reduce (sampled-bias
+        column sums) -> stack backward -> b200_seq_pool_backward + b200_feat_backward -> b200_adam_dense_dev
+
+    ``weights``: the layout of ``feat_models.YouTubeRetrieval`` (``seq_embeds`` [n_items, K], ``item_embeds``
+    [n_items, H], ``item_biases`` [n_items], ``sparse_embeds``, ``dense_embeds``, ``mlp`` ending in H units).  A
+    batch is (users, label items, one history per row ``seqs`` [B, T] padded with ``n_items``, ``lens`` [B]); a row
+    at position 0 of its user's history has ``lens`` 1 and the pad id (``b200_interacted_seqs``), which pools to
+    the zero vector of the reference's empty history and sends no gradient.  With ``norm_embed`` the user vectors
+    and the gathered item rows are L2-normalised (only gathered rows get gradients, so this is the reference's
+    normalisation of the whole table).  Raises ``ValueError`` before any launch for an unknown ``loss_type``, S
+    outside 1..min(n_items, 65536), or multi-sparse fields with a combiner other than "normal"."""
+
+    embed_table = "seq_embeds"
+    reg_vars = _REG_VARS + ("seq_embeds", "item_biases")
+
+    def __init__(self, spec, weights, loss_type="sampled_softmax", batch_size=256, num_sampled_per_batch=None,
+                 sampler="uniform", norm_embed=False, use_bn=True, lr=1e-3, epsilon=1e-5, seed=42, device=None):
+        from .feat_models import _spec_get
+
+        if loss_type not in RETRIEVAL_LOSSES:
+            raise ValueError(f"YouTubeRetrievalTrainer: loss_type must be one of {sorted(RETRIEVAL_LOSSES)}, "
+                             f"got `{loss_type}`")
+        g = _spec_get(spec) if not isinstance(spec, FeatSpec) else (lambda k, d=None: d)
+        if g("multi_sparse_combine_info") is not None and weights.get("multi_sparse_combiner", "sqrtn") != "normal":
+            raise ValueError("YouTubeRetrievalTrainer: multi-sparse fields need the combiner \"normal\"; the pooling "
+                             "backward is not built")
+        n_items = int(spec.n_items if isinstance(spec, FeatSpec) else g("n_items"))
+        S = int(num_sampled_per_batch) if num_sampled_per_batch and num_sampled_per_batch > 0 else int(batch_size)
+        if not 1 <= S <= min(n_items, UNIQUE_MAX_SAMPLED):
+            raise ValueError(f"YouTubeRetrievalTrainer: num_sampled {S} outside 1..min(n_items = {n_items}, "
+                             f"{UNIQUE_MAX_SAMPLED})")
+        for k, rows in (("seq_embeds", n_items), ("item_embeds", n_items), ("item_biases", n_items)):
+            if np.shape(weights[k])[0] != rows:
+                raise ValueError(f"YouTubeRetrievalTrainer: {k} has {np.shape(weights[k])[0]} rows, expected n_items = "
+                                 f"{n_items} (no OOV row)")
+        self.loss_type, self.loss_kind = loss_type, RETRIEVAL_LOSSES[loss_type]
+        self.sampler, self.sampler_kind = sampler, 0 if sampler == "uniform" else 1     # anything else: TF's default
+        self.S, self.seed, self.norm_embed = S, int(seed), bool(norm_embed)
+        self._combiner = weights.get("multi_sparse_combiner")
+        super().__init__(spec, weights, use_bn, lr, epsilon, device)
+        torch = self._torch
+        self._device_counters()
+        self.sampled = torch.empty(S, dtype=torch.int64, device=self.device)
+        self.num_tries = torch.empty(1, dtype=torch.int64, device=self.device)
+        self._owner = torch.full((self.n_items,), -1, dtype=torch.int32, device=self.device)     # 0xFF bytes: all free
+
+    def _init_params(self, weights):
+        p = self.params
+        p["seq_embeds"] = self._var(weights["seq_embeds"])
+        p["item_biases"] = self._var(weights["item_biases"], -1)
+        self.n_layers = self._init_stack("", weights["mlp"])
+        self.H = int(p[f"Wt{self.n_layers - 1}"].shape[0])
+        if tuple(p["item_embeds"].shape) != (self.n_items, self.H):
+            raise ValueError(f"YouTubeRetrievalTrainer: item_embeds {tuple(p['item_embeds'].shape)}, expected "
+                             f"(n_items, last hidden units) = ({self.n_items}, {self.H})")
+
+    def sample(self):
+        """This step's candidates: device ids [S] (distinct, in draw order) and the device ``num_tries``, drawn from
+        (seed, the device Adam step)."""
+        _lib.check(_lib.lib.b200_unique_candidates(
+            self.sampler_kind, self.n_items, self.S, self.seed, _lib.ptr(self._step_dev), _lib.ptr(self._owner),
+            self._owner.numel() * 4, _lib.ptr(self.sampled), _lib.ptr(self.num_tries), _lib.current_stream()))
+        return self.sampled, self.num_tries
+
+    def _normalize(self, x):
+        """(L2-normalised copy of x, x) with norm_embed, else (x, None)."""
+        if not self.norm_embed:
+            return x, None
+        y = x.clone()
+        _lib.check(_lib.lib.b200_l2_normalize_rows(_lib.ptr(y), y.stride(0), y.shape[0], y.shape[1],
+                                                   _lib.current_stream()))
+        return y, x
+
+    def _normalize_backward(self, dy, pre):
+        if pre is not None:
+            _lib.check(_lib.lib.b200_l2_normalize_backward(_lib.ptr(pre), pre.stride(0), _lib.ptr(dy), dy.stride(0),
+                                                           pre.shape[0], pre.shape[1], _lib.ptr(dy), dy.stride(0),
+                                                           _lib.current_stream()))
+        return dy
+
+    def user_forward(self, users_d, seqs_d, lens_d):
+        """User vectors [B, H] of the batch (training-mode BN) before any normalisation; returns (U, cache)."""
+        torch = self._torch
+        K = self.K
+        B = int(users_d.numel())
+        L, pos = self.spec.side("user", with_id=False)
+        x = torch.empty((B, (1 + len(pos)) * K), dtype=torch.float32, device=self.device)
+        rows = torch.arange(B, dtype=torch.int64, device=self.device)
+        E = self.params["seq_embeds"]
+        _lib.check(_lib.lib.b200_seq_pool(_lib.ptr(E), E.stride(0), K, self.n_items, _lib.ptr(seqs_d), seqs_d.stride(0),
+                                          _lib.ptr(lens_d), seqs_d.shape[1], _lib.ptr(rows), B, 0, 0, _lib.ptr(x),
+                                          x.stride(0), _lib.current_stream()))
+        if pos:
+            feat_forward(L, self.tables, users_d, users_d, B, concat=x[:, K:])
+        U, c = self._stack_forward("", self.n_layers, x)
+        c.update(users=users_d, seqs=seqs_d, lens=lens_d, rows=rows, fields=bool(pos))
+        return U, c
+
+    def forward_backward(self, users_d, items_d, seqs_d, lens_d):
+        """Loss (device scalar) with every gradient buffer filled; the candidates stay in ``sampled`` /
+        ``num_tries``."""
+        torch = self._torch
+        lib, st, p, g, K, H, S = _lib.lib, _lib.current_stream(), self.params, self.grads, self.K, self.H, self.S
+        f32, dev = torch.float32, self.device
+        B = int(users_d.numel())
+        ids, tries = self.sample()
+        U0, c = self.user_forward(users_d, seqs_d, lens_d)
+        W = p["item_embeds"]
+        Ws0 = torch.empty((S, H), dtype=f32, device=dev)
+        Wl0 = torch.empty((B, H), dtype=f32, device=dev)
+        _lib.check(lib.b200_gather_rows(_lib.ptr(W), W.stride(0), H, _lib.ptr(ids), S, _lib.ptr(Ws0), H, st))
+        _lib.check(lib.b200_gather_rows(_lib.ptr(W), W.stride(0), H, _lib.ptr(items_d), B, _lib.ptr(Wl0), H, st))
+        U, U_pre = self._normalize(U0)
+        Ws, Ws_pre = self._normalize(Ws0)
+        Wl, Wl_pre = self._normalize(Wl0)
+        rows = c["rows"]
+        logits = linear(U, Ws, None, False, cache_split=False)                  # [B, S] = U W_s^T
+        true = torch.empty(B, dtype=f32, device=dev)
+        _lib.check(lib.b200_gather_dot(_lib.ptr(U), U.stride(0), _lib.ptr(rows), _lib.ptr(Wl), Wl.stride(0),
+                                       _lib.ptr(rows), B, H, 0, 0.0, 0.0, _lib.ptr(true), st))
+        loss = torch.empty((), dtype=f32, device=dev)
+        dtrue = torch.empty(B, dtype=f32, device=dev)
+        ws = torch.empty(int(lib.b200_sampled_class_loss_workspace_bytes(B, S)), dtype=torch.uint8, device=dev)
+        _lib.check(lib.b200_sampled_class_loss(
+            self.loss_kind, _lib.ptr(logits), logits.stride(0), B, S, _lib.ptr(true), _lib.ptr(items_d), _lib.ptr(ids),
+            _lib.ptr(p["item_biases"]), self.sampler_kind, self.n_items, _lib.ptr(tries), _lib.ptr(loss),
+            _lib.ptr(dtrue), _lib.ptr(ws), ws.numel(), st))
+        dL = logits                                                              # now d loss / d logits
+        # dU = dL W_s + dtrue (x) W_label ; dW_s = dL^T U ; dW_label = dtrue (x) U  (row scalings: elementwise)
+        dU = linear(dL, Ws.t().contiguous(), None, False, cache_split=False)
+        _lib.check(lib.b200_axpy(_lib.ptr(dU), _lib.ptr(dtrue[:, None] * Wl), 1.0, dU.numel(), st))
+        dWs = _weight_grad(dL, U).contiguous()
+        dWl = dtrue[:, None] * U
+        dU = self._normalize_backward(dU, U_pre)
+        dWs = self._normalize_backward(dWs, Ws_pre)
+        dWl = self._normalize_backward(dWl, Wl_pre)
+        gW, gb = g["item_embeds"], g["item_biases"]
+        _lib.check(lib.b200_scatter_add_rows(_lib.ptr(gW), gW.stride(0), H, _lib.ptr(ids), S, _lib.ptr(dWs), H, st))
+        _lib.check(lib.b200_scatter_add_rows(_lib.ptr(gW), gW.stride(0), H, _lib.ptr(items_d), B, _lib.ptr(dWl), H, st))
+        db = torch.zeros(S, dtype=f32, device=dev)
+        self._col_sum(dL, db)
+        _lib.check(lib.b200_scatter_add_rows(_lib.ptr(gb), 1, 1, _lib.ptr(ids), S, _lib.ptr(db), 1, st))
+        _lib.check(lib.b200_scatter_add_rows(_lib.ptr(gb), 1, 1, _lib.ptr(items_d), B, _lib.ptr(dtrue), 1, st))
+        # user tower
+        dx = self._stack_backward("", self.n_layers, c, dU)
+        ge = g["seq_embeds"]
+        _lib.check(lib.b200_seq_pool_backward(_lib.ptr(dx), dx.stride(0), K, self.n_items, _lib.ptr(seqs_d),
+                                              seqs_d.stride(0), _lib.ptr(lens_d), seqs_d.shape[1], _lib.ptr(rows), B,
+                                              _lib.ptr(ge), ge.stride(0), st))
+        if c["fields"]:
+            feat_backward(self.spec.side("user", with_id=False)[0], self.tables, users_d, users_d, B, g,
+                          dconcat=dx[:, K:])
+        return loss
+
+    def step(self, users_d, items_d, seqs_d, lens_d):
+        """One optimisation step on (users, label items, histories [B, T], lengths [B]) device tensors; returns the
+        device loss."""
+        torch = self._torch
+        loss = self.forward_backward(users_d.to(torch.int64).contiguous(), items_d.to(torch.int64).contiguous(),
+                                     seqs_d.to(torch.int32).contiguous(), lens_d.to(torch.int32).contiguous())
+        self._adam_update()
+        return loss
+
+    def export_weights(self):
+        """The inference layout of ``feat_models.YouTubeRetrieval``."""
+        p = self.params
+        w = {k: v for k, v in self._export_tables().items() if k != "user_embeds"}
+        w.update(seq_embeds=p["seq_embeds"].cpu().numpy(), item_biases=p["item_biases"].cpu().numpy(),
+                 mlp=self._export_stack("", self.n_layers))
         if self._combiner is not None:
             w["multi_sparse_combiner"] = self._combiner
         return w

@@ -264,6 +264,69 @@ def autoint_tf_variables(raw):
     return out
 
 
+YOUTUBE_RETRIEVAL_TABLES = {
+    "seq_embeds": "embedding/seq_embeds_var:0", "item_embeds": "embedding/item_embeds_var:0",
+    "item_biases": "embedding/item_bias_var:0", "sparse_embeds": "embedding/sparse_embeds_var:0",
+    "dense_embeds": "embedding/dense_embeds_var:0",
+}
+
+
+def youtube_retrieval_tf_variables(w):
+    """YouTubeRetrieval weights in the layout of ``feat_models.YouTubeRetrieval`` (e.g.
+    ``training.YouTubeRetrievalTrainer.export_weights()``) -> ``{TF variable name: array}``: the ``embedding`` scope
+    of ``youtube_retrieval.py:194-260`` (``seq_embeds_var`` [n_items, K], ``item_embeds_var`` [n_items, H],
+    ``item_bias_var`` [n_items], ``sparse_embeds_var``, ``dense_embeds_var``) and the user tower's ``mlp`` dense_nn
+    stack.  The inverse of ``load_reference_tf_model(..., "YouTubeRetrieval", ...)``."""
+    out = {name: np.asarray(w[k], dtype=np.float32) for k, name in YOUTUBE_RETRIEVAL_TABLES.items()
+           if w.get(k) is not None}
+    out[YOUTUBE_RETRIEVAL_TABLES["item_biases"]] = out[YOUTUBE_RETRIEVAL_TABLES["item_biases"]].reshape(-1)
+    mlp = w["mlp"]
+    names = _mlp_names("mlp", len(mlp["kernels"]), mlp.get("bn_in") is not None)
+
+    def put(n, a):
+        if isinstance(n, dict):
+            for k in n:
+                put(n[k], a[k])
+        elif isinstance(n, list):
+            for ni, ai in zip(n, a):
+                put(ni, ai)
+        else:
+            out[n] = np.asarray(a, dtype=np.float32)
+    put(names, {k: mlp[k] for k in names})
+    return out
+
+
+def _youtube_retrieval_weights(npz, n_hidden, use_bn, extra_names=None):
+    """Engine weight dict of a saved YouTubeRetrieval: every name and shape checked (``KeyError`` naming the
+    variable and listing what the file holds)."""
+    seq = resolve_tf_names(npz, YOUTUBE_RETRIEVAL_TABLES["seq_embeds"])
+    n_items, K = seq.shape if seq.ndim == 2 else (None, None)
+    if n_items is None:
+        raise KeyError(f"TF variable `{YOUTUBE_RETRIEVAL_TABLES['seq_embeds']}` has shape {seq.shape}, expected "
+                       f"[n_items, K]")
+    names = {"mlp": _mlp_names("mlp", n_hidden, use_bn)}
+    names.update(extra_names or {})
+    mlp = resolve_tf_names(npz, names)["mlp"]
+    H = int(np.shape(mlp["kernels"][-1])[1]) if np.ndim(mlp["kernels"][-1]) == 2 else -1
+    dims = [None] + [np.shape(k)[1] if np.ndim(k) == 2 else -1 for k in mlp["kernels"]]
+    shapes = {"mlp": {"kernels": [(dims[i] if i else None, dims[i + 1]) for i in range(n_hidden)],
+                      "biases": [(dims[i + 1],) for i in range(n_hidden)]}}
+    if use_bn:
+        din = np.shape(mlp["kernels"][0])[0]
+        shapes["mlp"]["bn_in"] = {k: (din,) for k in ("gamma", "beta", "mean", "var")}
+        shapes["mlp"]["bns"] = [{k: (dims[i + 1],) for k in ("gamma", "beta", "mean", "var")} for i in range(n_hidden - 1)]
+    w = resolve_tf_names(npz, names, shapes)
+    tables = {"seq_embeds": (n_items, K), "item_embeds": (n_items, H), "item_biases": (n_items,)}
+    for k in ("sparse_embeds", "dense_embeds"):
+        if YOUTUBE_RETRIEVAL_TABLES[k] in npz:
+            tables[k] = (None, K)
+    w.update(resolve_tf_names(npz, {k: YOUTUBE_RETRIEVAL_TABLES[k] for k in tables}, tables))
+    if np.shape(mlp["kernels"][0])[0] % K:
+        raise KeyError(f"TF variable `{names['mlp']['kernels'][0]}` has {np.shape(mlp['kernels'][0])[0]} input rows, "
+                       f"not a multiple of K = {K}")
+    return w
+
+
 def load_reference_tf_model(path, model_name, arch, n_hidden, use_bn, use_tf_attention=False, extra_names=None,
                             num_heads=2, att_embed_size=(8, 8, 8), use_residual=True):
     """Engine weight dict of a model saved by the reference (``save_tf_variables``,
@@ -271,10 +334,13 @@ def load_reference_tf_model(path, model_name, arch, n_hidden, use_bn, use_tf_att
     fixed names, the heads / MLPs / batch-norms through :func:`default_tf_names` (override single entries
     with `extra_names`).  AutoInt takes its own constructor arguments ``num_heads``, ``att_embed_size`` and
     ``use_residual``; its naming scheme (keras or legacy) is read off the names in the file, and every name
-    and shape is checked."""
+    and shape is checked.  YouTubeRetrieval (``n_hidden`` Dense layers in the user tower) returns the layout of
+    ``feat_models.YouTubeRetrieval``, every name and shape checked."""
     from .feat_models import from_tf_variables
 
     npz = np.load(os.path.join(path, f"{model_name}_tf_variables.npz"))
+    if arch == "YouTubeRetrieval":
+        return _youtube_retrieval_weights(npz, n_hidden, use_bn, extra_names)
     w = from_tf_variables(npz)
     if arch == "AutoInt":
         hds = autoint_head_dims(att_embed_size)
