@@ -465,6 +465,7 @@ extern "C" int b200_bn_train_backward(const float* dy, int64_t lddy, const float
                                       void* stream) {
   B200_REQUIRE(dy && x && batch_mean && batch_var && gamma && dx && g_gamma && g_beta, "b200_bn_train_backward: null pointer");
   B200_REQUIRE(workspace && workspace_bytes >= (size_t)K * 16, "workspace too small (need 16 bytes per column)");
+  if (R == 0) return 0;                    // an empty batch adds nothing to g_gamma / g_beta
   cudaStream_t st = (cudaStream_t)stream;
   double* s1 = (double*)workspace;
   double* s2 = s1 + K;
@@ -551,6 +552,7 @@ extern "C" int b200_fm_head_backward(const float* dlogit, const float* z, const 
   B200_REQUIRE(dlogit && z && pw && pw_kernel && dpw && g_pw_kernel && g_pw_bias, "b200_fm_head_backward: null pointer");
   B200_REQUIRE(!batch_mean || (batch_var && gamma && beta && g_gamma && g_beta), "BN arguments incomplete");
   B200_REQUIRE(workspace && workspace_bytes >= b200_fm_head_backward_workspace_bytes(R, K), "workspace too small");
+  if (R == 0) return 0;                    // an empty batch adds nothing to the parameter gradients
   cudaStream_t st = (cudaStream_t)stream;
   double* red = (double*)workspace;                                   // 8-byte aligned start
   float* dz = (float*)((char*)workspace + (((size_t)(K + 2) * 8 + 255) / 256) * 256);
@@ -576,6 +578,19 @@ extern "C" int b200_feat_backward(const b200_feat_layout* layout, const b200_fea
   B200_REQUIRE(dpw || dconcat, "nothing to propagate");
   B200_REQUIRE(!dpw || S, "the pairwise gradient needs the field sum S");
   B200_REQUIRE(!dlogit || (lin_kernel && g_lin_kernel), "linear-term gradient needs lin_kernel");
+  // every field of the layout scatters into its table's gradient buffer (and its linear table's, with dlogit)
+  const bool has_u = layout->id_mask & 1, has_i = layout->id_mask & 2;
+  const bool has_s = layout->n_sparse > 0, has_d = layout->n_dense > 0;
+  B200_REQUIRE(!has_u || g_user_embeds, "b200_feat_backward: the layout has user ids but g_user_embeds is null");
+  B200_REQUIRE(!has_i || g_item_embeds, "b200_feat_backward: the layout has item ids but g_item_embeds is null");
+  B200_REQUIRE(!has_s || g_sparse_embeds, "b200_feat_backward: the layout has sparse fields but g_sparse_embeds is null");
+  B200_REQUIRE(!has_d || g_dense_embeds, "b200_feat_backward: the layout has dense fields but g_dense_embeds is null");
+  if (dlogit) {
+    B200_REQUIRE(!has_u || g_user_linear, "b200_feat_backward: dlogit given but g_user_linear is null");
+    B200_REQUIRE(!has_i || g_item_linear, "b200_feat_backward: dlogit given but g_item_linear is null");
+    B200_REQUIRE(!has_s || g_sparse_linear, "b200_feat_backward: dlogit given but g_sparse_linear is null");
+    B200_REQUIRE(!has_d || g_dense_linear, "b200_feat_backward: dlogit given but g_dense_linear is null");
+  }
   if (R == 0) return 0;
   const int K = layout->embed_size;
   int lpr = 1;
