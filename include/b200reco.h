@@ -82,10 +82,11 @@ int b200_score_rows_f32(const float* U, int64_t ldu, const int64_t* user_ids, in
  * both CTAs) + MMA groups per item tile, out[7] records per candidate list (n_out >= 8).
  * b200_recommend_embed_tune (process-wide, not thread-safe; 0 keeps a value): organisation code =
  * 100 x cluster size (1|2) + 10 x MMA groups per tile (1|2) + epilogue variant (3: divergent per-lane
- * group tests, 5: one warp vote per 64-column step + predicated record stores; default 213), and the rank
+ * group tests, 5: one warp vote per 64-column step + quad-mask record stores; default 215), and the rank
  * coefficient c of the speculative threshold (about c * k_row items are expected above it). */
 int b200_recommend_embed_tune(int32_t organisation_code, float pre_rank_coef);
-/* profiling diagnostics only (results are wrong while level > 0): ablate parts of the main pass */
+/* profiling diagnostics only (results are wrong while level > 0): ablate parts of the main pass
+ * (1: nothing is collected, cold epilogue steps only; 2: no epilogue at all, MMAs and stage releases only) */
 int b200_recommend_embed_debug(int32_t ablate_level);
 int b200_recommend_embed_plan(int64_t B, int64_t N, int32_t d, int32_t K, int32_t* out, int32_t n_out);
 int b200_embed_catalog_bytes(int64_t N, int32_t d, size_t* bytes);

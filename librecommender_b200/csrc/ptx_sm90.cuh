@@ -92,12 +92,16 @@ __device__ __forceinline__ void cluster_sync_all() {
   asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
 
-// arrive on the mbarrier at the same shared-memory offset in CTA `cta_rank` of this cluster
+// arrive on the mbarrier at the same shared-memory offset in CTA `cta_rank` of this cluster.
+// Default semantics (release at CTA scope): no fence orders this thread's earlier global stores before
+// the arrive (a .release.cluster arrive makes ptxas drain them with MEMBAR.ALL.GPU).  That suffices to
+// hand back a ring stage whose only readers were this warp's wgmmas: they are complete once
+// wgmma.wait_group returns, before the arrive, and the peer's TMA refill orders nothing else.
 __device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta_rank) {
   asm volatile(
       "{\n\t.reg .b32 ra;\n\t"
       "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t}"
+      "mbarrier.arrive.shared::cluster.b64 _, [ra];\n\t}"
       ::"r"(smem_u32(bar)), "r"(cta_rank)
       : "memory");
 }

@@ -332,27 +332,28 @@ __device__ __noinline__ int compact_row(float* __restrict__ ls, int n,
   return w;
 }
 
-__device__ __forceinline__ float fmax3(float a, float b, float c) { return fmaxf(fmaxf(a, b), c); }
-
 // CL = CTAs per thread-block cluster (1 or 2).  With CL = 2 the two CTAs of a cluster work on two
 // ADJACENT user tiles of the SAME item split in lock step: every item tile is fetched from L2 once
 // per cluster — each CTA loads half of it and the TMA multicasts that half into both CTAs' shared
 // memory — which halves the L2 -> SM traffic of the item table (the pass is L2-bandwidth bound
 // otherwise).  NH = MMA groups per item tile (1: one N=256 wgmma chain; 2: two N=128 chains into
 // separate accumulators, the epilogue of the first runs while the tensor core computes the second).
-// EPI = record stores of a hot 64-column step: 3 divergent per-group branches, 5 predicated stores.
+// EPI = record stores of a hot 64-column step: 3 divergent per-group branches (the quad maximum by
+// shuffles), 5 quad masks (one bit per (group, row) slot, one warp-uniform branch per slot).
 //
 // Threads: warpgroups 0 and 1 issue the wgmma of user rows [64 g, 64 g + 64) of the tile and run the
 // epilogue on the accumulator registers; one lane of warpgroup 2 is the TMA producer.  In the m64nN fragment, lane
 // (4 quad + tq) of warp w holds rows 16 w + quad and 16 w + quad + 8, columns 8 j + 2 tq + {0, 1}:
-// the 8 columns of a group are spread over the 4 lanes of a quad, which reduce the group maximum
-// with two shuffles and write the 48-byte record together (8 bytes each, the id from lane tq = 0).
+// the 8 columns of a group are spread over the 4 lanes of a quad, which write the 48-byte record
+// together (8 bytes each, the id from lane tq = 0).
 // Lane tq of a quad also owns one (row, list) pair — row quad + 8 (tq >> 1), list tq & 1 — for
 // the warp-wide bookkeeping (compaction votes, list lengths, pre-pass maxima).
-__device__ __forceinline__ int sel22(const int (&c)[2][2], int rs, int j) {
+template <class T>
+__device__ __forceinline__ T sel22(T const (&c)[2][2], int rs, int j) {
   return rs ? (j ? c[1][1] : c[1][0]) : (j ? c[0][1] : c[0][0]);
 }
-__device__ __forceinline__ void set22(int (&c)[2][2], int rs, int j, int v) {
+template <class T>
+__device__ __forceinline__ void set22(T (&c)[2][2], int rs, int j, T v) {
   if (rs) { if (j) c[1][1] = v; else c[1][0] = v; } else { if (j) c[0][1] = v; else c[0][0] = v; }
 }
 
@@ -571,8 +572,10 @@ sweep_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
       } else {
         // ---- main pass ----
         float tau[2];
-        int cnt[2][2] = {{0, 0}, {0, 0}}, n_counted[2][2] = {{0, 0}, {0, 0}};
+        int n_counted[2][2] = {{0, 0}, {0, 0}};
+        // lp: first record of the (row, list); rp: where its next record goes (records = (rp - lp) / REC)
         float* lp[2][2];
+        float* rp[2][2];
         const int64_t cap_words = (int64_t)p.capg * REC;
 #pragma unroll
         for (int rs = 0; rs < 2; ++rs) {
@@ -584,60 +587,93 @@ sweep_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
           }
           if (p.ablate >= 1) tau[rs] = pinf;   // diagnostics: nothing is ever collected (cold path only)
 #pragma unroll
-          for (int j = 0; j < 2; ++j) lp[rs][j] = p.cand_r + ((int64_t)(list_base + j) * p.B_pad + grow) * cap_words;
+          for (int j = 0; j < 2; ++j) rp[rs][j] = lp[rs][j] = p.cand_r + ((int64_t)(list_base + j) * p.B_pad + grow) * cap_words;
         }
+        auto records = [&](int rs, int j) { return (int)(sel22(rp, rs, j) - sel22(lp, rs, j)) / REC; };
 
         // Zero-padded item rows of the last tile (ids >= N, coarse score exactly 0) may be collected when
         // tau <= 0; compact_row and finalize_kernel ignore ids >= N, so the sweep needs no tail code.
         for (int t = t0; t < t1; ++t) {
-          const int c_before = cnt[0][0] + cnt[0][1] + cnt[1][0] + cnt[1][1];
+          bool hot = false;   // warp-uniform: some step of the tile stored records
           tile_mma([&](auto& d, auto c0) {
             constexpr int COL0 = decltype(c0)::value;
+            if (p.ablate >= 2) return;   // diagnostics: MMAs and stage releases only
 #pragma unroll
             for (int s = 0; s < NC / STEP; ++s) {
-              // one warp vote per 64-column step: a cold step (the common case) costs its max tree only
+              // one warp vote per 64-column step: a cold step (the common case) costs its max tree only.
+              // pm = the lane's maximum of each (group, row) slot; the group maximum reaches tau exactly
+              // when the pair maximum of some lane of the quad does
+              float pm[8][2];
               float m0 = ninf, m1 = ninf;
 #pragma unroll
-              for (int jj = 8 * s; jj < 8 * s + 8; ++jj) {
-                m0 = fmax3(m0, d[4 * jj + 0], d[4 * jj + 1]);
-                m1 = fmax3(m1, d[4 * jj + 2], d[4 * jj + 3]);
+              for (int jl = 0; jl < 8; ++jl) {
+                const int jj = 8 * s + jl;
+                pm[jl][0] = fmaxf(d[4 * jj + 0], d[4 * jj + 1]);
+                pm[jl][1] = fmaxf(d[4 * jj + 2], d[4 * jj + 3]);
+                m0 = fmaxf(m0, pm[jl][0]);
+                m1 = fmaxf(m1, pm[jl][1]);
               }
               if (!__any_sync(0xffffffffu, m0 >= tau[0] || m1 >= tau[1])) continue;
+              hot = true;   // some slot of the warp reaches tau: records are stored
+              // Slots are visited group by group, row by row, so every list receives its records in
+              // column order whichever variant runs.
+              if (EPI == 5) {
+                // bit 2 jl + rs: the group reaches tau in that row; OR over the quad, then over the warp
+                uint32_t mask = 0;
 #pragma unroll
-              for (int jj = 8 * s; jj < 8 * s + 8; ++jj) {
-                const int col = COL0 + 8 * jj;
-                const int j = col >= TN / 2;
-                const int32_t idv = t * TN + col;
+                for (int jl = 0; jl < 8; ++jl)
 #pragma unroll
-                for (int rs = 0; rs < 2; ++rs) {
-                  const float v0 = d[4 * jj + 2 * rs], v1 = d[4 * jj + 2 * rs + 1];
-                  float gm = fmaxf(v0, v1);
-                  gm = fmaxf(gm, __shfl_xor_sync(0xffffffffu, gm, 1));
-                  gm = fmaxf(gm, __shfl_xor_sync(0xffffffffu, gm, 2));
-                  int& c = j ? cnt[rs][1] : cnt[rs][0];
-                  float* dst = (j ? lp[rs][1] : lp[rs][0]) + (size_t)c * REC;
-                  if (EPI == 5) {
+                  for (int rs = 0; rs < 2; ++rs) mask |= (pm[jl][rs] >= tau[rs] ? 1u : 0u) << (2 * jl + rs);
+                mask |= __shfl_xor_sync(0xffffffffu, mask, 1);
+                mask |= __shfl_xor_sync(0xffffffffu, mask, 2);
+                const uint32_t any = __reduce_or_sync(0xffffffffu, mask);
+#pragma unroll
+                for (int jl = 0; jl < 8; ++jl) {
+                  const int jj = 8 * s + jl;
+                  const int col = COL0 + 8 * jj;
+#pragma unroll
+                  for (int rs = 0; rs < 2; ++rs) {
+                    const uint32_t bit = 1u << (2 * jl + rs);
+                    if (!(any & bit)) continue;   // warp-uniform: no quad of the warp has this slot
+                    float*& r = col >= TN / 2 ? rp[rs][1] : rp[rs][0];
+                    // predicated stores (not a branch on the lane's bit, which the compiler would merge
+                    // with the uniform test above into one divergent branch per slot)
                     asm volatile(
                         "{\n\t.reg .pred p, q;\n\t"
-                        "setp.ge.f32 p, %0, %1;\n\t"
-                        "setp.eq.and.u32 q, %6, 0, p;\n\t"
-                        "@p st.global.v2.f32 [%2], {%3, %4};\n\t"
-                        "@q st.global.b32 [%5], %7;\n\t}"
-                        ::"f"(gm), "f"(tau[rs]), "l"(dst + 2 * tq), "f"(v0), "f"(v1), "l"(dst + 8), "r"(tq), "r"(idv)
+                        "setp.ne.u32 p, %0, 0;\n\t"
+                        "setp.eq.and.u32 q, %5, 0, p;\n\t"
+                        "@p st.global.v2.f32 [%1], {%2, %3};\n\t"
+                        "@q st.global.b32 [%4], %6;\n\t}"
+                        ::"r"(mask & bit), "l"(r + 2 * tq), "f"(d[4 * jj + 2 * rs]), "f"(d[4 * jj + 2 * rs + 1]),
+                        "l"(r + 8), "r"(tq), "r"(t * TN + col)
                         : "memory");
-                    c += (gm >= tau[rs]) ? 1 : 0;
-                  } else if (gm >= tau[rs]) {
-                    *reinterpret_cast<float2*>(dst + 2 * tq) = make_float2(v0, v1);
-                    if (tq == 0) reinterpret_cast<int32_t*>(dst)[8] = idv;
-                    ++c;
+                    r += (mask & bit) ? REC : 0;
+                  }
+                }
+              } else {
+#pragma unroll
+                for (int jl = 0; jl < 8; ++jl) {
+                  const int jj = 8 * s + jl;
+                  const int col = COL0 + 8 * jj;
+#pragma unroll
+                  for (int rs = 0; rs < 2; ++rs) {
+                    float gm = pm[jl][rs];
+                    gm = fmaxf(gm, __shfl_xor_sync(0xffffffffu, gm, 1));
+                    gm = fmaxf(gm, __shfl_xor_sync(0xffffffffu, gm, 2));
+                    if (gm >= tau[rs]) {
+                      float*& r = col >= TN / 2 ? rp[rs][1] : rp[rs][0];
+                      *reinterpret_cast<float2*>(r + 2 * tq) = make_float2(d[4 * jj + 2 * rs], d[4 * jj + 2 * rs + 1]);
+                      if (tq == 0) reinterpret_cast<int32_t*>(r)[8] = t * TN + col;
+                      r += REC;
+                    }
                   }
                 }
               }
             }
           });
           // one overflow / compaction check per TILE (a tile adds at most 16 records to a list)
-          if (!__any_sync(0xffffffffu, cnt[0][0] + cnt[0][1] + cnt[1][0] + cnt[1][1] != c_before)) continue;
-          const int mc = sel22(cnt, my_rs, my_j), mn = sel22(n_counted, my_rs, my_j);
+          if (!hot) continue;
+          const int mc = records(my_rs, my_j), mn = sel22(n_counted, my_rs, my_j);
           uint32_t need = __ballot_sync(0xffffffffu, (mc - mn > p.trig) || (mc > p.capg - 24));
           while (need) {
             const int src = __ffs(need) - 1;
@@ -653,14 +689,14 @@ sweep_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
                                       sm.k_row, sm.eps2, sm.R, s_tau, p.ghist + (int64_t)sgrow * NB, lane, (int32_t)p.N,
                                       &new_tau);
             if (quad == sq) {
-              set22(cnt, srs, sj, w);
+              set22(rp, srs, sj, sel22(lp, srs, sj) + (size_t)w * REC);
               set22(n_counted, srs, sj, w);
               // also pick up what other lists of this row published meanwhile
               float nt = fmaxf(new_tau, key_to_float(max(__ldcg(p.row_tau_key + sgrow), 1u)));
               if (lane == src) atomicMax(p.row_tau_key + sgrow, float_to_key(new_tau));
               if (w > p.capg - 32) {  // too many near-ties to bound: hand the row to the exact path
                 nt = pinf;
-                set22(cnt, srs, sj, 0);
+                set22(rp, srs, sj, sel22(lp, srs, sj));
                 set22(n_counted, srs, sj, 0);
                 if (lane == src) p.row_status[sgrow] = 1;
               }
@@ -668,7 +704,7 @@ sweep_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
             }
           }
         }
-        p.cand_cnt[(int64_t)(list_base + my_j) * p.B_pad + grow0 + 8 * my_rs] = sel22(cnt, my_rs, my_j);
+        p.cand_cnt[(int64_t)(list_base + my_j) * p.B_pad + grow0 + 8 * my_rs] = records(my_rs, my_j);
       }
       // the user tile is reusable once every consumer warp's last MMA of the unit is complete
       __syncwarp();
@@ -1137,7 +1173,7 @@ static inline size_t al256(size_t x) { return (x + 255) & ~(size_t)255; }
 
 
 // ---- tuning knobs (defaults compiled in; b200_recommend_embed_tune overrides them per process) ----
-static int g_epi = 5;              // record stores of a hot epilogue step: 5 predicated stores (measured best on H100), 3 divergent group tests
+static int g_epi = 5;              // record stores of a hot epilogue step: 5 quad masks (measured best on H100), 3 divergent group tests
 static int g_cluster = 2;          // 2 = pairs of user tiles share every item tile through TMA multicast, 1 = off
 static int g_nh = 1;               // MMA groups per item tile (1 x N=256; 2 x N=128, epilogue of the first overlaps the second)
 static int g_ablate = 0;           // b200_recommend_embed_debug
@@ -1335,13 +1371,14 @@ extern "C" int b200_recommend_embed_tune(int32_t epilogue_warps_per_quadrant, fl
   return 0;
 }
 
-// Diagnostics (profiling only; results are WRONG while level 1 is set): 1 = the main pass collects nothing.
+// Diagnostics (profiling only; results are WRONG while level 1 or 2 is set): 1 = the main pass collects
+// nothing (cold epilogue steps only), 2 = the main pass runs no epilogue at all (wait, MMA, release).
 extern "C" int b200_recommend_embed_debug(int32_t ablate_level) {
   // levels >= 100: suspend-time hint (ns) of the mbarrier waits of the sweep kernels = level - 100
   // levels -1 .. -64: additive margin of the speculative rank (pre_k = margin + coef * f * k_row) = -level
   if (ablate_level < 0 && ablate_level >= -64) { g_pre_margin = -ablate_level; return 0; }
   if (ablate_level >= 100) { g_hint_ns = ablate_level - 100; return 0; }
-  B200_REQUIRE(ablate_level >= 0 && ablate_level <= 1, "b200_recommend_embed_debug: level 0..1 (or 100 + hint ns)");
+  B200_REQUIRE(ablate_level >= 0 && ablate_level <= 2, "b200_recommend_embed_debug: level 0..2 (or 100 + hint ns)");
   g_ablate = ablate_level;
   return 0;
 }
