@@ -43,14 +43,17 @@ int b200_build_consumed_csr_host(const int64_t* user_indices_host, const int64_t
 /* ---- a2: rank_recommendations (libreco/recommendation/ranking.py:10-78) ----------------
  * b200_mask_consumed: filter_items (:59-61) under the rule of :38 — row r (user user_ids[r])
  * is masked iff c_u > 0 and K + c_u <= N, c_u = indptr[u+1]-indptr[u] (duplicates counted);
- * users >= n_users (OOV) are never masked.  Masked scores are overwritten with -inf. */
+ * users >= n_users (OOV) are never masked; ids outside [0, N) are skipped.  Masked scores are
+ * overwritten with the REMOVED bit pattern 0xffffffff (a NaN no arithmetic produces), which
+ * b200_topk_rows ranks below every score, -inf and NaN included. */
 int b200_mask_consumed(float* scores, int64_t ld, const int64_t* user_ids, int64_t B, int64_t N,
                        int32_t K, const int64_t* indptr, const int32_t* idx, int64_t n_users,
                        void* stream);
 
 /* b200_topk_rows: partition_select + argsort (:48-49,:76-78): per row the K largest scores,
- * sorted by (score desc, item id asc).  out_ids int64 [B,K]; out_scores float [B,K] or NULL.
- * K <= 4096 and K <= N. */
+ * sorted by (score desc, item id asc) where -0.0 == +0.0, every NaN ranks above +inf and REMOVED
+ * below -inf.  out_ids int64 [B,K]; out_scores float [B,K] or NULL: the selected scores, with
+ * -0.0 written as +0.0 and a NaN as 0x7fffffff.  K <= 4096 and K <= N. */
 int b200_topk_rows_workspace_bytes(int64_t B, int64_t N, int32_t K, size_t* bytes);
 int b200_topk_rows(const float* scores, int64_t ld, int64_t B, int64_t N, int32_t K,
                    int64_t* out_ids, float* out_scores, void* workspace, size_t workspace_bytes,

@@ -134,6 +134,11 @@ for _name, (_res, _args) in SIGNATURES.items():
     _fn.argtypes = _args
 
 
+# float32 bit pattern, as an int32, of a REMOVED score (a consumed item, an empty candidate slot): the NaN 0xffffffff,
+# which b200_topk_rows ranks below every score (csrc/common.cuh kRemovedBits).  Write it through an int32 view.
+REMOVED_BITS = -1
+
+
 class B200Error(RuntimeError):
     pass
 

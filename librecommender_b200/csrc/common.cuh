@@ -39,10 +39,20 @@ inline int num_sms() {
 
 __host__ __device__ inline int64_t ceil_div64(int64_t a, int64_t b) { return (a + b - 1) / b; }
 
-// Order-preserving map float -> uint32 (larger float => larger key).
+// Float bit pattern of a REMOVED entry (a consumed item, an empty candidate slot).  It is a NaN
+// that no arithmetic produces (hardware NaNs are 0x7fffffff), and its key is 0: below every real value.
+constexpr uint32_t kRemovedBits = 0xffffffffu;
+
+// Order-preserving map float -> uint32 (larger float => larger key), one key per class of values
+// the ranking order calls equal: -0.0 takes the key of +0.0, every NaN the top key (a NaN ranks
+// above +inf, where numpy's sort puts it), and kRemovedBits key 0.  Keys in [1, key(-inf)) are unused.
+// key_to_float inverts it up to that canonicalisation (-0.0 -> +0.0, NaN -> 0x7fffffff).
 __device__ __forceinline__ uint32_t float_to_key(float f) {
   uint32_t b = __float_as_uint(f);
-  return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
+  b = b == 0x80000000u ? 0u : b;
+  const uint32_t k = (b & 0x80000000u) ? ~b : (b | 0x80000000u);
+  // NaNs land in (key(+inf), 2^32) (positive) and [1, key(-inf)) (negative; kRemovedBits gives 0)
+  return (k - 1u < 0x007ffffeu || k > 0xff800000u) ? 0xffffffffu : k;
 }
 __device__ __forceinline__ float key_to_float(uint32_t k) {
   uint32_t b = (k & 0x80000000u) ? (k & 0x7fffffffu) : ~k;

@@ -46,7 +46,9 @@ score_rows_f32_kernel(const float* __restrict__ U, int64_t ldu, const int64_t* _
 #pragma unroll
     for (int q = 0; q < 4; ++q) {
       const int k = k0 + lk + q;
-      float a = 0.f, b = 0.f;
+      // k >= d pads the last BK tile with a product of -0.0: fmaf(0, -0, acc) == acc for every acc, -0.0
+      // included (a +0.0 product would turn an accumulated -0.0 into +0.0)
+      float a = 0.f, b = -0.f;
       if (k < d) {
         if (arow >= 0) a = __ldg(U + arow * ldu + k);
         if (brow < N) b = __ldg(I + brow * ldi + k);

@@ -7,6 +7,8 @@
 // of the fp32 score, multi-CTA per row (grid = chunks x rows, per-row global histogram, the last
 // CTA of a row resolves the digit), then a count / collect pair that takes every element above
 // the K-th key plus the lowest-id ties, and a per-row bitonic sort by (score desc, id asc).
+// The key (float_to_key, common.cuh) makes -0.0 equal to +0.0, every NaN the largest value and the
+// REMOVED pattern written by mask_consumed_kernel the smallest.
 // HBM-bound integer/byte work: 5 coalesced sweeps over the row, no tensor cores.
 #include "common.cuh"
 #include "../../include/b200reco.h"
@@ -65,11 +67,12 @@ __global__ void mask_consumed_kernel(float* __restrict__ scores, int64_t ld,
   const int64_t beg = indptr[u], end = indptr[u + 1];
   const int64_t c = end - beg;
   if (c <= 0 || (int64_t)K + c > N) return;  // "cannot filter" branch: leave the row untouched
+  // removed, not -inf: a consumed item must rank below every real score, -inf and NaN included
   float* s = scores + row * ld;
-  const float ninf = __int_as_float(0xff800000);
+  const float removed = __uint_as_float(kRemovedBits);
   for (int64_t j = beg + threadIdx.x; j < end; j += blockDim.x) {
     const int32_t it = idx[j];
-    if (it >= 0 && it < N) s[it] = ninf;
+    if (it >= 0 && it < N) s[it] = removed;
   }
 }
 

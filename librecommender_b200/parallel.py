@@ -611,7 +611,9 @@ def merge_topk_shards(ids, scores, n_rec: int):
     """``ids`` int64 ``[G, B, K]`` (global item ids, -1 = no candidate), ``scores`` fp32 ``[G, B, K]`` (device
     tensors, each shard's rows sorted by (score desc, id asc)) -> ``(ids [B, n_rec], scores [B, n_rec])`` of the
     merged order.  One b200_topk_rows over the ``G*K`` candidates of a row; positions index the concatenation
-    (shard-major), which is ascending in item id among equal scores."""
+    (shard-major), which is ascending in item id among equal scores.  Empty slots are REMOVED, below every real
+    candidate (``-inf`` included), so id -1 comes back only where fewer than ``n_rec`` candidates exist; its score
+    is then ``-inf``."""
     import ctypes
 
     import torch
@@ -620,13 +622,12 @@ def merge_topk_shards(ids, scores, n_rec: int):
 
     G, B, K = ids.shape
     cat_ids = ids.permute(1, 0, 2).reshape(B, G * K).contiguous()
-    cat_sc = scores.permute(1, 0, 2).reshape(B, G * K).contiguous().clone()
-    cat_sc[cat_ids < 0] = float("-inf")
     ld = (G * K + 3) // 4 * 4
-    if ld != G * K:
-        pad = torch.full((B, ld), float("-inf"), dtype=torch.float32, device=cat_sc.device)
-        pad[:, :G * K] = cat_sc
-        cat_sc = pad
+    cat_sc = torch.empty((B, ld), dtype=torch.float32, device=scores.device)
+    cat_sc[:, :G * K] = scores.permute(1, 0, 2).reshape(B, G * K)
+    cat_bits = cat_sc.view(torch.int32)
+    cat_bits[:, G * K:] = _lib.REMOVED_BITS
+    cat_bits[:, :G * K].masked_fill_(cat_ids < 0, _lib.REMOVED_BITS)
     pos = torch.empty((B, n_rec), dtype=torch.int64, device=cat_sc.device)
     out_sc = torch.empty((B, n_rec), dtype=torch.float32, device=cat_sc.device)
     nbytes = ctypes.c_size_t(0)
@@ -634,7 +635,8 @@ def merge_topk_shards(ids, scores, n_rec: int):
     ws = torch.empty(nbytes.value, dtype=torch.uint8, device=cat_sc.device)
     _lib.check(_lib.lib.b200_topk_rows(_lib.ptr(cat_sc), cat_sc.stride(0), B, G * K, n_rec, _lib.ptr(pos), _lib.ptr(out_sc),
                                        _lib.ptr(ws), nbytes.value, _lib.current_stream()))
-    return torch.gather(cat_ids, 1, pos), out_sc
+    out_ids = torch.gather(cat_ids, 1, pos)
+    return out_ids, out_sc.masked_fill_(out_ids < 0, float("-inf"))
 
 
 class ItemShardScorer:

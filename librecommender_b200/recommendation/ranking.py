@@ -3,10 +3,16 @@
 
 * consumed filter incl. the "cannot filter" rule of ``ranking.py:38``  → ``b200_mask_consumed``
 * ``partition_select`` + descending ``argsort`` (``:48-49,:76-78``)      → ``b200_topk_rows``
-  with the total order (score desc, item id asc) where the reference leaves ties unspecified
+  with the total order (score desc, item id asc) where the reference leaves ties unspecified.
+  In that order -0.0 equals +0.0 and every NaN ranks above +inf (numpy's sort puts NaN last, so
+  the reference's reversed ``argsort`` returns it first).  Consumed items are removed, as
+  ``filter_items`` does: they are overwritten with the REMOVED pattern, which ranks below every
+  score, so a consumed item never comes back even where the answer reaches ``-inf`` scores.
+  Returned scores write -0.0 as +0.0 and every NaN as one NaN.
 * ``random_rec`` (``:65-73``: sample ``n_rec`` without replacement with
   p ∝ softmax(preds)^0.75 + 1e-8) → Gumbel-top-K over ``log p`` through the same
   kernel (the reference's own RNG here is unseeded, so only the distribution is defined).
+  A ``-inf`` prediction keeps the ``1e-8`` floor and can be drawn; a consumed item cannot.
 """
 from __future__ import annotations
 
@@ -56,22 +62,22 @@ def rank_recommendations(
     stream = _lib.current_stream()
     lib = _lib.lib
 
-    work = preds.clone() if (filter_consumed or random_rec) else preds  # never clobber caller data
-    work = work.contiguous()
+    # a copy (never clobber caller data) with one NaN pattern: a caller's NaN must not read as REMOVED
+    work = preds.masked_fill(torch.isnan(preds), float("nan")).contiguous()
     ld = work.stride(0)
     if filter_consumed and csr.nnz > 0:
         _lib.check(lib.b200_mask_consumed(_lib.ptr(work), ld, _lib.ptr(uid), B, n_items, n_rec,
                                           _lib.ptr(indptr_d), _lib.ptr(idx_d), csr.n_users, stream))
     select_on = work
     if random_rec:
-        # log p = log(softmax^0.75 + 1e-8) (unnormalised is enough); Gumbel-top-K samples
-        # without replacement from p.  Masked (-inf) entries get p = 0 exactly.
-        masked = torch.isinf(work) & (work < 0)
-        logp = torch.log(torch.softmax(work.double(), dim=1).pow(0.75) + 1e-8)
+        # log p = log(softmax^0.75 + 1e-8) (unnormalised is enough); Gumbel-top-K samples without replacement
+        # from p.  Removed (consumed) entries stay removed; the softmax sees them as -inf, i.e. it runs over the
+        # kept items only, like the reference's after filter_items.
+        removed = work.view(torch.int32) == _lib.REMOVED_BITS
+        logp = torch.log(torch.softmax(work.double().masked_fill(removed, float("-inf")), dim=1).pow(0.75) + 1e-8)
         g = -torch.log(-torch.log(torch.rand_like(logp).clamp_min(1e-300)))
-        select_on = (logp + g).float()
-        select_on[masked] = float("-inf")
-        select_on = select_on.contiguous()
+        select_on = (logp + g).float().contiguous()
+        select_on.view(torch.int32).masked_fill_(removed, _lib.REMOVED_BITS)
     out_ids = torch.empty((B, n_rec), dtype=torch.int64, device=device)
     out_scores = torch.empty((B, n_rec), dtype=torch.float32, device=device)
     nbytes = ctypes.c_size_t(0)

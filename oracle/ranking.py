@@ -19,7 +19,8 @@ the unmodified reference on random inputs (``tests/golden/gen_ranking.py``).
 Tie rule.  The reference leaves the order of equal scores unspecified
 (``np.argpartition`` + reversed unstable ``np.argsort``, ranking.py:48,76-78).
 The restatement uses the total order (score descending, item id ascending);
-it equals the reference wherever the reference's answer is unique.
+it equals the reference wherever the reference's answer is unique.  Special values
+follow the reference's numpy order: -0.0 == +0.0, and every NaN ranks above +inf.
 """
 from __future__ import annotations
 
@@ -42,10 +43,15 @@ def build_consumed_unique(user_indices, item_indices):
 
 
 def _row_topk(scores: np.ndarray, ids: np.ndarray, n_rec: int):
-    """Top ``n_rec`` of one row under (score desc, id asc)."""
+    """Top ``n_rec`` of one row under (score desc, id asc), where -0.0 == +0.0 and every NaN ranks
+    above +inf: numpy sorts NaN last, so the reference's reversed ``argsort`` returns it first."""
     # lexsort: last key is primary.  -scores ascending == scores descending.
     n = len(scores)
-    if n > 4 * n_rec + 1024:
+    nan = np.isnan(scores)
+    if nan.any():
+        neg = np.where(nan, 0.0, -scores.astype(np.float64))
+        order = np.lexsort((ids, neg, ~nan))[:n_rec]
+    elif n > 4 * n_rec + 1024:
         # same answer, less sorting: every item of the top n_rec has a score >= the n_rec-th largest
         # value v, so only the items with score >= v (ties at v included) need the full ordering
         v = np.partition(scores, n - n_rec)[n - n_rec]
@@ -81,10 +87,12 @@ def rank_recommendations(
         consumed = user_consumed[user] if user in user_consumed else []
         row, ids = preds[r], base_ids
         # ranking.py:38 — the filter is skipped unless K + len(consumed) <= N,
-        # where len() counts duplicates left by the consecutive-only dedup.
+        # where len() counts duplicates left by the consecutive-only dedup.  ``filter_items``
+        # (np.isin) removes the listed ids that exist; ids outside [0, n_items) match nothing.
         if filter_consumed and len(consumed) > 0 and n_rec + len(consumed) <= n_items:
             keep = np.ones(n_items, dtype=bool)
-            keep[np.asarray(consumed, dtype=np.int64)] = False
+            c = np.asarray(consumed, dtype=np.int64)
+            keep[c[(c >= 0) & (c < n_items)]] = False
             row, ids = row[keep], ids[keep]
         out_ids[r], out_scores[r] = _row_topk(row, ids, n_rec)
     if return_scores:
