@@ -230,9 +230,10 @@ int b200_scatter_add_rows(float* table, int64_t ld, int32_t d, const int64_t* id
                           const float* rows, int64_t ld_rows, void* stream);
 
 /* Y = act(X Wt^T + b): tf_dense (libreco/layers/dense.py:52-80) with BN folded by the caller.
- * Wt is the TRANSPOSED kernel [dout, din]; fp32 SIMT (exact fma chain in k). */
+ * Wt is the TRANSPOSED kernel [dout, din]; fp32 SIMT (exact fma chain in k).  act is an activation code:
+ * 0 none, 1 relu, 2 swish x / (1 + expf(-x)) (layers/activation.py:10-11); any other value returns -2. */
 int b200_linear_f32(const float* X, int64_t ldx, int64_t R, const float* Wt, int64_t ldw,
-                    const float* bias, int32_t din, int32_t dout, int32_t relu, float* Y,
+                    const float* bias, int32_t din, int32_t dout, int32_t act, float* Y,
                     int64_t ldy, void* stream);
 
 /* Same contract as b200_linear_f32 on the tensor cores (wgmma): operands split x = hi + lo into
@@ -246,15 +247,15 @@ int64_t b200_linear_tf32x3_split_ld(int32_t din);
 int b200_linear_tf32x3_split_weights(const float* Wt, int64_t ldw, int32_t din, int32_t dout, float* Wsplit,
                                      void* stream);
 int b200_linear_tf32x3(const float* X, int64_t ldx, int64_t R, const float* Wt, int64_t ldw,
-                       const float* Wsplit, const float* bias, int32_t din, int32_t dout, int32_t relu,
+                       const float* Wsplit, const float* bias, int32_t din, int32_t dout, int32_t act,
                        float* Y, int64_t ldy, void* stream);
 
 /* Split-K form for products with few output tiles and a long reduction (the weight gradients dWt = dY^T X of
  * the training steps: 1792 x 128 outputs over 8192 rows = 14 tiles): `splits` CTAs along the reduction per
  * output tile write partial products into workspace (splits * R * dout floats), a second kernel adds them in a
- * fixed order (+ bias, ReLU).  splits == 1 is b200_linear_tf32x3 without a pre-split weight copy. */
+ * fixed order (+ bias, activation).  splits == 1 is b200_linear_tf32x3 without a pre-split weight copy. */
 int b200_linear_tf32x3_splitk(const float* X, int64_t ldx, int64_t R, const float* Wt, int64_t ldw, const float* bias,
-                              int32_t din, int32_t dout, int32_t relu, int32_t splits, float* workspace,
+                              int32_t din, int32_t dout, int32_t act, int32_t splits, float* workspace,
                               size_t workspace_bytes, float* Y, int64_t ldy, void* stream);
 
 /* ---- training step of the FM-family models (SURVEY.md 8f-1; reference graph in training mode:
@@ -551,6 +552,42 @@ int b200_autoint_attention_backward(const float* Q, int64_t ldq, const float* K,
                                     int64_t ldv, const float* O, int64_t ldo, const float* lse, const float* dO,
                                     int64_t lddo, int64_t R, int32_t F, int32_t num_heads, int32_t head_dim,
                                     float scale, float* dQ, float* dK, float* dV, int64_t ldg, void* stream);
+
+/* ---- Transformer inference (libreco/algorithms/transformer.py:203-339, layers/transformer.py) --------
+ * G [n_items+1, Kp] is the item feature table (combine_seq_features), pos [T, Kpos] the positional table,
+ * D = Kp + Kpos.  Slot s encodes the sequence seqs[users[s], :T] with len = lens[s] (clamped to [0, T]):
+ *   X = [G[seq_t] || pos_t];  per layer:  a = MHA(rms_att(X)) + X;  X = a + gelu_erf(rms_ffn(a) W1) W2;
+ *   S[s] = rms_last(X)  [T, D]  (S: [n_slots, T, D] contiguous).
+ * rms(x) = x / sqrt(mean(x^2) + 1e-8) * scale.  MHA: num_heads heads of D / num_heads columns, no biases, scores
+ * <q, k> / sqrt(hd); key k is visible to query q when k < len, or k <= q with `causal` (the reference ORs the two
+ * masks); a hidden score becomes fl32(score - 1e9).  weights: per layer rms_att [D], Wq, Wk, Wv, Wo [D, D] (Wv the
+ * EFFECTIVE value map), rms_ffn [D], W1 [D, 4D], W2 [4D, D], row-major; rms_last [D].  Every dot product is one
+ * fmaf chain over an ascending index; the softmax is max, expf, an ascending sum, then a division.
+ * Supported: 1 <= T <= 64, 1 <= D <= 128, 1 <= n_layers <= 4, num_heads dividing D; anything else returns -2
+ * before launching.
+ * b200_transformer_pair_scores: scores[b * lds + n] for every slot b < B and item n < N:
+ *   p = softmax_t(<Qi[n], S[b, t]>) over t < lens[b] (over all T with every score - 1e9 when lens[b] = 0),
+ *   h1 = swish(Pu[b] + Pi[n] + sum_t p_t Vp[b*T + t]),  h2 = h1 W2 + b2,
+ *   H3 > 0: out = <swish(h2) W3 + b3, w_out> + b_out;  H3 = 0: out = <h2, w_out> + b_out.
+ * Qi [N, ldq] = [rms_item(G[n]) || 1..1], Vp [B*T, H1] = S W1_seq, Pu [B, H1] (first-layer bias included),
+ * Pi [N, ldpi], W2 [H1, H2], W3 [H2, H3] (row-major, BN folded).  Supported: H1 <= 256, H2 <= 64, H3 <= 32,
+ * B <= 65535 and b200_transformer_pair_smem_bytes(T, D, H1) within the device's shared-memory opt-in.
+ * b200_transformer_target_attention: out[r, :D] = sum_t p_t S[slot, t] for row r, slot = slot_of_row[r] and
+ * item = items[r] (explicit rows) or, both NULL, row g = row_offset + r of the grid: slot g / grid_items, item
+ * g % grid_items. */
+int b200_transformer_encode(const int64_t* users, int64_t n_slots, const int32_t* lens, const int32_t* seqs,
+                            int64_t ld_seq, const float* G, int64_t ldg, int32_t Kp, const float* pos, int32_t Kpos,
+                            int32_t T, int32_t num_heads, int32_t n_layers, int32_t causal, const float* weights,
+                            const float* rms_last, float* S, void* stream);
+int64_t b200_transformer_pair_smem_bytes(int32_t T, int32_t D, int32_t H1);
+int b200_transformer_pair_scores(const float* Qi, int64_t ldq, int64_t N, const float* S, const float* Vp,
+                                 const float* Pu, const int32_t* lens, int64_t B, const float* Pi, int64_t ldpi,
+                                 int32_t T, int32_t D, int32_t H1, int32_t H2, int32_t H3, const float* W2,
+                                 const float* b2, const float* W3, const float* b3, const float* w_out, float b_out,
+                                 float* scores, int64_t lds, void* stream);
+int b200_transformer_target_attention(const float* Qi, int64_t ldq, const float* S, int32_t T, int32_t D,
+                                      const int32_t* lens, const int32_t* slot_of_row, const int64_t* items, int64_t n,
+                                      int64_t grid_items, int64_t row_offset, float* out, int64_t ldo, void* stream);
 
 /* ---- a14: predict_from_embedding (libreco/prediction/predict.py:36-40) -----------------
  * out[r] = sum_k U[users[r],k] * I[items[r],k]; mode 0: raw, 1: expit (ranking),

@@ -122,6 +122,14 @@ SIGNATURES = {
                                   _P, _P]),
     "b200_autoint_grid": (c_int, [_P, c_int64, c_int64, _P, c_int64, c_int64, _P, c_int32, c_int32, c_int32, c_int32, _P,
                                   _P, _P, c_float, c_int32, _P, c_int64, _P]),
+    "b200_transformer_encode": (c_int, [_P, c_int64, _P, _P, c_int64, _P, c_int64, c_int32, _P, c_int32, c_int32,
+                                        c_int32, c_int32, c_int32, _P, _P, _P, _P]),
+    "b200_transformer_pair_smem_bytes": (c_int64, [c_int32, c_int32, c_int32]),
+    "b200_transformer_pair_scores": (c_int, [_P, c_int64, c_int64, _P, _P, _P, _P, c_int64, _P, c_int64, c_int32,
+                                             c_int32, c_int32, c_int32, c_int32, _P, _P, _P, _P, _P, c_float, _P,
+                                             c_int64, _P]),
+    "b200_transformer_target_attention": (c_int, [_P, c_int64, _P, c_int32, c_int32, _P, _P, _P, c_int64, c_int64,
+                                                  c_int64, _P, c_int64, _P]),
     "b200_autoint_attention_forward": (c_int, [_P, c_int64, _P, c_int64, _P, c_int64, c_int64, c_int32, c_int32,
                                                c_int32, c_float, _P, c_int64, _P, _P]),
     "b200_autoint_attention_backward": (c_int, [_P, c_int64, _P, c_int64, _P, c_int64, _P, c_int64, _P, _P, c_int64,

@@ -59,6 +59,12 @@ __device__ __forceinline__ float key_to_float(uint32_t k) {
   return __uint_as_float(b);
 }
 
+// Activation code of the b200_linear_* dense layers: 0 none, 1 relu, 2 swish x / (1 + exp(-x))
+// (layers/activation.py:10-11, the Transformer's MLP)
+__device__ __forceinline__ float apply_act(float v, int act) {
+  return act == 1 ? fmaxf(v, 0.f) : (act == 2 ? v / (1.0f + expf(-v)) : v);
+}
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

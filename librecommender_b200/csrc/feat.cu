@@ -902,11 +902,12 @@ feat_forward_async_kernel(const b200_feat_layout L, const b200_feat_tables T,
   }
 }
 
-// y[r, n] = act(sum_k x[r,k] * Wt[n,k] + b[n]) — 64x64x16 register-tiled SIMT GEMM (fp32, exact fma chain)
+// y[r, n] = act(sum_k x[r,k] * Wt[n,k] + b[n]) — 64x64x16 register-tiled SIMT GEMM (fp32, exact fma chain);
+// act: 0 none, 1 relu, 2 swish (apply_act)
 constexpr int LM = 64, LN = 64, LK = 16;
 __global__ void __launch_bounds__(256)
 linear_f32_kernel(const float* __restrict__ X, int64_t ldx, int64_t R, const float* __restrict__ Wt,
-                  int64_t ldw, const float* __restrict__ bias, int din, int dout, int relu,
+                  int64_t ldw, const float* __restrict__ bias, int din, int dout, int act,
                   float* __restrict__ Y, int64_t ldy) {
   __shared__ float Xs[LK][LM + 4];
   __shared__ float Ws[LK][LN + 4];
@@ -956,8 +957,7 @@ linear_f32_kernel(const float* __restrict__ X, int64_t ldx, int64_t R, const flo
       const int n = n0 + tx + 16 * j;
       if (n < dout) {
         float v = acc[i][j] + (bias ? bias[n] : 0.f);
-        if (relu) v = fmaxf(v, 0.f);
-        Y[r * ldy + n] = v;
+        Y[r * ldy + n] = apply_act(v, act);
       }
     }
   }
@@ -1220,9 +1220,10 @@ extern "C" int b200_scatter_add_rows(float* table, int64_t ld, int32_t d, const 
 }
 
 extern "C" int b200_linear_f32(const float* X, int64_t ldx, int64_t R, const float* Wt, int64_t ldw,
-                               const float* bias, int32_t din, int32_t dout, int32_t relu, float* Y,
+                               const float* bias, int32_t din, int32_t dout, int32_t act, float* Y,
                                int64_t ldy, void* stream) {
   B200_REQUIRE(X && Wt && Y, "b200_linear_f32: null pointer");
+  B200_REQUIRE(act >= 0 && act <= 2, "b200_linear_f32: activation code %d outside [0, 2]", act);
   if (R == 0) return 0;
   const int64_t gy = ceil_div64(R, LM);
   B200_REQUIRE(gy <= 65535 * 32ll, "b200_linear_f32: too many rows");
@@ -1232,7 +1233,7 @@ extern "C" int b200_linear_f32(const float* X, int64_t ldx, int64_t R, const flo
     const int64_t r0 = y0 * LM;
     dim3 grid((unsigned)ceil_div64(dout, LN), (unsigned)ny);
     linear_f32_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(X + r0 * ldx, ldx, R - r0, Wt, ldw, bias, din,
-                                                              dout, relu, Y + r0 * ldy, ldy);
+                                                              dout, act, Y + r0 * ldy, ldy);
     count_launch();
   }
   B200_CUDA_OK(cudaGetLastError());

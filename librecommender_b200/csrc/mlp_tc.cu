@@ -42,7 +42,7 @@ struct Params {
   const float* bias;
   float* Y;
   const float* dot_w;     // fused DIN epilogue: 16 weights of the Dense(1) on sigmoid(Dense(16)) (NULL = plain layer)
-  int din, dout, n_pad, relu;
+  int din, dout, n_pad, act;
   int n_tiles, n_chunks, nstage;
   int n_chunks_total;      // split-K: CTA z takes k-chunks [z * n_chunks, min((z + 1) * n_chunks, n_chunks_total))
   int64_t split_stride;    //          and writes its partial product to Y + z * split_stride (no bias / ReLU)
@@ -226,7 +226,7 @@ linear_tf32x3_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_const
 #pragma unroll
           for (int e = 0; e < 2; ++e) {
             const float v = y[4 * j + 2 * rs + e] + ss->bias_s[c + e];
-            o[e] = p.relu ? fmaxf(v, 0.f) : v;
+            o[e] = apply_act(v, p.act);
           }
           if (vec && c + 1 < ncol) {
             *(float2*)(yr + c) = make_float2(o[0], o[1]);
@@ -243,7 +243,7 @@ linear_tf32x3_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_const
 
 // split-K: Y[r, c] = act(sum_z part[z][r, c] + bias[c]) in a fixed order (deterministic)
 __global__ void splitk_reduce_kernel(const float* __restrict__ part, int splits, int64_t R, int dout,
-                                     const float* __restrict__ bias, int relu, float* __restrict__ Y, int64_t ldy) {
+                                     const float* __restrict__ bias, int act, float* __restrict__ Y, int64_t ldy) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= R * dout) return;
   const int64_t r = i / dout;
@@ -251,7 +251,7 @@ __global__ void splitk_reduce_kernel(const float* __restrict__ part, int splits,
   float v = 0.f;
   for (int z = 0; z < splits; ++z) v += part[(int64_t)z * R * dout + i];
   if (bias) v += __ldg(bias + c);
-  Y[r * ldy + c] = relu ? fmaxf(v, 0.f) : v;
+  Y[r * ldy + c] = apply_act(v, act);
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*,
@@ -308,14 +308,14 @@ extern "C" int b200_linear_tf32x3_split_weights(const float* Wt, int64_t ldw, in
 
 static int launch_linear_tf32x3(const float* X, int64_t ldx, int64_t R, const float* Wt, int64_t ldw,
                                 const float* Wsplit, const float* bias, int32_t din, int32_t dout,
-                                int32_t relu, const float* dot_w, float* Y, int64_t ldy, void* stream,
+                                int32_t act, const float* dot_w, float* Y, int64_t ldy, void* stream,
                                 int splits = 1, float* workspace = nullptr);
 
 extern "C" int b200_linear_tf32x3(const float* X, int64_t ldx, int64_t R, const float* Wt, int64_t ldw,
                                   const float* Wsplit, const float* bias, int32_t din, int32_t dout,
-                                  int32_t relu, float* Y, int64_t ldy, void* stream) {
+                                  int32_t act, float* Y, int64_t ldy, void* stream) {
   B200_REQUIRE(ldy >= dout, "leading dimension too small");
-  return launch_linear_tf32x3(X, ldx, R, Wt, ldw, Wsplit, bias, din, dout, relu, nullptr, Y, ldy, stream);
+  return launch_linear_tf32x3(X, ldx, R, Wt, ldw, Wsplit, bias, din, dout, act, nullptr, Y, ldy, stream);
 }
 
 extern "C" int b200_linear_tf32x3_sigmoid_dot(const float* X, int64_t ldx, int64_t R, const float* Wt, int64_t ldw,
@@ -327,23 +327,24 @@ extern "C" int b200_linear_tf32x3_sigmoid_dot(const float* X, int64_t ldx, int64
 }
 
 extern "C" int b200_linear_tf32x3_splitk(const float* X, int64_t ldx, int64_t R, const float* Wt, int64_t ldw,
-                                         const float* bias, int32_t din, int32_t dout, int32_t relu, int32_t splits,
+                                         const float* bias, int32_t din, int32_t dout, int32_t act, int32_t splits,
                                          float* workspace, size_t workspace_bytes, float* Y, int64_t ldy, void* stream) {
   B200_REQUIRE(splits >= 1 && splits <= 64, "b200_linear_tf32x3_splitk: splits outside [1, 64]");
   B200_REQUIRE(ldy >= dout, "leading dimension too small");
   B200_REQUIRE(splits == 1 || (workspace && workspace_bytes >= (size_t)splits * (size_t)R * (size_t)dout * 4),
                "b200_linear_tf32x3_splitk: workspace too small (splits * R * dout floats)");
-  return launch_linear_tf32x3(X, ldx, R, Wt, ldw, nullptr, bias, din, dout, relu, nullptr, Y, ldy, stream, splits,
+  return launch_linear_tf32x3(X, ldx, R, Wt, ldw, nullptr, bias, din, dout, act, nullptr, Y, ldy, stream, splits,
                               workspace);
 }
 
 static int launch_linear_tf32x3(const float* X, int64_t ldx, int64_t R, const float* Wt, int64_t ldw,
                                 const float* Wsplit, const float* bias, int32_t din, int32_t dout,
-                                int32_t relu, const float* dot_w, float* Y, int64_t ldy, void* stream,
+                                int32_t act, const float* dot_w, float* Y, int64_t ldy, void* stream,
                                 int splits, float* workspace) {
   using namespace b200;
   using namespace b200::mlp;
   B200_REQUIRE(R >= 0 && din > 0 && dout > 0, "bad shape");
+  B200_REQUIRE(act >= 0 && act <= 2, "b200_linear_tf32x3: activation code %d outside [0, 2]", act);
   B200_REQUIRE((ldx & 3) == 0 && ((uintptr_t)X & 15) == 0, "b200_linear_tf32x3 needs 16-byte aligned X rows (ldx % 4 == 0)");
   B200_REQUIRE(Wsplit ? (((uintptr_t)Wsplit & 15) == 0) : ((ldw & 3) == 0 && ((uintptr_t)Wt & 15) == 0),
                "b200_linear_tf32x3 needs 16-byte aligned weight rows (ldw % 4 == 0) or a split copy");
@@ -357,19 +358,19 @@ static int launch_linear_tf32x3(const float* X, int64_t ldx, int64_t R, const fl
   p.Y = Y;
   p.din = din;
   p.dout = dout;
-  p.relu = relu;
+  p.act = act;
   p.n_pad = dout >= NMAX ? NMAX : (dout + 31) / 32 * 32;
   p.n_tiles = (int)((R + TM - 1) / TM);
   p.n_chunks_total = (din + KC - 1) / KC;
   p.n_chunks = (p.n_chunks_total + splits - 1) / splits;
   splits = (p.n_chunks_total + p.n_chunks - 1) / p.n_chunks;        // no empty split
   p.split_stride = 0;
-  if (splits > 1) {   // partial products [splits][R, dout] into the workspace, bias / ReLU in the reduction
+  if (splits > 1) {   // partial products [splits][R, dout] into the workspace, bias / activation in the reduction
     p.split_stride = R * (int64_t)dout;
     p.Y = workspace;
     p.ldy = dout;
     p.bias = nullptr;
-    p.relu = 0;
+    p.act = 0;
   }
   const int stage_bytes = 2 * A_BYTES + 2 * p.n_pad * KC * 4;
   p.nstage = min(MAXSTAGE, (200 * 1024) / stage_bytes);
@@ -414,7 +415,7 @@ static int launch_linear_tf32x3(const float* X, int64_t ldx, int64_t R, const fl
   if (rc) return rc;
   if (splits > 1) {
     const int64_t n = R * (int64_t)dout;
-    splitk_reduce_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(workspace, splits, R, dout, bias, relu, Y, ldy);
+    splitk_reduce_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(workspace, splits, R, dout, bias, act, Y, ldy);
     count_launch();
   }
   B200_CUDA_OK(cudaGetLastError());

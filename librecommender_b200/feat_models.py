@@ -137,8 +137,12 @@ def split_weights(Wt):
     return hit[0]
 
 
-def linear(x, Wt, b, relu, cache_split=True):
-    """tf_dense (libreco/layers/dense.py:52-80) with BN folded: act(x Wt^T + b), fp32 device tensors."""
+ACT_NONE, ACT_RELU, ACT_SWISH = 0, 1, 2     # activation codes of b200_linear_* (include/b200reco.h)
+
+
+def linear(x, Wt, b, act, cache_split=True):
+    """tf_dense (libreco/layers/dense.py:52-80) with BN folded: act(x Wt^T + b), fp32 device tensors.  ``act`` is an
+    activation code (a bool reads as relu on / off): 0 none, 1 relu, 2 swish."""
     import torch
 
     R, din, dout = x.shape[0], Wt.shape[1], Wt.shape[0]
@@ -158,18 +162,18 @@ def linear(x, Wt, b, relu, cache_split=True):
         if splits > 1:
             part = torch.empty(splits * R * dout, dtype=torch.float32, device=x.device)
             _lib.check(_lib.lib.b200_linear_tf32x3_splitk(_lib.ptr(x), x.stride(0), R, _lib.ptr(Wt), Wt.stride(0), bp, din,
-                                                          dout, 1 if relu else 0, splits, _lib.ptr(part),
+                                                          dout, int(act), splits, _lib.ptr(part),
                                                           part.numel() * 4, _lib.ptr(y), y.stride(0),
                                                           _lib.current_stream()))
             return y
     if use_tc and aligned and w_ok:
         ws = split_weights(Wt) if cache_split else None
         _lib.check(_lib.lib.b200_linear_tf32x3(_lib.ptr(x), x.stride(0), R, _lib.ptr(Wt), Wt.stride(0), _lib.ptr(ws), bp,
-                                               din, dout, 1 if relu else 0, _lib.ptr(y), y.stride(0),
+                                               din, dout, int(act), _lib.ptr(y), y.stride(0),
                                                _lib.current_stream()))
     else:
         _lib.check(_lib.lib.b200_linear_f32(_lib.ptr(x), x.stride(0), R, _lib.ptr(Wt), Wt.stride(0), bp, din, dout,
-                                            1 if relu else 0, _lib.ptr(y), y.stride(0), _lib.current_stream()))
+                                            int(act), _lib.ptr(y), y.stride(0), _lib.current_stream()))
     return y
 
 
@@ -193,9 +197,10 @@ def fold_bn(bn):
     return scale, shift
 
 
-def fold_mlp(mlp):
-    """dense_nn (libreco/layers/dense.py:12-49) -> [(Wt [dout, din], bias, relu)], BN folded into
-    the Dense that FOLLOWS it: Dense(BN(a)) = a (diag(s) W) + (t W + b)."""
+def fold_mlp(mlp, act=ACT_RELU):
+    """dense_nn (libreco/layers/dense.py:12-49) -> [(Wt [dout, din], bias, act)], BN folded into
+    the Dense that FOLLOWS it: Dense(BN(a)) = a (diag(s) W) + (t W + b).  ``act``: the activation code of the
+    hidden layers (relu, or swish for the Transformer); the last layer has none."""
     layers = []
     scale, shift = fold_bn(mlp.get("bn_in"))
     n = len(mlp["kernels"])
@@ -205,7 +210,7 @@ def fold_mlp(mlp):
         if scale is not None:
             b = (shift @ W + b).astype(np.float32)
             W = (scale[:, None] * W).astype(np.float32)
-        layers.append((np.ascontiguousarray(W.T), b, i != n - 1))
+        layers.append((np.ascontiguousarray(W.T), b, i != n - 1 if act == ACT_RELU else (act if i != n - 1 else 0)))
         scale, shift = (None, None)
         if i != n - 1 and mlp.get("bns"):
             scale, shift = fold_bn(mlp["bns"][i])
@@ -641,14 +646,14 @@ class _FeatModelBase:
 
     def _mlp(self, x, layers):
         torch = self._torch
-        for Wt, b, relu in layers:
-            x = linear(x, Wt, b, relu)
+        for Wt, b, act in layers:
+            x = linear(x, Wt, b, act)
         return x
 
-    def _upload_mlp(self, mlp):
+    def _upload_mlp(self, mlp, act=ACT_RELU):
         torch = self._torch
-        return [(_dev(Wt, self.device, torch.float32), _dev(b, self.device, torch.float32), relu)
-                for Wt, b, relu in fold_mlp(mlp)]
+        return [(_dev(Wt, self.device, torch.float32), _dev(b, self.device, torch.float32), a)
+                for Wt, b, a in fold_mlp(mlp, act)]
 
 
 class FM(_FeatModelBase):
@@ -1079,6 +1084,198 @@ class DIN(_SeqModelBase):
             self.seqs.stride(0), _lib.ptr(self.lens), self.T, _lib.ptr(users_d), n, grid_items, row_offset,
             _lib.ptr(self.att["k1"]), _lib.ptr(self.att["b1"]), _lib.ptr(self.att["k2"]), self.att["b2"],
             _lib.ptr(out_view), out_view.stride(0), _lib.current_stream()))
+
+
+TRANSFORMER_MAX_T = 64          # the shapes b200_transformer_* accept (include/b200reco.h)
+TRANSFORMER_MAX_D = 128
+TRANSFORMER_MAX_LAYERS = 4
+
+
+def sinusoidal_positions(T, d):
+    """The non-trainable positional table of ``positional_encoding`` (libreco/layers/transformer.py:113-144), [T, d]:
+    column c holds t / 10000^(2 floor(c/2) / d), through sin for even c and cos for odd c (odd d included)."""
+    ang = np.arange(T, dtype=np.float64)[:, None] / np.power(10000.0, (np.arange(d) // 2 * 2) / d)[None, :]
+    pe = np.where(np.arange(d)[None, :] % 2 == 0, np.sin(ang), np.cos(ang))
+    return pe.astype(np.float32)
+
+
+def _rms(x, scale):
+    """rms_norm (layers/normalization.py:21-29) on device tensors: x / sqrt(mean(x^2) + 1e-8) * scale."""
+    return x * (x.square().mean(dim=-1, keepdim=True) + 1e-8).rsqrt() * scale
+
+
+class Transformer(_SeqModelBase):
+    """libreco/algorithms/transformer.py:203-339 (inference): the BST-style sequence model.  The user's recent items
+    (rows of the item feature table G, ``combine_seq_features`` in ``concat`` or ``elementwise`` mode) and a positional
+    table [T, K] form X [T, D = K' + K]; ``L`` layers of pre-norm multi-head self-attention + gelu FFN and a final RMS
+    norm give S_u [T, D]; the target item's query [rms_item(G[n]) || 1..1] attends over S_u (Keras dot-product
+    attention, no scale); ``dense_nn`` with swish on [user, item, sparse.., dense.., s_u], then Dense(1).
+
+    Weights (besides the embedding tables): ``tfm_layers`` = [{rms_att, wq, wk, wv, wo, rms_ffn, w1, w2}] per layer
+    (``wv`` the effective value map), ``rms_last``, ``rms_item``, ``positional_encoding`` (absent: sinusoidal),
+    ``num_heads``, ``use_causal_mask``, ``feat_agg_mode``, ``ln_sparse`` / ``ln_dense`` ({scale, bias}; elementwise
+    mode), ``mlp``, ``out_kernel``, ``out_bias`` — :func:`weights_io.transformer_weights` makes them from either
+    TensorFlow graph's variables.
+
+    The encoder runs ONCE per user of a call (``b200_transformer_encode``).  All-items scoring splits the first MLP
+    layer into a per-model item part Pi, a per-call user part Pu and V'_u = S_u W1_seq, and ``b200_transformer_pair_scores``
+    finishes every pair; rows mode (``predict``, feature rows, ``recommend_dynamic`` with features, an MLP outside the
+    pair kernel's envelope) encodes each distinct user of a chunk once and writes s_u into the concat
+    (``b200_transformer_target_attention``) for the swish MLP on the library's dense layers."""
+
+    def __init__(self, spec, weights, recent_seqs, recent_seq_lens, user_consumed=None, task="ranking",
+                 device=None):
+        raw_is = None
+        if not isinstance(spec, FeatSpec):
+            g = _spec_get(spec)
+            raw_is = g("item_sparse_unique") if g("item_sparse_col_index") else None
+        super().__init__(spec, weights, recent_seqs, recent_seq_lens, user_consumed, task, device)
+        torch = self._torch
+        f32 = torch.float32
+        K, T, F = self.K, self.T, self.F
+        self.feat_agg_mode = weights.get("feat_agg_mode", "concat")
+        if self.feat_agg_mode not in ("concat", "elementwise"):
+            raise ValueError("Transformer: `feat_agg_mode` must be `concat` or `elementwise`")
+        # combine_seq_features reads the item sparse columns as they are (multi-sparse sub-columns one by one)
+        self._item_sparse = _dev(raw_is, self.device, torch.int32) if raw_is is not None else self.spec.is_
+        self.ln = {k: {n: _dev(np.asarray(v[n]).reshape(-1), self.device, f32) for n in ("scale", "bias")}
+                   for k, v in (("sparse", weights.get("ln_sparse")), ("dense", weights.get("ln_dense"))) if v is not None}
+        self.rms_item = _dev(np.asarray(weights["rms_item"]).reshape(-1), self.device, f32)
+        self._rebuild_item_features()
+        self.Kp = int(self.G.shape[1])
+        D = self.D = self.Kp + K
+        H = self.num_heads = int(weights["num_heads"])
+        layers = list(weights["tfm_layers"])
+        if T > TRANSFORMER_MAX_T:
+            raise ValueError(f"Transformer: sequence length {T} > {TRANSFORMER_MAX_T} is not supported")
+        if D > TRANSFORMER_MAX_D:
+            raise ValueError(f"Transformer: model width {D} (item features {self.Kp} + positions {K}) > "
+                             f"{TRANSFORMER_MAX_D} is not supported")
+        if not 1 <= len(layers) <= TRANSFORMER_MAX_LAYERS:
+            raise ValueError(f"Transformer: {len(layers)} layers, supported 1..{TRANSFORMER_MAX_LAYERS}")
+        if H < 1 or D % H:
+            raise ValueError(f"Transformer: width {D} must be divisible by num_heads {H}")
+        if self.rms_item.numel() != self.Kp:
+            raise ValueError(f"Transformer: rms_item has {self.rms_item.numel()} entries, expected {self.Kp}")
+        shapes = dict(rms_att=(D,), wq=(D, D), wk=(D, D), wv=(D, D), wo=(D, D), rms_ffn=(D,), w1=(D, 4 * D),
+                      w2=(4 * D, D))
+        packed = []
+        for i, lw in enumerate(layers):
+            for k, shp in shapes.items():
+                a = np.asarray(lw[k], dtype=np.float32)
+                if a.shape != shp:
+                    raise ValueError(f"Transformer layer {i}: {k} has shape {a.shape}, expected {shp}")
+                packed.append(a.reshape(-1))
+        self.n_layers = len(layers)
+        self.w_layers = _dev(np.concatenate(packed), self.device, f32)
+        self.rms_last = _dev(np.asarray(weights["rms_last"], dtype=np.float32).reshape(-1), self.device, f32)
+        if self.rms_last.numel() != D:
+            raise ValueError(f"Transformer: rms_last has {self.rms_last.numel()} entries, expected {D}")
+        pos = weights.get("positional_encoding")
+        pos = sinusoidal_positions(T, K) if pos is None else np.asarray(pos, dtype=np.float32)
+        if pos.shape != (T, K):
+            raise ValueError(f"Transformer: positional table has shape {pos.shape}, expected ({T}, {K})")
+        self.pos = _dev(pos, self.device, f32)
+        self.causal = bool(weights.get("use_causal_mask", False))
+        self.extra = D
+        self.mlp = self._upload_mlp(weights["mlp"], ACT_SWISH)
+        if self.mlp[0][0].shape[1] != F * K + D:
+            raise ValueError(f"Transformer: the first MLP layer takes {self.mlp[0][0].shape[1]} inputs, expected "
+                             f"F*K + D = {F}*{K} + {D}")
+
+    def _rebuild_item_features(self):
+        """G [n_items+1, K'] (combine_seq_features, tfops/features.py:151-236) and the target queries
+        Qi = [rms_item(G) || 1..1] [n_items+1, D]: once per set of tables (again after ``assign_oov``)."""
+        torch = self._torch
+        E = self.t["item_embeds"]
+        n = self.n_items + 1
+        sp = self.t["sparse_embeds"][self._item_sparse.long()] if self._item_sparse is not None else None
+        de = None
+        if self.spec.id_ is not None:
+            cols = torch.as_tensor(self.spec.item_dense_cols, device=self.device)
+            de = self.spec.id_[:, :, None] * self.t["dense_embeds"][cols][None]
+        if self.feat_agg_mode == "concat":
+            self.G = torch.cat([E] + [x.reshape(n, -1) for x in (sp, de) if x is not None], dim=1).contiguous()
+        else:
+            agg = torch.ones_like(E)
+            for name, x in (("sparse", sp), ("dense", de)):
+                if x is None:
+                    continue
+                mean = x.mean(dim=-1, keepdim=True)
+                var = (x - mean).square().mean(dim=-1, keepdim=True)   # layer_normalization, eps 1e-8
+                ln = self.ln[name]
+                agg = agg + ((x - mean) * (var + 1e-8).rsqrt() * ln["scale"] + ln["bias"]).sum(dim=1)
+            self.G = (E * agg).contiguous()
+        self.Qi = torch.cat([_rms(self.G, self.rms_item), torch.ones((n, self.K), dtype=torch.float32,
+                                                                       device=self.device)], dim=1).contiguous()
+
+    def _encode(self, users_d):
+        """S [n, T, D] of the given users' sequences (one encoder pass each) and their lengths (int32 [n])."""
+        torch = self._torch
+        users = users_d.to(torch.int64).contiguous()
+        lens = self.lens[users].contiguous()
+        n = int(users.numel())
+        S = torch.empty((n, self.T, self.D), dtype=torch.float32, device=self.device)
+        _lib.check(_lib.lib.b200_transformer_encode(
+            _lib.ptr(users), n, _lib.ptr(lens), _lib.ptr(self.seqs), self.seqs.stride(0), _lib.ptr(self.G),
+            self.G.stride(0), self.Kp, _lib.ptr(self.pos), self.K, self.T, self.num_heads, self.n_layers,
+            int(self.causal), _lib.ptr(self.w_layers), _lib.ptr(self.rms_last), _lib.ptr(S), _lib.current_stream()))
+        return S, lens
+
+    def _hoistable(self):
+        if not super()._hoistable():
+            return False
+        need = _lib.lib.b200_transformer_pair_smem_bytes(self.T, self.D, self.mlp[0][0].shape[0])
+        return 0 < need <= self._torch.cuda.get_device_properties(self.device).shared_memory_per_block_optin
+
+    def score_all_items(self, user_ids_d):
+        """transformer.py:203-339 over (these users) x (every item): the encoder once per user, V'_u = S_u W1_seq on
+        the library GEMM, then every pair in ``b200_transformer_pair_scores``; the item part Pi of the first layer
+        once per model.  The [b*N, F*K + D] concat is never built."""
+        torch = self._torch
+        if not self._hoistable():
+            return super().score_all_items(user_ids_d)
+        N, FK, D, T = self.n_items, self.F * self.K, self.D, self.T
+        if "_item_part" not in self.__dict__:
+            xi = self._side_concat("item", torch.arange(N, device=self.device))
+            self._item_part = self._first_layer_partial("item", xi, False)
+            self._w_seq = self.mlp[0][0][:, FK:FK + D].contiguous()             # [H1, D]
+            three = len(self.mlp) == 3
+            self._tail = (self.mlp[1][0].t().contiguous(), self.mlp[2][0].t().contiguous() if three else None)
+        Pi = self._item_part
+        W2, W3 = self._tail
+        H1 = Pi.shape[1]
+        b = int(user_ids_d.numel())
+        scores = torch.empty((b, N), dtype=torch.float32, device=self.device)
+        for r0 in range(0, b, 65535):
+            u = user_ids_d[r0:r0 + 65535]
+            nb = int(u.numel())
+            Pu = self._first_layer_partial("user", self._side_concat("user", u), True)     # [nb, H1] incl. bias
+            S, lens = self._encode(u)
+            Vp = linear(S.view(nb * T, D), self._w_seq, None, ACT_NONE)                     # [nb*T, H1]
+            out = scores[r0:r0 + nb]
+            _lib.check(_lib.lib.b200_transformer_pair_scores(
+                _lib.ptr(self.Qi), self.Qi.stride(0), N, _lib.ptr(S), _lib.ptr(Vp), _lib.ptr(Pu), _lib.ptr(lens), nb,
+                _lib.ptr(Pi), Pi.stride(0), T, D, H1, W2.shape[1], W3.shape[1] if W3 is not None else 0, _lib.ptr(W2),
+                _lib.ptr(self.mlp[1][1]), _lib.ptr(W3), _lib.ptr(self.mlp[2][1]) if W3 is not None else None,
+                _lib.ptr(self.out_kernel), self.out_bias, _lib.ptr(out), out.stride(0), _lib.current_stream()))
+        return scores
+
+    def _seq_block(self, users_d, items_d, n, grid_items, row_offset, out_view):
+        """s_u of each row, every distinct user (grid slot) of the chunk encoded once."""
+        torch = self._torch
+        if grid_items > 0:
+            u0 = row_offset // grid_items
+            u1 = (row_offset + n - 1) // grid_items
+            S, lens = self._encode(users_d[u0:u1 + 1])
+            slot, items, off = None, None, row_offset - u0 * grid_items
+        else:
+            uniq, inv = torch.unique(users_d, return_inverse=True)
+            S, lens = self._encode(uniq)
+            slot, items, off = inv.to(torch.int32).contiguous(), items_d.to(torch.int64).contiguous(), 0
+        _lib.check(_lib.lib.b200_transformer_target_attention(
+            _lib.ptr(self.Qi), self.Qi.stride(0), _lib.ptr(S), self.T, self.D, _lib.ptr(lens), _lib.ptr(slot),
+            _lib.ptr(items), n, grid_items, off, _lib.ptr(out_view), out_view.stride(0), _lib.current_stream()))
 
 
 class TwoTower:

@@ -194,3 +194,49 @@ def make_autoint_weights(rng, spec, K, att_embed_size=(8, 8, 8), num_heads=2, us
     w.update(autoint_scheme=scheme, autoint_mha=mha, num_heads=H, use_residual=bool(use_residual),
              out_kernel=_glorot(rng, (F * K, 1)), out_bias=np.float32(0.02).reshape(1))
     return w
+
+
+def make_transformer_weights(rng, spec, K, num_heads=1, n_layers=1, max_seq_len=10, hidden=(128, 64, 32), use_bn=True,
+                             positional_embedding="trainable", use_causal_mask=False, feat_agg_mode="concat",
+                             version="keras", combiner="sqrtn"):
+    """Transformer variables (libreco/algorithms/transformer.py:203-339) in the raw shapes of the graph TensorFlow
+    `version` builds: "keras" query / key / value [D, H, hd] and attention_output [H, hd, D], "legacy" q, k, v, out
+    [D, D] (v applied to the projected keys); FFN [D, 4D], [4D, D]; RMS scales; the trainable positional table
+    [T, K] unless `positional_embedding` is sinusoidal.  D = K' + K with K' = K (1 + item sparse columns + item dense
+    columns) in concat mode, K in elementwise mode.  ``weights_io.transformer_weights`` turns them into the engine's
+    dict.  F counts a multi-sparse group as one field unless ``combiner == "normal"``."""
+    from .weights_io import autoint_scheme
+
+    scheme = autoint_scheme(version)
+    w = make_embeddings(rng, spec, K, linear=False)
+    n_sparse = spec["n_sparse"]
+    info = spec.get("multi_sparse_combine_info")
+    if info is not None and combiner != "normal":
+        n_sparse = int(info["field_offset"][0]) + len(info["field_offset"])
+    F = 2 + n_sparse + spec["n_dense"]
+    n_is, n_id = len(spec["item_sparse_col_index"]), len(spec["item_dense_col_index"])
+    Kp = K * (1 + n_is + n_id) if feat_agg_mode == "concat" else K
+    D, H = Kp + K, int(num_heads)
+    scale = lambda n: rng.uniform(0.5, 1.5, n).astype(np.float32)      # noqa: E731
+    layers = []
+    for _ in range(n_layers):
+        if scheme == "keras":
+            lw = dict(query=_glorot(rng, (D, D)).reshape(D, H, D // H), key=_glorot(rng, (D, D)).reshape(D, H, D // H),
+                      value=_glorot(rng, (D, D)).reshape(D, H, D // H),
+                      attention_output=_glorot(rng, (D, D)).reshape(H, D // H, D))
+        else:
+            lw = dict(query=_glorot(rng, (D, D)), key=_glorot(rng, (D, D)), value=_glorot(rng, (D, D)),
+                      output=_glorot(rng, (D, D)))
+        lw.update(rms_att=scale(D), rms_ffn=scale(D), ffn1=_glorot(rng, (D, 4 * D)), ffn2=_glorot(rng, (4 * D, D)))
+        layers.append(lw)
+    w.update(tfm_scheme=scheme, tfm_layers=layers, rms_last=scale(D), rms_item=scale(Kp), num_heads=H,
+             use_causal_mask=bool(use_causal_mask), feat_agg_mode=feat_agg_mode,
+             mlp=make_mlp(rng, F * K + D, hidden, use_bn), out_kernel=_glorot(rng, (hidden[-1], 1)),
+             out_bias=np.float32(0.03).reshape(1))
+    if positional_embedding not in ("sinusoidal", "sin", "sinusoid"):
+        w["positional_encoding"] = _glorot(rng, (max_seq_len, K))
+    if feat_agg_mode == "elementwise":
+        for side, n in (("sparse", n_is), ("dense", n_id)):
+            if n:
+                w[f"ln_{side}"] = dict(scale=scale(K), bias=rng.normal(0, 0.1, K).astype(np.float32))
+    return w

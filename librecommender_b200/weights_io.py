@@ -91,7 +91,8 @@ def load_default_recs(path, model_name):
 # ``<name>_layer<i>`` (layers/dense.py:28-33).  The creation order per model is read off the graph
 # builders: fm.py:152-171, deepfm.py:158-174, din.py:205-218 (+ the "attention" dense_nn,
 # layers/attention.py:47-53), youtube_ranking.py:208-217, two_tower.py:400-409, autoint.py:160-168 (+
-# multi_head_attention, layers/attention.py:67-138, whose graph depends on the TensorFlow version).  No TensorFlow exists in
+# multi_head_attention, layers/attention.py:67-138, whose graph depends on the TensorFlow version), transformer.py:
+# 203-339 (multi_head_attention and the two FFN tf_dense per layer, layers/transformer.py:147-166, then the head).  No TensorFlow exists in
 # this environment, so this table is RESTATED from TensorFlow's documented uniquifying rule and is
 # unverified against a real checkpoint; ``resolve_tf_names`` therefore checks every expected name AND
 # shape against the file and reports exactly what is missing instead of guessing.
@@ -137,15 +138,54 @@ def autoint_scheme(version):
 AUTOINT_SCHEMES = ("keras", "legacy")
 
 
-def default_tf_names(model_name, n_hidden, use_bn, use_tf_attention=False, n_layers=None, scheme="keras"):
+def default_tf_names(model_name, n_hidden, use_bn, use_tf_attention=False, n_layers=None, scheme="keras",
+                     positional_embedding="trainable", feat_agg_mode="concat", item_sparse=False, item_dense=False):
     """{engine weight key: TF variable name (or nested dict / list of names)} for the auto-named
-    variables of `model_name` in {"FM", "DeepFM", "DIN", "YouTubeRanking", "TwoTower", "AutoInt"}.
+    variables of `model_name` in {"FM", "DeepFM", "DIN", "YouTubeRanking", "TwoTower", "AutoInt", "Transformer"}.
+
+    Transformer (transformer.py:203-339; layer l = 1..L opens ``transformer_layer{l}``): per layer
+    ``rms_norm_att/scale:0``, ``rms_norm_ffn/scale:0``, the attention and the two bias-free FFN ``tf_dense``.  "keras":
+    ``multi_head_attention[_{l-1}]/{query,key,value,attention_output}/kernel:0`` and FFN ``dense_{2(l-1)}``,
+    ``dense_{2(l-1)+1}``, the head ``dense_{2L}``; "legacy": q, k, v, out, ffn1, ffn2 are ``dense_{6(l-1)}`` ..
+    ``dense_{6(l-1)+5}`` and the head ``dense_{6L}``.  Both: ``rms_norm_last/scale:0``, ``rms_norm_item/scale:0``,
+    ``transformer/positional_encoding:0`` (trainable positions only; the sinusoidal table is not saved), the
+    ``mlp`` stack, and in elementwise mode ``elementwise_{sparse,dense}_feats/layer_norm/{scale,bias}:0`` for the
+    sides with item features.  Returned under ``tfm_layers`` (per layer {query, key, value, attention_output | output,
+    rms_att, rms_ffn, ffn1, ffn2}), ``rms_last``, ``rms_item``, ``positional_encoding``, ``ln_sparse`` / ``ln_dense``,
+    ``mlp``, ``out_kernel``, ``out_bias``.
 
     AutoInt (autoint.py:160-168, one ``multi_head_attention`` per layer, then ``tf_dense(1)``) has two schemes:
     "keras" (TF >= 2.10): ``multi_head_attention[_i]/{query,key,value,attention_output}/kernel:0`` and the head
     ``dense/{kernel,bias}:0``; "legacy": four bias-free ``tf_dense`` per layer created as q, k, v, out, so layer l
     owns ``dense_{4l}`` .. ``dense_{4l+3}`` and the head is ``dense_{4L}``.  Returned under ``autoint_mha``
     (per-layer {query, key, value, attention_output | output}), ``out_kernel``, ``out_bias``."""
+    if model_name == "Transformer":
+        layers = []
+        for i in range(n_layers):
+            sc = f"transformer_layer{i + 1}"
+            if scheme == "keras":
+                mha = f"{sc}/multi_head_attention{'' if i == 0 else f'_{i}'}"
+                lw = {k: f"{mha}/{k}/kernel:0" for k in ("query", "key", "value", "attention_output")}
+                ffn = [2 * i, 2 * i + 1]
+            elif scheme == "legacy":
+                lw = {k: f"{sc}/{_dense_name(6 * i + j)}/kernel:0" for j, k in enumerate(("query", "key", "value",
+                                                                                          "output"))}
+                ffn = [6 * i + 4, 6 * i + 5]
+            else:
+                raise ValueError(f"unknown Transformer naming scheme `{scheme}`")
+            lw.update(rms_att=f"{sc}/rms_norm_att/scale:0", rms_ffn=f"{sc}/rms_norm_ffn/scale:0",
+                      ffn1=f"{sc}/{_dense_name(ffn[0])}/kernel:0", ffn2=f"{sc}/{_dense_name(ffn[1])}/kernel:0")
+            layers.append(lw)
+        head = _dense_name((2 if scheme == "keras" else 6) * n_layers)
+        out = {"tfm_layers": layers, "rms_last": "rms_norm_last/scale:0", "rms_item": "rms_norm_item/scale:0",
+               "mlp": _mlp_names("mlp", n_hidden, use_bn), "out_kernel": f"{head}/kernel:0", "out_bias": f"{head}/bias:0"}
+        if positional_embedding not in ("sinusoidal", "sin", "sinusoid"):
+            out["positional_encoding"] = "transformer/positional_encoding:0"
+        if feat_agg_mode == "elementwise":
+            for side, present in (("sparse", item_sparse), ("dense", item_dense)):
+                if present:
+                    out[f"ln_{side}"] = {k: f"elementwise_{side}_feats/layer_norm/{k}:0" for k in ("scale", "bias")}
+        return out
     if model_name == "AutoInt":
         if scheme == "keras":
             mha = [{k: f"multi_head_attention{'' if i == 0 else f'_{i}'}/{k}/kernel:0"
@@ -264,6 +304,91 @@ def autoint_tf_variables(raw):
     return out
 
 
+def transformer_tf_shapes(scheme, names, K, Kp, num_heads, T=None):
+    """Expected shapes for the Transformer entries of `names` (:func:`default_tf_names`); D = Kp + K.  keras
+    ``query/key/value [D, H, hd]``, ``attention_output [H, hd, D]``; legacy ``q, k, v, out [D, D]`` (v applied to the
+    projected keys); FFN ``[D, 4D]``, ``[4D, D]``; positions ``[T, K]``; the MLP's first kernel ``[F*K + D, H1]``
+    (F is not known here)."""
+    D, H = Kp + K, num_heads
+    hd = D // H
+    if scheme == "keras":
+        att = dict(query=(D, H, hd), key=(D, H, hd), value=(D, H, hd), attention_output=(H, hd, D))
+    else:
+        att = dict(query=(D, D), key=(D, D), value=(D, D), output=(D, D))
+    layer = dict(att, rms_att=(D,), rms_ffn=(D,), ffn1=(D, 4 * D), ffn2=(4 * D, D))
+    out = {"tfm_layers": [layer] * len(names["tfm_layers"]), "rms_last": (D,), "rms_item": (Kp,), "out_kernel": (None, 1),
+           "out_bias": (1,), "mlp": None}
+    if "positional_encoding" in names:
+        out["positional_encoding"] = (T, K)
+    for k in ("ln_sparse", "ln_dense"):
+        if k in names:
+            out[k] = {"scale": (K,), "bias": (K,)}
+    return out
+
+
+def transformer_layers(layers, scheme):
+    """Per-layer variables of either graph -> the engine's ``tfm_layers`` [{rms_att, wq, wk, wv, wo [D, D], rms_ffn,
+    w1 [D, 4D], w2 [4D, D]}], columns head-major.  legacy: the value Dense acts on the PROJECTED keys
+    (attention.py:104-106), so the effective value map Wk Wv' is multiplied in float64 and then cast."""
+    out = []
+    for lw in layers:
+        f32 = lambda a: np.asarray(a, dtype=np.float32)      # noqa: E731
+        if scheme == "keras":
+            D = np.shape(lw["query"])[0]
+            att = dict(wq=f32(lw["query"]).reshape(D, D), wk=f32(lw["key"]).reshape(D, D),
+                       wv=f32(lw["value"]).reshape(D, D), wo=f32(lw["attention_output"]).reshape(D, D))
+        elif scheme == "legacy":
+            wk = f32(lw["key"])
+            att = dict(wq=f32(lw["query"]), wk=wk, wo=f32(lw["output"]),
+                       wv=(wk.astype(np.float64) @ np.asarray(lw["value"], dtype=np.float64)).astype(np.float32))
+        else:
+            raise ValueError(f"unknown Transformer naming scheme `{scheme}`")
+        out.append(dict(att, rms_att=f32(lw["rms_att"]).reshape(-1), rms_ffn=f32(lw["rms_ffn"]).reshape(-1),
+                        w1=f32(lw["ffn1"]), w2=f32(lw["ffn2"])))
+    return out
+
+
+def transformer_weights(raw):
+    """Engine weight dict for :class:`feat_models.Transformer` from the raw variables of either graph: ``raw`` holds
+    the embedding tables, ``tfm_scheme``, ``tfm_layers`` (per layer, as :func:`default_tf_names` names them),
+    ``rms_last``, ``rms_item``, ``positional_encoding`` (trainable positions), ``ln_sparse`` / ``ln_dense``
+    (elementwise mode), ``num_heads``, ``use_causal_mask``, ``feat_agg_mode``, ``mlp``, ``out_kernel`` and
+    ``out_bias``; other entries pass through."""
+    w = {k: v for k, v in raw.items() if k not in ("tfm_layers", "tfm_scheme")}
+    w["tfm_layers"] = transformer_layers(raw["tfm_layers"], raw["tfm_scheme"])
+    w["out_kernel"] = np.asarray(raw["out_kernel"], dtype=np.float32).reshape(-1)
+    w["out_bias"] = np.float32(np.asarray(raw["out_bias"]).reshape(-1)[0])
+    return w
+
+
+def transformer_tf_variables(raw):
+    """Raw Transformer variables of either graph (the layout :func:`transformer_weights` takes) -> ``{TF variable
+    name: array}`` named by :func:`default_tf_names` for the raw dict's scheme and options: what ``save_tf_variables``
+    writes as ``<name>_tf_variables.npz``, and the inverse of ``load_reference_tf_model(..., "Transformer", ...)``."""
+    mlp = raw["mlp"]
+    names = default_tf_names("Transformer", len(mlp["kernels"]), mlp.get("bn_in") is not None,
+                             n_layers=len(raw["tfm_layers"]), scheme=raw["tfm_scheme"],
+                             positional_embedding="trainable" if raw.get("positional_encoding") is not None else "sinusoidal",
+                             feat_agg_mode=raw.get("feat_agg_mode", "concat"), item_sparse="ln_sparse" in raw,
+                             item_dense="ln_dense" in raw)
+    out = to_tf_variables({k: raw[k] for k in EMBEDDING_SCOPE if k in raw})
+
+    def put(n, a):
+        if isinstance(n, dict):
+            for k in n:
+                put(n[k], a[k])
+        elif isinstance(n, list):
+            for ni, ai in zip(n, a):
+                put(ni, ai)
+        else:
+            out[n] = np.asarray(a, dtype=np.float32)
+    put({k: v for k, v in names.items() if k not in ("out_kernel", "out_bias")},
+        {k: raw[k] for k in names if k not in ("out_kernel", "out_bias")})
+    out[names["out_kernel"]] = np.asarray(raw["out_kernel"], dtype=np.float32).reshape(-1, 1)
+    out[names["out_bias"]] = np.asarray(raw["out_bias"], dtype=np.float32).reshape(1)
+    return out
+
+
 YOUTUBE_RETRIEVAL_TABLES = {
     "seq_embeds": "embedding/seq_embeds_var:0", "item_embeds": "embedding/item_embeds_var:0",
     "item_biases": "embedding/item_bias_var:0", "sparse_embeds": "embedding/sparse_embeds_var:0",
@@ -328,13 +453,16 @@ def _youtube_retrieval_weights(npz, n_hidden, use_bn, extra_names=None):
 
 
 def load_reference_tf_model(path, model_name, arch, n_hidden, use_bn, use_tf_attention=False, extra_names=None,
-                            num_heads=2, att_embed_size=(8, 8, 8), use_residual=True):
+                            num_heads=None, att_embed_size=(8, 8, 8), use_residual=True, num_tfm_layers=1,
+                            positional_embedding="trainable", use_causal_mask=False, feat_agg_mode="concat"):
     """Engine weight dict of a model saved by the reference (``save_tf_variables``,
     utils/save_load.py:70-98) WITHOUT a hand-written name map: the embedding-scope variables by their
     fixed names, the heads / MLPs / batch-norms through :func:`default_tf_names` (override single entries
     with `extra_names`).  AutoInt takes its own constructor arguments ``num_heads``, ``att_embed_size`` and
     ``use_residual``; its naming scheme (keras or legacy) is read off the names in the file, and every name
-    and shape is checked.  YouTubeRetrieval (``n_hidden`` Dense layers in the user tower) returns the layout of
+    and shape is checked.  Transformer likewise, with ``num_heads``, ``num_tfm_layers``, ``positional_embedding``,
+    ``use_causal_mask`` and ``feat_agg_mode`` (``num_heads`` defaults to each model's own default: 2 for AutoInt, 1
+    for Transformer).  YouTubeRetrieval (``n_hidden`` Dense layers in the user tower) returns the layout of
     ``feat_models.YouTubeRetrieval``, every name and shape checked."""
     from .feat_models import from_tf_variables
 
@@ -342,6 +470,26 @@ def load_reference_tf_model(path, model_name, arch, n_hidden, use_bn, use_tf_att
     if arch == "YouTubeRetrieval":
         return _youtube_retrieval_weights(npz, n_hidden, use_bn, extra_names)
     w = from_tf_variables(npz)
+    if arch == "Transformer":
+        scheme = "keras" if "transformer_layer1/multi_head_attention/query/kernel:0" in npz.files else "legacy"
+        H = 1 if num_heads is None else int(num_heads)
+        K = int(np.shape(npz[EMBEDDING_SCOPE["user_embeds"]])[1])
+        # the elementwise layer norms exist for the item feature kinds the data has, which only the file tells
+        item_sparse, item_dense = (f"elementwise_{k}_feats/layer_norm/scale:0" in npz.files for k in ("sparse", "dense"))
+        names = default_tf_names(arch, n_hidden, use_bn, n_layers=int(num_tfm_layers), scheme=scheme,
+                                 positional_embedding=positional_embedding, feat_agg_mode=feat_agg_mode,
+                                 item_sparse=item_sparse, item_dense=item_dense)
+        names.update(extra_names or {})
+        D = int(np.shape(resolve_tf_names(npz, names["rms_last"]))[0])
+        if D <= K or D % H:
+            raise ValueError(f"Transformer: model width {D} (from `{names['rms_last']}`) must exceed K = {K} and be "
+                             f"divisible by num_heads {H}")
+        raw = resolve_tf_names(npz, names, transformer_tf_shapes(scheme, names, K, D - K, H))
+        w.update(raw, tfm_scheme=scheme, num_heads=H, use_causal_mask=bool(use_causal_mask),
+                 feat_agg_mode=feat_agg_mode)
+        return transformer_weights(w)
+    if num_heads is None:
+        num_heads = 2
     if arch == "AutoInt":
         hds = autoint_head_dims(att_embed_size)
         scheme = "keras" if "multi_head_attention/query/kernel:0" in npz.files else "legacy"
