@@ -589,6 +589,45 @@ int b200_transformer_target_attention(const float* Qi, int64_t ldq, const float*
                                       const int32_t* lens, const int32_t* slot_of_row, const int64_t* items, int64_t n,
                                       int64_t grid_items, int64_t row_offset, float* out, int64_t ldo, void* stream);
 
+/* ---- Transformer training (libreco/algorithms/transformer.py:203-339 in training mode) ------------------------
+ * The dense products over the R*T sequence rows (Q / K / V / O projections, FFN, MLP and their gradients) run on
+ * b200_linear_*; these are the rest.  Every `lens` here is clamped to [1, T] on the device, as the training
+ * collator gives it (position 0 of a history is len 1 holding the pad id): key 0 is always visible.
+ * b200_transformer_attention_forward / _backward: the attention core of b200_autoint_attention_* (same layouts,
+ * Q, K, V, O [R*T, ld], lse [R, H, T], dQ / dK / dV WRITTEN, one warp per (row, head), no atomics, bit-identical
+ * repeats) with a mask: key g is visible to query f of row r when g < lens[r], or g <= f with `causal`; a hidden
+ * key gets probability exactly 0.  Supported: 1 <= T <= 64, num_heads, head_dim >= 1, num_heads * head_dim <= 128,
+ * every stride >= that product, a finite scale; anything else returns -2 before launching.  The backward needs
+ * (6 T odd(hd) + 32 odd(T)) * 4 bytes of shared memory per (row, head): 206 464 B at T = 64, hd = 128.
+ * b200_rms_norm_forward: Y = X * rstd * scale per row of width D, rstd[r] = rsqrt(mean(X[r]^2) + 1e-8) saved.
+ * b200_rms_norm_backward: dX = rstd (dY o scale - X rstd^2 <dY o scale, X> / D).  The scale's gradient
+ * sum_r rstd[r] dY[r, c] X[r, c] is b200_col_reduce(dY, wrow = rstd, Y = X).
+ * b200_activation_forward / _backward: y = act(x), dx = dy * act'(x) elementwise over n floats from the
+ * pre-activation x; act 1 relu, 2 swish x / (1 + exp(-x)), 3 gelu 0.5 x (1 + erf(x / sqrt 2)).
+ * b200_transformer_target_attention_backward: the backward of b200_transformer_target_attention with one slot per
+ * row (query Q[r], sequence S[r] = S + r T D, [T, D] contiguous): p = softmax_t(<q, S_t>) over t < len,
+ * out = sum_t p_t S_t recomputed, ds_t = p_t (<dout, S_t> - <dout, out>); WRITES dq[r] = sum_t ds_t S_t and
+ * dS[r, t] = p_t dout + ds_t q for t < len, 0 for t >= len.  One warp per row, no atomics.
+ * Supported: 1 <= T <= 64, 1 <= D <= 128. */
+int b200_transformer_attention_forward(const float* Q, int64_t ldq, const float* K, int64_t ldk, const float* V,
+                                       int64_t ldv, const int32_t* lens, int64_t R, int32_t T, int32_t num_heads,
+                                       int32_t head_dim, int32_t causal, float scale, float* O, int64_t ldo, float* lse,
+                                       void* stream);
+int b200_transformer_attention_backward(const float* Q, int64_t ldq, const float* K, int64_t ldk, const float* V,
+                                        int64_t ldv, const float* O, int64_t ldo, const float* lse, const float* dO,
+                                        int64_t lddo, const int32_t* lens, int64_t R, int32_t T, int32_t num_heads,
+                                        int32_t head_dim, int32_t causal, float scale, float* dQ, float* dK, float* dV,
+                                        int64_t ldg, void* stream);
+int b200_rms_norm_forward(const float* X, int64_t ldx, int64_t R, int32_t D, const float* scale, float* Y, int64_t ldy,
+                          float* rstd, void* stream);
+int b200_rms_norm_backward(const float* dY, int64_t lddy, const float* X, int64_t ldx, const float* rstd, int64_t R,
+                           int32_t D, const float* scale, float* dX, int64_t lddx, void* stream);
+int b200_activation_forward(const float* x, int64_t n, int32_t act, float* y, void* stream);
+int b200_activation_backward(const float* dy, const float* x, int64_t n, int32_t act, float* dx, void* stream);
+int b200_transformer_target_attention_backward(const float* Q, int64_t ldq, const float* S, int32_t T, int32_t D,
+                                               const int32_t* lens, const float* dout, int64_t lddo, int64_t R,
+                                               float* dq, int64_t lddq, float* dS, void* stream);
+
 /* ---- a14: predict_from_embedding (libreco/prediction/predict.py:36-40) -----------------
  * out[r] = sum_k U[users[r],k] * I[items[r],k]; mode 0: raw, 1: expit (ranking),
  * 2: clip to [lo, hi] (rating) — normalize_prediction (:18-23). */

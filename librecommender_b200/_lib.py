@@ -134,6 +134,17 @@ SIGNATURES = {
                                                c_int32, c_float, _P, c_int64, _P, _P]),
     "b200_autoint_attention_backward": (c_int, [_P, c_int64, _P, c_int64, _P, c_int64, _P, c_int64, _P, _P, c_int64,
                                                 c_int64, c_int32, c_int32, c_int32, c_float, _P, _P, _P, c_int64, _P]),
+    "b200_transformer_attention_forward": (c_int, [_P, c_int64, _P, c_int64, _P, c_int64, _P, c_int64, c_int32,
+                                                   c_int32, c_int32, c_int32, c_float, _P, c_int64, _P, _P]),
+    "b200_transformer_attention_backward": (c_int, [_P, c_int64, _P, c_int64, _P, c_int64, _P, c_int64, _P, _P,
+                                                    c_int64, _P, c_int64, c_int32, c_int32, c_int32, c_int32, c_float,
+                                                    _P, _P, _P, c_int64, _P]),
+    "b200_rms_norm_forward": (c_int, [_P, c_int64, c_int64, c_int32, _P, _P, c_int64, _P, _P]),
+    "b200_rms_norm_backward": (c_int, [_P, c_int64, _P, c_int64, _P, c_int64, c_int32, _P, _P, c_int64, _P]),
+    "b200_activation_forward": (c_int, [_P, c_int64, c_int32, _P, _P]),
+    "b200_activation_backward": (c_int, [_P, _P, c_int64, c_int32, _P, _P]),
+    "b200_transformer_target_attention_backward": (c_int, [_P, c_int64, _P, c_int32, c_int32, _P, _P, c_int64,
+                                                           c_int64, _P, c_int64, _P, _P]),
 }
 
 for _name, (_res, _args) in SIGNATURES.items():

@@ -18,7 +18,8 @@ from __future__ import annotations
 import numpy as np
 
 from . import _lib
-from .feat_models import FeatSpec, _dev, feat_backward, feat_forward, linear, permute_mlp_input, tables_struct
+from .feat_models import (ACT_NONE, ACT_RELU, ACT_SWISH, FeatSpec, _dev, feat_backward, feat_forward, linear,
+                          permute_mlp_input, tables_struct)
 
 BN_EPS = 1e-3          # tf.layers.batch_normalization defaults
 BN_MOMENTUM = 0.99
@@ -334,37 +335,58 @@ class _StackTrainer(_Trainer):
             _lib.current_stream()))
         return dx
 
-    def _stack_forward(self, prefix, n_layers, x):
-        """BN(input) -> [Dense -> ReLU -> BN] x (L-1) -> Dense with batch statistics; returns (out, cache)."""
+    def _stack_forward(self, prefix, n_layers, x, act=ACT_RELU):
+        """BN(input) -> [Dense -> act -> BN] x (L-1) -> Dense with batch statistics; returns (out, cache).  ``act``:
+        relu (fused into the dense kernel) or swish (``dense_nn(..., activation=swish)``; its pre-activation is kept
+        for the backward)."""
         p = self.params
-        c = dict(concat=x, bn_stats={}, dense_in=[], relu_out=[])
+        c = dict(concat=x, bn_stats={}, dense_in=[], act_out=[], pre_act=[])
         a = x
         if self.use_bn:
             a, c["bn_stats"][0] = self._bn_forward(a, f"{prefix}bn0")
         for i in range(n_layers):
             last = i == n_layers - 1
             c["dense_in"].append(a)
-            a = linear(a, p[f"{prefix}Wt{i}"], p[f"{prefix}b{i}"], not last, cache_split=False)  # weights change every step
+            fused = last or act == ACT_RELU
+            a = linear(a, p[f"{prefix}Wt{i}"], p[f"{prefix}b{i}"], ACT_RELU if not last and fused else ACT_NONE,
+                       cache_split=False)                                    # weights change every step
             if not last:
-                c["relu_out"].append(a)
+                if not fused:
+                    c["pre_act"].append(a)
+                    a = self._activation(a, act)
+                c["act_out"].append(a)
                 if self.use_bn:
                     a, c["bn_stats"][i + 1] = self._bn_forward(a, f"{prefix}bn{i + 1}")
         return a, c
 
-    def _stack_backward(self, prefix, n_layers, c, da):
-        """Gradients of the stack's variables ADDED into ``self.grads``; returns d loss / d input."""
+    def _activation(self, z, act):
+        y = self._torch.empty_like(z)
+        _lib.check(_lib.lib.b200_activation_forward(_lib.ptr(z), z.numel(), act, _lib.ptr(y), _lib.current_stream()))
+        return y
+
+    def _stack_backward(self, prefix, n_layers, c, da, act=ACT_RELU):
+        """Gradients of the stack's variables ADDED into ``self.grads``; returns d loss / d input.  ``act`` as in
+        ``_stack_forward``: a relu output masks the BN backward (or b200_relu_backward), a swish block runs the BN
+        backward unmasked and then b200_activation_backward from the saved pre-activation."""
         torch = self._torch
         lib, st, p, g = _lib.lib, _lib.current_stream(), self.params, self.grads
         da = da.contiguous()
         for i in range(n_layers - 1, -1, -1):
             if i != n_layers - 1:
-                r_out = c["relu_out"][i]
+                a_out = c["act_out"][i]
+                relu = act == ACT_RELU
                 if self.use_bn:
-                    da = self._bn_backward(da, r_out, c["bn_stats"][i + 1], f"{prefix}bn{i + 1}", True)
-                else:
+                    da = self._bn_backward(da, a_out, c["bn_stats"][i + 1], f"{prefix}bn{i + 1}", relu)
+                elif relu:
                     dh = torch.empty_like(da)
-                    _lib.check(lib.b200_relu_backward(_lib.ptr(da), _lib.ptr(r_out), da.numel(), _lib.ptr(dh), st))
+                    _lib.check(lib.b200_relu_backward(_lib.ptr(da), _lib.ptr(a_out), da.numel(), _lib.ptr(dh), st))
                     da = dh
+                if not relu:
+                    z = c["pre_act"][i]
+                    dz = torch.empty_like(da)
+                    _lib.check(lib.b200_activation_backward(_lib.ptr(da), _lib.ptr(z), da.numel(), act, _lib.ptr(dz),
+                                                            st))
+                    da = dz
             x = c["dense_in"][i]
             da = da.contiguous()
             # dWt [dout, din] = dY^T X ; db = column sums of dY ; dX = dY Wt
@@ -572,7 +594,11 @@ class _SeqTrainer(_StackTrainer):
     """YouTubeRanking and DIN: the F field blocks and a sequence block -> one ``dense_nn`` stack -> Dense(1), mean
     sigmoid CE, TF-Adam.  The batch carries one behaviour sequence per ROW (``seqs`` [R, T] padded with ``n_items``,
     ``lens`` [R]; ``libreco/batch/sequence.py:75-91``).  A subclass fills the sequence block of the stack input
-    (``forward``) and sends its gradient back (``backward``)."""
+    (``forward``) and sends its gradient back (``backward``).  ``mlp_act``: the activation of the ``dense_nn``
+    stack.  The item feature table G (``combine_seq_features``, concat mode) of the models that attend over item
+    features is built by ``_build_G`` and its gradient folded back by ``_fold_dG``."""
+
+    mlp_act = ACT_RELU
 
     def __init__(self, spec, weights, use_bn=True, lr=1e-3, epsilon=1e-5, device=None):
         super().__init__(spec, weights, use_bn, lr, epsilon, device)
@@ -582,10 +608,55 @@ class _SeqTrainer(_StackTrainer):
         self.params["out_kernel"] = self._var(weights["out_kernel"], -1)
         self.params["out_bias"] = self._var(weights["out_bias"], 1)
 
+    def _init_item_table(self):
+        """Columns of G: the item embedding, then one block per item sparse field (index columns of the spec) and
+        per item dense field (value x that field's embedding)."""
+        torch = self._torch
+        sp = self.spec
+        self._is = [sp.is_[:, j].to(torch.int64).contiguous() for j in range(sp.is_.shape[1])] if sp.is_ is not None else []
+        self._id = [sp.id_[:, j].contiguous() for j in range(sp.id_.shape[1])] if sp.id_ is not None else []
+        self._id_cols = list(sp.item_dense_cols)
+        self.Kp = self.K * (1 + len(self._is) + len(self._id))
+
+    def _build_G(self):
+        torch = self._torch
+        p, K, st = self.params, self.K, _lib.current_stream()
+        n = self.n_items + 1
+        G = torch.empty((n, self.Kp), dtype=torch.float32, device=self.device)
+        G[:, :K].copy_(p["item_embeds"][:n])
+        off = K
+        for idx in self._is:
+            blk = G[:, off:off + K]
+            _lib.check(_lib.lib.b200_gather_rows(_lib.ptr(p["sparse_embeds"]), K, K, _lib.ptr(idx), n, _lib.ptr(blk),
+                                                 G.stride(0), st))
+            off += K
+        for vals, col in zip(self._id, self._id_cols):
+            G[:, off:off + K] = vals[:, None] * p["dense_embeds"][col][None, :]
+            off += K
+        return G
+
+    def _fold_dG(self, dG):
+        """dG [n_items+1, K'] back into the tables G was built from: the item-embedding block added, sparse blocks
+        through b200_scatter_add_rows, dense blocks through b200_col_reduce."""
+        lib, st, g, K = _lib.lib, _lib.current_stream(), self.grads, self.K
+        n = self.n_items + 1
+        g["item_embeds"][:n] += dG[:, :K]
+        off = K
+        for idx in self._is:
+            blk = dG[:, off:off + K]
+            _lib.check(lib.b200_scatter_add_rows(_lib.ptr(g["sparse_embeds"]), K, K, _lib.ptr(idx), n, _lib.ptr(blk),
+                                                 dG.stride(0), st))
+            off += K
+        for vals, col in zip(self._id, self._id_cols):
+            blk = dG[:, off:off + K]
+            _lib.check(lib.b200_col_reduce(_lib.ptr(blk), dG.stride(0), n, K, _lib.ptr(vals), None, 0,
+                                           _lib.ptr(g["dense_embeds"][col]), st))
+            off += K
+
     def _head_forward(self, x, **cache):
         """Stack + Dense(1) on the filled input ``x``; caches what the backward needs and returns the logits."""
         R = int(x.shape[0])
-        h, c = self._stack_forward("", self.n_layers, x)
+        h, c = self._stack_forward("", self.n_layers, x, self.mlp_act)
         logit = self._dense1_forward(h)
         c.update(R=R, h=h, logit=logit, **cache)
         self._cache = c
@@ -596,7 +667,7 @@ class _SeqTrainer(_StackTrainer):
         g, c = self.grads, self._cache
         R = c["R"]
         loss, da = self._dense1_backward(c["h"], c["logit"], labels_d)
-        dx = self._stack_backward("", self.n_layers, c, da)
+        dx = self._stack_backward("", self.n_layers, c, da, self.mlp_act)
         feat_backward(self.spec.layout, self.tables, c["users"], c["items"], R, g, dconcat=dx)
         return loss, dx
 
@@ -684,7 +755,6 @@ class DINTrainer(_SeqTrainer):
     """
 
     def _init_params(self, weights):
-        torch = self._torch
         super()._init_params(weights)
         p = self.params
         att = weights["attention"]
@@ -693,28 +763,7 @@ class DINTrainer(_SeqTrainer):
         p["att_k2"] = self._var(att["k2"], -1)
         p["att_b2"] = self._var(att["b2"], 1)
         self._b2_host = float(np.asarray(att["b2"]).reshape(-1)[0])      # Dense(1) bias enters the kernels by value
-        sp = self.spec
-        self._is = [sp.is_[:, j].to(torch.int64).contiguous() for j in range(sp.is_.shape[1])] if sp.is_ is not None else []
-        self._id = [sp.id_[:, j].contiguous() for j in range(sp.id_.shape[1])] if sp.id_ is not None else []
-        self._id_cols = list(sp.item_dense_cols)
-        self.Kp = self.K * (1 + len(self._is) + len(self._id))
-
-    def _build_G(self):
-        torch = self._torch
-        p, K, st = self.params, self.K, _lib.current_stream()
-        n = self.n_items + 1
-        G = torch.empty((n, self.Kp), dtype=torch.float32, device=self.device)
-        G[:, :K].copy_(p["item_embeds"][:n])
-        off = K
-        for idx in self._is:
-            blk = G[:, off:off + K]
-            _lib.check(_lib.lib.b200_gather_rows(_lib.ptr(p["sparse_embeds"]), K, K, _lib.ptr(idx), n, _lib.ptr(blk),
-                                                 G.stride(0), st))
-            off += K
-        for vals, col in zip(self._id, self._id_cols):
-            G[:, off:off + K] = vals[:, None] * p["dense_embeds"][col][None, :]
-            off += K
-        return G
+        self._init_item_table()
 
     def forward(self, users_d, items_d, seqs_d, lens_d):
         torch = self._torch
@@ -751,19 +800,7 @@ class DINTrainer(_SeqTrainer):
             _lib.ptr(c["lens"]), c["T"], _lib.ptr(c["rows"]), R, _lib.ptr(p["att_k1"]), _lib.ptr(p["att_b1"]),
             _lib.ptr(p["att_k2"]), c["b2"], _lib.ptr(datt), datt.stride(0), _lib.ptr(dG), dG.stride(0),
             _lib.ptr(g["att_k1"]), _lib.ptr(g["att_b1"]), _lib.ptr(g["att_k2"]), _lib.ptr(g["att_b2"]), st))
-        # ---- dG back into the tables G was built from
-        g["item_embeds"][:n] += dG[:, :K]
-        off = K
-        for idx in self._is:
-            blk = dG[:, off:off + K]
-            _lib.check(lib.b200_scatter_add_rows(_lib.ptr(g["sparse_embeds"]), K, K, _lib.ptr(idx), n, _lib.ptr(blk),
-                                                 dG.stride(0), st))
-            off += K
-        for vals, col in zip(self._id, self._id_cols):
-            blk = dG[:, off:off + K]
-            _lib.check(lib.b200_col_reduce(_lib.ptr(blk), dG.stride(0), n, K, _lib.ptr(vals), None, 0,
-                                           _lib.ptr(g["dense_embeds"][col]), st))
-            off += K
+        self._fold_dG(dG)
         return loss
 
     def export_weights(self):
@@ -771,6 +808,293 @@ class DINTrainer(_SeqTrainer):
         w = super().export_weights()
         w["attention"] = dict(k1=p["att_k1"].cpu().numpy(), b1=p["att_b1"].cpu().numpy(), k2=p["att_k2"].cpu().numpy(),
                               b2=np.float32(p["att_b2"].cpu().numpy()[0]))
+        return w
+
+
+TFM_ATT_NAMES = {"keras": ("query", "key", "value", "attention_output"), "legacy": ("query", "key", "value", "output")}
+ACT_GELU = 3      # b200_activation_* code of the erf gelu (include/b200reco.h)
+
+
+class TransformerTrainer(_SeqTrainer):
+    """Transformer training step on the device: ``libreco/algorithms/transformer.py:203-339`` in training mode (no
+    dropout), mean sigmoid CE, TF-Adam.  One behaviour sequence per ROW (``seqs`` [R, T], ``lens`` [R], clamped to
+    [1, T] as the training collator gives them).
+
+        G (the item feature table, concat mode, from the CURRENT tables) -> X = [G[seq_t] || pos_t] over R*T rows
+        (b200_gather_rows) -> per layer: b200_rms_norm_forward -> Q / K / V projections (b200_linear_*) ->
+        b200_transformer_attention_forward (masked) -> output projection + residual -> rms -> W1 ->
+        b200_activation_forward (gelu) -> W2 + residual -> rms_last -> target attention of [rms_item(G[item]) || 1]
+        (b200_transformer_target_attention) -> K1 gather + swish ``dense_nn`` -> Dense(1) -> b200_pointwise_loss
+        -> the reverse (b200_transformer_target_attention_backward, b200_rms_norm_backward + b200_col_reduce for
+        the scales, b200_transformer_attention_backward, b200_activation_backward, the dense kernels for every
+        projection) -> dX[:, :K'] and dq[:K'] scattered into dG (b200_scatter_add_rows), the trainable positions'
+        gradient a column reduction -> dG folded into the tables as DIN does -> b200_feat_backward ->
+        b200_adam_dense_dev
+
+    ``weights``: the RAW variables of either graph, as ``synthetic.make_transformer_weights`` makes them (the
+    tables, ``tfm_scheme``, ``tfm_layers``, ``rms_last``, ``rms_item``, ``positional_encoding`` when the positions
+    are trainable — absent, the sinusoidal table is a constant —, ``num_heads``, ``use_causal_mask``, ``mlp``,
+    ``out_kernel``, ``out_bias``).  keras ``query`` / ``key`` / ``value`` [D, H, hd] and ``attention_output``
+    [H, hd, D] are held as [D, D]; legacy ``value`` acts on the PROJECTED keys, so Wk is trained through both of its
+    paths.  ``export_weights`` returns the same raw layout.  ``reg`` applies to the embedding tables only.
+
+    Raises ``ValueError`` before anything is launched for shapes outside the kernels' envelope (T <= 64,
+    D = K' + K <= 128, 1..4 layers, heads dividing D), ``feat_agg_mode="elementwise"`` (its layer-norm backward is
+    not built) and multi-sparse fields with a combiner other than "normal" (the pooling backward is not built)."""
+
+    mlp_act = ACT_SWISH
+
+    def __init__(self, spec, weights, use_bn=True, lr=1e-3, epsilon=1e-5, device=None):
+        from .feat_models import _spec_get
+
+        g = _spec_get(spec) if not isinstance(spec, FeatSpec) else (lambda k, d=None: d)
+        if weights.get("feat_agg_mode", "concat") != "concat":
+            raise ValueError("TransformerTrainer: only feat_agg_mode \"concat\" trains; the layer-norm backward of "
+                             "\"elementwise\" is not built")
+        if g("multi_sparse_combine_info") is not None and weights.get("multi_sparse_combiner", "sqrtn") != "normal":
+            raise ValueError("TransformerTrainer: multi-sparse fields need the combiner \"normal\"; the pooling "
+                             "backward is not built")
+        self._combiner = weights.get("multi_sparse_combiner")
+        super().__init__(spec, weights, use_bn, lr, epsilon, device)
+        self._sin = {}
+
+    def _init_params(self, weights):
+        from .feat_models import TRANSFORMER_MAX_D, TRANSFORMER_MAX_LAYERS, TRANSFORMER_MAX_T
+
+        super()._init_params(weights)
+        self._init_item_table()
+        p, K, F, Kp = self.params, self.K, self.F, self.Kp
+        D = self.D = Kp + K
+        H = self.H = int(weights["num_heads"])
+        self.scheme = weights["tfm_scheme"]
+        if self.scheme not in TFM_ATT_NAMES:
+            raise ValueError(f"TransformerTrainer: unknown naming scheme `{self.scheme}`")
+        layers = list(weights["tfm_layers"])
+        if D > TRANSFORMER_MAX_D or not 1 <= len(layers) <= TRANSFORMER_MAX_LAYERS or H < 1 or D % H:
+            raise ValueError(f"TransformerTrainer: width D = {D} (item features {Kp} + positions {K}), {len(layers)} "
+                             f"layers, {H} heads outside D <= {TRANSFORMER_MAX_D}, 1..{TRANSFORMER_MAX_LAYERS} layers, "
+                             f"heads dividing D")
+        hd = D // H
+        self.att_names = TFM_ATT_NAMES[self.scheme]
+        att = [(D, H, hd)] * 3 + [(H, hd, D)] if self.scheme == "keras" else [(D, D)] * 4
+        want = dict(zip(self.att_names, att), rms_att=(D,), rms_ffn=(D,), ffn1=(D, 4 * D), ffn2=(4 * D, D))
+        for l, lw in enumerate(layers):
+            got = {n: tuple(np.shape(lw[n])) for n in want}
+            if got != want:
+                raise ValueError(f"TransformerTrainer layer {l}: shapes {got}, expected {want}")
+            for n in want:
+                p[f"tfm{l}_{n}"] = self._var(lw[n], (D, D) if n in self.att_names else want[n])
+        self.n_tfm = len(layers)
+        for n, shp in (("rms_last", D), ("rms_item", Kp)):
+            if np.size(weights[n]) != shp:
+                raise ValueError(f"TransformerTrainer: {n} has {np.size(weights[n])} entries, expected {shp}")
+            p[n] = self._var(weights[n], -1)
+        pos = weights.get("positional_encoding")
+        self.T_pos = None
+        if pos is not None:
+            T = np.shape(pos)[0]
+            if np.ndim(pos) != 2 or np.shape(pos)[1] != K or not 1 <= T <= TRANSFORMER_MAX_T:
+                raise ValueError(f"TransformerTrainer: positional table of shape {np.shape(pos)}, expected (T, {K}) "
+                                 f"with T <= {TRANSFORMER_MAX_T}")
+            p["positional_encoding"] = self._var(pos)
+            self.T_pos = T
+        n_in = np.shape(weights["mlp"]["kernels"][0])[0]
+        if n_in != F * K + D:
+            raise ValueError(f"TransformerTrainer: the first MLP layer takes {n_in} inputs, expected F*K + D = "
+                             f"{F}*{K} + {D}")
+        self.causal = bool(weights.get("use_causal_mask", False))
+
+    def _positions(self, T):
+        """The positional table [T, K] of this batch: the trainable variable, or the constant sinusoidal table
+        (uploaded once per T, outside any graph capture)."""
+        from .feat_models import TRANSFORMER_MAX_T, sinusoidal_positions
+
+        if not 1 <= T <= TRANSFORMER_MAX_T:
+            raise ValueError(f"TransformerTrainer: sequence length {T} outside 1..{TRANSFORMER_MAX_T}")
+        if self.T_pos is not None:
+            if T != self.T_pos:
+                raise ValueError(f"TransformerTrainer: sequences of length {T}, the positional table has {self.T_pos} "
+                                 f"rows")
+            return self.params["positional_encoding"]
+        if T not in self._sin:
+            self._sin[T] = _dev(sinusoidal_positions(T, self.K), self.device, self._torch.float32)
+        return self._sin[T]
+
+    def _rms(self, x, name, out=None):
+        """(rms_norm(x) with the scale variable ``name``, rstd [rows]); written into ``out`` when given."""
+        torch = self._torch
+        R, D = x.shape
+        y = out if out is not None else torch.empty((R, D), dtype=torch.float32, device=self.device)
+        rstd = torch.empty(R, dtype=torch.float32, device=self.device)
+        _lib.check(_lib.lib.b200_rms_norm_forward(_lib.ptr(x), x.stride(0), R, D, _lib.ptr(self.params[name]),
+                                                  _lib.ptr(y), y.stride(0), _lib.ptr(rstd), _lib.current_stream()))
+        return y, rstd
+
+    def _rms_backward(self, dy, x, rstd, name):
+        """d input of ``_rms``; the scale's gradient sum_r rstd dy x is ADDED into ``grads[name]``."""
+        lib, st = _lib.lib, _lib.current_stream()
+        R, D = x.shape
+        dx = self._torch.empty((R, D), dtype=self._torch.float32, device=self.device)
+        _lib.check(lib.b200_rms_norm_backward(_lib.ptr(dy), dy.stride(0), _lib.ptr(x), x.stride(0), _lib.ptr(rstd), R, D,
+                                              _lib.ptr(self.params[name]), _lib.ptr(dx), dx.stride(0), st))
+        _lib.check(lib.b200_col_reduce(_lib.ptr(dy), dy.stride(0), R, D, _lib.ptr(rstd), _lib.ptr(x), x.stride(0),
+                                       _lib.ptr(self.grads[name]), st))
+        return dx
+
+    def _axpy(self, y, x):
+        """y += x (same shapes, contiguous) on the library's kernel."""
+        _lib.check(_lib.lib.b200_axpy(_lib.ptr(y), _lib.ptr(x), 1.0, y.numel(), _lib.current_stream()))
+
+    def forward(self, users_d, items_d, seqs_d, lens_d):
+        """Training-mode logits of the batch (batch statistics in the BN); caches what the backward needs."""
+        torch = self._torch
+        lib, st, p = _lib.lib, _lib.current_stream(), self.params
+        K, F, Kp, D, H = self.K, self.F, self.Kp, self.D, self.H
+        R, T = int(seqs_d.shape[0]), int(seqs_d.shape[1])
+        pos = self._positions(T)
+        hd = D // H
+        scale = float(np.float32(1.0 / np.sqrt(hd)))
+        f32, dev = torch.float32, self.device
+        lens = lens_d.clamp(1, T).to(torch.int32).contiguous()
+        G = self._build_G()
+        RT = R * T
+        seq_idx = seqs_d.reshape(-1).to(torch.int64)
+        X = torch.empty((RT, D), dtype=f32, device=dev)
+        _lib.check(lib.b200_gather_rows(_lib.ptr(G), G.stride(0), Kp, _lib.ptr(seq_idx), RT, _lib.ptr(X), D, st))
+        X.view(R, T, D)[:, :, Kp:] = pos                       # broadcast copy of the positions (plumbing)
+        layers = []
+        for l in range(self.n_tfm):
+            wq, wk, wv, wo = (p[f"tfm{l}_{n}"] for n in self.att_names)
+            h1, r1 = self._rms(X, f"tfm{l}_rms_att")
+            q = linear(h1, wq.t().contiguous(), None, ACT_NONE, cache_split=False)
+            k = linear(h1, wk.t().contiguous(), None, ACT_NONE, cache_split=False)
+            v = linear(k if self.scheme == "legacy" else h1, wv.t().contiguous(), None, ACT_NONE, cache_split=False)
+            o = torch.empty((RT, D), dtype=f32, device=dev)
+            lse = torch.empty(R * H * T, dtype=f32, device=dev)
+            _lib.check(lib.b200_transformer_attention_forward(
+                _lib.ptr(q), q.stride(0), _lib.ptr(k), k.stride(0), _lib.ptr(v), v.stride(0), _lib.ptr(lens), R, T, H,
+                hd, int(self.causal), scale, _lib.ptr(o), o.stride(0), _lib.ptr(lse), st))
+            a = linear(o, wo.t().contiguous(), None, ACT_NONE, cache_split=False)
+            self._axpy(a, X)
+            h2, r2 = self._rms(a, f"tfm{l}_rms_ffn")
+            z = linear(h2, p[f"tfm{l}_ffn1"].t().contiguous(), None, ACT_NONE, cache_split=False)
+            gz = self._activation(z, ACT_GELU)
+            y = linear(gz, p[f"tfm{l}_ffn2"].t().contiguous(), None, ACT_NONE, cache_split=False)
+            self._axpy(y, a)
+            layers.append(dict(x=X, h1=h1, r1=r1, q=q, k=k, v=v, o=o, lse=lse, a=a, h2=h2, r2=r2, z=z, gz=gz))
+            X = y
+        S, rl = self._rms(X, "rms_last")
+        # the target query [rms_item(G[item]) || 1..1]
+        Gi = torch.empty((R, Kp), dtype=f32, device=dev)
+        _lib.check(lib.b200_gather_rows(_lib.ptr(G), G.stride(0), Kp, _lib.ptr(items_d), R, _lib.ptr(Gi), Kp, st))
+        Q = torch.empty((R, D), dtype=f32, device=dev)
+        Q[:, Kp:] = 1.0
+        _, ri = self._rms(Gi, "rms_item", out=Q[:, :Kp])
+        x = torch.empty((R, F * K + D), dtype=f32, device=dev)
+        feat_forward(self.spec.layout, self.tables, users_d, items_d, R, concat=x)
+        su = x[:, F * K:]
+        rows = torch.arange(R, dtype=torch.int64, device=dev)
+        slots = rows.to(torch.int32)
+        _lib.check(lib.b200_transformer_target_attention(_lib.ptr(Q), Q.stride(0), _lib.ptr(S), T, D, _lib.ptr(lens),
+                                                         _lib.ptr(slots), _lib.ptr(rows), R, 0, 0, _lib.ptr(su),
+                                                         su.stride(0), st))
+        return self._head_forward(x, users=users_d, items=items_d, T=T, lens=lens, seq_idx=seq_idx, layers=layers,
+                                  XL=X, S=S, rl=rl, Gi=Gi, ri=ri, Q=Q)
+
+    def backward(self, labels_d):
+        """Loss + every gradient buffer filled (before the optimiser); returns the device loss."""
+        torch = self._torch
+        lib, st, p, g = _lib.lib, _lib.current_stream(), self.params, self.grads
+        K, F, Kp, D, H = self.K, self.F, self.Kp, self.D, self.H
+        c = self._cache
+        R, T = c["R"], c["T"]
+        RT, hd = R * T, D // H
+        scale = float(np.float32(1.0 / np.sqrt(hd)))
+        f32, dev = torch.float32, self.device
+        loss, dx = self._head_backward(labels_d)
+        dsu = dx[:, F * K:]
+        dq = torch.empty((R, D), dtype=f32, device=dev)
+        dX = torch.empty((RT, D), dtype=f32, device=dev)
+        _lib.check(lib.b200_transformer_target_attention_backward(
+            _lib.ptr(c["Q"]), c["Q"].stride(0), _lib.ptr(c["S"]), T, D, _lib.ptr(c["lens"]), _lib.ptr(dsu),
+            dsu.stride(0), R, _lib.ptr(dq), dq.stride(0), _lib.ptr(dX), st))
+        n = self.n_items + 1
+        dG = torch.zeros((n, Kp), dtype=f32, device=dev)
+        dGi = self._rms_backward(dq[:, :Kp], c["Gi"], c["ri"], "rms_item")      # the ones padding is a constant
+        _lib.check(lib.b200_scatter_add_rows(_lib.ptr(dG), Kp, Kp, _lib.ptr(c["items"]), R, _lib.ptr(dGi), Kp, st))
+        dX = self._rms_backward(dX, c["XL"], c["rl"], "rms_last")
+        for l in range(self.n_tfm - 1, -1, -1):
+            a_ = c["layers"][l]
+            nq, nk, nv, no = (f"tfm{l}_{n}" for n in self.att_names)
+            n1, n2 = f"tfm{l}_ffn1", f"tfm{l}_ffn2"
+            # y = a + gelu(rms_ffn(a) W1) W2
+            g[n2] += _weight_grad(dX, a_["gz"]).t()
+            dgz = linear(dX, p[n2], None, ACT_NONE, cache_split=False)
+            dz = torch.empty_like(dgz)
+            _lib.check(lib.b200_activation_backward(_lib.ptr(dgz), _lib.ptr(a_["z"]), dz.numel(), ACT_GELU, _lib.ptr(dz),
+                                                    st))
+            g[n1] += _weight_grad(dz, a_["h2"]).t()
+            dh2 = linear(dz, p[n1], None, ACT_NONE, cache_split=False)
+            da = self._rms_backward(dh2, a_["a"], a_["r2"], f"tfm{l}_rms_ffn")
+            self._axpy(da, dX)
+            # a = x + MHA(rms_att(x))
+            g[no] += _weight_grad(da, a_["o"]).t()
+            dO = linear(da, p[no], None, ACT_NONE, cache_split=False)
+            dqh, dk, dv = (torch.empty((RT, D), dtype=f32, device=dev) for _ in range(3))
+            _lib.check(lib.b200_transformer_attention_backward(
+                _lib.ptr(a_["q"]), a_["q"].stride(0), _lib.ptr(a_["k"]), a_["k"].stride(0), _lib.ptr(a_["v"]),
+                a_["v"].stride(0), _lib.ptr(a_["o"]), a_["o"].stride(0), _lib.ptr(a_["lse"]), _lib.ptr(dO),
+                dO.stride(0), _lib.ptr(c["lens"]), R, T, H, hd, int(self.causal), scale, _lib.ptr(dqh), _lib.ptr(dk),
+                _lib.ptr(dv), D, st))
+            if self.scheme == "legacy":                                # V = Kproj Wv': Wk gets the V path too
+                g[nv] += _weight_grad(dv, a_["k"]).t()
+                self._axpy(dk, linear(dv, p[nv], None, ACT_NONE, cache_split=False))
+            g[nq] += _weight_grad(dqh, a_["h1"]).t()
+            g[nk] += _weight_grad(dk, a_["h1"]).t()
+            dh1 = linear(dqh, p[nq], None, ACT_NONE, cache_split=False)
+            self._axpy(dh1, linear(dk, p[nk], None, ACT_NONE, cache_split=False))
+            if self.scheme == "keras":
+                g[nv] += _weight_grad(dv, a_["h1"]).t()
+                self._axpy(dh1, linear(dv, p[nv], None, ACT_NONE, cache_split=False))
+            dXn = self._rms_backward(dh1, a_["x"], a_["r1"], f"tfm{l}_rms_att")
+            self._axpy(dXn, da)
+            dX = dXn
+        # X = [G[seq_t] || pos_t]: the item block into dG, the positions' gradient a column reduction over the rows
+        _lib.check(lib.b200_scatter_add_rows(_lib.ptr(dG), Kp, Kp, _lib.ptr(c["seq_idx"]), RT, _lib.ptr(dX), D, st))
+        if self.T_pos is not None:
+            dpos = torch.zeros(T * D, dtype=f32, device=dev)
+            _lib.check(lib.b200_col_reduce(_lib.ptr(dX), T * D, R, T * D, None, None, 0, _lib.ptr(dpos), st))
+            g["positional_encoding"] += dpos.view(T, D)[:, Kp:]
+        self._fold_dG(dG)
+        return loss
+
+    def step_graph(self, users_d, items_d, seqs_d, lens_d, labels_d):
+        self._positions(int(seqs_d.shape[1]))       # the sinusoidal table is uploaded before any capture
+        return super().step_graph(users_d, items_d, seqs_d, lens_d, labels_d)
+
+    def export_weights(self):
+        """The raw variables in the scheme they came in (``weights_io.transformer_weights`` makes the inference
+        dict, ``weights_io.transformer_tf_variables`` the reference's variable names)."""
+        p, D, H = self.params, self.D, self.H
+        hd = D // H
+        w = super().export_weights()
+        layers = []
+        for l in range(self.n_tfm):
+            lw = {}
+            for n in self.att_names + ("rms_att", "rms_ffn", "ffn1", "ffn2"):
+                a = p[f"tfm{l}_{n}"].cpu().numpy()
+                if self.scheme == "keras" and n in self.att_names:
+                    a = a.reshape((H, hd, D) if n == "attention_output" else (D, H, hd))
+                lw[n] = a
+            layers.append(lw)
+        w.update(tfm_scheme=self.scheme, tfm_layers=layers, rms_last=p["rms_last"].cpu().numpy(),
+                 rms_item=p["rms_item"].cpu().numpy(), num_heads=H, use_causal_mask=self.causal,
+                 feat_agg_mode="concat", out_kernel=w["out_kernel"].reshape(-1, 1),
+                 out_bias=np.asarray(w["out_bias"], dtype=np.float32).reshape(1))
+        if self.T_pos is not None:
+            w["positional_encoding"] = p["positional_encoding"].cpu().numpy()
+        if self._combiner is not None:
+            w["multi_sparse_combiner"] = self._combiner
         return w
 
 
