@@ -628,6 +628,31 @@ int b200_transformer_target_attention_backward(const float* Q, int64_t ldq, cons
                                                const int32_t* lens, const float* dout, int64_t lddo, int64_t R,
                                                float* dq, int64_t lddq, float* dS, void* stream);
 
+/* ---- RNN4Rec inference (libreco/algorithms/rnn4rec.py:151-237, layers/recurrent.py:4-63) ----------------------
+ * Slot s encodes the sequence seqs[users[s], :T] (row-major, ld_seq) with len = lens[users[s]] clamped to [0, T]
+ * over the input table X [*, ldx] (seq_embeds, in_dim columns) through n_layers stacked recurrent layers and
+ * writes out[s, :H_last] (ldo): the last layer's state after step len - 1.  Steps t >= len leave every state
+ * unchanged and len = 0 gives the zero state (dynamic_rnn(sequence_length=len); the Keras graph with a mask when
+ * masked steps repeat the previous output).  Layer l (input width in_l = l ? hidden[l-1] : in_dim, hidden size H,
+ * G gates) has cell_kinds[l]:
+ *   0 GRU reset-after (Keras), blocks z | r | h:  h~ = act(ax_h + r * ah_h),  h' = z h + (1 - z) h~
+ *   1 GRU reset-before (TF1 GRUCell), blocks z | r | c:  c = act(ax_c + (r o h) . U_c + bh_c),  h' = z h + (1 - z) c
+ *   2 LSTM, blocks i | f | c | o:  c' = f c + i act(ax_c + ah_c),  h' = o act(c')
+ * with ax_g = x . W_g + bx_g and ah_g = h . U_g + bh_g, each dot product one fmaf chain over the index ascending,
+ * and z, r, i, f, o = sigmoid(ax_g + ah_g) = 1 / (1 + expf(-v)).  acts[l]: 0 act = tanhf; 1 act = identity and the
+ * layer's output is tanh(LayerNorm(h)) (eps 1e-3, mean and variance over H), which is the next layer's input and,
+ * for the last layer, the result.  weights packs the layers back to back, each W [in_l, G*H], U [H, G*H],
+ * bx [G*H], bh [G*H], gamma [H], beta [H] row-major (b200_rnn_layer_floats floats; gamma / beta are read only when
+ * acts[l] = 1).  cell_kinds, hidden and acts are HOST arrays of n_layers entries.  A slot's result depends only on
+ * its own sequence: the same bits whatever the other slots, n or the call.
+ * Supported: 1 <= T <= 128, 1 <= in_dim, hidden[l] <= 256, 1 <= n_layers <= 4; anything else returns -2 before
+ * launching; n = 0 launches nothing. */
+int64_t b200_rnn_layer_floats(int32_t cell_kind, int32_t in_dim, int32_t hidden);
+int b200_rnn_encode(const int64_t* users, int64_t n, const int32_t* lens, const int32_t* seqs, int64_t ld_seq,
+                    int32_t T, const float* X, int64_t ldx, int32_t in_dim, int32_t n_layers, const int32_t* cell_kinds,
+                    const int32_t* hidden, const int32_t* acts, const float* weights, float* out, int64_t ldo,
+                    void* stream);
+
 /* ---- a14: predict_from_embedding (libreco/prediction/predict.py:36-40) -----------------
  * out[r] = sum_k U[users[r],k] * I[items[r],k]; mode 0: raw, 1: expit (ranking),
  * 2: clip to [lo, hi] (rating) — normalize_prediction (:18-23). */

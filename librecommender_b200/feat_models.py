@@ -140,19 +140,21 @@ def split_weights(Wt):
 ACT_NONE, ACT_RELU, ACT_SWISH = 0, 1, 2     # activation codes of b200_linear_* (include/b200reco.h)
 
 
-def linear(x, Wt, b, act, cache_split=True):
+def linear(x, Wt, b, act, cache_split=True, impl=None):
     """tf_dense (libreco/layers/dense.py:52-80) with BN folded: act(x Wt^T + b), fp32 device tensors.  ``act`` is an
-    activation code (a bool reads as relu on / off): 0 none, 1 relu, 2 swish."""
+    activation code (a bool reads as relu on / off): 0 none, 1 relu, 2 swish.  ``impl`` overrides ``LINEAR_IMPL``
+    for this call ("f32": one fmaf chain per output, so a row's bits do not depend on how many rows come with it)."""
     import torch
 
+    impl = LINEAR_IMPL if impl is None else impl
     R, din, dout = x.shape[0], Wt.shape[1], Wt.shape[0]
     y = torch.empty((R, dout), dtype=torch.float32, device=x.device)
     bp = _lib.ptr(b) if b is not None else None
     aligned = x.stride(0) % 4 == 0 and x.data_ptr() % 16 == 0 and x.stride(1) == 1 and Wt.stride(1) == 1
     # few output rows but a long reduction (the weight gradients dWt = dY^T X of the training steps: 128 x 1792
     # outputs over 8192 rows) would run on a handful of SIMT CTAs: send those to the tensor-core kernel too
-    use_tc = LINEAR_IMPL == "tf32x3" or (LINEAR_IMPL == "auto" and din >= TC_MIN_DIN and
-                                         (R >= TC_MIN_ROWS or din >= TC_LONG_K or R * din * dout >= TC_MIN_MACS))
+    use_tc = impl == "tf32x3" or (impl == "auto" and din >= TC_MIN_DIN and
+                                  (R >= TC_MIN_ROWS or din >= TC_LONG_K or R * din * dout >= TC_MIN_MACS))
     w_ok = cache_split or (Wt.stride(0) % 4 == 0 and Wt.data_ptr() % 16 == 0)
     if use_tc and aligned and w_ok and not cache_split and din >= TC_LONG_K:
         # few output tiles, long reduction: split the reduction over enough CTAs to fill the SMs
@@ -1380,12 +1382,176 @@ class YouTubeRetrieval:
         ``I [n_items + 1, H + 1]`` (``[item_embeds | item_biases]`` + the mean row) for :class:`engine.EmbedScorer`."""
         torch = self._torch
         rows = [self.user_vectors(np.arange(i, min(self.n_users, i + chunk))) for i in range(0, self.n_users, chunk)]
-        U = torch.cat(rows, dim=0)
-        if self.norm_embed:          # dyn_embed_base.py:264-265: the item side is normalised too (before the bias column)
-            I = self.item_embeds / self.item_embeds.norm(dim=1, keepdim=True)
+        return dyn_embed_tables(torch.cat(rows, dim=0), self.item_embeds, self.item_biases, self.norm_embed)
+
+
+def dyn_embed_tables(U, item_embeds, item_biases, norm_embed):
+    """The serving tables of ``DynEmbedBase.set_embeddings`` (``bases/dyn_embed_base.py:240-269``) and
+    ``embed_base.py:257-265`` from the device user vectors ``U [n_users, d]``: ``[U | 1]`` and ``[I | b]`` with
+    ``I = item_embeds`` (L2-normalised when ``norm_embed``; the user vectors arrive normalised already), each with
+    its column-mean row appended -> ``[n_users + 1, d + 1]``, ``[n_items + 1, d + 1]``."""
+    import torch
+
+    I = _dyn_item_rows(item_embeds, item_biases, norm_embed)
+    U = torch.cat([U, torch.ones((U.shape[0], 1), dtype=torch.float32, device=U.device)], dim=1)
+    return (torch.cat([U, U.mean(dim=0, keepdim=True)], dim=0).contiguous(),
+            torch.cat([I, I.mean(dim=0, keepdim=True)], dim=0).contiguous())
+
+
+def _dyn_item_rows(item_embeds, item_biases, norm_embed):
+    """``[I | b]`` [n_items, d + 1] of :func:`dyn_embed_tables`, without the mean row."""
+    import torch
+
+    if norm_embed:          # dyn_embed_base.py:264-265: the item side is normalised too (before the bias column)
+        I = item_embeds / item_embeds.norm(dim=1, keepdim=True)
+    else:
+        I = item_embeds
+    return torch.cat([I, item_biases[:, None]], dim=1)
+
+
+RNN_MAX_T, RNN_MAX_DIM, RNN_MAX_LAYERS = 128, 256, 4     # the envelope of b200_rnn_encode
+
+
+class RNN4Rec:
+    """libreco/algorithms/rnn4rec.py:151-237 (inference) + the serving step of ``DynEmbedBase``
+    (``bases/dyn_embed_base.py:166-269``).  The user vector is ``tf_dense(embed_size)(rnn(seq_embeds[seq]))``
+    (optionally L2-normalised): ``b200_rnn_encode`` runs the stacked GRU / LSTM over each user's recent sequence
+    (``recent_sequences``: right-padded with ``n_items``, len 0 for no history) and :func:`linear` the head.  The
+    item side is ``[item_embeds | item_bias]`` and the user side gets the pseudo bias 1, so all-items retrieval is
+    the embed scorer on d = embed_size + 1.  ``weights``: the dict of ``weights_io.rnn4rec_weights`` (or the raw
+    variables it takes).  RNN4Rec has no user table and no user features."""
+
+    def __init__(self, data_info_or_spec, weights, recent_seqs, recent_seq_lens, norm_embed=False, device=None):
+        import torch
+
+        from .weights_io import rnn4rec_weights
+
+        self._torch = torch
+        if "rnn_scheme" in weights:
+            weights = rnn4rec_weights(weights)
+        g = (data_info_or_spec.get if isinstance(data_info_or_spec, dict)
+             else lambda k: getattr(data_info_or_spec, k))
+        self.n_users, self.n_items = int(g("n_users")), int(g("n_items"))
+        self.device = torch.device(device) if device is not None else _lib.require_cuda()
+        self.norm_embed = bool(norm_embed)
+        layers = weights["rnn_layers"]
+        self.in_dim = int(np.shape(weights["seq_embeds"])[1])
+        self.hidden = [int(np.shape(lw["U"])[0]) for lw in layers]
+        self.T = int(np.shape(recent_seqs)[1])
+        if not 1 <= self.T <= RNN_MAX_T:
+            raise ValueError(f"RNN4Rec: max_seq_len {self.T} outside [1, {RNN_MAX_T}]")
+        if not 1 <= len(layers) <= RNN_MAX_LAYERS:
+            raise ValueError(f"RNN4Rec: {len(layers)} recurrent layers, supported 1 to {RNN_MAX_LAYERS}")
+        if max([self.in_dim] + self.hidden) > RNN_MAX_DIM:
+            raise ValueError(f"RNN4Rec: input width {self.in_dim} / hidden sizes {self.hidden} exceed {RNN_MAX_DIM}")
+        packed, d = [], self.in_dim
+        for lw, H in zip(layers, self.hidden):
+            parts = [np.asarray(lw[k], dtype=np.float32).reshape(-1) for k in ("W", "U", "bx", "bh", "gamma", "beta")]
+            flat = np.concatenate(parts)
+            if flat.size != int(_lib.lib.b200_rnn_layer_floats(int(lw["kind"]), d, H)):
+                raise ValueError(f"RNN4Rec: layer of kind {lw['kind']} with input {d} and hidden {H} has {flat.size} "
+                                 "packed floats")
+            packed.append(flat)
+            d = H
+        f32 = torch.float32
+        self.rnn_w = _dev(np.concatenate(packed), self.device, f32)
+        self.kinds = (ctypes.c_int32 * len(layers))(*[int(lw["kind"]) for lw in layers])
+        self.hid = (ctypes.c_int32 * len(layers))(*self.hidden)
+        self.acts = (ctypes.c_int32 * len(layers))(*[int(lw["act"]) for lw in layers])
+        self.seq_embeds = _dev(weights["seq_embeds"], self.device, f32)          # [n_items + 1, in_dim]
+        self.dense_Wt = _dev(np.asarray(weights["dense_kernel"]).T, self.device, f32)    # [K, H_last]
+        self.dense_b = _dev(np.asarray(weights["dense_bias"]).reshape(-1), self.device, f32)
+        self.K = int(self.dense_Wt.shape[0])
+        self.item_embeds = _dev(weights["item_embeds"], self.device, f32)        # [n_items, K]
+        self.item_biases = _dev(np.asarray(weights["item_biases"]).reshape(-1), self.device, f32)
+        self.seqs = _dev(recent_seqs, self.device, torch.int32)
+        self.lens = _dev(np.asarray(recent_seq_lens).reshape(-1), self.device, torch.int32)
+
+    def encode(self, ids_d, seqs=None, lens=None):
+        """[n, H_last]: ``b200_rnn_encode`` of the rows ``ids_d`` (device int64) of ``seqs`` / ``lens`` (default: the
+        model's recent sequences)."""
+        torch = self._torch
+        seqs = self.seqs if seqs is None else seqs
+        lens = self.lens if lens is None else lens
+        n = int(ids_d.numel())
+        h = torch.empty((n, self.hidden[-1]), dtype=torch.float32, device=self.device)
+        _lib.check(_lib.lib.b200_rnn_encode(
+            _lib.ptr(ids_d), n, _lib.ptr(lens), _lib.ptr(seqs), seqs.stride(0), self.T, _lib.ptr(self.seq_embeds),
+            self.seq_embeds.stride(0), self.in_dim, len(self.hidden), self.kinds, self.hid, self.acts,
+            _lib.ptr(self.rnn_w), _lib.ptr(h), h.stride(0), _lib.current_stream()))
+        return h
+
+    def user_vectors(self, ids, seqs=None, lens=None):
+        """[n, embed_size] user vectors of the rows ``ids`` of the recent sequences, or of the supplied ``seqs``
+        [*, T] / ``lens`` (host or device) when given: the encoder, the Dense head, then the L2 normalisation with
+        ``norm_embed``.  A row's bits depend only on its own sequence."""
+        torch = self._torch
+        ids_d = torch.as_tensor(np.asarray(ids, dtype=np.int64)).to(self.device)
+        if (seqs is None) != (lens is None):
+            raise ValueError("give both `seqs` and `lens`, or neither")
+        if seqs is not None:
+            seqs = _dev(seqs, self.device, torch.int32)
+            lens = _dev(np.asarray(lens).reshape(-1) if not isinstance(lens, torch.Tensor) else lens.reshape(-1),
+                        self.device, torch.int32)
+            if seqs.shape[1] != self.T:
+                raise ValueError(f"`seqs` has {seqs.shape[1]} columns, the model's max_seq_len is {self.T}")
+        x = linear(self.encode(ids_d, seqs, lens), self.dense_Wt, self.dense_b, ACT_NONE, impl="f32")
+        if self.norm_embed:
+            _lib.check(_lib.lib.b200_l2_normalize_rows(_lib.ptr(x), x.stride(0), x.shape[0], x.shape[1],
+                                                       _lib.current_stream()))
+        return x
+
+    def set_embeddings(self, chunk=1 << 20):
+        """Device tensors ``U [n_users + 1, K + 1]`` (pseudo bias 1 in the last column, last row = mean OOV row) and
+        ``I [n_items + 1, K + 1]`` (``[item_embeds | item_biases]`` + the mean row) for :class:`engine.EmbedScorer`."""
+        torch = self._torch
+        rows = [self.user_vectors(np.arange(i, min(self.n_users, i + chunk))) for i in range(0, self.n_users, chunk)]
+        return dyn_embed_tables(torch.cat(rows, dim=0), self.item_embeds, self.item_biases, self.norm_embed)
+
+    def recommend_dynamic(self, user_id, n_rec, data_info, user_feats=None, seq=None, filter_consumed=True,
+                          inner_id=False, return_scores=False):
+        """``recommend_user`` for ONE user with an optional behaviour sequence supplied for this call
+        (``dyn_embed_base.py:166-214``, ``recommendation/preprocess.py:26-46``): the sequence is cut to its last
+        ``max_seq_len`` items, unknown original ids become the pad id ``n_items``, and it is encoded once; without
+        one the user's cached sequence is used.  ``user_feats`` is accepted and ignored (the model has no user
+        features).  The vector scores ``I[:n_items]`` with the pseudo bias and the consumed filter (none for the
+        unknown user ``n_users``) and top-K select.  The model's sequence table is not touched."""
+        from .dynamic_feats import build_rec_seq
+
+        torch = self._torch
+        if n_rec > self.n_items:
+            raise ValueError(f"`n_rec` {n_rec} exceeds num of items {self.n_items}")
+        u = int(user_id)
+        if seq is not None and len(seq) > 0:
+            row, ln = build_rec_seq(seq, self.n_items, self.T, getattr(data_info, "item2id", None), inner_id)
+            v = self.user_vectors([0], row, ln)
         else:
-            I = self.item_embeds
-        U = torch.cat([U, torch.ones((U.shape[0], 1), dtype=torch.float32, device=self.device)], dim=1)
-        I = torch.cat([I, self.item_biases[:, None]], dim=1)
-        return (torch.cat([U, U.mean(dim=0, keepdim=True)], dim=0).contiguous(),
-                torch.cat([I, I.mean(dim=0, keepdim=True)], dim=0).contiguous())
+            v = self.user_vectors([u])
+        if not hasattr(self, "_I"):
+            self._I = _dyn_item_rows(self.item_embeds, self.item_biases, self.norm_embed).contiguous()
+        q = torch.cat([v, torch.ones((1, 1), dtype=torch.float32, device=self.device)], dim=1).contiguous()
+        N, d = self.n_items, q.shape[1]
+        scores = torch.empty((1, N), dtype=torch.float32, device=self.device)
+        zero = torch.zeros(1, dtype=torch.int64, device=self.device)
+        _lib.check(_lib.lib.b200_score_rows_f32(_lib.ptr(q), q.stride(0), _lib.ptr(zero), 1, _lib.ptr(self._I),
+                                                self._I.stride(0), N, d, _lib.ptr(scores), scores.stride(0),
+                                                _lib.current_stream()))
+        consumed = getattr(data_info, "user_consumed", None)
+        owner = _ConsumedOwner(consumed, self.n_users, self.n_items, self.device)
+        out_ids = torch.empty((1, n_rec), dtype=torch.int64, device=self.device)
+        out_sc = torch.empty((1, n_rec), dtype=torch.float32, device=self.device)
+        uid = torch.tensor([u], dtype=torch.int64, device=self.device)
+        masked_topk(owner, scores, uid, n_rec, filter_consumed, out_ids, out_sc)
+        ids = out_ids.cpu().numpy()
+        return (ids, out_sc.cpu().numpy()) if return_scores else ids
+
+
+class _ConsumedOwner:
+    """What :func:`engine.masked_topk` reads: the catalogue size and the consumed CSR on the device."""
+
+    def __init__(self, user_consumed, n_users, n_items, device):
+        csr = user_consumed if user_consumed is not None else ConsumedCSR(np.zeros(1, dtype=np.int64),
+                                                                          np.zeros(0, dtype=np.int32))
+        self.n_items = n_items
+        self.csr = as_csr(csr, n_users)
+        self.indptr_d, self.idx_d = self.csr.device(device)

@@ -240,3 +240,36 @@ def make_transformer_weights(rng, spec, K, num_heads=1, n_layers=1, max_seq_len=
             if n:
                 w[f"ln_{side}"] = dict(scale=scale(K), bias=rng.normal(0, 0.1, K).astype(np.float32))
     return w
+
+
+def make_rnn4rec_weights(rng, n_items, K, hidden_units=(16,), rnn_type="gru", use_layer_norm=False, scheme="keras"):
+    """RNN4Rec variables (libreco/algorithms/rnn4rec.py:151-237, layers/recurrent.py:4-63) in the raw shapes of the
+    graph `scheme` names: "keras" GRU ``kernel [in, 3H]``, ``recurrent_kernel [H, 3H]``, ``bias [2, 3H]``, keras LSTM
+    ``[in, 4H]``, ``[H, 4H]``, ``[4H]`` (+ LayerNorm gamma / beta with `use_layer_norm`); "legacy" GRU ``gates_*``
+    ``[in+H, 2H]`` / ``candidate_*`` ``[in+H, H]``, LSTM ``[in+H, 4H]``.  ``seq_embeds`` [n_items+1, hidden_units[0]]
+    (the pad row is an ordinary row), ``item_embeds`` [n_items, K], ``item_biases``, the head ``dense_kernel``
+    [H_last, K] and ``dense_bias``.  Biases are non-zero so that their placement is tested.
+    ``weights_io.rnn4rec_weights`` turns them into the engine's dict."""
+    hidden_units = [int(h) for h in hidden_units]
+    small = lambda *s: (rng.standard_normal(s) * 0.1).astype(np.float32)      # noqa: E731
+    layers, d = [], hidden_units[0]
+    for H in hidden_units:
+        if scheme == "keras":
+            G = 3 if rnn_type == "gru" else 4
+            lw = dict(kernel=_glorot(rng, (d, G * H)), recurrent_kernel=_glorot(rng, (H, G * H)),
+                      bias=small(2, G * H) if rnn_type == "gru" else small(G * H))
+            if use_layer_norm:
+                lw.update(gamma=rng.uniform(0.5, 1.5, H).astype(np.float32), beta=small(H))
+        elif scheme == "legacy":
+            if rnn_type == "gru":
+                lw = dict(gates_kernel=_glorot(rng, (d + H, 2 * H)), gates_bias=small(2 * H),
+                          candidate_kernel=_glorot(rng, (d + H, H)), candidate_bias=small(H))
+            else:
+                lw = dict(kernel=_glorot(rng, (d + H, 4 * H)), bias=small(4 * H))
+        else:
+            raise ValueError(f"unknown RNN4Rec naming scheme `{scheme}`")
+        layers.append(lw)
+        d = H
+    return dict(rnn_scheme=scheme, rnn_type=rnn_type, use_layer_norm=bool(use_layer_norm and scheme == "keras"),
+                seq_embeds=_glorot(rng, (n_items + 1, hidden_units[0])), item_embeds=_glorot(rng, (n_items, K)),
+                item_biases=small(n_items), rnn_layers=layers, dense_kernel=_glorot(rng, (d, K)), dense_bias=small(K))

@@ -139,9 +139,19 @@ AUTOINT_SCHEMES = ("keras", "legacy")
 
 
 def default_tf_names(model_name, n_hidden, use_bn, use_tf_attention=False, n_layers=None, scheme="keras",
-                     positional_embedding="trainable", feat_agg_mode="concat", item_sparse=False, item_dense=False):
+                     positional_embedding="trainable", feat_agg_mode="concat", item_sparse=False, item_dense=False,
+                     rnn_type="gru", use_layer_norm=False):
     """{engine weight key: TF variable name (or nested dict / list of names)} for the auto-named
-    variables of `model_name` in {"FM", "DeepFM", "DIN", "YouTubeRanking", "TwoTower", "AutoInt", "Transformer"}.
+    variables of `model_name` in {"FM", "DeepFM", "DIN", "YouTubeRanking", "TwoTower", "AutoInt", "Transformer",
+    "RNN4Rec"}.
+
+    RNN4Rec (rnn4rec.py:151-237 with layers/recurrent.py:4-63; `n_layers` = len(hidden_units)): "keras" layer i is
+    ``{t}[_i]/{t}_cell/{kernel,recurrent_kernel,bias}:0`` (t = gru or lstm) plus, with `use_layer_norm`,
+    ``layer_normalization[_i]/{gamma,beta}:0``; "legacy" cell i is ``rnn/multi_rnn_cell/cell_{i}/gru_cell/{gates,
+    candidate}/{kernel,bias}:0`` or ``.../lstm_cell/{kernel,bias}:0``.  Both: the head ``dense/{kernel,bias}:0``.
+    Returned under ``rnn_layers`` (per layer {kernel, recurrent_kernel, bias[, gamma, beta]} or {gates_kernel,
+    gates_bias, candidate_kernel, candidate_bias} or {kernel, bias}), ``dense_kernel`` and ``dense_bias``.  Keras
+    cell scopes differ between Keras versions: `extra_names` overrides them.
 
     Transformer (transformer.py:203-339; layer l = 1..L opens ``transformer_layer{l}``): per layer
     ``rms_norm_att/scale:0``, ``rms_norm_ffn/scale:0``, the attention and the two bias-free FFN ``tf_dense``.  "keras":
@@ -159,6 +169,8 @@ def default_tf_names(model_name, n_hidden, use_bn, use_tf_attention=False, n_lay
     ``dense/{kernel,bias}:0``; "legacy": four bias-free ``tf_dense`` per layer created as q, k, v, out, so layer l
     owns ``dense_{4l}`` .. ``dense_{4l+3}`` and the head is ``dense_{4L}``.  Returned under ``autoint_mha``
     (per-layer {query, key, value, attention_output | output}), ``out_kernel``, ``out_bias``."""
+    if model_name == "RNN4Rec":
+        return _rnn4rec_names(scheme, rnn_type, n_layers, use_layer_norm)
     if model_name == "Transformer":
         layers = []
         for i in range(n_layers):
@@ -452,9 +464,158 @@ def _youtube_retrieval_weights(npz, n_hidden, use_bn, extra_names=None):
     return w
 
 
+RNN4REC_TABLES = {"seq_embeds": "embedding/seq_embeds_var:0", "item_embeds": "embedding/item_embeds_var:0",
+                  "item_biases": "embedding/item_bias_var:0"}
+RNN_CELL_KINDS = {"gru_reset_after": 0, "gru_reset_before": 1, "lstm": 2}   # cell kinds of b200_rnn_encode
+RNN_ACT_TANH, RNN_ACT_LN_TANH = 0, 1
+
+
+def _rnn4rec_names(scheme, rnn_type, n_layers, use_layer_norm):
+    if rnn_type not in ("gru", "lstm"):
+        raise ValueError(f"`rnn_type` must be gru or lstm, not `{rnn_type}`")
+    layers = []
+    for i in range(n_layers):
+        if scheme == "keras":
+            sc = f"{rnn_type}{'' if i == 0 else f'_{i}'}/{rnn_type}_cell"
+            lw = {k: f"{sc}/{k}:0" for k in ("kernel", "recurrent_kernel", "bias")}
+            if use_layer_norm:
+                ln = f"layer_normalization{'' if i == 0 else f'_{i}'}"
+                lw.update(gamma=f"{ln}/gamma:0", beta=f"{ln}/beta:0")
+        elif scheme == "legacy":
+            sc = f"rnn/multi_rnn_cell/cell_{i}/{rnn_type}_cell"
+            if rnn_type == "gru":
+                lw = {f"{g}_{k}": f"{sc}/{g}/{k}:0" for g in ("gates", "candidate") for k in ("kernel", "bias")}
+            else:
+                lw = {k: f"{sc}/{k}:0" for k in ("kernel", "bias")}
+        else:
+            raise ValueError(f"unknown RNN4Rec naming scheme `{scheme}`")
+        layers.append(lw)
+    return {"rnn_layers": layers, "dense_kernel": "dense/kernel:0", "dense_bias": "dense/bias:0"}
+
+
+def rnn4rec_tf_shapes(scheme, rnn_type, in_dim, hidden_units, use_layer_norm, K):
+    """Expected shapes for :func:`default_tf_names` ("RNN4Rec"): keras GRU ``kernel [in, 3H]``, ``recurrent_kernel
+    [H, 3H]``, ``bias [2, 3H]`` (reset_after: input row, recurrent row), keras LSTM ``[in, 4H]``, ``[H, 4H]``,
+    ``[4H]``, LayerNorm ``[H]``; legacy GRU ``gates [in+H, 2H]`` + ``[2H]``, ``candidate [in+H, H]`` + ``[H]``,
+    legacy LSTM ``[in+H, 4H]`` + ``[4H]``; the head ``[H_last, K]``, ``[K]``."""
+    layers, d = [], int(in_dim)
+    for H in hidden_units:
+        H = int(H)
+        if scheme == "keras":
+            G = 3 if rnn_type == "gru" else 4
+            lw = dict(kernel=(d, G * H), recurrent_kernel=(H, G * H), bias=(2, G * H) if rnn_type == "gru" else (G * H,))
+            if use_layer_norm:
+                lw.update(gamma=(H,), beta=(H,))
+        elif rnn_type == "gru":
+            lw = dict(gates_kernel=(d + H, 2 * H), gates_bias=(2 * H,), candidate_kernel=(d + H, H), candidate_bias=(H,))
+        else:
+            lw = dict(kernel=(d + H, 4 * H), bias=(4 * H,))
+        layers.append(lw)
+        d = H
+    return {"rnn_layers": layers, "dense_kernel": (d, int(K)), "dense_bias": (int(K),)}
+
+
+def rnn_layers(layers, scheme, rnn_type, in_dim, use_layer_norm):
+    """Per-layer raw variables of either graph -> the engine's ``rnn_layers`` [{kind, act, W [in, G*H], U [H, G*H],
+    bx [G*H], bh [G*H], gamma [H], beta [H]}] in the canonical layout of ``b200_rnn_encode``.  keras GRU: blocks
+    z | r | h as stored, bias rows -> bx, bh.  keras LSTM: i | f | c | o as stored, the one bias -> bx.  legacy GRU:
+    the ``[x, h]`` kernels split at row ``in``, gate blocks r | u reordered to u | r, then the candidate; biases -> bx.
+    legacy LSTM: blocks i | j | f | o reordered to i | f | j | o, and ``forget_bias = 1.0`` (added at run time by
+    ``LSTMCell``) folded into the f bias in float32."""
+    f32 = lambda a: np.asarray(a, dtype=np.float32)      # noqa: E731
+    out, d = [], int(in_dim)
+    for lw in layers:
+        if scheme == "keras":
+            W, U = f32(lw["kernel"]), f32(lw["recurrent_kernel"])
+            H = U.shape[0]
+            if rnn_type == "gru":
+                b = f32(lw["bias"]).reshape(2, 3 * H)
+                kind, bx, bh = RNN_CELL_KINDS["gru_reset_after"], b[0], b[1]
+            else:
+                kind, bx, bh = RNN_CELL_KINDS["lstm"], f32(lw["bias"]).reshape(-1), np.zeros(4 * H, np.float32)
+            act = RNN_ACT_LN_TANH if use_layer_norm else RNN_ACT_TANH
+        elif scheme == "legacy":
+            if rnn_type == "gru":
+                gk, gb = f32(lw["gates_kernel"]), f32(lw["gates_bias"]).reshape(-1)
+                ck, cb = f32(lw["candidate_kernel"]), f32(lw["candidate_bias"]).reshape(-1)
+                H = ck.shape[1]
+                perm = np.r_[H:2 * H, 0:H]
+                W = np.concatenate([gk[:d, perm], ck[:d]], axis=1)
+                U = np.concatenate([gk[d:, perm], ck[d:]], axis=1)
+                kind, bx = RNN_CELL_KINDS["gru_reset_before"], np.concatenate([gb[perm], cb])
+                bh = np.zeros(3 * H, np.float32)
+            else:
+                k, b = f32(lw["kernel"]), f32(lw["bias"]).reshape(-1)
+                H = k.shape[1] // 4
+                perm = np.r_[0:H, 2 * H:3 * H, H:2 * H, 3 * H:4 * H]
+                W, U, bx = k[:d, perm], k[d:, perm], b[perm].copy()
+                bx[H:2 * H] += np.float32(1.0)
+                kind, bh = RNN_CELL_KINDS["lstm"], np.zeros(4 * H, np.float32)
+            act = RNN_ACT_TANH
+        else:
+            raise ValueError(f"unknown RNN4Rec naming scheme `{scheme}`")
+        ln = act == RNN_ACT_LN_TANH
+        out.append(dict(kind=kind, act=act, W=np.ascontiguousarray(W), U=np.ascontiguousarray(U),
+                        bx=np.ascontiguousarray(bx), bh=np.ascontiguousarray(bh),
+                        gamma=f32(lw["gamma"]).reshape(-1) if ln else np.ones(H, np.float32),
+                        beta=f32(lw["beta"]).reshape(-1) if ln else np.zeros(H, np.float32)))
+        d = H
+    return out
+
+
+def rnn4rec_weights(raw):
+    """Engine weight dict for :class:`feat_models.RNN4Rec` from the raw variables of either graph: ``raw`` holds
+    ``seq_embeds`` [n_items+1, hidden_units[0]], ``item_embeds`` [n_items, K], ``item_biases`` [n_items],
+    ``rnn_scheme``, ``rnn_type``, ``use_layer_norm``, ``rnn_layers`` (per layer, as :func:`default_tf_names` names
+    them), ``dense_kernel`` [H_last, K] and ``dense_bias`` [K]."""
+    w = {k: np.asarray(raw[k], dtype=np.float32) for k in ("seq_embeds", "item_embeds", "item_biases", "dense_kernel",
+                                                             "dense_bias")}
+    w["item_biases"] = w["item_biases"].reshape(-1)
+    w["dense_bias"] = w["dense_bias"].reshape(-1)
+    w["rnn_layers"] = rnn_layers(raw["rnn_layers"], raw["rnn_scheme"], raw["rnn_type"], w["seq_embeds"].shape[1],
+                                 bool(raw.get("use_layer_norm", False)))
+    return w
+
+
+def rnn4rec_tf_variables(raw):
+    """Raw RNN4Rec variables of either graph (the layout :func:`rnn4rec_weights` takes) -> ``{TF variable name:
+    array}`` named by :func:`default_tf_names`: what ``save_tf_variables`` writes as ``<name>_tf_variables.npz``, and
+    the inverse of ``load_reference_tf_model(..., "RNN4Rec", ...)``."""
+    names = default_tf_names("RNN4Rec", None, False, n_layers=len(raw["rnn_layers"]), scheme=raw["rnn_scheme"],
+                             rnn_type=raw["rnn_type"], use_layer_norm=bool(raw.get("use_layer_norm", False)))
+    out = {name: np.asarray(raw[k], dtype=np.float32) for k, name in RNN4REC_TABLES.items()}
+    out[RNN4REC_TABLES["item_biases"]] = out[RNN4REC_TABLES["item_biases"]].reshape(-1)
+    for lw, ln in zip(raw["rnn_layers"], names["rnn_layers"]):
+        for k, n in ln.items():
+            out[n] = np.asarray(lw[k], dtype=np.float32)
+    out[names["dense_kernel"]] = np.asarray(raw["dense_kernel"], dtype=np.float32)
+    out[names["dense_bias"]] = np.asarray(raw["dense_bias"], dtype=np.float32).reshape(-1)
+    return out
+
+
+def _rnn4rec_raw(npz, rnn_type, hidden_units, use_layer_norm, extra_names=None):
+    """Raw RNN4Rec variables of a saved model, every name and shape checked; the scheme is read off the names."""
+    scheme = "legacy" if any(k.startswith("rnn/multi_rnn_cell/") for k in npz.files) else "keras"
+    hidden_units = [int(h) for h in hidden_units]
+    names = default_tf_names("RNN4Rec", None, False, n_layers=len(hidden_units), scheme=scheme, rnn_type=rnn_type,
+                             use_layer_norm=use_layer_norm)
+    names.update(extra_names or {})
+    item = resolve_tf_names(npz, RNN4REC_TABLES["item_embeds"])
+    if item.ndim != 2:
+        raise KeyError(f"TF variable `{RNN4REC_TABLES['item_embeds']}` has shape {item.shape}, expected [n_items, K]")
+    n_items, K = item.shape
+    tables = {"seq_embeds": (n_items + 1, hidden_units[0]), "item_embeds": (n_items, K), "item_biases": (n_items,)}
+    raw = resolve_tf_names(npz, {k: RNN4REC_TABLES[k] for k in tables}, tables)
+    raw.update(resolve_tf_names(npz, names, rnn4rec_tf_shapes(scheme, rnn_type, hidden_units[0], hidden_units,
+                                                              use_layer_norm, K)))
+    raw.update(rnn_scheme=scheme, rnn_type=rnn_type, use_layer_norm=bool(use_layer_norm and scheme == "keras"))
+    return raw
+
+
 def load_reference_tf_model(path, model_name, arch, n_hidden, use_bn, use_tf_attention=False, extra_names=None,
                             num_heads=None, att_embed_size=(8, 8, 8), use_residual=True, num_tfm_layers=1,
-                            positional_embedding="trainable", use_causal_mask=False, feat_agg_mode="concat"):
+                            positional_embedding="trainable", use_causal_mask=False, feat_agg_mode="concat",
+                            rnn_type="gru", hidden_units=(16,), use_layer_norm=False):
     """Engine weight dict of a model saved by the reference (``save_tf_variables``,
     utils/save_load.py:70-98) WITHOUT a hand-written name map: the embedding-scope variables by their
     fixed names, the heads / MLPs / batch-norms through :func:`default_tf_names` (override single entries
@@ -463,12 +624,16 @@ def load_reference_tf_model(path, model_name, arch, n_hidden, use_bn, use_tf_att
     and shape is checked.  Transformer likewise, with ``num_heads``, ``num_tfm_layers``, ``positional_embedding``,
     ``use_causal_mask`` and ``feat_agg_mode`` (``num_heads`` defaults to each model's own default: 2 for AutoInt, 1
     for Transformer).  YouTubeRetrieval (``n_hidden`` Dense layers in the user tower) returns the layout of
-    ``feat_models.YouTubeRetrieval``, every name and shape checked."""
+    ``feat_models.YouTubeRetrieval``, every name and shape checked.  RNN4Rec takes its constructor's ``rnn_type``,
+    ``hidden_units`` and ``use_layer_norm`` (``n_hidden`` and ``use_bn`` are unused), reads the graph (keras or
+    legacy) off the names, checks every name and shape and returns the layout of ``feat_models.RNN4Rec``."""
     from .feat_models import from_tf_variables
 
     npz = np.load(os.path.join(path, f"{model_name}_tf_variables.npz"))
     if arch == "YouTubeRetrieval":
         return _youtube_retrieval_weights(npz, n_hidden, use_bn, extra_names)
+    if arch == "RNN4Rec":
+        return rnn4rec_weights(_rnn4rec_raw(npz, rnn_type, hidden_units, bool(use_layer_norm), extra_names))
     w = from_tf_variables(npz)
     if arch == "Transformer":
         scheme = "keras" if "transformer_layer1/multi_head_attention/query/kernel:0" in npz.files else "legacy"
