@@ -653,6 +653,32 @@ int b200_rnn_encode(const int64_t* users, int64_t n, const int32_t* lens, const 
                     const int32_t* hidden, const int32_t* acts, const float* weights, float* out, int64_t ldo,
                     void* stream);
 
+/* ---- RNN4Rec training (rnn4rec.py:151-237 in training mode, no dropout) ------------------------------------------
+ * b200_rnn_train_forward: b200_rnn_encode (the same out, bit for bit) that also saves what the backward needs.
+ * saved is a HOST array of 6 * n_layers device pointers; layer l's six tensors have n * T rows, row s * T + t:
+ *   [0] h_{t-1} [H]   [1] the layer output y_t [H] (h_t, or tanh(LayerNorm(h_t)))   [2] the post-activation gates
+ *   [G*H] (z | r | h~, z | r | c, i | f | c~ | o)   [3] LSTM c_t, Keras GRU U_c h_{t-1} + bh_c, TF1 GRU r o h_{t-1}
+ *   [H]   [4] x^ = (h_t - mean) rstd [H] and [5] rstd [1] (acts[l] = 1 only; NULL otherwise).
+ * Rows t >= len are 0.  Same envelope and errors as b200_rnn_encode.
+ * b200_rnn_backward: one layer's backward through time.  The layer (cell_kind, input width in_dim, hidden, act,
+ * layer_weights = its packed weights) reads its six saved tensors (saved: HOST array of 6 device pointers) and ONE of
+ * dout [n, lddo] (top layer: the gradient of the encoder output, taken at step len - 1) or dy [n * T, hidden] (the
+ * gradient of the layer's outputs y_t).  It WRITES, rows s * T + t, dgx [n * T, G*H] = d loss / d (x W + bx) per
+ * gate and, for the Keras GRU only, dgh [n * T, G*H] = d loss / d (h U + bh) (the candidate block scaled by r); for
+ * the other cells the h part equals dgx (TF1 GRU: the candidate block acts on r o h_{t-1}).  With act = 1 it also
+ * writes dln = dy (1 - y^2) and dlnx = dln x^ [n * T, hidden] (beta / gamma column sums); a len-0 row of the top
+ * layer writes its dln (through tanh(beta)) at t = 0.  Rows t >= len are otherwise 0.  No atomics.  Supported as
+ * b200_rnn_encode: 1 <= T <= 128, 1 <= in_dim, hidden <= 256; anything else returns -2 before launching; n = 0
+ * launches nothing. */
+int b200_rnn_train_forward(const int64_t* users, int64_t n, const int32_t* lens, const int32_t* seqs, int64_t ld_seq,
+                           int32_t T, const float* X, int64_t ldx, int32_t in_dim, int32_t n_layers,
+                           const int32_t* cell_kinds, const int32_t* hidden, const int32_t* acts, const float* weights,
+                           float* out, int64_t ldo, float* const* saved, void* stream);
+int b200_rnn_backward(const int64_t* users, int64_t n, const int32_t* lens, int32_t T, int32_t cell_kind,
+                      int32_t in_dim, int32_t hidden, int32_t act, const float* layer_weights, const float* dout,
+                      int64_t lddo, const float* dy, const float* const* saved, float* dgx, float* dgh, float* dln,
+                      float* dlnx, void* stream);
+
 /* ---- a14: predict_from_embedding (libreco/prediction/predict.py:36-40) -----------------
  * out[r] = sum_k U[users[r],k] * I[items[r],k]; mode 0: raw, 1: expit (ranking),
  * 2: clip to [lo, hi] (rating) — normalize_prediction (:18-23). */

@@ -148,6 +148,10 @@ SIGNATURES = {
     "b200_rnn_layer_floats": (c_int64, [c_int32, c_int32, c_int32]),
     "b200_rnn_encode": (c_int, [_P, c_int64, _P, _P, c_int64, c_int32, _P, c_int64, c_int32, c_int32, _P, _P, _P, _P,
                                 _P, c_int64, _P]),
+    "b200_rnn_train_forward": (c_int, [_P, c_int64, _P, _P, c_int64, c_int32, _P, c_int64, c_int32, c_int32, _P, _P,
+                                       _P, _P, _P, c_int64, _P, _P]),
+    "b200_rnn_backward": (c_int, [_P, c_int64, _P, c_int32, c_int32, c_int32, c_int32, c_int32, _P, _P, c_int64, _P,
+                                  _P, _P, _P, _P, _P, _P]),
 }
 
 for _name, (_res, _args) in SIGNATURES.items():

@@ -60,7 +60,12 @@ struct RnnParams {
   const float* w;
   float* out;
   int64_t ldo;
+  float* sv[RNN_MAX_LAYERS][6];   // training forward only: the saved tensors of each layer (SV_*), rows s * T + t
 };
+
+// What the training forward saves per layer, row s * T + t for t < len (rows t >= len are 0): the state before the
+// step, the layer output, the post-activation gates, one cell-specific block, and with layer norm x^ and rstd.
+enum SavedTensor { SV_HP = 0, SV_Y = 1, SV_G = 2, SV_X = 3, SV_XH = 4, SV_RS = 5 };
 
 // acc[g][v] = sum_k xs[v * ldxs + k] * W[k * ldw + col[g]], one chain per (g, v) over k ascending
 template <int NG>
@@ -86,7 +91,9 @@ __device__ __forceinline__ void chain(float (&acc)[NG][RNN_UPT], const float* __
 __device__ __forceinline__ float cell_act(int act, float x) { return act == ACT_TANH ? tanhf(x) : x; }
 
 // One step of layer l for every active user of the tile: new states into hn (and c in place).  GRU reset-before
-// runs in two passes because its candidate chain reads r o h of every unit.
+// runs in two passes because its candidate chain reads r o h of every unit.  SAVE (the training forward) also
+// writes h_{t-1}, the gates and the cell-specific block (LSTM c_t, Keras GRU U_c h + bh_c, TF1 GRU r o h_{t-1}).
+template <bool SAVE>
 __device__ void layer_step(const RnnParams& p, float* sm, int l, int t, const float* xin, int ldin) {
   const int kind = p.kind[l], H = p.H[l], act = p.act[l], in = p.in[l], tid = threadIdx.x;
   const int G = cell_gates(kind), GH = G * H, ldh = odd_ld(H), lds = odd_ld(p.Hmax);
@@ -120,6 +127,13 @@ __device__ void layer_step(const RnnParams& p, float* sm, int l, int t, const fl
         const float cn = fg * c[u * ldh + j] + ig * gg;
         c[u * ldh + j] = cn;
         hn[u * lds + j] = og * cell_act(act, cn);
+        if constexpr (SAVE) {
+          const int64_t row = ((int64_t)blockIdx.x * p.tile + u) * p.T + t;
+          float* g = p.sv[l][SV_G] + row * GH;
+          g[j] = ig; g[H + j] = fg; g[2 * H + j] = gg; g[3 * H + j] = og;
+          p.sv[l][SV_X][row * H + j] = cn;
+          p.sv[l][SV_HP][row * H + j] = h[u * ldh + j];
+        }
       }
     }
   } else if (kind == GRU_RESET_AFTER) {
@@ -140,6 +154,13 @@ __device__ void layer_step(const RnnParams& p, float* sm, int l, int t, const fl
         const float rg = sigmoid_f((ax[1][v] + b[1]) + (ah[1][v] + r[1]));
         const float hh = cell_act(act, (ax[2][v] + b[2]) + rg * (ah[2][v] + r[2]));
         hn[u * lds + j] = z * h[u * ldh + j] + (1.0f - z) * hh;
+        if constexpr (SAVE) {
+          const int64_t row = ((int64_t)blockIdx.x * p.tile + u) * p.T + t;
+          float* g = p.sv[l][SV_G] + row * GH;
+          g[j] = z; g[H + j] = rg; g[2 * H + j] = hh;
+          p.sv[l][SV_X][row * H + j] = ah[2][v] + r[2];
+          p.sv[l][SV_HP][row * H + j] = h[u * ldh + j];
+        }
       }
     }
   } else {   // GRU_RESET_BEFORE: z, r and the x part of the candidate; then the candidate over r o h
@@ -165,6 +186,14 @@ __device__ void layer_step(const RnnParams& p, float* sm, int l, int t, const fl
         zb[u * lds + j] = z;
         rh[u * lds + j] = rg * h[u * ldh + j];
         hn[u * lds + j] = ax[2][v] + b[2];
+        if constexpr (SAVE) {
+          if (t < slen[u]) {
+            const int64_t row = ((int64_t)blockIdx.x * p.tile + u) * p.T + t;
+            p.sv[l][SV_G][row * GH + H + j] = rg;
+            p.sv[l][SV_X][row * H + j] = rh[u * lds + j];
+            p.sv[l][SV_HP][row * H + j] = h[u * ldh + j];
+          }
+        }
       }
     }
     __syncthreads();
@@ -181,6 +210,11 @@ __device__ void layer_step(const RnnParams& p, float* sm, int l, int t, const fl
         const float cc = cell_act(act, hn[u * lds + j] + (ac[0][v] + r));
         const float z = zb[u * lds + j];
         hn[u * lds + j] = z * h[u * ldh + j] + (1.0f - z) * cc;
+        if constexpr (SAVE) {
+          const int64_t row = ((int64_t)blockIdx.x * p.tile + u) * p.T + t;
+          p.sv[l][SV_G][row * GH + j] = z;
+          p.sv[l][SV_G][row * GH + 2 * H + j] = cc;
+        }
       }
     }
   }
@@ -221,6 +255,49 @@ __device__ void layer_norm_tanh(const RnnParams& p, float* sm, int l) {
   __syncthreads();
 }
 
+// SAVE: the layer output of step t (h_t, or tanh(LN(h_t)) with x^ = (h_t - mean) rstd and rstd) for t < len
+__device__ void save_outputs(const RnnParams& p, const float* sm, int l, int t) {
+  const int H = p.H[l], ldh = odd_ld(H);
+  const bool ln = p.act[l] == ACT_LN_TANH;
+  const int* slen = reinterpret_cast<const int*>(sm + p.s_len);
+  const float* h = sm + p.s_h[l];
+  const float* st = sm + p.s_st;
+  for (int i = threadIdx.x; i < p.tile * H; i += blockDim.x) {
+    const int u = i / H, j = i - u * H;
+    if (t >= slen[u]) continue;
+    const int64_t row = ((int64_t)blockIdx.x * p.tile + u) * p.T + t;
+    p.sv[l][SV_Y][row * H + j] = ln ? sm[p.s_y[l] + u * ldh + j] : h[u * ldh + j];
+    if (ln) {
+      p.sv[l][SV_XH][row * H + j] = (h[u * ldh + j] - st[2 * u]) * st[2 * u + 1];
+      if (j == 0) p.sv[l][SV_RS][row] = st[2 * u + 1];
+    }
+  }
+}
+
+// SAVE: rows t >= len of every saved tensor are written as 0
+__device__ void save_zero_tail(const RnnParams& p, const float* sm) {
+  const int* slen = reinterpret_cast<const int*>(sm + p.s_len);
+  const int64_t s0 = (int64_t)blockIdx.x * p.tile;
+  for (int l = 0; l < p.L; ++l) {
+    const int H = p.H[l], GH = cell_gates(p.kind[l]) * H;
+    const bool ln = p.act[l] == ACT_LN_TANH;
+    for (int u = 0; u < p.tile; ++u) {
+      if (s0 + u >= p.n) break;
+      const int64_t r0 = (s0 + u) * p.T + slen[u], nr = p.T - slen[u];
+      for (int64_t i = threadIdx.x; i < nr * H; i += blockDim.x) {
+        p.sv[l][SV_HP][r0 * H + i] = 0.f;
+        p.sv[l][SV_Y][r0 * H + i] = 0.f;
+        p.sv[l][SV_X][r0 * H + i] = 0.f;
+        if (ln) p.sv[l][SV_XH][r0 * H + i] = 0.f;
+      }
+      for (int64_t i = threadIdx.x; i < nr * GH; i += blockDim.x) p.sv[l][SV_G][r0 * GH + i] = 0.f;
+      if (ln)
+        for (int64_t i = threadIdx.x; i < nr; i += blockDim.x) p.sv[l][SV_RS][r0 + i] = 0.f;
+    }
+  }
+}
+
+template <bool SAVE>
 __global__ void __launch_bounds__(RNN_THREADS) rnn_encode_kernel(const __grid_constant__ RnnParams p) {
   extern __shared__ float sm[];
   const int tid = threadIdx.x, nt = blockDim.x;
@@ -259,7 +336,7 @@ __global__ void __launch_bounds__(RNN_THREADS) rnn_encode_kernel(const __grid_co
     const float* xin = sm + p.s_x0;
     int ldin = ld0;
     for (int l = 0; l < p.L; ++l) {
-      layer_step(p, sm, l, t, xin, ldin);
+      layer_step<SAVE>(p, sm, l, t, xin, ldin);
       if (l + 1 < p.L) {
         if (p.act[l] == ACT_LN_TANH) {
           layer_norm_tanh(p, sm, l);
@@ -268,9 +345,13 @@ __global__ void __launch_bounds__(RNN_THREADS) rnn_encode_kernel(const __grid_co
           xin = sm + p.s_h[l];
         }
         ldin = odd_ld(p.H[l]);
+      } else if constexpr (SAVE) {
+        if (p.act[l] == ACT_LN_TANH) layer_norm_tanh(p, sm, l);
       }
+      if constexpr (SAVE) save_outputs(p, sm, l, t);
     }
   }
+  if constexpr (SAVE) save_zero_tail(p, sm);
   // output[:, -1] = the last layer's state after step len - 1 (after its LayerNorm and tanh when it has them)
   const int Lz = p.L - 1, H = p.H[Lz], ldh = odd_ld(H);
   const float* res = sm + p.s_h[Lz];
@@ -306,6 +387,242 @@ int64_t rnn_layout(RnnParams& p, int tile) {
   return off;
 }
 
+// ---- training: the backward through time of one layer ----------------------------------------------------------
+// One CTA owns a tile of users and runs the layer's steps in reverse from the tile's longest len.  dh (and dc) stay
+// in shared memory; at step t < len the incoming dY_t is added (through the LN + tanh backward for a layer-norm
+// layer), the gate pre-activation gradients are formed and written as dGx (x part) and dGh (h part, Keras GRU only:
+// the two differ in the candidate block, scaled by r), and dh_{t-1} = direct terms + dGh_t U^T is one ascending fmaf
+// chain per (unit, user) over U's row, read through L1 / L2.  The dense products over all rows (dW, dU, dX, the
+// bias, gamma and beta sums) run on the dense kernels outside.  No atomics: a user's rows depend on its own data.
+struct RnnBwdParams {
+  int T, tile, kind, H, GH, act, ldg;
+  int s_dh, s_dc, s_dd, s_q, s_g, s_st, s_len;
+  const int64_t* users;
+  int64_t n;
+  const int32_t* lens;
+  const float* U;
+  const float* gamma;   // gamma [H], beta [H] (layer norm)
+  const float* dout;    // top layer: the head gradient [n, lddo], added at step len - 1
+  int64_t lddo;
+  const float* dy;      // lower layer: dX of the layer above [n * T, H]
+  const float* sv[6];
+  float* dgx;
+  float* dgh;
+  float* dln;           // layer norm: dLN = dy (1 - y^2) and dLN x^, rows [n * T, H]
+  float* dlnx;
+};
+
+int64_t rnn_bwd_layout(RnnBwdParams& p, int tile) {
+  int64_t off = 0;
+  auto take = [&](int64_t floats) { const int64_t o = off; off += floats; return (int)o; };
+  const int64_t blk = (int64_t)tile * odd_ld(p.H);
+  p.tile = tile;
+  p.ldg = odd_ld(p.GH);
+  p.s_dh = take(blk);
+  p.s_dc = take(blk);
+  p.s_dd = take(blk);
+  p.s_q = take(blk);
+  p.s_g = take((int64_t)tile * p.ldg);
+  p.s_st = take(2 * (int64_t)tile);
+  p.s_len = take(tile);
+  return off;
+}
+
+// acc[v] = sum_{c < nc} g[(u0 + v) * ldg + c] * ur[c], one chain per user over c ascending
+__device__ __forceinline__ void row_chain(float (&acc)[RNN_UPT], const float* g, int ldg, const float* __restrict__ ur,
+                                          int nc) {
+#pragma unroll
+  for (int v = 0; v < RNN_UPT; ++v) acc[v] = 0.f;
+  for (int c = 0; c < nc; ++c) {
+    const float w = __ldg(ur + c);
+#pragma unroll
+    for (int v = 0; v < RNN_UPT; ++v) acc[v] = fmaf(g[v * ldg + c], w, acc[v]);
+  }
+}
+
+__global__ void __launch_bounds__(RNN_THREADS) rnn_backward_kernel(const __grid_constant__ RnnBwdParams p) {
+  extern __shared__ float sm[];
+  const int tid = threadIdx.x, nt = blockDim.x, H = p.H, GH = p.GH, ldh = odd_ld(H), ldg = p.ldg, T = p.T;
+  const bool ln = p.act == ACT_LN_TANH;
+  const int64_t s0 = (int64_t)blockIdx.x * p.tile;
+  int* slen = reinterpret_cast<int*>(sm + p.s_len);
+  float *dh = sm + p.s_dh, *dc = sm + p.s_dc, *dd = sm + p.s_dd, *q = sm + p.s_q, *sg = sm + p.s_g, *st = sm + p.s_st;
+  for (int u = tid; u < p.tile; u += nt) {
+    const int64_t s = s0 + u;
+    slen[u] = s < p.n ? min(max(p.lens[p.users[s]], 0), T) : 0;
+  }
+  for (int i = tid; i < p.tile * ldh; i += nt) { dh[i] = 0.f; dc[i] = 0.f; }
+  __syncthreads();
+  // rows t >= len of every output are 0
+  for (int u = 0; u < p.tile; ++u) {
+    if (s0 + u >= p.n) break;
+    const int64_t r0 = (s0 + u) * T + slen[u], nr = T - slen[u];
+    for (int64_t i = tid; i < nr * GH; i += nt) {
+      p.dgx[r0 * GH + i] = 0.f;
+      if (p.dgh) p.dgh[r0 * GH + i] = 0.f;
+    }
+    if (ln)
+      for (int64_t i = tid; i < nr * H; i += nt) { p.dln[r0 * H + i] = 0.f; p.dlnx[r0 * H + i] = 0.f; }
+  }
+  __syncthreads();
+  // a len-0 user of the top layer-norm layer outputs tanh(beta) (h = 0): its dLN goes to row t = 0 (x^ = 0)
+  if (ln && p.dout) {
+    for (int i = tid; i < p.tile * H; i += nt) {
+      const int u = i / H, j = i - u * H;
+      const int64_t s = s0 + u;
+      if (s >= p.n || slen[u] != 0) continue;
+      const float y = tanhf(__ldg(p.gamma + H + j));
+      p.dln[s * T * H + j] = p.dout[s * p.lddo + j] * (1.0f - y * y);
+    }
+  }
+  int steps = 0;
+  for (int u = 0; u < p.tile; ++u) steps = max(steps, slen[u]);
+  const float* Sg = p.sv[SV_G];
+  const float* Sx = p.sv[SV_X];
+  const float* Shp = p.sv[SV_HP];
+  const int items = H * (p.tile / RNN_UPT);
+  for (int t = steps - 1; t >= 0; --t) {
+    // 1. dh += dY_t (through the LN + tanh backward)
+    for (int i = tid; i < p.tile * H; i += nt) {
+      const int u = i / H, j = i - u * H;
+      if (t >= slen[u]) continue;
+      const int64_t s = s0 + u, row = s * T + t;
+      const float add = p.dy ? p.dy[row * H + j] : (t == slen[u] - 1 ? p.dout[s * p.lddo + j] : 0.f);
+      if (ln) {
+        const float y = p.sv[SV_Y][row * H + j], xh = p.sv[SV_XH][row * H + j];
+        const float dl = add * (1.0f - y * y);
+        p.dln[row * H + j] = dl;
+        p.dlnx[row * H + j] = dl * xh;
+        q[u * ldh + j] = dl * __ldg(p.gamma + j);
+      } else {
+        dh[u * ldh + j] += add;
+      }
+    }
+    __syncthreads();
+    if (ln) {
+      for (int u = tid; u < p.tile; u += nt) {
+        if (t >= slen[u]) continue;
+        const float* xh = p.sv[SV_XH] + ((s0 + u) * T + t) * H;
+        float a = 0.f, b = 0.f;
+        for (int j = 0; j < H; ++j) {
+          a += q[u * ldh + j];
+          b = fmaf(q[u * ldh + j], xh[j], b);
+        }
+        st[2 * u] = a / (float)H;
+        st[2 * u + 1] = b / (float)H;
+      }
+      __syncthreads();
+      for (int i = tid; i < p.tile * H; i += nt) {
+        const int u = i / H, j = i - u * H;
+        if (t >= slen[u]) continue;
+        const int64_t row = (s0 + u) * T + t;
+        const float xh = p.sv[SV_XH][row * H + j];
+        dh[u * ldh + j] += p.sv[SV_RS][row] * (q[u * ldh + j] - st[2 * u] - xh * st[2 * u + 1]);
+      }
+      __syncthreads();
+    }
+    // 2. the cell: gate pre-activation gradients, the direct terms of dh_{t-1} (and dc_{t-1})
+    int nc = GH;
+    if (p.kind == LSTM) {
+      for (int i = tid; i < p.tile * H; i += nt) {
+        const int u = i / H, j = i - u * H;
+        float* gs = sg + u * ldg;
+        if (t >= slen[u]) {
+          for (int g = 0; g < 4; ++g) gs[g * H + j] = 0.f;
+          continue;
+        }
+        const int64_t row = (s0 + u) * T + t;
+        const float* G = Sg + row * GH;
+        const float ig = G[j], fg = G[H + j], gg = G[2 * H + j], og = G[3 * H + j];
+        const float c1 = Sx[row * H + j], c0 = t ? Sx[(row - 1) * H + j] : 0.f;
+        const float tc = cell_act(p.act, c1);
+        const float dhv = dh[u * ldh + j];
+        const float dcv = dc[u * ldh + j] + dhv * og * (p.act == ACT_TANH ? 1.0f - tc * tc : 1.0f);
+        const float di = dcv * gg * ig * (1.0f - ig);
+        const float df = dcv * c0 * fg * (1.0f - fg);
+        const float dg = dcv * ig * (p.act == ACT_TANH ? 1.0f - gg * gg : 1.0f);
+        const float dov = dhv * tc * og * (1.0f - og);
+        dc[u * ldh + j] = dcv * fg;
+        float* dG = p.dgx + row * GH;
+        dG[j] = di; dG[H + j] = df; dG[2 * H + j] = dg; dG[3 * H + j] = dov;
+        gs[j] = di; gs[H + j] = df; gs[2 * H + j] = dg; gs[3 * H + j] = dov;
+        dd[u * ldh + j] = 0.f;
+      }
+    } else if (p.kind == GRU_RESET_AFTER) {
+      for (int i = tid; i < p.tile * H; i += nt) {
+        const int u = i / H, j = i - u * H;
+        float* gs = sg + u * ldg;
+        if (t >= slen[u]) {
+          for (int g = 0; g < 3; ++g) gs[g * H + j] = 0.f;
+          continue;
+        }
+        const int64_t row = (s0 + u) * T + t;
+        const float* G = Sg + row * GH;
+        const float z = G[j], r = G[H + j], hh = G[2 * H + j];
+        const float hp = Shp[row * H + j], dhv = dh[u * ldh + j];
+        const float dn = dhv * (1.0f - z) * (p.act == ACT_TANH ? 1.0f - hh * hh : 1.0f);
+        const float dz = dhv * (hp - hh) * z * (1.0f - z);
+        const float dr = dn * Sx[row * H + j] * r * (1.0f - r);
+        float* dG = p.dgx + row * GH;
+        float* dU = p.dgh + row * GH;
+        dG[j] = dz; dG[H + j] = dr; dG[2 * H + j] = dn;
+        dU[j] = dz; dU[H + j] = dr; dU[2 * H + j] = dn * r;
+        gs[j] = dz; gs[H + j] = dr; gs[2 * H + j] = dn * r;
+        dd[u * ldh + j] = dhv * z;
+      }
+    } else {   // GRU_RESET_BEFORE: z and the candidate first; r needs d(r o h) = dc U_c^T of every unit
+      for (int i = tid; i < p.tile * H; i += nt) {
+        const int u = i / H, j = i - u * H;
+        float* gs = sg + u * ldg;
+        if (t >= slen[u]) {
+          for (int g = 0; g < 3; ++g) gs[g * H + j] = 0.f;
+          continue;
+        }
+        const int64_t row = (s0 + u) * T + t;
+        const float* G = Sg + row * GH;
+        const float z = G[j], cc = G[2 * H + j];
+        const float hp = Shp[row * H + j], dhv = dh[u * ldh + j];
+        const float dn = dhv * (1.0f - z) * (p.act == ACT_TANH ? 1.0f - cc * cc : 1.0f);
+        const float dz = dhv * (hp - cc) * z * (1.0f - z);
+        float* dG = p.dgx + row * GH;
+        dG[j] = dz; dG[2 * H + j] = dn;
+        gs[j] = dz; gs[2 * H + j] = dn;
+      }
+      __syncthreads();
+      for (int it = tid; it < items; it += nt) {
+        const int j = it % H, u0 = (it / H) * RNN_UPT;
+        float acc[RNN_UPT];
+        row_chain(acc, sg + u0 * ldg + 2 * H, ldg, p.U + (int64_t)j * GH + 2 * H, H);
+#pragma unroll
+        for (int v = 0; v < RNN_UPT; ++v) {
+          const int u = u0 + v;
+          if (t >= slen[u]) continue;
+          const int64_t row = (s0 + u) * T + t;
+          const float z = Sg[row * GH + j], r = Sg[row * GH + H + j];
+          const float dr = acc[v] * Shp[row * H + j] * r * (1.0f - r);
+          p.dgx[row * GH + H + j] = dr;
+          sg[u * ldg + H + j] = dr;
+          dd[u * ldh + j] = dh[u * ldh + j] * z + acc[v] * r;
+        }
+      }
+      nc = 2 * H;
+    }
+    __syncthreads();
+    // 3. dh_{t-1} = direct + dGh_t U^T
+    for (int it = tid; it < items; it += nt) {
+      const int j = it % H, u0 = (it / H) * RNN_UPT;
+      float acc[RNN_UPT];
+      row_chain(acc, sg + u0 * ldg, ldg, p.U + (int64_t)j * GH, nc);
+#pragma unroll
+      for (int v = 0; v < RNN_UPT; ++v) {
+        const int u = u0 + v;
+        if (t < slen[u]) dh[u * ldh + j] = dd[u * ldh + j] + acc[v];
+      }
+    }
+    __syncthreads();
+  }
+}
+
 }  // namespace
 }  // namespace b200
 
@@ -316,11 +633,12 @@ extern "C" int64_t b200_rnn_layer_floats(int32_t cell_kind, int32_t in_dim, int3
   return rnn_layer_floats(cell_kind, in_dim, hidden);
 }
 
-extern "C" int b200_rnn_encode(const int64_t* users, int64_t n, const int32_t* lens, const int32_t* seqs,
-                               int64_t ld_seq, int32_t T, const float* X, int64_t ldx, int32_t in_dim,
-                               int32_t n_layers, const int32_t* cell_kinds, const int32_t* hidden,
-                               const int32_t* acts, const float* weights, float* out, int64_t ldo, void* stream) {
-  const char* who = "b200_rnn_encode";
+// the checks, weight offsets and launch shared by b200_rnn_encode and b200_rnn_train_forward
+static int rnn_encode_launch(const char* who, bool save, float* const* saved, const int64_t* users, int64_t n,
+                             const int32_t* lens, const int32_t* seqs, int64_t ld_seq, int32_t T, const float* X,
+                             int64_t ldx, int32_t in_dim, int32_t n_layers, const int32_t* cell_kinds,
+                             const int32_t* hidden, const int32_t* acts, const float* weights, float* out, int64_t ldo,
+                             void* stream) {
   B200_REQUIRE(T >= 1 && T <= RNN_MAX_T, "%s: sequence length %d outside [1, %d]", who, T, RNN_MAX_T);
   B200_REQUIRE(in_dim >= 1 && in_dim <= RNN_MAX_DIM, "%s: input width %d outside [1, %d]", who, in_dim, RNN_MAX_DIM);
   B200_REQUIRE(n_layers >= 1 && n_layers <= RNN_MAX_LAYERS, "%s: layer count %d outside [1, %d]", who, n_layers,
@@ -348,6 +666,17 @@ extern "C" int b200_rnn_encode(const int64_t* users, int64_t n, const int32_t* l
   B200_REQUIRE(ld_seq >= T && ldx >= in_dim && ldo >= hidden[n_layers - 1], "%s: bad leading dimension", who);
   p.users = users; p.n = n; p.lens = lens; p.seqs = seqs; p.ld_seq = ld_seq; p.X = X; p.ldx = ldx; p.w = weights;
   p.out = out; p.ldo = ldo;
+  for (int l = 0; l < RNN_MAX_LAYERS; ++l)
+    for (int k = 0; k < 6; ++k) p.sv[l][k] = nullptr;
+  if (save) {
+    B200_REQUIRE(saved, "%s: null saved-tensor table", who);
+    for (int l = 0; l < n_layers; ++l)
+      for (int k = 0; k < 6; ++k) {
+        p.sv[l][k] = saved[6 * l + k];
+        B200_REQUIRE(p.sv[l][k] || (k >= SV_XH && acts[l] != ACT_LN_TANH), "%s: layer %d saved tensor %d is null",
+                     who, l, k);
+      }
+  }
   int dev = 0, optin = 0;
   B200_CUDA_OK(cudaGetDevice(&dev));
   B200_CUDA_OK(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
@@ -357,9 +686,71 @@ extern "C" int b200_rnn_encode(const int64_t* users, int64_t n, const int32_t* l
   const size_t smem = (size_t)rnn_layout(p, tile) * sizeof(float);
   B200_REQUIRE(smem <= (size_t)optin, "%s: a tile of %d users needs %zu B of shared memory, the device allows %d", who,
                tile, smem, optin);
+  auto kernel = save ? rnn_encode_kernel<true> : rnn_encode_kernel<false>;
   if (smem > 48 * 1024)
-    B200_CUDA_OK(cudaFuncSetAttribute(rnn_encode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  rnn_encode_kernel<<<(unsigned)ceil_div64(n, tile), RNN_THREADS, smem, (cudaStream_t)stream>>>(p);
+    B200_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  kernel<<<(unsigned)ceil_div64(n, tile), RNN_THREADS, smem, (cudaStream_t)stream>>>(p);
+  count_launch();
+  B200_CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int b200_rnn_encode(const int64_t* users, int64_t n, const int32_t* lens, const int32_t* seqs,
+                               int64_t ld_seq, int32_t T, const float* X, int64_t ldx, int32_t in_dim,
+                               int32_t n_layers, const int32_t* cell_kinds, const int32_t* hidden,
+                               const int32_t* acts, const float* weights, float* out, int64_t ldo, void* stream) {
+  return rnn_encode_launch("b200_rnn_encode", false, nullptr, users, n, lens, seqs, ld_seq, T, X, ldx, in_dim,
+                           n_layers, cell_kinds, hidden, acts, weights, out, ldo, stream);
+}
+
+extern "C" int b200_rnn_train_forward(const int64_t* users, int64_t n, const int32_t* lens, const int32_t* seqs,
+                                      int64_t ld_seq, int32_t T, const float* X, int64_t ldx, int32_t in_dim,
+                                      int32_t n_layers, const int32_t* cell_kinds, const int32_t* hidden,
+                                      const int32_t* acts, const float* weights, float* out, int64_t ldo,
+                                      float* const* saved, void* stream) {
+  return rnn_encode_launch("b200_rnn_train_forward", true, saved, users, n, lens, seqs, ld_seq, T, X, ldx, in_dim,
+                           n_layers, cell_kinds, hidden, acts, weights, out, ldo, stream);
+}
+
+extern "C" int b200_rnn_backward(const int64_t* users, int64_t n, const int32_t* lens, int32_t T, int32_t cell_kind,
+                                 int32_t in_dim, int32_t hidden, int32_t act, const float* layer_weights,
+                                 const float* dout, int64_t lddo, const float* dy, const float* const* saved,
+                                 float* dgx, float* dgh, float* dln, float* dlnx, void* stream) {
+  const char* who = "b200_rnn_backward";
+  B200_REQUIRE(T >= 1 && T <= RNN_MAX_T, "%s: sequence length %d outside [1, %d]", who, T, RNN_MAX_T);
+  B200_REQUIRE(in_dim >= 1 && in_dim <= RNN_MAX_DIM, "%s: input width %d outside [1, %d]", who, in_dim, RNN_MAX_DIM);
+  B200_REQUIRE(hidden >= 1 && hidden <= RNN_MAX_DIM, "%s: hidden size %d outside [1, %d]", who, hidden, RNN_MAX_DIM);
+  B200_REQUIRE(cell_kind >= 0 && cell_kind <= 2, "%s: unknown cell kind %d", who, cell_kind);
+  B200_REQUIRE(act == ACT_TANH || act == ACT_LN_TANH, "%s: unknown activation %d", who, act);
+  B200_REQUIRE(n >= 0 && n <= (int64_t)0x7fffffff * 8, "%s: bad slot count %lld", who, (long long)n);
+  if (n == 0) return 0;
+  const bool ln = act == ACT_LN_TANH;
+  B200_REQUIRE(users && lens && layer_weights && saved && dgx, "%s: null pointer", who);
+  B200_REQUIRE((dout == nullptr) != (dy == nullptr), "%s: give exactly one of dout (top layer) and dy", who);
+  B200_REQUIRE(!dout || lddo >= hidden, "%s: bad leading dimension", who);
+  B200_REQUIRE(cell_kind != GRU_RESET_AFTER || dgh, "%s: the Keras GRU needs dgh", who);
+  for (int k = 0; k < 6; ++k)
+    B200_REQUIRE(saved[k] || (k >= SV_XH && !ln), "%s: saved tensor %d is null", who, k);
+  B200_REQUIRE(!ln || (dln && dlnx), "%s: a layer-norm layer needs dln and dlnx", who);
+  RnnBwdParams p;
+  p.T = T; p.kind = cell_kind; p.H = hidden; p.GH = cell_gates(cell_kind) * hidden; p.act = act;
+  p.users = users; p.n = n; p.lens = lens;
+  p.U = layer_weights + (int64_t)in_dim * p.GH;
+  p.gamma = layer_weights + rnn_layer_floats(cell_kind, in_dim, hidden) - 2 * hidden;
+  p.dout = dout; p.lddo = lddo; p.dy = dy;
+  for (int k = 0; k < 6; ++k) p.sv[k] = saved[k];
+  p.dgx = dgx; p.dgh = cell_kind == GRU_RESET_AFTER ? dgh : nullptr; p.dln = dln; p.dlnx = dlnx;
+  int dev = 0, optin = 0;
+  B200_CUDA_OK(cudaGetDevice(&dev));
+  B200_CUDA_OK(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+  int tile = RNN_MAX_TILE;
+  while (tile > RNN_UPT && rnn_bwd_layout(p, tile) * (int64_t)sizeof(float) > 96 * 1024) tile -= RNN_UPT;
+  const size_t smem = (size_t)rnn_bwd_layout(p, tile) * sizeof(float);
+  B200_REQUIRE(smem <= (size_t)optin, "%s: a tile of %d users needs %zu B of shared memory, the device allows %d", who,
+               tile, smem, optin);
+  if (smem > 48 * 1024)
+    B200_CUDA_OK(cudaFuncSetAttribute(rnn_backward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  rnn_backward_kernel<<<(unsigned)ceil_div64(n, tile), RNN_THREADS, smem, (cudaStream_t)stream>>>(p);
   count_launch();
   B200_CUDA_OK(cudaGetLastError());
   return 0;

@@ -1457,3 +1457,351 @@ class YouTubeRetrievalTrainer(_StackTrainer):
         if self._combiner is not None:
             w["multi_sparse_combiner"] = self._combiner
         return w
+
+
+RNN4REC_LOSSES = {"cross_entropy": 0, "focal": 1, "bpr": 2}
+
+
+class RNN4RecTrainer(_Trainer):
+    """RNN4Rec training step on the device: ``libreco/algorithms/rnn4rec.py:151-237`` in training mode (no dropout)
+    with ``layers/recurrent.py:4-63``, the losses of ``tfops/loss.py:4-25`` and TF-Adam
+    (``training/tf_trainer.py:103-124``).  The user vector of a row is ``Dense(embed_size)(rnn(seq_embeds[seq]))``
+    over the row's own sequence:
+
+        b200_gather_rows (the layer-0 input rows) -> b200_rnn_train_forward (the stacked cells, saving per step)
+        -> b200_linear_f32 (the head) -> [b200_l2_normalize_rows] -> scores <u, i> + b_i (b200_gather_dot)
+        -> b200_pointwise_loss / b200_pairwise_loss -> head and item gradients (b200_scatter_add_rows)
+        -> per layer, top down: b200_rnn_backward (dGx, dGh), then dW = X^T dGx, dU = H_prev^T dGh, dX = dGx W^T
+        on the dense kernels and the bias / gamma / beta sums on b200_col_reduce -> b200_scatter_add_rows of dX_0
+        into seq_embeds -> b200_adam_dense_dev
+
+    ``weights``: the raw variables of either TensorFlow graph (``synthetic.make_rnn4rec_weights``,
+    ``weights_io._rnn4rec_raw``).  The Adam variables are the TF variables' elements in the kernel's canonical order
+    (gate reordering and the split of the TF1 ``[x, h]`` kernels are permutations): W, U and the bias of every layer,
+    bh only for the Keras GRU, gamma / beta only with layer norm, the head, and the three tables.  The TF1 LSTM's
+    ``forget_bias = 1.0`` stays folded into the trained f bias; :meth:`export_weights` subtracts it again.
+
+    A pointwise step is ``step(users, items, seqs, lens, labels)`` (``cross_entropy``, ``focal``); a ``bpr`` step is
+    ``step(users, items_pos, seqs, lens, items_neg)``: row r scores its sequence against items_pos[r] and
+    items_neg[r].  ``seqs`` [B, T] holds item ids padded with the pad row ``n_items`` and ``lens`` [B] the valid
+    prefix of each row (a row at history position 0 has len 1 and the pad id).  ``users`` is not read (the model has
+    no user table).  With ``norm_embed`` users and items are L2-normalised; the BPR branch, as the reference's
+    (``rnn4rec.py:189-195``), scores the normalised items against the UN-normalised user vectors.  ``ValueError``
+    before any launch for shapes outside the envelope of ``b200_rnn_encode``, an unknown ``loss_type``,
+    ``rnn_type`` or scheme, the rating task, a ``seq_embeds`` row count other than ``n_items + 1`` and a batch whose
+    saved state does not fit in the free device memory."""
+
+    embed_table = "item_embeds"
+    reg_vars = ("seq_embeds", "item_embeds", "item_biases")
+
+    def __init__(self, spec, weights, loss_type="cross_entropy", norm_embed=False, task="ranking", lr=1e-3,
+                 epsilon=1e-5, device=None):
+        from .feat_models import RNN_MAX_DIM, RNN_MAX_LAYERS, RNN_MAX_T, _spec_get   # noqa: F401
+        from .weights_io import rnn4rec_weights
+
+        if task != "ranking":
+            raise ValueError(f"RNN4RecTrainer: task `{task}` is not supported (ranking only)")
+        if loss_type not in RNN4REC_LOSSES:
+            raise ValueError(f"RNN4RecTrainer: loss_type must be one of {sorted(RNN4REC_LOSSES)}, got `{loss_type}`")
+        if weights.get("rnn_scheme") not in ("keras", "legacy"):
+            raise ValueError(f"RNN4RecTrainer: unknown rnn_scheme `{weights.get('rnn_scheme')}`")
+        if weights.get("rnn_type") not in ("gru", "lstm"):
+            raise ValueError(f"RNN4RecTrainer: rnn_type must be gru or lstm, not `{weights.get('rnn_type')}`")
+        n_items = int(spec.n_items if isinstance(spec, FeatSpec) else _spec_get(spec)("n_items"))
+        if np.shape(weights["seq_embeds"])[0] != n_items + 1:
+            raise ValueError(f"RNN4RecTrainer: seq_embeds has {np.shape(weights['seq_embeds'])[0]} rows, expected "
+                             f"n_items + 1 = {n_items + 1}")
+        self.scheme, self.rnn_type = weights["rnn_scheme"], weights["rnn_type"]
+        self.use_layer_norm = bool(weights.get("use_layer_norm", False)) and self.scheme == "keras"
+        canon = rnn4rec_weights(weights)
+        self.in_dim = int(canon["seq_embeds"].shape[1])
+        self.hidden = [int(lw["U"].shape[0]) for lw in canon["rnn_layers"]]
+        if not 1 <= len(self.hidden) <= RNN_MAX_LAYERS:
+            raise ValueError(f"RNN4RecTrainer: {len(self.hidden)} recurrent layers, supported 1 to {RNN_MAX_LAYERS}")
+        if max([self.in_dim] + self.hidden) > RNN_MAX_DIM:
+            raise ValueError(f"RNN4RecTrainer: input width {self.in_dim} / hidden sizes {self.hidden} exceed "
+                             f"{RNN_MAX_DIM}")
+        self.loss_type, self.norm_embed = loss_type, bool(norm_embed)
+        self._canon = canon
+        super().__init__(spec, canon, False, lr, epsilon, device)
+        self._canon = None
+
+    def _init_params(self, weights):
+        import ctypes
+
+        torch = self._torch
+        p = self.params
+        layers = weights["rnn_layers"]
+        self.kinds = [int(lw["kind"]) for lw in layers]
+        self.acts = [int(lw["act"]) for lw in layers]
+        self._kinds = (ctypes.c_int32 * len(layers))(*self.kinds)
+        self._hid = (ctypes.c_int32 * len(layers))(*self.hidden)
+        self._acts = (ctypes.c_int32 * len(layers))(*self.acts)
+        packed, self._offs, d = [], [], self.in_dim
+        for lw, H in zip(layers, self.hidden):
+            flat = np.concatenate([np.asarray(lw[k], np.float32).reshape(-1)
+                                   for k in ("W", "U", "bx", "bh", "gamma", "beta")])
+            if flat.size != int(_lib.lib.b200_rnn_layer_floats(int(lw["kind"]), d, H)):
+                raise ValueError(f"RNN4RecTrainer: layer of kind {lw['kind']} with input {d} and hidden {H} has "
+                                 f"{flat.size} packed floats")
+            self._offs.append(sum(a.size for a in packed))
+            packed.append(flat)
+            d = H
+        # the packed weights the kernels read; the variables are views into it
+        self.rnn_w = _dev(np.concatenate(packed), self.device, torch.float32).clone()
+        d = self.in_dim
+        for l, (H, kind) in enumerate(zip(self.hidden, self.kinds)):
+            GH = (4 if kind == 2 else 3) * H
+            o = self._offs[l]
+            views = dict(W=(o, (d, GH)), U=(o + d * GH, (H, GH)), bx=(o + (d + H) * GH, (GH,)),
+                         bh=(o + (d + H + 1) * GH, (GH,)), gamma=(o + (d + H + 2) * GH, (H,)),
+                         beta=(o + (d + H + 2) * GH + H, (H,)))
+            names = ["W", "U", "bx"] + (["bh"] if kind == 0 else []) + (["gamma", "beta"] if self.acts[l] else [])
+            for k in names:
+                off, shape = views[k]
+                p[f"rnn{l}_{k}"] = self.rnn_w[off:off + int(np.prod(shape))].view(shape)
+            d = H
+        p["seq_embeds"] = self._var(weights["seq_embeds"])
+        p["item_biases"] = self._var(weights["item_biases"], -1)
+        p["dense_Wt"] = self._var(np.asarray(weights["dense_kernel"]).T.copy())       # [K, H_last]
+        p["dense_b"] = self._var(weights["dense_bias"], -1)
+
+    # -- memory ------------------------------------------------------------------------------------------------------
+    def saved_bytes_per_row(self, T):
+        """Device bytes one batch row keeps for the backward at sequence length T: the saved tensors of every layer
+        (h_{t-1}, y_t, the gates, the cell block, and x^ + rstd with layer norm), the layer-0 input rows, and the
+        largest layer's transient gradients (dGx, dGh, dX, dLN, dLN x^)."""
+        per_t, trans, d = self.in_dim, 0, self.in_dim
+        for l, (H, kind) in enumerate(zip(self.hidden, self.kinds)):
+            GH = (4 if kind == 2 else 3) * H
+            per_t += 3 * H + GH + (H + 1 if self.acts[l] else 0)
+            trans = max(trans, GH * (2 if kind == 0 else 1) + d + (2 * H if self.acts[l] else 0))
+            d = H
+        return 4 * T * (per_t + trans)
+
+    def _check_batch(self, B, T):
+        from .feat_models import RNN_MAX_T
+
+        torch = self._torch
+        if not 1 <= T <= RNN_MAX_T:
+            raise ValueError(f"RNN4RecTrainer: sequence length {T} outside [1, {RNN_MAX_T}]")
+        need = B * self.saved_bytes_per_row(T)
+        free = torch.cuda.mem_get_info(self.device)[0] + torch.cuda.memory_reserved(self.device) - \
+            torch.cuda.memory_allocated(self.device)
+        if need > free:
+            raise ValueError(f"RNN4RecTrainer: a batch of {B} rows x T = {T} keeps {need} B for the backward, "
+                             f"{free} B are free")
+
+    # -- forward -----------------------------------------------------------------------------------------------------
+    def encode(self, seqs_d, lens_d):
+        """[B, H_last] encoder outputs of the rows ``seqs_d`` [B, T] / ``lens_d`` [B] with the saved state; returns
+        (h, cache)."""
+        torch = self._torch
+        f32, dev = torch.float32, self.device
+        B, T = int(seqs_d.shape[0]), int(seqs_d.shape[1])
+        rows = torch.arange(B, dtype=torch.int64, device=dev)
+        idx = seqs_d.reshape(-1).to(torch.int64)
+        E = self.params["seq_embeds"]
+        X0 = torch.empty((B * T, self.in_dim), dtype=f32, device=dev)
+        _lib.check(_lib.lib.b200_gather_rows(_lib.ptr(E), E.stride(0), self.in_dim, _lib.ptr(idx), B * T,
+                                             _lib.ptr(X0), X0.stride(0), _lib.current_stream()))
+        saved, ptrs = [], []
+        for l, (H, kind) in enumerate(zip(self.hidden, self.kinds)):
+            GH = (4 if kind == 2 else 3) * H
+            sv = [torch.empty((B * T, H), dtype=f32, device=dev), torch.empty((B * T, H), dtype=f32, device=dev),
+                  torch.empty((B * T, GH), dtype=f32, device=dev), torch.empty((B * T, H), dtype=f32, device=dev)]
+            sv += ([torch.empty((B * T, H), dtype=f32, device=dev), torch.empty(B * T, dtype=f32, device=dev)]
+                   if self.acts[l] else [None, None])
+            saved.append(sv)
+            ptrs += [t.data_ptr() if t is not None else None for t in sv]
+        table = (_ctypes_ptr_array(len(ptrs)))(*ptrs)
+        h = torch.empty((B, self.hidden[-1]), dtype=f32, device=dev)
+        _lib.check(_lib.lib.b200_rnn_train_forward(
+            _lib.ptr(rows), B, _lib.ptr(lens_d), _lib.ptr(seqs_d), seqs_d.stride(0), T, _lib.ptr(E), E.stride(0),
+            self.in_dim, len(self.hidden), self._kinds, self._hid, self._acts, _lib.ptr(self.rnn_w), _lib.ptr(h),
+            h.stride(0), table, _lib.current_stream()))
+        return h, dict(rows=rows, idx=idx, X0=X0, saved=saved, B=B, T=T, lens=lens_d)
+
+    def user_vectors(self, seqs_d, lens_d):
+        """The head over the encoder output (before any normalisation): [B, K] and the cache."""
+        h, c = self.encode(seqs_d, lens_d)
+        p = self.params
+        u = linear(h, p["dense_Wt"], p["dense_b"], ACT_NONE, impl="f32")
+        c["h"] = h
+        return u, c
+
+    def _normalize(self, x):
+        if not self.norm_embed:
+            return x, None
+        y = x.clone()
+        _lib.check(_lib.lib.b200_l2_normalize_rows(_lib.ptr(y), y.stride(0), y.shape[0], y.shape[1],
+                                                   _lib.current_stream()))
+        return y, x
+
+    def _normalize_backward(self, dy, pre):
+        if pre is not None:
+            _lib.check(_lib.lib.b200_l2_normalize_backward(_lib.ptr(pre), pre.stride(0), _lib.ptr(dy), dy.stride(0),
+                                                           pre.shape[0], pre.shape[1], _lib.ptr(dy), dy.stride(0),
+                                                           _lib.current_stream()))
+        return dy
+
+    def _items(self, items_d):
+        """(item rows [B, K] normalised with norm_embed, their pre-normalisation rows or None, biases [B])."""
+        torch = self._torch
+        p, K, B = self.params, self.K, int(items_d.numel())
+        I0 = torch.empty((B, K), dtype=torch.float32, device=self.device)
+        b = torch.empty((B, 1), dtype=torch.float32, device=self.device)
+        st = _lib.current_stream()
+        _lib.check(_lib.lib.b200_gather_rows(_lib.ptr(p["item_embeds"]), K, K, _lib.ptr(items_d), B, _lib.ptr(I0), K,
+                                             st))
+        _lib.check(_lib.lib.b200_gather_rows(_lib.ptr(p["item_biases"]), 1, 1, _lib.ptr(items_d), B, _lib.ptr(b), 1,
+                                             st))
+        I, pre = self._normalize(I0)
+        return I, pre, b.view(-1)
+
+    def _score(self, u, I, b):
+        torch = self._torch
+        B = int(u.shape[0])
+        rows = torch.arange(B, dtype=torch.int64, device=self.device)
+        s = torch.empty(B, dtype=torch.float32, device=self.device)
+        _lib.check(_lib.lib.b200_gather_dot(_lib.ptr(u), u.stride(0), _lib.ptr(rows), _lib.ptr(I), I.stride(0),
+                                            _lib.ptr(rows), B, self.K, 0, 0.0, 0.0, _lib.ptr(s), _lib.current_stream()))
+        _lib.check(_lib.lib.b200_axpy(_lib.ptr(s), _lib.ptr(b), 1.0, B, _lib.current_stream()))
+        return s
+
+    # -- one step ----------------------------------------------------------------------------------------------------
+    def forward_backward(self, items_d, seqs_d, lens_d, labels_or_neg):
+        """Loss (device scalar) with every gradient buffer filled."""
+        torch = self._torch
+        lib, st, p, g, K = _lib.lib, _lib.current_stream(), self.params, self.grads, self.K
+        f32, dev = torch.float32, self.device
+        B = int(seqs_d.shape[0])
+        u0, c = self.user_vectors(seqs_d, lens_d)
+        loss = torch.empty((), dtype=f32, device=dev)
+        gI, gb = g["item_embeds"], g["item_biases"]
+        if self.loss_type == "bpr":
+            neg_d = labels_or_neg
+            Ip, Ip_pre, bp = self._items(items_d)
+            In, In_pre, bn = self._items(neg_d)
+            pos, neg = self._score(u0, Ip, bp), self._score(u0, In, bn)
+            dpos = torch.empty(B, dtype=f32, device=dev)
+            dneg = torch.empty(B, dtype=f32, device=dev)
+            _lib.check(lib.b200_pairwise_loss(_lib.ptr(pos), B, _lib.ptr(neg), B, 0, 0.0, 0.25, 2.0, 1, _lib.ptr(loss),
+                                              _lib.ptr(dpos), _lib.ptr(dneg), _lib.ptr(self._lws), self._lws.numel(),
+                                              st))
+            du = dpos[:, None] * Ip + dneg[:, None] * In           # the user side is not normalised (see above)
+            dIp = self._normalize_backward(dpos[:, None] * u0, Ip_pre)
+            dIn = self._normalize_backward(dneg[:, None] * u0, In_pre)
+            for ids, dI, db in ((items_d, dIp, dpos), (neg_d, dIn, dneg)):
+                _lib.check(lib.b200_scatter_add_rows(_lib.ptr(gI), K, K, _lib.ptr(ids), B, _lib.ptr(dI), K, st))
+                _lib.check(lib.b200_scatter_add_rows(_lib.ptr(gb), 1, 1, _lib.ptr(ids), B, _lib.ptr(db), 1, st))
+        else:
+            u, u_pre = self._normalize(u0)
+            I, I_pre, b = self._items(items_d)
+            logit = self._score(u, I, b)
+            dlogit = torch.empty(B, dtype=f32, device=dev)
+            _lib.check(lib.b200_pointwise_loss(_lib.ptr(logit), _lib.ptr(labels_or_neg), B,
+                                               RNN4REC_LOSSES[self.loss_type], 0.25, 2.0, _lib.ptr(loss),
+                                               _lib.ptr(dlogit), _lib.ptr(self._lws), self._lws.numel(), st))
+            du = self._normalize_backward(dlogit[:, None] * I, u_pre)
+            dI = self._normalize_backward(dlogit[:, None] * u, I_pre)
+            _lib.check(lib.b200_scatter_add_rows(_lib.ptr(gI), K, K, _lib.ptr(items_d), B, _lib.ptr(dI), K, st))
+            _lib.check(lib.b200_scatter_add_rows(_lib.ptr(gb), 1, 1, _lib.ptr(items_d), B, _lib.ptr(dlogit), 1, st))
+        du = du.contiguous()
+        # the Dense head
+        h = c["h"]
+        g["dense_Wt"].copy_(_weight_grad(du, h))
+        self._col_sum(du, g["dense_b"])
+        dh = linear(du, p["dense_Wt"].t().contiguous(), None, False, cache_split=False)
+        self.rnn_backward(c, dout=dh)
+        return loss
+
+    def rnn_backward(self, c, dout):
+        """Backward of :meth:`encode` given d loss / d h [B, H_last]: every recurrent variable's gradient and the
+        seq_embeds rows'."""
+        torch = self._torch
+        lib, st, g = _lib.lib, _lib.current_stream(), self.grads
+        f32, dev = torch.float32, self.device
+        B, T = c["B"], c["T"]
+        S = B * T
+        dy = None
+        for l in range(len(self.hidden) - 1, -1, -1):
+            H, kind, act = self.hidden[l], self.kinds[l], self.acts[l]
+            GH = (4 if kind == 2 else 3) * H
+            d = self.in_dim if l == 0 else self.hidden[l - 1]
+            sv = c["saved"][l]
+            dgx = torch.empty((S, GH), dtype=f32, device=dev)
+            dgh = torch.empty((S, GH), dtype=f32, device=dev) if kind == 0 else None
+            dln = torch.empty((S, H), dtype=f32, device=dev) if act else None
+            dlnx = torch.empty((S, H), dtype=f32, device=dev) if act else None
+            table = (_ctypes_ptr_array(6))(*[t.data_ptr() if t is not None else None for t in sv])
+            lw = self.rnn_w[self._offs[l]:]
+            _lib.check(lib.b200_rnn_backward(
+                _lib.ptr(c["rows"]), B, _lib.ptr(c["lens"]), T, kind, d, H, act, _lib.ptr(lw),
+                _lib.ptr(dout) if dy is None else None, dout.stride(0) if dy is None else 0, _lib.ptr(dy), table,
+                _lib.ptr(dgx), _lib.ptr(dgh), _lib.ptr(dln), _lib.ptr(dlnx), st))
+            X = c["X0"] if l == 0 else c["saved"][l - 1][1]
+            pre = f"rnn{l}_"
+            g[pre + "W"].copy_(_weight_grad(dgx, X).t())
+            hp = sv[0]
+            if kind == 1:        # TF1 GRU: the candidate block of U acts on r o h_{t-1}
+                g[pre + "U"][:, :2 * H].copy_(_weight_grad(dgx[:, :2 * H].contiguous(), hp).t())
+                g[pre + "U"][:, 2 * H:].copy_(_weight_grad(dgx[:, 2 * H:].contiguous(), sv[3]).t())
+            else:
+                g[pre + "U"].copy_(_weight_grad(dgx if dgh is None else dgh, hp).t())
+            self._col_sum(dgx, g[pre + "bx"])
+            if kind == 0:
+                self._col_sum(dgh, g[pre + "bh"])
+            if act:
+                self._col_sum(dlnx, g[pre + "gamma"])
+                self._col_sum(dln, g[pre + "beta"])
+            W = self.params[pre + "W"]
+            dy = linear(dgx, W, None, False, cache_split=False)          # dX = dGx W^T [S, d]
+        ge = g["seq_embeds"]
+        _lib.check(lib.b200_scatter_add_rows(_lib.ptr(ge), ge.stride(0), self.in_dim, _lib.ptr(c["idx"]), S,
+                                             _lib.ptr(dy), dy.stride(0), st))
+
+    def step(self, users_d, items_d, seqs_d, lens_d, labels_or_neg):
+        """One optimisation step; returns the device loss.  Pointwise losses: ``step(users, items, seqs, lens,
+        labels)``; bpr: ``step(users, items_pos, seqs, lens, items_neg)``."""
+        torch = self._torch
+        seqs_d = seqs_d.to(torch.int32).contiguous()
+        self._check_batch(int(seqs_d.shape[0]), int(seqs_d.shape[1]))
+        x = labels_or_neg.to(torch.int64 if self.loss_type == "bpr" else torch.float32).contiguous()
+        loss = self.forward_backward(items_d.to(torch.int64).contiguous(), seqs_d, lens_d.to(torch.int32).contiguous(),
+                                     x)
+        self._adam_update()
+        return loss
+
+    def canonical_layers(self):
+        """The trained layers in the canonical layout of ``weights_io.rnn_layers``."""
+        out, d = [], self.in_dim
+        w = self.rnn_w.cpu().numpy()
+        for l, (H, kind) in enumerate(zip(self.hidden, self.kinds)):
+            GH = (4 if kind == 2 else 3) * H
+            o = self._offs[l]
+            seg = lambda a, n: w[o + a:o + a + n]        # noqa: E731
+            out.append(dict(kind=kind, act=self.acts[l], W=seg(0, d * GH).reshape(d, GH).copy(),
+                            U=seg(d * GH, H * GH).reshape(H, GH).copy(), bx=seg((d + H) * GH, GH).copy(),
+                            bh=seg((d + H + 1) * GH, GH).copy(), gamma=seg((d + H + 2) * GH, H).copy(),
+                            beta=seg((d + H + 2) * GH + H, H).copy()))
+            d = H
+        return out
+
+    def export_weights(self):
+        """The raw variables of the trainer's scheme (``rnn4rec_weights``, ``rnn4rec_tf_variables`` and
+        ``feat_models.RNN4Rec`` take them as they stand)."""
+        from .weights_io import rnn_raw_layers
+
+        p = self.params
+        return dict(rnn_scheme=self.scheme, rnn_type=self.rnn_type, use_layer_norm=self.use_layer_norm,
+                    seq_embeds=p["seq_embeds"].cpu().numpy(), item_embeds=p["item_embeds"].cpu().numpy(),
+                    item_biases=p["item_biases"].cpu().numpy(),
+                    rnn_layers=rnn_raw_layers(self.canonical_layers(), self.scheme, self.rnn_type, self.in_dim),
+                    dense_kernel=p["dense_Wt"].cpu().numpy().T.copy(), dense_bias=p["dense_b"].cpu().numpy())
+
+
+def _ctypes_ptr_array(n):
+    import ctypes
+
+    return ctypes.c_void_p * n

@@ -563,6 +563,40 @@ def rnn_layers(layers, scheme, rnn_type, in_dim, use_layer_norm):
     return out
 
 
+def rnn_raw_layers(layers, scheme, rnn_type, in_dim, forget_bias=1.0):
+    """The inverse of :func:`rnn_layers`: canonical layers -> the per-layer raw variables of the graph `scheme`.  The
+    gate reorderings are involutions and the ``[x, h]`` kernels are stacked back; the TF1 LSTM's f bias has
+    ``forget_bias`` (1.0, what :func:`rnn_layers` folded in) subtracted in float32, so a raw -> canonical -> raw round
+    trip is exact for every variable except that bias, which it returns as ``fl32(fl32(b + 1) - 1)``.
+    ``forget_bias=0`` maps gradients, which the fold does not change."""
+    f32 = lambda a: np.asarray(a, dtype=np.float32)      # noqa: E731
+    out, d = [], int(in_dim)
+    for lw in layers:
+        W, U, bx, bh = f32(lw["W"]), f32(lw["U"]), f32(lw["bx"]).reshape(-1), f32(lw["bh"]).reshape(-1)
+        H = U.shape[0]
+        if scheme == "keras":
+            raw = dict(kernel=W.copy(), recurrent_kernel=U.copy(),
+                       bias=np.stack([bx, bh]) if rnn_type == "gru" else bx.copy())
+            if int(lw["act"]) == RNN_ACT_LN_TANH:
+                raw.update(gamma=f32(lw["gamma"]).copy(), beta=f32(lw["beta"]).copy())
+        elif scheme == "legacy":
+            if rnn_type == "gru":
+                perm = np.r_[H:2 * H, 0:H]
+                raw = dict(gates_kernel=np.concatenate([W[:, perm], U[:, perm]], axis=0), gates_bias=bx[perm],
+                           candidate_kernel=np.concatenate([W[:, 2 * H:], U[:, 2 * H:]], axis=0),
+                           candidate_bias=bx[2 * H:].copy())
+            else:
+                perm = np.r_[0:H, 2 * H:3 * H, H:2 * H, 3 * H:4 * H]
+                b = bx[perm].copy()
+                b[2 * H:3 * H] -= np.float32(forget_bias)
+                raw = dict(kernel=np.concatenate([W, U], axis=0)[:, perm], bias=b)
+        else:
+            raise ValueError(f"unknown RNN4Rec naming scheme `{scheme}`")
+        out.append({k: np.ascontiguousarray(v) for k, v in raw.items()})
+        d = H
+    return out
+
+
 def rnn4rec_weights(raw):
     """Engine weight dict for :class:`feat_models.RNN4Rec` from the raw variables of either graph: ``raw`` holds
     ``seq_embeds`` [n_items+1, hidden_units[0]], ``item_embeds`` [n_items, K], ``item_biases`` [n_items],
