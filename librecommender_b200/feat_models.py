@@ -138,6 +138,7 @@ def split_weights(Wt):
 
 
 ACT_NONE, ACT_RELU, ACT_SWISH = 0, 1, 2     # activation codes of b200_linear_* (include/b200reco.h)
+ACT_GELU = 3                                # b200_activation_* only: the erf gelu
 
 
 def linear(x, Wt, b, act, cache_split=True, impl=None):

@@ -165,6 +165,15 @@ def make_two_tower_weights(rng, spec, K, hidden=(64, 32), use_bn=True):
     return w
 
 
+def _mha_raw(rng, scheme, d_in, D, H):
+    """One ``multi_head_attention`` layer's raw variables of `scheme` (``weights_io._mha_tf_shapes``), each drawn
+    glorot over its 2-D view, in the order query, key, value, output."""
+    from .weights_io import _mha_2d, _mha_tf_shapes
+
+    raw = _mha_tf_shapes(scheme, d_in, D, H)
+    return {n: _glorot(rng, shp).reshape(raw[n]) for n, shp in _mha_2d(scheme, d_in, D).items()}
+
+
 def make_autoint_weights(rng, spec, K, att_embed_size=(8, 8, 8), num_heads=2, use_residual=True, version="keras",
                          combiner="sqrtn"):
     """AutoInt variables in the raw shapes of the graph TensorFlow `version` builds (layers/attention.py:67-138):
@@ -181,16 +190,7 @@ def make_autoint_weights(rng, spec, K, att_embed_size=(8, 8, 8), num_heads=2, us
         n_sparse = int(info["field_offset"][0]) + len(info["field_offset"])
     F = 2 + n_sparse + spec["n_dense"]
     H = int(num_heads)
-    mha = []
-    for hd in autoint_head_dims(att_embed_size):
-        D = H * hd
-        if scheme == "keras":
-            mha.append(dict(query=_glorot(rng, (K, D)).reshape(K, H, hd), key=_glorot(rng, (K, D)).reshape(K, H, hd),
-                            value=_glorot(rng, (K, D)).reshape(K, H, hd),
-                            attention_output=_glorot(rng, (D, K)).reshape(H, hd, K)))
-        else:
-            mha.append(dict(query=_glorot(rng, (K, D)), key=_glorot(rng, (K, D)), value=_glorot(rng, (D, D)),
-                            output=_glorot(rng, (D, K))))
+    mha = [_mha_raw(rng, scheme, K, H * hd, H) for hd in autoint_head_dims(att_embed_size)]
     w.update(autoint_scheme=scheme, autoint_mha=mha, num_heads=H, use_residual=bool(use_residual),
              out_kernel=_glorot(rng, (F * K, 1)), out_bias=np.float32(0.02).reshape(1))
     return w
@@ -220,13 +220,7 @@ def make_transformer_weights(rng, spec, K, num_heads=1, n_layers=1, max_seq_len=
     scale = lambda n: rng.uniform(0.5, 1.5, n).astype(np.float32)      # noqa: E731
     layers = []
     for _ in range(n_layers):
-        if scheme == "keras":
-            lw = dict(query=_glorot(rng, (D, D)).reshape(D, H, D // H), key=_glorot(rng, (D, D)).reshape(D, H, D // H),
-                      value=_glorot(rng, (D, D)).reshape(D, H, D // H),
-                      attention_output=_glorot(rng, (D, D)).reshape(H, D // H, D))
-        else:
-            lw = dict(query=_glorot(rng, (D, D)), key=_glorot(rng, (D, D)), value=_glorot(rng, (D, D)),
-                      output=_glorot(rng, (D, D)))
+        lw = _mha_raw(rng, scheme, D, D, H)
         lw.update(rms_att=scale(D), rms_ffn=scale(D), ffn1=_glorot(rng, (D, 4 * D)), ffn2=_glorot(rng, (4 * D, D)))
         layers.append(lw)
     w.update(tfm_scheme=scheme, tfm_layers=layers, rms_last=scale(D), rms_item=scale(Kp), num_heads=H,

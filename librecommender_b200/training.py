@@ -15,11 +15,14 @@ variable moves, i.e. a dense Adam step with a zero-filled gradient.  torch: memo
 """
 from __future__ import annotations
 
+import functools
+
 import numpy as np
 
 from . import _lib
-from .feat_models import (ACT_NONE, ACT_RELU, ACT_SWISH, FeatSpec, _dev, feat_backward, feat_forward, linear,
+from .feat_models import (ACT_GELU, ACT_NONE, ACT_RELU, ACT_SWISH, FeatSpec, _dev, feat_backward, feat_forward, linear,
                           permute_mlp_input, tables_struct)
+from .weights_io import _MHA_VARS, _check_mha_scheme, _mha_2d, _mha_tf_shapes
 
 BN_EPS = 1e-3          # tf.layers.batch_normalization defaults
 BN_MOMENTUM = 0.99
@@ -113,6 +116,74 @@ class _Trainer:
         X2 = X if X.dim() == 2 else X.view(-1, 1)
         _lib.check(_lib.lib.b200_col_reduce(_lib.ptr(X2), X2.stride(0), X2.shape[0], X2.shape[1], _lib.ptr(wrow), None, 0,
                                             _lib.ptr(out), _lib.current_stream()))
+
+    def _axpy(self, y, x):
+        """y += x (same shapes, contiguous) on the library's kernel."""
+        _lib.check(_lib.lib.b200_axpy(_lib.ptr(y), _lib.ptr(x), 1.0, y.numel(), _lib.current_stream()))
+
+    def _normalize(self, x):
+        """(L2-normalised copy of the rows of x, x) with ``norm_embed``, else (x, None)."""
+        if not self.norm_embed:
+            return x, None
+        y = x.clone()
+        _lib.check(_lib.lib.b200_l2_normalize_rows(_lib.ptr(y), y.stride(0), y.shape[0], y.shape[1],
+                                                   _lib.current_stream()))
+        return y, x
+
+    def _normalize_backward(self, dy, pre):
+        """d loss / d x of ``_normalize`` (in place of dy) given its second result."""
+        if pre is not None:
+            _lib.check(_lib.lib.b200_l2_normalize_backward(_lib.ptr(pre), pre.stride(0), _lib.ptr(dy), dy.stride(0),
+                                                           pre.shape[0], pre.shape[1], _lib.ptr(dy), dy.stride(0),
+                                                           _lib.current_stream()))
+        return dy
+
+    # ---- one multi_head_attention layer (layers/attention.py:67-138; layout in weights_io) of ``self.scheme`` with
+    # ``self.H`` heads: variables ``{prefix}{query, key, value, attention_output | output}`` held as 2-D views; the
+    # model's attention core comes in as callables ----------------------------------------------------------------
+    def _init_mha(self, prefix, lw, d_in, D, layer):
+        """Adds one layer's variables from its raw ``lw`` of input width d_in and width D; ``ValueError`` if a shape
+        differs."""
+        want = _mha_tf_shapes(self.scheme, d_in, D, self.H)
+        got = {n: tuple(np.shape(lw[n])) for n in want}
+        if got != want:
+            raise ValueError(f"{type(self).__name__} layer {layer}: attention shapes {got}, expected {want}")
+        for n, shp in _mha_2d(self.scheme, d_in, D).items():
+            self.params[prefix + n] = self._var(lw[n], shp)
+
+    def _mha_forward(self, prefix, X, core):
+        """q = X Wq, k = X Wk, v = (k if legacy else X) Wv, (o, lse) = core(q, k, v), then o Wo; returns (o Wo, cache)."""
+        wq, wk, wv, wo = (self.params[prefix + n] for n in _MHA_VARS[self.scheme])
+        q = linear(X, wq.t().contiguous(), None, ACT_NONE, cache_split=False)
+        k = linear(X, wk.t().contiguous(), None, ACT_NONE, cache_split=False)
+        v = linear(k if self.scheme == "legacy" else X, wv.t().contiguous(), None, ACT_NONE, cache_split=False)
+        o, lse = core(q, k, v)
+        return linear(o, wo.t().contiguous(), None, ACT_NONE, cache_split=False), dict(x=X, q=q, k=k, v=v, o=o, lse=lse)
+
+    def _mha_backward(self, prefix, c, dY, core_backward):
+        """Backward of ``_mha_forward`` given dY = d loss / d (o Wo): the four weight gradients ADDED into ``grads``;
+        returns d loss / d X.  ``core_backward(c, dO)`` returns (dq, dk, dv)."""
+        p, g = self.params, self.grads
+        nq, nk, nv, no = (prefix + n for n in _MHA_VARS[self.scheme])
+        g[no] += _weight_grad(dY, c["o"]).t()                     # dWo = O^T dY
+        dO = linear(dY, p[no], None, ACT_NONE, cache_split=False)  # dO = dY Wo^T
+        dq, dk, dv = core_backward(c, dO)
+        if self.scheme == "legacy":                                # V = Kproj Wv': Wk gets the V path too
+            g[nv] += _weight_grad(dv, c["k"]).t()                 # dWv' = Kproj^T dV
+            self._axpy(dk, linear(dv, p[nv], None, ACT_NONE, cache_split=False))
+        g[nq] += _weight_grad(dq, c["x"]).t()
+        g[nk] += _weight_grad(dk, c["x"]).t()
+        dX = linear(dq, p[nq], None, ACT_NONE, cache_split=False)
+        self._axpy(dX, linear(dk, p[nk], None, ACT_NONE, cache_split=False))
+        if self.scheme == "keras":
+            g[nv] += _weight_grad(dv, c["x"]).t()
+            self._axpy(dX, linear(dv, p[nv], None, ACT_NONE, cache_split=False))
+        return dX
+
+    def _export_mha(self, prefix, d_in, D):
+        """One layer's variables in their raw shapes (the inverse of ``_init_mha``)."""
+        return {n: self.params[prefix + n].cpu().numpy().reshape(shp)
+                for n, shp in _mha_tf_shapes(self.scheme, d_in, D, self.H).items()}
 
     def _dense1_forward(self, h):
         """Logits of the Dense(1) head (variables ``out_kernel`` [C], ``out_bias`` [1]) on ``h`` [R, C]."""
@@ -532,21 +603,12 @@ class TwoTowerTrainer(_StackTrainer):
         feat_forward(L, self.tables, ids_d, ids_d, n, concat=x)
         a, c = self._stack_forward(f"{which}_", self.n_layers[which], x)
         c["ids"] = ids_d
-        if self.norm_embed:
-            c["pre_norm"] = a
-            a = a.clone()
-            _lib.check(_lib.lib.b200_l2_normalize_rows(_lib.ptr(a), a.stride(0), n, a.shape[1], _lib.current_stream()))
-        c["out"] = a
+        c["out"], c["pre_norm"] = self._normalize(a)
         return c
 
     def tower_backward(self, which, c, da):
         n = int(c["ids"].numel())
-        da = da.contiguous()
-        if self.norm_embed:
-            x = c["pre_norm"]
-            _lib.check(_lib.lib.b200_l2_normalize_backward(_lib.ptr(x), x.stride(0), _lib.ptr(da), da.stride(0), n,
-                                                           x.shape[1], _lib.ptr(da), da.stride(0),
-                                                           _lib.current_stream()))
+        da = self._normalize_backward(da.contiguous(), c["pre_norm"])
         dconcat = self._stack_backward(f"{which}_", self.n_layers[which], c, da)
         feat_backward(self.spec.side(which)[0], self.tables, c["ids"], c["ids"], n, self.grads, dconcat=dconcat)
 
@@ -811,10 +873,6 @@ class DINTrainer(_SeqTrainer):
         return w
 
 
-TFM_ATT_NAMES = {"keras": ("query", "key", "value", "attention_output"), "legacy": ("query", "key", "value", "output")}
-ACT_GELU = 3      # b200_activation_* code of the erf gelu (include/b200reco.h)
-
-
 class TransformerTrainer(_SeqTrainer):
     """Transformer training step on the device: ``libreco/algorithms/transformer.py:203-339`` in training mode (no
     dropout), mean sigmoid CE, TF-Adam.  One behaviour sequence per ROW (``seqs`` [R, T], ``lens`` [R], clamped to
@@ -867,23 +925,20 @@ class TransformerTrainer(_SeqTrainer):
         D = self.D = Kp + K
         H = self.H = int(weights["num_heads"])
         self.scheme = weights["tfm_scheme"]
-        if self.scheme not in TFM_ATT_NAMES:
-            raise ValueError(f"TransformerTrainer: unknown naming scheme `{self.scheme}`")
+        _check_mha_scheme(self.scheme, "TransformerTrainer")
         layers = list(weights["tfm_layers"])
         if D > TRANSFORMER_MAX_D or not 1 <= len(layers) <= TRANSFORMER_MAX_LAYERS or H < 1 or D % H:
             raise ValueError(f"TransformerTrainer: width D = {D} (item features {Kp} + positions {K}), {len(layers)} "
                              f"layers, {H} heads outside D <= {TRANSFORMER_MAX_D}, 1..{TRANSFORMER_MAX_LAYERS} layers, "
                              f"heads dividing D")
-        hd = D // H
-        self.att_names = TFM_ATT_NAMES[self.scheme]
-        att = [(D, H, hd)] * 3 + [(H, hd, D)] if self.scheme == "keras" else [(D, D)] * 4
-        want = dict(zip(self.att_names, att), rms_att=(D,), rms_ffn=(D,), ffn1=(D, 4 * D), ffn2=(4 * D, D))
+        want = dict(rms_att=(D,), rms_ffn=(D,), ffn1=(D, 4 * D), ffn2=(4 * D, D))
         for l, lw in enumerate(layers):
+            self._init_mha(f"tfm{l}_", lw, D, D, l)
             got = {n: tuple(np.shape(lw[n])) for n in want}
             if got != want:
                 raise ValueError(f"TransformerTrainer layer {l}: shapes {got}, expected {want}")
             for n in want:
-                p[f"tfm{l}_{n}"] = self._var(lw[n], (D, D) if n in self.att_names else want[n])
+                p[f"tfm{l}_{n}"] = self._var(lw[n], want[n])
         self.n_tfm = len(layers)
         for n, shp in (("rms_last", D), ("rms_item", Kp)):
             if np.size(weights[n]) != shp:
@@ -941,10 +996,6 @@ class TransformerTrainer(_SeqTrainer):
                                        _lib.ptr(self.grads[name]), st))
         return dx
 
-    def _axpy(self, y, x):
-        """y += x (same shapes, contiguous) on the library's kernel."""
-        _lib.check(_lib.lib.b200_axpy(_lib.ptr(y), _lib.ptr(x), 1.0, y.numel(), _lib.current_stream()))
-
     def forward(self, users_d, items_d, seqs_d, lens_d):
         """Training-mode logits of the batch (batch statistics in the BN); caches what the backward needs."""
         torch = self._torch
@@ -962,26 +1013,26 @@ class TransformerTrainer(_SeqTrainer):
         X = torch.empty((RT, D), dtype=f32, device=dev)
         _lib.check(lib.b200_gather_rows(_lib.ptr(G), G.stride(0), Kp, _lib.ptr(seq_idx), RT, _lib.ptr(X), D, st))
         X.view(R, T, D)[:, :, Kp:] = pos                       # broadcast copy of the positions (plumbing)
-        layers = []
-        for l in range(self.n_tfm):
-            wq, wk, wv, wo = (p[f"tfm{l}_{n}"] for n in self.att_names)
-            h1, r1 = self._rms(X, f"tfm{l}_rms_att")
-            q = linear(h1, wq.t().contiguous(), None, ACT_NONE, cache_split=False)
-            k = linear(h1, wk.t().contiguous(), None, ACT_NONE, cache_split=False)
-            v = linear(k if self.scheme == "legacy" else h1, wv.t().contiguous(), None, ACT_NONE, cache_split=False)
+
+        def core(q, k, v):
             o = torch.empty((RT, D), dtype=f32, device=dev)
             lse = torch.empty(R * H * T, dtype=f32, device=dev)
             _lib.check(lib.b200_transformer_attention_forward(
                 _lib.ptr(q), q.stride(0), _lib.ptr(k), k.stride(0), _lib.ptr(v), v.stride(0), _lib.ptr(lens), R, T, H,
                 hd, int(self.causal), scale, _lib.ptr(o), o.stride(0), _lib.ptr(lse), st))
-            a = linear(o, wo.t().contiguous(), None, ACT_NONE, cache_split=False)
+            return o, lse
+
+        layers = []
+        for l in range(self.n_tfm):
+            h1, r1 = self._rms(X, f"tfm{l}_rms_att")
+            a, mha = self._mha_forward(f"tfm{l}_", h1, core)
             self._axpy(a, X)
             h2, r2 = self._rms(a, f"tfm{l}_rms_ffn")
             z = linear(h2, p[f"tfm{l}_ffn1"].t().contiguous(), None, ACT_NONE, cache_split=False)
             gz = self._activation(z, ACT_GELU)
             y = linear(gz, p[f"tfm{l}_ffn2"].t().contiguous(), None, ACT_NONE, cache_split=False)
             self._axpy(y, a)
-            layers.append(dict(x=X, h1=h1, r1=r1, q=q, k=k, v=v, o=o, lse=lse, a=a, h2=h2, r2=r2, z=z, gz=gz))
+            layers.append(dict(x=X, r1=r1, mha=mha, a=a, h2=h2, r2=r2, z=z, gz=gz))
             X = y
         S, rl = self._rms(X, "rms_last")
         # the target query [rms_item(G[item]) || 1..1]
@@ -1023,9 +1074,18 @@ class TransformerTrainer(_SeqTrainer):
         dGi = self._rms_backward(dq[:, :Kp], c["Gi"], c["ri"], "rms_item")      # the ones padding is a constant
         _lib.check(lib.b200_scatter_add_rows(_lib.ptr(dG), Kp, Kp, _lib.ptr(c["items"]), R, _lib.ptr(dGi), Kp, st))
         dX = self._rms_backward(dX, c["XL"], c["rl"], "rms_last")
+
+        def core_backward(m, dO):
+            dqh, dk, dv = (torch.empty((RT, D), dtype=f32, device=dev) for _ in range(3))
+            _lib.check(lib.b200_transformer_attention_backward(
+                _lib.ptr(m["q"]), m["q"].stride(0), _lib.ptr(m["k"]), m["k"].stride(0), _lib.ptr(m["v"]),
+                m["v"].stride(0), _lib.ptr(m["o"]), m["o"].stride(0), _lib.ptr(m["lse"]), _lib.ptr(dO), dO.stride(0),
+                _lib.ptr(c["lens"]), R, T, H, hd, int(self.causal), scale, _lib.ptr(dqh), _lib.ptr(dk), _lib.ptr(dv), D,
+                st))
+            return dqh, dk, dv
+
         for l in range(self.n_tfm - 1, -1, -1):
             a_ = c["layers"][l]
-            nq, nk, nv, no = (f"tfm{l}_{n}" for n in self.att_names)
             n1, n2 = f"tfm{l}_ffn1", f"tfm{l}_ffn2"
             # y = a + gelu(rms_ffn(a) W1) W2
             g[n2] += _weight_grad(dX, a_["gz"]).t()
@@ -1038,24 +1098,7 @@ class TransformerTrainer(_SeqTrainer):
             da = self._rms_backward(dh2, a_["a"], a_["r2"], f"tfm{l}_rms_ffn")
             self._axpy(da, dX)
             # a = x + MHA(rms_att(x))
-            g[no] += _weight_grad(da, a_["o"]).t()
-            dO = linear(da, p[no], None, ACT_NONE, cache_split=False)
-            dqh, dk, dv = (torch.empty((RT, D), dtype=f32, device=dev) for _ in range(3))
-            _lib.check(lib.b200_transformer_attention_backward(
-                _lib.ptr(a_["q"]), a_["q"].stride(0), _lib.ptr(a_["k"]), a_["k"].stride(0), _lib.ptr(a_["v"]),
-                a_["v"].stride(0), _lib.ptr(a_["o"]), a_["o"].stride(0), _lib.ptr(a_["lse"]), _lib.ptr(dO),
-                dO.stride(0), _lib.ptr(c["lens"]), R, T, H, hd, int(self.causal), scale, _lib.ptr(dqh), _lib.ptr(dk),
-                _lib.ptr(dv), D, st))
-            if self.scheme == "legacy":                                # V = Kproj Wv': Wk gets the V path too
-                g[nv] += _weight_grad(dv, a_["k"]).t()
-                self._axpy(dk, linear(dv, p[nv], None, ACT_NONE, cache_split=False))
-            g[nq] += _weight_grad(dqh, a_["h1"]).t()
-            g[nk] += _weight_grad(dk, a_["h1"]).t()
-            dh1 = linear(dqh, p[nq], None, ACT_NONE, cache_split=False)
-            self._axpy(dh1, linear(dk, p[nk], None, ACT_NONE, cache_split=False))
-            if self.scheme == "keras":
-                g[nv] += _weight_grad(dv, a_["h1"]).t()
-                self._axpy(dh1, linear(dv, p[nv], None, ACT_NONE, cache_split=False))
+            dh1 = self._mha_backward(f"tfm{l}_", a_["mha"], da, core_backward)
             dXn = self._rms_backward(dh1, a_["x"], a_["r1"], f"tfm{l}_rms_att")
             self._axpy(dXn, da)
             dX = dXn
@@ -1076,17 +1119,10 @@ class TransformerTrainer(_SeqTrainer):
         """The raw variables in the scheme they came in (``weights_io.transformer_weights`` makes the inference
         dict, ``weights_io.transformer_tf_variables`` the reference's variable names)."""
         p, D, H = self.params, self.D, self.H
-        hd = D // H
         w = super().export_weights()
-        layers = []
-        for l in range(self.n_tfm):
-            lw = {}
-            for n in self.att_names + ("rms_att", "rms_ffn", "ffn1", "ffn2"):
-                a = p[f"tfm{l}_{n}"].cpu().numpy()
-                if self.scheme == "keras" and n in self.att_names:
-                    a = a.reshape((H, hd, D) if n == "attention_output" else (D, H, hd))
-                lw[n] = a
-            layers.append(lw)
+        layers = [dict(self._export_mha(f"tfm{l}_", D, D), **{n: p[f"tfm{l}_{n}"].cpu().numpy()
+                                                              for n in ("rms_att", "rms_ffn", "ffn1", "ffn2")})
+                  for l in range(self.n_tfm)]
         w.update(tfm_scheme=self.scheme, tfm_layers=layers, rms_last=p["rms_last"].cpu().numpy(),
                  rms_item=p["rms_item"].cpu().numpy(), num_heads=H, use_causal_mask=self.causal,
                  feat_agg_mode="concat", out_kernel=w["out_kernel"].reshape(-1, 1),
@@ -1132,7 +1168,6 @@ class AutoIntTrainer(_Trainer):
 
     def _init_params(self, weights):
         from .feat_models import AUTOINT_MAX_D, AUTOINT_MAX_F, AUTOINT_MAX_K, AUTOINT_MAX_LAYERS
-        from .weights_io import AUTOINT_SCHEMES
 
         p, K, F = self.params, self.K, self.F
         self.scheme = weights["autoint_scheme"]
@@ -1140,64 +1175,48 @@ class AutoIntTrainer(_Trainer):
         self.use_residual = bool(weights.get("use_residual", True))
         self._combiner = weights.get("multi_sparse_combiner")
         mha = list(weights["autoint_mha"])
-        if self.scheme not in AUTOINT_SCHEMES:
-            raise ValueError(f"AutoIntTrainer: unknown naming scheme `{self.scheme}`")
+        _check_mha_scheme(self.scheme, "AutoIntTrainer")
         if K > AUTOINT_MAX_K or F > AUTOINT_MAX_F or not 1 <= len(mha) <= AUTOINT_MAX_LAYERS or H < 1:
             raise ValueError(f"AutoIntTrainer: K {K}, F {F}, {len(mha)} layers, {H} heads outside K <= "
                              f"{AUTOINT_MAX_K}, F <= {AUTOINT_MAX_F}, 1..{AUTOINT_MAX_LAYERS} layers, heads >= 1")
-        self.names = ("query", "key", "value", "attention_output" if self.scheme == "keras" else "output")
         self.head_dims = []
         for l, lw in enumerate(mha):
-            q = np.asarray(lw["query"])
-            D = int(np.prod(q.shape[1:]))
-            hd = D // H
-            if self.scheme == "keras":
-                want = [(K, H, hd), (K, H, hd), (K, H, hd), (H, hd, K)]
-                views = [(K, D), (K, D), (K, D), (D, K)]
-            else:
-                want = views = [(K, D), (K, D), (D, D), (D, K)]
-            got = [tuple(np.shape(lw[n])) for n in self.names]
-            if D % H or not 1 <= D <= AUTOINT_MAX_D or got != [tuple(s) for s in want]:
-                raise ValueError(f"AutoIntTrainer layer {l}: shapes {got} with {H} heads, expected {want} and "
-                                 f"num_heads x head size <= {AUTOINT_MAX_D}")
-            for n, shp in zip(self.names, views):
-                p[f"mha{l}_{n}"] = self._var(lw[n], shp)
-            self.head_dims.append(hd)
+            D = int(np.prod(np.shape(lw["query"])[1:]))
+            if D % H or not 1 <= D <= AUTOINT_MAX_D:
+                raise ValueError(f"AutoIntTrainer layer {l}: width {D} with {H} heads, expected a multiple of the "
+                                 f"heads <= {AUTOINT_MAX_D}")
+            self._init_mha(f"mha{l}_", lw, K, D, l)
+            self.head_dims.append(D // H)
         if np.size(weights["out_kernel"]) != F * K:
             raise ValueError(f"AutoIntTrainer: out_kernel has {np.size(weights['out_kernel'])} entries, expected "
                              f"F*K = {F}*{K}")
         p["out_kernel"] = self._var(weights["out_kernel"], -1)
         p["out_bias"] = self._var(weights["out_bias"], 1)
 
-    def _axpy(self, y, x):
-        """y += x (same shapes, contiguous) on the library's kernel."""
-        _lib.check(_lib.lib.b200_axpy(_lib.ptr(y), _lib.ptr(x), 1.0, y.numel(), _lib.current_stream()))
-
     def forward(self, users_d, items_d):
         """Training-mode logits of the batch; caches what the backward needs."""
         torch = self._torch
-        p, K, F, H = self.params, self.K, self.F, self.H
+        K, F, H = self.K, self.F, self.H
         R = int(users_d.numel())
         f32, dev = torch.float32, self.device
         x = torch.empty((R, F * K), dtype=f32, device=dev)
         feat_forward(self.spec.layout, self.tables, users_d, items_d, R, concat=x)
         X = x.view(R * F, K)
-        layers = []
-        for l, hd in enumerate(self.head_dims):
-            wq, wk, wv, wo = (p[f"mha{l}_{n}"] for n in self.names)
-            D = H * hd
-            q = linear(X, wq.t().contiguous(), None, False, cache_split=False)
-            k = linear(X, wk.t().contiguous(), None, False, cache_split=False)
-            v = linear(k if self.scheme == "legacy" else X, wv.t().contiguous(), None, False, cache_split=False)
-            o = torch.empty((R * F, D), dtype=f32, device=dev)
+
+        def core(q, k, v, hd):
+            o = torch.empty((R * F, H * hd), dtype=f32, device=dev)
             lse = torch.empty(R * H * F, dtype=f32, device=dev)
             _lib.check(_lib.lib.b200_autoint_attention_forward(
                 _lib.ptr(q), q.stride(0), _lib.ptr(k), k.stride(0), _lib.ptr(v), v.stride(0), R, F, H, hd,
                 float(1.0 / np.sqrt(hd)), _lib.ptr(o), o.stride(0), _lib.ptr(lse), _lib.current_stream()))
-            y = linear(o, wo.t().contiguous(), None, False, cache_split=False)
+            return o, lse
+
+        layers = []
+        for l, hd in enumerate(self.head_dims):
+            y, a = self._mha_forward(f"mha{l}_", X, functools.partial(core, hd=hd))
             if self.use_residual:
                 self._axpy(y, X)
-            layers.append(dict(x=X, q=q, k=k, v=v, o=o, lse=lse))
+            layers.append(a)
             X = y
         h = X.view(R, F * K)
         logit = self._dense1_forward(h)
@@ -1207,38 +1226,29 @@ class AutoIntTrainer(_Trainer):
     def backward(self, labels_d):
         """Loss + every gradient buffer filled (before the optimiser); returns the device loss."""
         torch = self._torch
-        p, g, K, F, H = self.params, self.grads, self.K, self.F, self.H
+        K, F, H = self.K, self.F, self.H
         c = self._cache
         R = c["R"]
         loss, dh = self._dense1_backward(c["h"], c["logit"], labels_d)
-        dX = dh.view(R * F, K)
-        for l in range(len(self.head_dims) - 1, -1, -1):
-            hd, a = self.head_dims[l], c["layers"][l]
-            nq, nk, nv, no = (f"mha{l}_{n}" for n in self.names)
+
+        def core_backward(a, dO, hd):
             D = H * hd
-            dY = dX
-            g[no] += _weight_grad(dY, a["o"]).t()                     # dWo = O^T dY
-            dO = linear(dY, p[no], None, False, cache_split=False)     # dO = dY Wo^T
             dq, dk, dv = (torch.empty((R * F, D), dtype=torch.float32, device=self.device) for _ in range(3))
             _lib.check(_lib.lib.b200_autoint_attention_backward(
                 _lib.ptr(a["q"]), a["q"].stride(0), _lib.ptr(a["k"]), a["k"].stride(0), _lib.ptr(a["v"]),
                 a["v"].stride(0), _lib.ptr(a["o"]), a["o"].stride(0), _lib.ptr(a["lse"]), _lib.ptr(dO), dO.stride(0),
                 R, F, H, hd, float(1.0 / np.sqrt(hd)), _lib.ptr(dq), _lib.ptr(dk), _lib.ptr(dv), D,
                 _lib.current_stream()))
-            if self.scheme == "legacy":                                # V = Kproj Wv': Wk gets the V path too
-                g[nv] += _weight_grad(dv, a["k"]).t()                 # dWv' = Kproj^T dV
-                self._axpy(dk, linear(dv, p[nv], None, False, cache_split=False))
-            g[nq] += _weight_grad(dq, a["x"]).t()
-            g[nk] += _weight_grad(dk, a["x"]).t()
-            dXn = linear(dq, p[nq], None, False, cache_split=False)
-            self._axpy(dXn, linear(dk, p[nk], None, False, cache_split=False))
-            if self.scheme == "keras":
-                g[nv] += _weight_grad(dv, a["x"]).t()
-                self._axpy(dXn, linear(dv, p[nv], None, False, cache_split=False))
+            return dq, dk, dv
+
+        dX = dh.view(R * F, K)
+        for l in range(len(self.head_dims) - 1, -1, -1):
+            dXn = self._mha_backward(f"mha{l}_", c["layers"][l], dX,
+                                     functools.partial(core_backward, hd=self.head_dims[l]))
             if self.use_residual:
-                self._axpy(dXn, dY)
+                self._axpy(dXn, dX)
             dX = dXn
-        feat_backward(self.spec.layout, self.tables, c["users"], c["items"], R, g, dconcat=dX.view(R, F * K))
+        feat_backward(self.spec.layout, self.tables, c["users"], c["items"], R, self.grads, dconcat=dX.view(R, F * K))
         return loss
 
     def step(self, users_d, items_d, labels_d):
@@ -1252,14 +1262,9 @@ class AutoIntTrainer(_Trainer):
 
     def export_weights(self):
         """The raw variables in the scheme they came in (``weights_io.autoint_weights`` makes the inference dict)."""
-        p, K, H = self.params, self.K, self.H
+        p, H = self.params, self.H
         w = self._export_tables()
-        mha = []
-        for l, hd in enumerate(self.head_dims):
-            lw = {n: p[f"mha{l}_{n}"].cpu().numpy() for n in self.names}
-            if self.scheme == "keras":
-                lw = {n: a.reshape((H, hd, K) if n == "attention_output" else (K, H, hd)) for n, a in lw.items()}
-            mha.append(lw)
+        mha = [self._export_mha(f"mha{l}_", self.K, H * hd) for l, hd in enumerate(self.head_dims)]
         w.update(autoint_scheme=self.scheme, autoint_mha=mha, num_heads=H, use_residual=self.use_residual,
                  out_kernel=p["out_kernel"].cpu().numpy().reshape(-1, 1), out_bias=p["out_bias"].cpu().numpy().reshape(1))
         if self._combiner is not None:
@@ -1348,22 +1353,6 @@ class YouTubeRetrievalTrainer(_StackTrainer):
             self.sampler_kind, self.n_items, self.S, self.seed, _lib.ptr(self._step_dev), _lib.ptr(self._owner),
             self._owner.numel() * 4, _lib.ptr(self.sampled), _lib.ptr(self.num_tries), _lib.current_stream()))
         return self.sampled, self.num_tries
-
-    def _normalize(self, x):
-        """(L2-normalised copy of x, x) with norm_embed, else (x, None)."""
-        if not self.norm_embed:
-            return x, None
-        y = x.clone()
-        _lib.check(_lib.lib.b200_l2_normalize_rows(_lib.ptr(y), y.stride(0), y.shape[0], y.shape[1],
-                                                   _lib.current_stream()))
-        return y, x
-
-    def _normalize_backward(self, dy, pre):
-        if pre is not None:
-            _lib.check(_lib.lib.b200_l2_normalize_backward(_lib.ptr(pre), pre.stride(0), _lib.ptr(dy), dy.stride(0),
-                                                           pre.shape[0], pre.shape[1], _lib.ptr(dy), dy.stride(0),
-                                                           _lib.current_stream()))
-        return dy
 
     def user_forward(self, users_d, seqs_d, lens_d):
         """User vectors [B, H] of the batch (training-mode BN) before any normalisation; returns (U, cache)."""
@@ -1629,21 +1618,6 @@ class RNN4RecTrainer(_Trainer):
         u = linear(h, p["dense_Wt"], p["dense_b"], ACT_NONE, impl="f32")
         c["h"] = h
         return u, c
-
-    def _normalize(self, x):
-        if not self.norm_embed:
-            return x, None
-        y = x.clone()
-        _lib.check(_lib.lib.b200_l2_normalize_rows(_lib.ptr(y), y.stride(0), y.shape[0], y.shape[1],
-                                                   _lib.current_stream()))
-        return y, x
-
-    def _normalize_backward(self, dy, pre):
-        if pre is not None:
-            _lib.check(_lib.lib.b200_l2_normalize_backward(_lib.ptr(pre), pre.stride(0), _lib.ptr(dy), dy.stride(0),
-                                                           pre.shape[0], pre.shape[1], _lib.ptr(dy), dy.stride(0),
-                                                           _lib.current_stream()))
-        return dy
 
     def _items(self, items_d):
         """(item rows [B, K] normalised with norm_embed, their pre-normalisation rows or None, biases [B])."""

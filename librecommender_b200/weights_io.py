@@ -129,13 +129,62 @@ def autoint_head_dims(att_embed_size):
 def autoint_scheme(version):
     """Which graph ``multi_head_attention`` (layers/attention.py:67-138) built: "keras" for TensorFlow >= 2.10
     (``tf.keras.layers.MultiHeadAttention``), "legacy" before.  Takes a scheme name or a TF version string."""
-    if version in AUTOINT_SCHEMES:
+    if version in _MHA_VARS:
         return version
     parts = [int(p) for p in str(version).split(".")[:2] if p.isdigit()]
     return "keras" if tuple(parts + [0, 0][len(parts):]) >= (2, 10) else "legacy"
 
 
-AUTOINT_SCHEMES = ("keras", "legacy")
+# ------------------------------------------------------------------------------------------------
+# One ``multi_head_attention`` layer (layers/attention.py:67-138), shared by AutoInt and Transformer.  X [rows, d_in],
+# width D = H * hd, no biases.  "keras" (TF >= 2.10, tf.keras.layers.MultiHeadAttention): query / key / value
+# [d_in, H, hd] and attention_output [H, hd, d_in].  "legacy": four tf_dense created as q, k, v, out: query / key
+# [d_in, D], value [D, D] and output [D, d_in]; ``values = tf_dense(D)(keys)`` acts on the PROJECTED keys
+# (attention.py:104-106), so V = (X Wk) Wv'.
+# ------------------------------------------------------------------------------------------------
+_MHA_VARS = {"keras": ("query", "key", "value", "attention_output"), "legacy": ("query", "key", "value", "output")}
+
+
+def _check_mha_scheme(scheme, who):
+    if scheme not in _MHA_VARS:
+        raise ValueError(f"{who}: unknown naming scheme `{scheme}`")
+
+
+def _mha_tf_names(scheme, prefix, layer, first_dense):
+    """TF variable names of attention layer `layer` (0-based) under the scope `prefix`: keras
+    ``{prefix}multi_head_attention[_layer]/{query,key,value,attention_output}/kernel:0``, legacy
+    ``{prefix}dense_{first_dense + j}/kernel:0`` for q, k, v, out."""
+    if scheme == "keras":
+        scope = f"{prefix}multi_head_attention{'' if layer == 0 else f'_{layer}'}"
+        return {k: f"{scope}/{k}/kernel:0" for k in _MHA_VARS[scheme]}
+    return {k: f"{prefix}{_dense_name(first_dense + j)}/kernel:0" for j, k in enumerate(_MHA_VARS[scheme])}
+
+
+def _mha_tf_shapes(scheme, d_in, D, H):
+    """Raw shapes of one layer's variables (any scheme other than "keras" reads as legacy)."""
+    if scheme == "keras":
+        hd = D // H
+        return dict(query=(d_in, H, hd), key=(d_in, H, hd), value=(d_in, H, hd), attention_output=(H, hd, d_in))
+    return dict(query=(d_in, D), key=(d_in, D), value=(D, D), output=(D, d_in))
+
+
+def _mha_2d(scheme, d_in, D):
+    """The 2-D shapes the trainers hold one layer's variables in, columns head-major: [d_in, D] projections ([D, D]
+    for the legacy value) and the [D, d_in] output.  Reshaping to :func:`_mha_tf_shapes` is the inverse."""
+    return dict(zip(_MHA_VARS[scheme], ((d_in, D), (d_in, D), (D, D) if scheme == "legacy" else (d_in, D), (D, d_in))))
+
+
+def _mha_engine(lw, scheme):
+    """One layer's raw variables -> the engines' {wq, wk, wv [d_in, D], wo [D, d_in]}: keras kernels flattened; legacy
+    the effective value map Wk Wv', multiplied in float64 and then cast."""
+    f32 = lambda a: np.asarray(a, dtype=np.float32)      # noqa: E731
+    if scheme == "keras":
+        d_in, D = np.shape(lw["query"])[0], int(np.prod(np.shape(lw["query"])[1:]))
+        return dict(wq=f32(lw["query"]).reshape(d_in, D), wk=f32(lw["key"]).reshape(d_in, D),
+                    wv=f32(lw["value"]).reshape(d_in, D), wo=f32(lw["attention_output"]).reshape(D, d_in))
+    wk = f32(lw["key"])
+    return dict(wq=f32(lw["query"]), wk=wk, wv=(wk.astype(np.float64) @ np.asarray(lw["value"], dtype=np.float64)
+                                                ).astype(np.float32), wo=f32(lw["output"]))
 
 
 def default_tf_names(model_name, n_hidden, use_bn, use_tf_attention=False, n_layers=None, scheme="keras",
@@ -172,21 +221,14 @@ def default_tf_names(model_name, n_hidden, use_bn, use_tf_attention=False, n_lay
     if model_name == "RNN4Rec":
         return _rnn4rec_names(scheme, rnn_type, n_layers, use_layer_norm)
     if model_name == "Transformer":
+        _check_mha_scheme(scheme, "Transformer")
         layers = []
         for i in range(n_layers):
             sc = f"transformer_layer{i + 1}"
-            if scheme == "keras":
-                mha = f"{sc}/multi_head_attention{'' if i == 0 else f'_{i}'}"
-                lw = {k: f"{mha}/{k}/kernel:0" for k in ("query", "key", "value", "attention_output")}
-                ffn = [2 * i, 2 * i + 1]
-            elif scheme == "legacy":
-                lw = {k: f"{sc}/{_dense_name(6 * i + j)}/kernel:0" for j, k in enumerate(("query", "key", "value",
-                                                                                          "output"))}
-                ffn = [6 * i + 4, 6 * i + 5]
-            else:
-                raise ValueError(f"unknown Transformer naming scheme `{scheme}`")
+            lw = _mha_tf_names(scheme, f"{sc}/", i, 6 * i)
+            ffn = 2 * i if scheme == "keras" else 6 * i + 4
             lw.update(rms_att=f"{sc}/rms_norm_att/scale:0", rms_ffn=f"{sc}/rms_norm_ffn/scale:0",
-                      ffn1=f"{sc}/{_dense_name(ffn[0])}/kernel:0", ffn2=f"{sc}/{_dense_name(ffn[1])}/kernel:0")
+                      ffn1=f"{sc}/{_dense_name(ffn)}/kernel:0", ffn2=f"{sc}/{_dense_name(ffn + 1)}/kernel:0")
             layers.append(lw)
         head = _dense_name((2 if scheme == "keras" else 6) * n_layers)
         out = {"tfm_layers": layers, "rms_last": "rms_norm_last/scale:0", "rms_item": "rms_norm_item/scale:0",
@@ -199,17 +241,10 @@ def default_tf_names(model_name, n_hidden, use_bn, use_tf_attention=False, n_lay
                     out[f"ln_{side}"] = {k: f"elementwise_{side}_feats/layer_norm/{k}:0" for k in ("scale", "bias")}
         return out
     if model_name == "AutoInt":
-        if scheme == "keras":
-            mha = [{k: f"multi_head_attention{'' if i == 0 else f'_{i}'}/{k}/kernel:0"
-                    for k in ("query", "key", "value", "attention_output")} for i in range(n_layers)]
-            head = _dense_name(0)
-        elif scheme == "legacy":
-            mha = [{k: f"{_dense_name(4 * i + j)}/kernel:0" for j, k in enumerate(("query", "key", "value", "output"))}
-                   for i in range(n_layers)]
-            head = _dense_name(4 * n_layers)
-        else:
-            raise ValueError(f"unknown AutoInt naming scheme `{scheme}`")
-        return {"autoint_mha": mha, "out_kernel": f"{head}/kernel:0", "out_bias": f"{head}/bias:0"}
+        _check_mha_scheme(scheme, "AutoInt")
+        head = _dense_name(0 if scheme == "keras" else 4 * n_layers)
+        return {"autoint_mha": [_mha_tf_names(scheme, "", i, 4 * i) for i in range(n_layers)],
+                "out_kernel": f"{head}/kernel:0", "out_bias": f"{head}/bias:0"}
     if model_name == "FM":
         out = {"lin_kernel": "dense/kernel:0", "lin_bias": "dense/bias:0",
                "pw_kernel": "dense_1/kernel:0", "pw_bias": "dense_1/bias:0"}
@@ -255,16 +290,26 @@ def resolve_tf_names(npz, names, shapes=None):
     return take(names, shapes)
 
 
+def _put_tf_names(out, names, values):
+    """The inverse of :func:`resolve_tf_names`: ``out[name] = values`` as float32 for every name of the (possibly
+    nested) table `names`, `values` nested the same way (dicts indexed by the table's keys)."""
+    if isinstance(names, dict):
+        for k in names:
+            _put_tf_names(out, names[k], values[k])
+    elif isinstance(names, list):
+        for n, v in zip(names, values):
+            _put_tf_names(out, n, v)
+    else:
+        out[names] = np.asarray(values, dtype=np.float32)
+    return out
+
+
 def autoint_tf_shapes(scheme, K, num_heads, head_dims):
     """Expected shapes for :func:`default_tf_names` ("AutoInt"): keras ``query/key/value [K, H, hd]``,
     ``attention_output [H, hd, K]``; legacy ``q, k [K, D]``, ``v [D, D]`` (applied to the projected keys),
     ``out [D, K]``; the head ``[F*K, 1]`` (F is not known here) and ``[1]``."""
-    H = num_heads
-    if scheme == "keras":
-        mha = [dict(query=(K, H, hd), key=(K, H, hd), value=(K, H, hd), attention_output=(H, hd, K)) for hd in head_dims]
-    else:
-        mha = [dict(query=(K, H * hd), key=(K, H * hd), value=(H * hd, H * hd), output=(H * hd, K)) for hd in head_dims]
-    return {"autoint_mha": mha, "out_kernel": (None, 1), "out_bias": (1,)}
+    return {"autoint_mha": [_mha_tf_shapes(scheme, K, num_heads * hd, num_heads) for hd in head_dims],
+            "out_kernel": (None, 1), "out_bias": (1,)}
 
 
 def autoint_layers(mha, scheme):
@@ -272,21 +317,8 @@ def autoint_layers(mha, scheme):
     columns head-major (h * hd + j, the order ``_split_heads`` reshapes into).  keras: the [K, H, hd] / [H, hd, K]
     kernels flattened.  legacy: ``values = tf_dense(D)(keys)`` acts on the PROJECTED keys (attention.py:104-106),
     so V = (X Wk) Wv' and the effective value map is Wk Wv', multiplied in float64 and then cast."""
-    out = []
-    for lw in mha:
-        if scheme == "keras":
-            K, H, hd = np.shape(lw["query"])
-            flat = lambda a: np.asarray(a, dtype=np.float32).reshape(K, H * hd)      # noqa: E731
-            out.append(dict(wq=flat(lw["query"]), wk=flat(lw["key"]), wv=flat(lw["value"]),
-                            wo=np.asarray(lw["attention_output"], dtype=np.float32).reshape(H * hd, K)))
-        elif scheme == "legacy":
-            wk = np.asarray(lw["key"], dtype=np.float32)
-            wv = (wk.astype(np.float64) @ np.asarray(lw["value"], dtype=np.float64)).astype(np.float32)
-            out.append(dict(wq=np.asarray(lw["query"], dtype=np.float32), wk=wk, wv=wv,
-                            wo=np.asarray(lw["output"], dtype=np.float32)))
-        else:
-            raise ValueError(f"unknown AutoInt naming scheme `{scheme}`")
-    return out
+    _check_mha_scheme(scheme, "AutoInt")
+    return [_mha_engine(lw, scheme) for lw in mha]
 
 
 def autoint_weights(raw):
@@ -305,12 +337,9 @@ def autoint_tf_variables(raw):
     ``training.AutoIntTrainer.export_weights()``) -> ``{TF variable name: array}`` named by
     :func:`default_tf_names` for the raw dict's scheme: what ``save_tf_variables`` writes as
     ``<name>_tf_variables.npz``, and the inverse of ``load_reference_tf_model(..., "AutoInt")``."""
-    mha = raw["autoint_mha"]
-    names = default_tf_names("AutoInt", None, False, n_layers=len(mha), scheme=raw["autoint_scheme"])
+    names = default_tf_names("AutoInt", None, False, n_layers=len(raw["autoint_mha"]), scheme=raw["autoint_scheme"])
     out = to_tf_variables({k: raw[k] for k in EMBEDDING_SCOPE if k in raw})
-    for lw, ln in zip(mha, names["autoint_mha"]):
-        for k, n in ln.items():
-            out[n] = np.asarray(lw[k], dtype=np.float32)
+    _put_tf_names(out, names["autoint_mha"], raw["autoint_mha"])
     out[names["out_kernel"]] = np.asarray(raw["out_kernel"], dtype=np.float32).reshape(-1, 1)
     out[names["out_bias"]] = np.asarray(raw["out_bias"], dtype=np.float32).reshape(1)
     return out
@@ -321,13 +350,8 @@ def transformer_tf_shapes(scheme, names, K, Kp, num_heads, T=None):
     ``query/key/value [D, H, hd]``, ``attention_output [H, hd, D]``; legacy ``q, k, v, out [D, D]`` (v applied to the
     projected keys); FFN ``[D, 4D]``, ``[4D, D]``; positions ``[T, K]``; the MLP's first kernel ``[F*K + D, H1]``
     (F is not known here)."""
-    D, H = Kp + K, num_heads
-    hd = D // H
-    if scheme == "keras":
-        att = dict(query=(D, H, hd), key=(D, H, hd), value=(D, H, hd), attention_output=(H, hd, D))
-    else:
-        att = dict(query=(D, D), key=(D, D), value=(D, D), output=(D, D))
-    layer = dict(att, rms_att=(D,), rms_ffn=(D,), ffn1=(D, 4 * D), ffn2=(4 * D, D))
+    D = Kp + K
+    layer = dict(_mha_tf_shapes(scheme, D, D, num_heads), rms_att=(D,), rms_ffn=(D,), ffn1=(D, 4 * D), ffn2=(4 * D, D))
     out = {"tfm_layers": [layer] * len(names["tfm_layers"]), "rms_last": (D,), "rms_item": (Kp,), "out_kernel": (None, 1),
            "out_bias": (1,), "mlp": None}
     if "positional_encoding" in names:
@@ -342,22 +366,10 @@ def transformer_layers(layers, scheme):
     """Per-layer variables of either graph -> the engine's ``tfm_layers`` [{rms_att, wq, wk, wv, wo [D, D], rms_ffn,
     w1 [D, 4D], w2 [4D, D]}], columns head-major.  legacy: the value Dense acts on the PROJECTED keys
     (attention.py:104-106), so the effective value map Wk Wv' is multiplied in float64 and then cast."""
-    out = []
-    for lw in layers:
-        f32 = lambda a: np.asarray(a, dtype=np.float32)      # noqa: E731
-        if scheme == "keras":
-            D = np.shape(lw["query"])[0]
-            att = dict(wq=f32(lw["query"]).reshape(D, D), wk=f32(lw["key"]).reshape(D, D),
-                       wv=f32(lw["value"]).reshape(D, D), wo=f32(lw["attention_output"]).reshape(D, D))
-        elif scheme == "legacy":
-            wk = f32(lw["key"])
-            att = dict(wq=f32(lw["query"]), wk=wk, wo=f32(lw["output"]),
-                       wv=(wk.astype(np.float64) @ np.asarray(lw["value"], dtype=np.float64)).astype(np.float32))
-        else:
-            raise ValueError(f"unknown Transformer naming scheme `{scheme}`")
-        out.append(dict(att, rms_att=f32(lw["rms_att"]).reshape(-1), rms_ffn=f32(lw["rms_ffn"]).reshape(-1),
-                        w1=f32(lw["ffn1"]), w2=f32(lw["ffn2"])))
-    return out
+    _check_mha_scheme(scheme, "Transformer")
+    f32 = lambda a: np.asarray(a, dtype=np.float32)      # noqa: E731
+    return [dict(_mha_engine(lw, scheme), rms_att=f32(lw["rms_att"]).reshape(-1), rms_ffn=f32(lw["rms_ffn"]).reshape(-1),
+                 w1=f32(lw["ffn1"]), w2=f32(lw["ffn2"])) for lw in layers]
 
 
 def transformer_weights(raw):
@@ -384,18 +396,7 @@ def transformer_tf_variables(raw):
                              feat_agg_mode=raw.get("feat_agg_mode", "concat"), item_sparse="ln_sparse" in raw,
                              item_dense="ln_dense" in raw)
     out = to_tf_variables({k: raw[k] for k in EMBEDDING_SCOPE if k in raw})
-
-    def put(n, a):
-        if isinstance(n, dict):
-            for k in n:
-                put(n[k], a[k])
-        elif isinstance(n, list):
-            for ni, ai in zip(n, a):
-                put(ni, ai)
-        else:
-            out[n] = np.asarray(a, dtype=np.float32)
-    put({k: v for k, v in names.items() if k not in ("out_kernel", "out_bias")},
-        {k: raw[k] for k in names if k not in ("out_kernel", "out_bias")})
+    _put_tf_names(out, {k: v for k, v in names.items() if k not in ("out_kernel", "out_bias")}, raw)
     out[names["out_kernel"]] = np.asarray(raw["out_kernel"], dtype=np.float32).reshape(-1, 1)
     out[names["out_bias"]] = np.asarray(raw["out_bias"], dtype=np.float32).reshape(1)
     return out
@@ -418,19 +419,7 @@ def youtube_retrieval_tf_variables(w):
            if w.get(k) is not None}
     out[YOUTUBE_RETRIEVAL_TABLES["item_biases"]] = out[YOUTUBE_RETRIEVAL_TABLES["item_biases"]].reshape(-1)
     mlp = w["mlp"]
-    names = _mlp_names("mlp", len(mlp["kernels"]), mlp.get("bn_in") is not None)
-
-    def put(n, a):
-        if isinstance(n, dict):
-            for k in n:
-                put(n[k], a[k])
-        elif isinstance(n, list):
-            for ni, ai in zip(n, a):
-                put(ni, ai)
-        else:
-            out[n] = np.asarray(a, dtype=np.float32)
-    put(names, {k: mlp[k] for k in names})
-    return out
+    return _put_tf_names(out, _mlp_names("mlp", len(mlp["kernels"]), mlp.get("bn_in") is not None), mlp)
 
 
 def _youtube_retrieval_weights(npz, n_hidden, use_bn, extra_names=None):
@@ -619,9 +608,7 @@ def rnn4rec_tf_variables(raw):
                              rnn_type=raw["rnn_type"], use_layer_norm=bool(raw.get("use_layer_norm", False)))
     out = {name: np.asarray(raw[k], dtype=np.float32) for k, name in RNN4REC_TABLES.items()}
     out[RNN4REC_TABLES["item_biases"]] = out[RNN4REC_TABLES["item_biases"]].reshape(-1)
-    for lw, ln in zip(raw["rnn_layers"], names["rnn_layers"]):
-        for k, n in ln.items():
-            out[n] = np.asarray(lw[k], dtype=np.float32)
+    _put_tf_names(out, names["rnn_layers"], raw["rnn_layers"])
     out[names["dense_kernel"]] = np.asarray(raw["dense_kernel"], dtype=np.float32)
     out[names["dense_bias"]] = np.asarray(raw["dense_bias"], dtype=np.float32).reshape(-1)
     return out
