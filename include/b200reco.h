@@ -82,10 +82,14 @@ int b200_score_rows_f32(const float* U, int64_t ldu, const int64_t* user_ids, in
  * speculative pre-pass (sweep<PRE> + guess_kernel) is used, out[1] item splits, out[2] item tiles
  * per split, out[3] user tiles, out[4] sampled tiles per split, out[5] TMA stages, out[6] = 10 x CTAs
  * per cluster (2: every item tile is fetched from L2 once per pair of user tiles and TMA-multicast to
- * both CTAs) + MMA groups per item tile, out[7] records per candidate list (n_out >= 8).
+ * both CTAs) + MMA organisation actually used (1, 2 or 3 as in the tune code; 3 runs as 1 when
+ * d > 128), out[7] records per candidate list (n_out >= 8).  Without a device the plan is the one
+ * of a 132-SM H100.
  * b200_recommend_embed_tune (process-wide, not thread-safe; 0 keeps a value): organisation code =
- * 100 x cluster size (1|2) + 10 x MMA groups per tile (1|2) + epilogue variant (3: divergent per-lane
- * group tests, 5: one warp vote per 64-column step + quad-mask record stores; default 215), and the rank
+ * 100 x cluster size (1|2) + 10 x MMA organisation (1: one N=256 group per item tile; 2: two N=128
+ * groups; 3: two N=128 groups pipelined across item tiles, each half-tile epilogue running under the
+ * MMAs of the other half; d > 128 falls back to 1) + epilogue variant (3: divergent per-lane group
+ * tests, 5: one warp vote per 64-column step + quad-mask record stores; default 215), and the rank
  * coefficient c of the speculative threshold (about c * k_row items are expected above it). */
 int b200_recommend_embed_tune(int32_t organisation_code, float pre_rank_coef);
 /* profiling diagnostics only (results are wrong while level > 0): ablate parts of the main pass

@@ -110,6 +110,20 @@ __device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta_
 __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t count) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
 }
+// named barrier ID over COUNT threads that also ORs `pred` over them: true on every thread if any had it
+template <int ID, int COUNT>
+__device__ __forceinline__ bool named_bar_any(bool pred) {
+  uint32_t r;
+  asm volatile(
+      "{\n\t.reg .pred p, q;\n\t"
+      "setp.ne.u32 p, %1, 0;\n\t"
+      "bar.red.or.pred q, %2, %3, p;\n\t"
+      "selp.u32 %0, 1, 0, q;\n\t}"
+      : "=r"(r)
+      : "r"((uint32_t)pred), "n"(ID), "n"(COUNT)
+      : "memory");
+  return r != 0;
+}
 
 // ---------------------------------------------------------------- wgmma
 // move registers between warpgroups (every thread of the warpgroup executes it)

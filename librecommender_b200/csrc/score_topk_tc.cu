@@ -336,8 +336,10 @@ __device__ __noinline__ int compact_row(float* __restrict__ ls, int n,
 // ADJACENT user tiles of the SAME item split in lock step: every item tile is fetched from L2 once
 // per cluster — each CTA loads half of it and the TMA multicasts that half into both CTAs' shared
 // memory — which halves the L2 -> SM traffic of the item table (the pass is L2-bandwidth bound
-// otherwise).  NH = MMA groups per item tile (1: one N=256 wgmma chain; 2: two N=128 chains into
-// separate accumulators, the epilogue of the first runs while the tensor core computes the second).
+// otherwise).  NH = MMA organisation of an item tile (1: one N=256 wgmma chain; 2: two N=128 chains into
+// separate accumulators, the epilogue of the first runs while the tensor core computes the second;
+// 3: the same two N=128 groups pipelined across item tiles, so every half-tile epilogue of the main
+// pass runs while the tensor core computes the other half, see the main pass).
 // EPI = record stores of a hot 64-column step: 3 divergent per-group branches (the quad maximum by
 // shuffles), 5 quad masks (one bit per (group, row) slot, one warp-uniform branch per slot).
 //
@@ -445,7 +447,10 @@ sweep_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
   } else {
     ptx::setmaxnreg_inc<SWEEP_CONSUMER_REGS>();
     // ===================== MMA + epilogue: 2 warpgroups x 64 user rows ==========
-    constexpr int NC = TN / NH;             // accumulator columns per MMA group
+    constexpr bool PIPE = NH == 3;          // two N=128 groups pipelined across item tiles (main pass only)
+    static_assert(!(PRE && PIPE), "the pre-pass runs the unpipelined two-group organisation");
+    constexpr int NG = NH == 1 ? 1 : 2;     // MMA groups (accumulators) per item tile
+    constexpr int NC = TN / NG;             // accumulator columns per MMA group
     const int g = warp >> 2;
     const int quad = lane >> 2, tq = lane & 3;
     const int my_rs = tq >> 1, my_j = tq & 1;          // the (row, list) pair this lane reports
@@ -454,7 +459,7 @@ sweep_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
     const float ninf = __int_as_float(0xff800000);
     const uint32_t a_addr = ptx::smem_u32(smemA) + (uint32_t)(g * 64 * KBLK * 2);
     const uint32_t b_addr = ptx::smem_u32(smemB);
-    float acc[NH][NC / 2];
+    float acc[NG][NC / 2];
     int stage = 0;
     uint32_t phase = 0;
 
@@ -472,19 +477,19 @@ sweep_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
     // the four k16 MMAs of one 64-wide k-block; the first k-block of a tile starts the accumulator
     auto mma_kblock = [&](float (&d)[NC / 2], uint64_t da, uint64_t db, bool first) {
       if (first) {
-        if (NH == 1) ptx::wgmma_f16_n256_first(*reinterpret_cast<float(*)[128]>(&d[0]), da, db);
+        if (NG == 1) ptx::wgmma_f16_n256_first(*reinterpret_cast<float(*)[128]>(&d[0]), da, db);
         else ptx::wgmma_f16_n128_first(*reinterpret_cast<float(*)[64]>(&d[0]), da, db);
       }
 #pragma unroll
       for (int k4 = first ? 1 : 0; k4 < KBLK / 16; ++k4) {
         // advance 16 fp16 = 32 bytes inside the 128-byte swizzled row: +2 in the >>4 field
-        if (NH == 1) ptx::wgmma_f16_n256(*reinterpret_cast<float(*)[128]>(&d[0]), da + 2 * k4, db + 2 * k4);
+        if (NG == 1) ptx::wgmma_f16_n256(*reinterpret_cast<float(*)[128]>(&d[0]), da + 2 * k4, db + 2 * k4);
         else ptx::wgmma_f16_n128(*reinterpret_cast<float(*)[64]>(&d[0]), da + 2 * k4, db + 2 * k4);
       }
     };
-    // MMAs of column group hh of the item tile in the current (whole-tile) stage
-    auto issue_group = [&](float (&d)[NC / 2], int hh) {
-      const uint32_t b_hh = b_addr + (uint32_t)(stage * p.KB * B_KB_BYTES + hh * NC * KBLK * 2);
+    // MMAs of column group hh of the item tile in (whole-tile) stage st, as one commit group
+    auto issue_group = [&](float (&d)[NC / 2], int hh, int st) {
+      const uint32_t b_hh = b_addr + (uint32_t)(st * p.KB * B_KB_BYTES + hh * NC * KBLK * 2);
       mma_kblock(d, ptx::wgmma_desc_sw128_kmajor(a_addr), ptx::wgmma_desc_sw128_kmajor(b_hh), true);
 #pragma unroll 1
       for (int kb = 1; kb < p.KB; ++kb)
@@ -515,13 +520,13 @@ sweep_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
       ptx::mbar_wait_hint(&ss->full[stage], phase, p.hint_ns);
       ptx::wgmma_fence();
 #pragma unroll
-      for (int hh = 0; hh < NH; ++hh) issue_group(acc[hh], hh);
-      if (NH == 2) {
+      for (int hh = 0; hh < NG; ++hh) issue_group(acc[hh], hh, stage);
+      if (NG == 2) {
         ptx::wgmma_wait<1>(acc[0]);
         epi(acc[0], std::integral_constant<int, 0>{});
-        ptx::wgmma_wait<0>(acc[NH - 1]);
+        ptx::wgmma_wait<0>(acc[NG - 1]);
         release();
-        epi(acc[NH - 1], std::integral_constant<int, NC>{});
+        epi(acc[NG - 1], std::integral_constant<int, NC>{});
       } else {
         ptx::wgmma_wait<0>(acc[0]);
         release();
@@ -573,10 +578,13 @@ sweep_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
         // ---- main pass ----
         float tau[2];
         int n_counted[2][2] = {{0, 0}, {0, 0}};
-        // lp: first record of the (row, list); rp: where its next record goes (records = (rp - lp) / REC)
-        float* lp[2][2];
+        // lp(rs, j): first record of the (row, list), computed rather than held (registers are scarce);
+        // rp: where its next record goes (records = (rp - lp) / REC)
         float* rp[2][2];
         const int64_t cap_words = (int64_t)p.capg * REC;
+        auto lp = [&](int rs, int j) {
+          return p.cand_r + ((int64_t)(list_base + j) * p.B_pad + grow0 + 8 * rs) * cap_words;
+        };
 #pragma unroll
         for (int rs = 0; rs < 2; ++rs) {
           const int grow = grow0 + 8 * rs;
@@ -587,15 +595,15 @@ sweep_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
           }
           if (p.ablate >= 1) tau[rs] = pinf;   // diagnostics: nothing is ever collected (cold path only)
 #pragma unroll
-          for (int j = 0; j < 2; ++j) rp[rs][j] = lp[rs][j] = p.cand_r + ((int64_t)(list_base + j) * p.B_pad + grow) * cap_words;
+          for (int j = 0; j < 2; ++j) rp[rs][j] = lp(rs, j);
         }
-        auto records = [&](int rs, int j) { return (int)(sel22(rp, rs, j) - sel22(lp, rs, j)) / REC; };
+        auto records = [&](int rs, int j) { return (int)(sel22(rp, rs, j) - lp(rs, j)) / REC; };
 
         // Zero-padded item rows of the last tile (ids >= N, coarse score exactly 0) may be collected when
         // tau <= 0; compact_row and finalize_kernel ignore ids >= N, so the sweep needs no tail code.
-        for (int t = t0; t < t1; ++t) {
-          bool hot = false;   // warp-uniform: some step of the tile stored records
-          tile_mma([&](auto& d, auto c0) {
+        bool hot = false;   // warp-uniform: some step of the current tile stored records
+        // epilogue of the MMA group at column offset c0 of item tile t: records of its hot groups
+        auto epilogue = [&](auto& d, auto c0, int t) {
             constexpr int COL0 = decltype(c0)::value;
             if (p.ablate >= 2) return;   // diagnostics: MMAs and stage releases only
 #pragma unroll
@@ -627,8 +635,13 @@ sweep_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
                 mask |= __shfl_xor_sync(0xffffffffu, mask, 1);
                 mask |= __shfl_xor_sync(0xffffffffu, mask, 2);
                 const uint32_t any = __reduce_or_sync(0xffffffffu, mask);
+                // two-level slot tests: a hot step usually holds one or two slots, so test the four
+                // slots of a group pair only when the pair has one (4 + 4 uniform tests instead of 16)
 #pragma unroll
-                for (int jl = 0; jl < 8; ++jl) {
+                for (int jp = 0; jp < 4; ++jp) {
+                  if (!(any & (0xfu << (4 * jp)))) continue;   // warp-uniform: no slot in groups 2 jp, 2 jp + 1
+#pragma unroll
+                for (int jl = 2 * jp; jl < 2 * jp + 2; ++jl) {
                   const int jj = 8 * s + jl;
                   const int col = COL0 + 8 * jj;
 #pragma unroll
@@ -650,6 +663,7 @@ sweep_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
                     r += (mask & bit) ? REC : 0;
                   }
                 }
+                }
               } else {
 #pragma unroll
                 for (int jl = 0; jl < 8; ++jl) {
@@ -670,11 +684,17 @@ sweep_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
                 }
               }
             }
-          });
-          // one overflow / compaction check per TILE (a tile adds at most 16 records to a list)
-          if (!hot) continue;
+        };
+        // the lane's (row, list) is due for a compaction once it holds `extra` more records
+        auto compaction_due = [&](int extra) {
+          const int mc = records(my_rs, my_j) + extra, mn = sel22(n_counted, my_rs, my_j);
+          return (mc - mn > p.trig) || (mc > p.capg - 24);
+        };
+        // one overflow / compaction check per TILE, after all of the tile's records
+        auto check = [&]() {
+          if (!hot) return;
           const int mc = records(my_rs, my_j), mn = sel22(n_counted, my_rs, my_j);
-          uint32_t need = __ballot_sync(0xffffffffu, (mc - mn > p.trig) || (mc > p.capg - 24));
+          uint32_t need = __ballot_sync(0xffffffffu, compaction_due(0));
           while (need) {
             const int src = __ffs(need) - 1;
             need &= need - 1;
@@ -682,25 +702,93 @@ sweep_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
             const int s_cntd = __shfl_sync(0xffffffffu, mn, src);
             const float s_tau = __shfl_sync(0xffffffffu, my_rs ? tau[1] : tau[0], src);
             const int sq = src >> 2, srs = (src >> 1) & 1, sj = src & 1;
-            const int sgrow = m * TM + 64 * g + 16 * (warp & 3) + sq + 8 * srs;
+            const int sgrow = grow0 - quad + sq + 8 * srs;
             const RowMeta sm = p.meta[sgrow];
             float new_tau;
             const int w = compact_row(p.cand_r + ((int64_t)(list_base + sj) * p.B_pad + sgrow) * cap_words, s_cnt, s_cntd,
                                       sm.k_row, sm.eps2, sm.R, s_tau, p.ghist + (int64_t)sgrow * NB, lane, (int32_t)p.N,
                                       &new_tau);
             if (quad == sq) {
-              set22(rp, srs, sj, sel22(lp, srs, sj) + (size_t)w * REC);
+              set22(rp, srs, sj, lp(srs, sj) + (size_t)w * REC);
               set22(n_counted, srs, sj, w);
               // also pick up what other lists of this row published meanwhile
               float nt = fmaxf(new_tau, key_to_float(max(__ldcg(p.row_tau_key + sgrow), 1u)));
               if (lane == src) atomicMax(p.row_tau_key + sgrow, float_to_key(new_tau));
               if (w > p.capg - 32) {  // too many near-ties to bound: hand the row to the exact path
                 nt = pinf;
-                set22(rp, srs, sj, sel22(lp, srs, sj));
+                set22(rp, srs, sj, lp(srs, sj));
                 set22(n_counted, srs, sj, 0);
                 if (lane == src) p.row_status[sgrow] = 1;
               }
               if (srs) tau[1] = nt; else tau[0] = nt;
+            }
+          }
+        };
+
+        if constexpr (!PIPE) {
+          for (int t = t0; t < t1; ++t) {
+            hot = false;
+            tile_mma([&](auto& d, auto c0) { epilogue(d, c0, t); });
+            check();
+          }
+        } else {
+          // Two N=128 groups per tile (G0 / G1 = columns [0, 128) / [128, 256); group h feeds list h only,
+          // so every list still receives its records in column order), pipelined across the unit's tiles.
+          // Steady state of tile t:
+          //   wait full(t+1); issue G0(t+1) | wait<1>: G1(t) done, release stage(t) | epilogue G1(t)
+          //   issue G1(t+1) | wait<1>: G0(t+1) done | epilogue G0(t+1)
+          // so each half-tile epilogue runs while the tensor core computes the other half.
+          //  - Every group is its own commit group and its first MMA writes the accumulator, so wait<1>
+          //    means "all but the newest group are complete".
+          //  - Two ring stages are held at once: stage(t) until G1(t) completes, then stage(t+1).
+          //    release() hands stage(t) back exactly once per warp, to every CTA of the cluster, right after
+          //    G1(t) completes (nstage >= 2 whenever a stage holds a whole tile, d_pad <= 128).
+          //  - compact_row is __noinline__ and register-hungry: no wgmma may be in flight and no accumulator
+          //    live across it (ptxas would serialise every wgmma of the kernel, or spill).  So before G0(t+1)
+          //    is issued the warpgroup decides from the worst case whether the check of tile t can compact:
+          //    list 0 has all of tile t's records, list 1 gets at most TN / 2 / GW = 16 more.  If it can
+          //    (rare), the pipeline drains (wait<0>, epilogue G1(t), check) and restarts at t+1; otherwise
+          //    the check provably finds nothing to do and is skipped.  Either way it sits where the
+          //    unpipelined organisations have it, after all of tile t's records and before any of t+1's, so
+          //    lists and thresholds evolve exactly as there.  The vote is warpgroup-wide (named barrier 1 + g)
+          //    because wgmma issue and wait are warpgroup-collective.
+          //  - The user tile changes at unit boundaries: the last tile of a unit always drains, so nothing
+          //    is issued into the next unit and every MMA of the unit is complete before a_empty.
+          constexpr int MAX_TILE_RECORDS = TN / 2 / GW;   // records one tile adds to one (row, list)
+          // (every split has at least one tile)
+          ptx::mbar_wait_hint(&ss->full[stage], phase, p.hint_ns);
+          ptx::wgmma_fence();
+          issue_group(acc[0], 0, stage);
+          // the loop leaves only through the drain branch (after wait<0>): ptxas then sees that no group is
+          // pending at the end of the unit (otherwise it serialises every wgmma of the kernel, C7514)
+          for (int t = t0;; ++t) {
+            // here G0(t) is issued into `stage`, no other group is pending
+            ptx::wgmma_fence();
+            issue_group(acc[1], 1, stage);
+            ptx::wgmma_wait<1>(acc[0]);
+            hot = false;
+            epilogue(acc[0], std::integral_constant<int, 0>{}, t);
+            const bool due = compaction_due(my_j ? MAX_TILE_RECORDS : 0);
+            const bool drain = t + 1 == t1 ||
+                __any_sync(0xffffffffu, g ? ptx::named_bar_any<2, 128>(due) : ptx::named_bar_any<1, 128>(due));
+            if (!drain) {
+              const int nst = stage + 1 == p.nstage ? 0 : stage + 1;
+              ptx::mbar_wait_hint(&ss->full[nst], nst ? phase : phase ^ 1, p.hint_ns);
+              ptx::wgmma_fence();
+              issue_group(acc[0], 0, nst);
+              ptx::wgmma_wait<1>(acc[1]);
+              release();
+              epilogue(acc[1], std::integral_constant<int, NC>{}, t);
+            } else {
+              ptx::wgmma_wait<0>(acc[1]);
+              release();
+              epilogue(acc[1], std::integral_constant<int, NC>{}, t);
+              check();
+              if (t + 1 == t1) break;
+              // restart the pipeline at t + 1
+              ptx::mbar_wait_hint(&ss->full[stage], phase, p.hint_ns);
+              ptx::wgmma_fence();
+              issue_group(acc[0], 0, stage);
             }
           }
         }
@@ -1175,7 +1263,8 @@ static inline size_t al256(size_t x) { return (x + 255) & ~(size_t)255; }
 // ---- tuning knobs (defaults compiled in; b200_recommend_embed_tune overrides them per process) ----
 static int g_epi = 5;              // record stores of a hot epilogue step: 5 quad masks (measured best on H100), 3 divergent group tests
 static int g_cluster = 2;          // 2 = pairs of user tiles share every item tile through TMA multicast, 1 = off
-static int g_nh = 1;               // MMA groups per item tile (1 x N=256; 2 x N=128, epilogue of the first overlaps the second)
+static int g_nh = 1;               // MMA organisation of an item tile (1 x N=256, measured best on H100; 2 x N=128, epilogue of
+                                   // the first overlaps the second; 3 = 2 x N=128 pipelined across tiles)
 static int g_ablate = 0;           // b200_recommend_embed_debug
 static int g_hint_ns = 20000;      // suspend-time hint of the mbarrier waits in the sweep kernels
 static int g_pre_margin = 12;      // additive part of the speculative rank: pre_k = margin + coef * f * k_row sampled block maxima
@@ -1200,7 +1289,11 @@ static int make_plan(int64_t B, int64_t N, int d, Plan* pl) {
                MAX_KB * KBLK, d);
   // clusters of 2 CTAs take two adjacent user tiles: worth it from two user tiles on (B > 128)
   pl->CL = (g_cluster == 2 && B > TM) ? 2 : 1;
-  pl->NH = g_nh;
+  // d_pad <= 128: a ring stage = one whole 256-item tile (KB k-blocks); wider embeddings: one k-block per stage
+  // (a whole tile of d_pad = 256 is 128 KB: two of them do not fit beside the 64 KB user tile)
+  pl->kb_stages = pl->KB > 2;
+  // the pipelined organisation holds two whole-tile stages at once: k-block stages run one N=256 group
+  pl->NH = (g_nh == 3 && pl->kb_stages) ? 1 : g_nh;
   pl->B_pad = pad_to(B, TM * pl->CL);
   pl->N_pad = (N + TN - 1) / TN * TN;
   pl->m_tiles = pl->B_pad / TM;
@@ -1210,8 +1303,8 @@ static int make_plan(int64_t B, int64_t N, int d, Plan* pl) {
   const int ovh = 12;
   long best = -1;
   int bestS = 1;
-  const int sms = num_sms();
-  B200_REQUIRE(sms > 0, "no CUDA device");
+  // without a device (plan and workspace queries only) the plan is the one of a 132-SM H100 SXM
+  const int sms = num_sms() > 0 ? num_sms() : 132;
   const int maxS = pl->total_tiles < 2 * sms ? pl->total_tiles : 2 * sms;
   for (int S = 1; S <= maxS; ++S) {
     const long units = (long)pl->m_tiles * S;
@@ -1241,9 +1334,6 @@ static int make_plan(int64_t B, int64_t N, int d, Plan* pl) {
   pl->capg = (pl->use_pre && pl->n_lists >= 16) ? 128 : CAPG_MAX;
   pl->trig = pl->use_pre ? pl->capg : 96;
   const size_t budget = 227 * 1024 - 1024 /*align*/ - sizeof(SweepSmem) - (size_t)pl->KB * A_KB_BYTES;
-  // d_pad <= 128: a ring stage = one whole 256-item tile (KB k-blocks); wider embeddings: one k-block per stage
-  // (a whole tile of d_pad = 256 is 128 KB: two of them do not fit beside the 64 KB user tile)
-  pl->kb_stages = pl->KB > 2;
   B200_REQUIRE(!pl->kb_stages || pl->NH == 1, "the two-MMA-group organisation supports embed width <= 128 only");
   const size_t stage_bytes = pl->kb_stages ? (size_t)B_KB_BYTES : (size_t)pl->KB * B_KB_BYTES;
   int ns = (int)(budget / stage_bytes);
@@ -1290,10 +1380,11 @@ static int launch_sweep(int grid, const Plan& pl, cudaStream_t stream, const CUt
   return 0;
 }
 
-// organisation = (record stores EPI, cluster size CL, MMA groups NH); the default is (5, 2, 1)
+// organisation = (record stores EPI, cluster size CL, MMA organisation NH); the default is (5, 2, 1)
 static int launch_pre_dispatch(int grid, const Plan& pl, cudaStream_t stream, const CUtensorMap& tmA,
                                const CUtensorMap& tmB, const CUtensorMap& tmBh, const SweepParams& sp) {
-  // the pre-pass stores no records: one epilogue
+  // the pre-pass stores no records: one epilogue; the pipelined organisation (NH = 3) runs its pre-pass on
+  // the unpipelined two-group kernel
   if (pl.CL == 2) {
     if (pl.NH == 1) return launch_sweep<true, 3, 2, 1>(grid, pl, stream, tmA, tmB, tmBh, sp);
     return launch_sweep<true, 3, 2, 2>(grid, pl, stream, tmA, tmB, tmBh, sp);
@@ -1306,11 +1397,13 @@ static int launch_main_dispatch(int grid, const Plan& pl, int epi, cudaStream_t 
                                 const CUtensorMap& tmB, const CUtensorMap& tmBh, const SweepParams& sp) {
 #define B200_SWEEP(E_, C_, N_) return launch_sweep<false, E_, C_, N_>(grid, pl, stream, tmA, tmB, tmBh, sp)
   if (epi == 5) {
-    if (pl.CL == 2) { if (pl.NH == 2) B200_SWEEP(5, 2, 2); B200_SWEEP(5, 2, 1); }
+    if (pl.CL == 2) { if (pl.NH == 3) B200_SWEEP(5, 2, 3); if (pl.NH == 2) B200_SWEEP(5, 2, 2); B200_SWEEP(5, 2, 1); }
+    if (pl.NH == 3) B200_SWEEP(5, 1, 3);
     if (pl.NH == 2) B200_SWEEP(5, 1, 2);
     B200_SWEEP(5, 1, 1);
   }
-  if (pl.CL == 2) { if (pl.NH == 2) B200_SWEEP(3, 2, 2); B200_SWEEP(3, 2, 1); }
+  if (pl.CL == 2) { if (pl.NH == 3) B200_SWEEP(3, 2, 3); if (pl.NH == 2) B200_SWEEP(3, 2, 2); B200_SWEEP(3, 2, 1); }
+  if (pl.NH == 3) B200_SWEEP(3, 1, 3);
   if (pl.NH == 2) B200_SWEEP(3, 1, 2);
   B200_SWEEP(3, 1, 1);
 #undef B200_SWEEP
@@ -1356,11 +1449,12 @@ extern "C" int b200_embed_catalog_prepare(const float* I, int64_t ldi, int64_t N
 }
 
 extern "C" int b200_recommend_embed_tune(int32_t epilogue_warps_per_quadrant, float pre_rank_coef) {
-  if (epilogue_warps_per_quadrant != 0) {   // organisation code: 100 * cluster size + 10 * MMA groups per tile + epilogue variant
+  if (epilogue_warps_per_quadrant != 0) {   // organisation code: 100 * cluster size + 10 * MMA organisation + epilogue variant
     const int code = epilogue_warps_per_quadrant % 1000;
     const int cl = (code / 100) % 10, nh = (code / 10) % 10, epi = code % 10;
-    B200_REQUIRE((cl == 1 || cl == 2) && (nh == 1 || nh == 2) && (epi == 3 || epi == 5),
-                 "b200_recommend_embed_tune: code = 100 * cluster (1|2) + 10 * MMA groups (1|2) + record stores (3|5)");
+    B200_REQUIRE((cl == 1 || cl == 2) && (nh >= 1 && nh <= 3) && (epi == 3 || epi == 5),
+                 "b200_recommend_embed_tune: code = 100 * cluster (1|2) + 10 * MMA groups (1|2, 3 = 2 pipelined) "
+                 "+ record stores (3|5)");
     g_cluster = cl; g_nh = nh; g_epi = epi;
   }
   if (pre_rank_coef != 0.f) {

@@ -27,7 +27,9 @@ def main():
     import librecommender_b200.engine as eng
 
     sc = EmbedScorer(U, I, args.items, ConsumedCSR.from_device_tensors(indptr, idx), n_users=args.users, device=dev)
-    variants = [(w, 2.0, b) for b in (8192, 16384) for w in (215, 115, 213, 225)]
+    # organisation code : rank coefficient : users per launch : ablate level (1: cold epilogue steps only,
+    # 2: no epilogue) -- the per-phase breakdown of the default and the two-group organisations
+    variants = [(w, 2.0, 32768, a) for w in (215, 225, 235) for a in (0, 1, 2)]
     if os.environ.get("VARIANTS"):
         variants = [tuple(float(x) if "." in x else int(x) for x in v.split(":")) for v in os.environ["VARIANTS"].split(",")]
     rng = np.random.default_rng(5)
