@@ -683,6 +683,34 @@ int b200_rnn_backward(const int64_t* users, int64_t n, const int32_t* lens, int3
                       int64_t lddo, const float* dy, const float* const* saved, float* dgx, float* dgh, float* dln,
                       float* dlnx, void* stream);
 
+/* ---- Caser / WaveNet inference (libreco/algorithms/caser.py:177-221, wave_net.py:181-222) ----------------------
+ * Slot s reads the sequence seqs[users[s], :T] (row-major, ld_seq; pad positions are ordinary rows: neither model
+ * masks by length) and x = X[seq] [T, K] (X = seq_embeds [*, ldx]).  Every pre-activation below is ONE fmaf chain
+ * that starts at the bias and runs over the terms in the order written; max and ReLU are order-free.  A slot's
+ * result depends only on its own sequence: the same bits whatever the other slots, n or the call.
+ * b200_caser_encode writes out[s, :T*nh + K*nv] (ldo), the concat the Dense head reads:
+ *   column (h-1)*nh + f, h = 1..T:  max_{p <= T-h} relu(b_h[f] + sum_{j<h} sum_{k<K} x[p+j, k] W_h[j, k, f]),
+ *                                    j ascending, then k ascending (Conv1D(nh, h, valid, relu) + MaxPool1D);
+ *   column T*nh + k*nv + f:          relu(bv[f] + sum_{t<T} x[t, k] Wv[t, f]), t ascending (Conv1D(nv, 1) over x^T).
+ * weights packs W_1 .. W_T ([h, K, nh] each, Keras layout) back to back, then b_h [T, nh], Wv [T, nv], bv [nv]
+ * (b200_caser_weight_floats floats).
+ * b200_wavenet_encode runs n_conv causal layers Conv1D(F, 2, causal, dilation d_l = dilations[l], relu) (C_in = K
+ * for the first layer, F after):  y[t, f] = relu(b[f] + sum_c x[t-d, c] W[0, c, f] + sum_c x[t, c] W[1, c, f]),
+ * the first sum (c ascending, absent while t < d) before the second (c ascending); then the 1x1 layer
+ * z[t, f] = relu(b1[f] + sum_c y[t, c] W1[c, f]) (c ascending), and writes out[s, f] = max_t z[t, f] (ldo).
+ * weights packs per causal layer W [2, C_in, F], b [F], then W1 [F, F], b1 [F] (b200_wavenet_weight_floats
+ * floats).  dilations is a HOST array of n_conv entries.
+ * Supported: 1 <= T <= 64, 1 <= K <= 128, 1 <= nh, nv <= 32, 1 <= F <= 128, 1 <= n_conv <= 16, dilations >= 1;
+ * anything else returns -2 before launching (the weight-float helpers too); n = 0 launches nothing. */
+int64_t b200_caser_weight_floats(int32_t T, int32_t K, int32_t nh, int32_t nv);
+int64_t b200_wavenet_weight_floats(int32_t K, int32_t F, int32_t n_conv);
+int b200_caser_encode(const int64_t* users, int64_t n, const int32_t* seqs, int64_t ld_seq, int32_t T, const float* X,
+                      int64_t ldx, int32_t K, int32_t nh, int32_t nv, const float* weights, float* out, int64_t ldo,
+                      void* stream);
+int b200_wavenet_encode(const int64_t* users, int64_t n, const int32_t* seqs, int64_t ld_seq, int32_t T,
+                        const float* X, int64_t ldx, int32_t K, int32_t n_conv, int32_t F, const int32_t* dilations,
+                        const float* weights, float* out, int64_t ldo, void* stream);
+
 /* ---- a14: predict_from_embedding (libreco/prediction/predict.py:36-40) -----------------
  * out[r] = sum_k U[users[r],k] * I[items[r],k]; mode 0: raw, 1: expit (ranking),
  * 2: clip to [lo, hi] (rating) — normalize_prediction (:18-23). */

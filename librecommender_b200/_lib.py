@@ -152,6 +152,12 @@ SIGNATURES = {
                                        _P, _P, _P, c_int64, _P, _P]),
     "b200_rnn_backward": (c_int, [_P, c_int64, _P, c_int32, c_int32, c_int32, c_int32, c_int32, _P, _P, c_int64, _P,
                                   _P, _P, _P, _P, _P, _P]),
+    "b200_caser_weight_floats": (c_int64, [c_int32, c_int32, c_int32, c_int32]),
+    "b200_wavenet_weight_floats": (c_int64, [c_int32, c_int32, c_int32]),
+    "b200_caser_encode": (c_int, [_P, c_int64, _P, c_int64, c_int32, _P, c_int64, c_int32, c_int32, c_int32, _P, _P,
+                                  c_int64, _P]),
+    "b200_wavenet_encode": (c_int, [_P, c_int64, _P, c_int64, c_int32, _P, c_int64, c_int32, c_int32, c_int32, _P, _P,
+                                    _P, c_int64, _P]),
 }
 
 for _name, (_res, _args) in SIGNATURES.items():

@@ -1519,7 +1519,6 @@ class RNN4Rec:
         unknown user ``n_users``) and top-K select.  The model's sequence table is not touched."""
         from .dynamic_feats import build_rec_seq
 
-        torch = self._torch
         if n_rec > self.n_items:
             raise ValueError(f"`n_rec` {n_rec} exceeds num of items {self.n_items}")
         u = int(user_id)
@@ -1528,23 +1527,237 @@ class RNN4Rec:
             v = self.user_vectors([0], row, ln)
         else:
             v = self.user_vectors([u])
-        if not hasattr(self, "_I"):
-            self._I = _dyn_item_rows(self.item_embeds, self.item_biases, self.norm_embed).contiguous()
-        q = torch.cat([v, torch.ones((1, 1), dtype=torch.float32, device=self.device)], dim=1).contiguous()
-        N, d = self.n_items, q.shape[1]
-        scores = torch.empty((1, N), dtype=torch.float32, device=self.device)
-        zero = torch.zeros(1, dtype=torch.int64, device=self.device)
-        _lib.check(_lib.lib.b200_score_rows_f32(_lib.ptr(q), q.stride(0), _lib.ptr(zero), 1, _lib.ptr(self._I),
-                                                self._I.stride(0), N, d, _lib.ptr(scores), scores.stride(0),
-                                                _lib.current_stream()))
-        consumed = getattr(data_info, "user_consumed", None)
-        owner = _ConsumedOwner(consumed, self.n_users, self.n_items, self.device)
-        out_ids = torch.empty((1, n_rec), dtype=torch.int64, device=self.device)
-        out_sc = torch.empty((1, n_rec), dtype=torch.float32, device=self.device)
-        uid = torch.tensor([u], dtype=torch.int64, device=self.device)
-        masked_topk(owner, scores, uid, n_rec, filter_consumed, out_ids, out_sc)
-        ids = out_ids.cpu().numpy()
-        return (ids, out_sc.cpu().numpy()) if return_scores else ids
+        return _dynamic_topk(self, v, u, n_rec, data_info, filter_consumed, return_scores)
+
+
+def _dynamic_topk(model, v, u, n_rec, data_info, filter_consumed, return_scores):
+    """The scoring tail of ``recommend_dynamic`` for the ``DynEmbedBase`` sequence models: the user vector ``v``
+    [1, d] with the pseudo bias 1 appended scores ``[I | b]`` (``model.item_embeds`` / ``item_biases``, normalised
+    with ``model.norm_embed``; cached on the model) over ``I[:n_items]``, then the consumed filter of user ``u``
+    (none for the unknown user ``n_users``) and top-K select."""
+    import torch
+
+    dev = model.device
+    if not hasattr(model, "_I"):
+        model._I = _dyn_item_rows(model.item_embeds, model.item_biases, model.norm_embed).contiguous()
+    q = torch.cat([v, torch.ones((1, 1), dtype=torch.float32, device=dev)], dim=1).contiguous()
+    N, d = model.n_items, q.shape[1]
+    scores = torch.empty((1, N), dtype=torch.float32, device=dev)
+    zero = torch.zeros(1, dtype=torch.int64, device=dev)
+    _lib.check(_lib.lib.b200_score_rows_f32(_lib.ptr(q), q.stride(0), _lib.ptr(zero), 1, _lib.ptr(model._I),
+                                            model._I.stride(0), N, d, _lib.ptr(scores), scores.stride(0),
+                                            _lib.current_stream()))
+    consumed = getattr(data_info, "user_consumed", None)
+    owner = _ConsumedOwner(consumed, model.n_users, model.n_items, dev)
+    out_ids = torch.empty((1, n_rec), dtype=torch.int64, device=dev)
+    out_sc = torch.empty((1, n_rec), dtype=torch.float32, device=dev)
+    uid = torch.tensor([u], dtype=torch.int64, device=dev)
+    masked_topk(owner, scores, uid, n_rec, filter_consumed, out_ids, out_sc)
+    ids = out_ids.cpu().numpy()
+    return (ids, out_sc.cpu().numpy()) if return_scores else ids
+
+
+CONV_MAX_T, CONV_MAX_K, CONV_MAX_FILTERS, CONV_MAX_F, CONV_MAX_LAYERS = 64, 128, 32, 128, 16   # b200_*_encode envelope
+
+
+class _ConvSeqModel:
+    """What Caser and WaveNet share (``bases/dyn_embed_base.py:166-283``, ``recommendation/preprocess.py:26-46``):
+    the user vector ``[user_embeds[u] | head(encoder(seq_embeds[seq]))]`` (2K wide, L2-normalised as a whole with
+    ``norm_embed``), where the encoder is the subclass's kernel over the user's recent sequence (right-padded with
+    ``n_items``; the pad positions are ordinary rows, neither model masks by length) and the Dense head runs on
+    :func:`linear`; the item side is ``[item_embeds (2K) | item_bias]`` and the user side gets the pseudo bias 1, so
+    all-items retrieval is the embed scorer on d = 2K + 1.  The user table's last row ``n_users`` is the unknown
+    user's: ``set_embeddings`` first sets it to the mean of the other rows (``_assign_user_oov``)."""
+
+    NAME = ""
+    HEAD_ACT = ACT_NONE
+
+    def __init__(self, data_info_or_spec, weights, recent_seqs, recent_seq_lens, norm_embed=False, device=None):
+        import torch
+
+        self._torch = torch
+        g = (data_info_or_spec.get if isinstance(data_info_or_spec, dict)
+             else lambda k: getattr(data_info_or_spec, k))
+        self.n_users, self.n_items = int(g("n_users")), int(g("n_items"))
+        self.norm_embed = bool(norm_embed)
+        self.T = int(np.shape(recent_seqs)[1])
+        self.K = int(np.shape(weights["seq_embeds"])[1])
+        if not 1 <= self.T <= CONV_MAX_T:
+            raise ValueError(f"{self.NAME}: max_seq_len {self.T} outside [1, {CONV_MAX_T}]")
+        if not 1 <= self.K <= CONV_MAX_K:
+            raise ValueError(f"{self.NAME}: embed_size {self.K} outside [1, {CONV_MAX_K}]")
+        shapes = {"user_embeds": (self.n_users + 1, self.K), "seq_embeds": (self.n_items + 1, self.K),
+                  "item_embeds": (self.n_items, 2 * self.K), "dense_bias": (self.K,)}
+        for k, shp in shapes.items():
+            if tuple(np.shape(weights[k])) != shp:
+                raise ValueError(f"{self.NAME}: `{k}` has shape {np.shape(weights[k])}, expected {shp}")
+        if np.shape(recent_seqs)[0] != self.n_users + 1:
+            raise ValueError(f"{self.NAME}: {np.shape(recent_seqs)[0]} recent sequences for {self.n_users} users + "
+                             "the OOV row")
+        self._check_encoder(weights)
+        self.device = torch.device(device) if device is not None else _lib.require_cuda()
+        f32 = torch.float32
+        self.user_embeds = _dev(weights["user_embeds"], self.device, f32)       # [n_users + 1, K]
+        self.seq_embeds = _dev(weights["seq_embeds"], self.device, f32)         # [n_items + 1, K]
+        self.item_embeds = _dev(weights["item_embeds"], self.device, f32)       # [n_items, 2K]
+        self.item_biases = _dev(np.asarray(weights["item_biases"]).reshape(-1), self.device, f32)
+        self.conv_w = _dev(weights["conv"], self.device, f32)
+        self.dense_Wt = _dev(np.asarray(weights["dense_kernel"]).T, self.device, f32)    # [K, D]
+        self.dense_b = _dev(np.asarray(weights["dense_bias"]).reshape(-1), self.device, f32)
+        self.seqs = _dev(recent_seqs, self.device, torch.int32)
+        self.lens = _dev(np.asarray(recent_seq_lens).reshape(-1), self.device, torch.int32)   # kept, never read
+
+    def _check_encoder(self, weights):
+        raise NotImplementedError
+
+    def _encode_into(self, rows_d, seqs, out):
+        raise NotImplementedError
+
+    def encode(self, rows_d, seqs=None):
+        """[n, D] pre-head features of the rows ``rows_d`` (device int64) of ``seqs`` (default: the model's recent
+        sequences)."""
+        seqs = self.seqs if seqs is None else seqs
+        out = self._torch.empty((int(rows_d.numel()), self.dense_Wt.shape[1]), dtype=self._torch.float32,
+                                device=self.device)
+        self._encode_into(rows_d, seqs, out)
+        return out
+
+    def user_vectors(self, ids, seqs=None, lens=None):
+        """[n, 2K] user vectors of the users ``ids`` (0..n_users; n_users is the unknown user): the user table row
+        beside the encoded sequence, which is the user's recent sequence or, when given, row i of ``seqs`` [n, T]
+        (host or device) for ``ids[i]``; then the L2 normalisation with ``norm_embed``.  ``lens`` is accepted and
+        not read: neither graph masks by length.  A row's bits depend only on its own user row and sequence."""
+        torch = self._torch
+        ids = np.asarray(ids, dtype=np.int64).reshape(-1)
+        n, K = int(ids.size), self.K
+        if n and (ids.min() < 0 or ids.max() > self.n_users):
+            raise ValueError(f"{self.NAME}: user ids must lie in [0, {self.n_users}]")
+        ids_d = torch.as_tensor(ids).to(self.device)
+        rows_d = ids_d
+        if seqs is not None:
+            seqs = _dev(seqs, self.device, torch.int32)
+            if tuple(seqs.shape) != (n, self.T):
+                raise ValueError(f"`seqs` has shape {tuple(seqs.shape)}, expected ({n}, {self.T})")
+            rows_d = torch.arange(n, dtype=torch.int64, device=self.device)
+        x = torch.empty((n, 2 * K), dtype=torch.float32, device=self.device)
+        if n == 0:
+            return x
+        _lib.check(_lib.lib.b200_gather_rows(_lib.ptr(self.user_embeds), self.user_embeds.stride(0), K,
+                                             _lib.ptr(ids_d), n, _lib.ptr(x), x.stride(0), _lib.current_stream()))
+        x[:, K:] = linear(self.encode(rows_d, seqs), self.dense_Wt, self.dense_b, self.HEAD_ACT, impl="f32")
+        if self.norm_embed:
+            _lib.check(_lib.lib.b200_l2_normalize_rows(_lib.ptr(x), x.stride(0), n, x.shape[1],
+                                                       _lib.current_stream()))
+        return x
+
+    def assign_user_oov(self):
+        """``_assign_user_oov`` (dyn_embed_base.py:271-283): the unknown user's row := mean of the known rows."""
+        self.user_embeds[self.n_users] = self.user_embeds[:self.n_users].mean(dim=0)
+
+    def set_embeddings(self, chunk=1 << 20):
+        """Assigns the OOV user row, then returns device tensors ``U [n_users + 1, 2K + 1]`` (pseudo bias 1 in the
+        last column, last row = the mean row) and ``I [n_items + 1, 2K + 1]`` (``[item_embeds | item_biases]`` + the
+        mean row) for :class:`engine.EmbedScorer`."""
+        torch = self._torch
+        self.assign_user_oov()
+        rows = [self.user_vectors(np.arange(i, min(self.n_users, i + chunk))) for i in range(0, self.n_users, chunk)]
+        return dyn_embed_tables(torch.cat(rows, dim=0), self.item_embeds, self.item_biases, self.norm_embed)
+
+    def recommend_dynamic(self, user_id, n_rec, data_info, user_feats=None, seq=None, filter_consumed=True,
+                          inner_id=False, return_scores=False):
+        """``recommend_user`` for ONE user (inner id; ``n_users`` = the unknown user, whose table row is the mean row
+        once ``set_embeddings`` ran) with an optional behaviour sequence supplied for this call
+        (``dyn_embed_base.py:166-214``, ``recommendation/preprocess.py:26-46``): the sequence is cut to its last
+        ``max_seq_len`` items and unknown original ids become the pad id ``n_items``; without one the user's cached
+        sequence is used.  The user's own table row always goes beside it, so a cold and a warm user with the same
+        sequence get different vectors.  ``user_feats`` is accepted and ignored (no user features).  The model's
+        tables are not touched."""
+        from .dynamic_feats import build_rec_seq
+
+        if n_rec > self.n_items:
+            raise ValueError(f"`n_rec` {n_rec} exceeds num of items {self.n_items}")
+        u = int(user_id)
+        if seq is not None and len(seq) > 0:
+            row, _ = build_rec_seq(seq, self.n_items, self.T, getattr(data_info, "item2id", None), inner_id)
+            v = self.user_vectors([u], row)
+        else:
+            v = self.user_vectors([u])
+        return _dynamic_topk(self, v, u, n_rec, data_info, filter_consumed, return_scores)
+
+
+class Caser(_ConvSeqModel):
+    """libreco/algorithms/caser.py:135-221 (inference): ``b200_caser_encode`` runs the T horizontal convolutions
+    (kernel sizes 1..T, ReLU, max over the valid positions) and the vertical one over each user's recent sequence;
+    the head is ``Dense(K, relu)``.  ``weights``: the dict of ``weights_io.caser_weights`` (or the raw variables it
+    takes, ``synthetic.make_caser_weights``).  ``use_bn`` and ``dropout_rate`` are never read by the graph."""
+
+    NAME = "Caser"
+    HEAD_ACT = ACT_RELU
+
+    def __init__(self, data_info_or_spec, weights, recent_seqs, recent_seq_lens, norm_embed=False, device=None):
+        from .weights_io import caser_weights
+
+        if "conv" not in weights:
+            weights = caser_weights(weights)
+        super().__init__(data_info_or_spec, weights, recent_seqs, recent_seq_lens, norm_embed, device)
+
+    def _check_encoder(self, weights):
+        self.nh, self.nv = int(weights["nh"]), int(weights["nv"])
+        if int(weights["T"]) != self.T:
+            raise ValueError(f"Caser: {weights['T']} horizontal convolutions, max_seq_len is {self.T}")
+        if not (1 <= self.nh <= CONV_MAX_FILTERS and 1 <= self.nv <= CONV_MAX_FILTERS):
+            raise ValueError(f"Caser: nh_filters {self.nh} / nv_filters {self.nv} outside [1, {CONV_MAX_FILTERS}]")
+        D = self.T * self.nh + self.K * self.nv
+        if np.size(weights["conv"]) != int(_lib.lib.b200_caser_weight_floats(self.T, self.K, self.nh, self.nv)):
+            raise ValueError(f"Caser: {np.size(weights['conv'])} packed convolution floats do not match T {self.T}, "
+                             f"K {self.K}, nh {self.nh}, nv {self.nv}")
+        if tuple(np.shape(weights["dense_kernel"])) != (D, self.K):
+            raise ValueError(f"Caser: `dense_kernel` has shape {np.shape(weights['dense_kernel'])}, expected "
+                             f"({D}, {self.K})")
+
+    def _encode_into(self, rows_d, seqs, out):
+        _lib.check(_lib.lib.b200_caser_encode(
+            _lib.ptr(rows_d), int(rows_d.numel()), _lib.ptr(seqs), seqs.stride(0), self.T, _lib.ptr(self.seq_embeds),
+            self.seq_embeds.stride(0), self.K, self.nh, self.nv, _lib.ptr(self.conv_w), _lib.ptr(out), out.stride(0),
+            _lib.current_stream()))
+
+
+class WaveNet(_ConvSeqModel):
+    """libreco/algorithms/wave_net.py:139-222 (inference): ``b200_wavenet_encode`` runs the causal dilated
+    convolutions (kernel size 2, ReLU), the 1x1 convolution (ReLU) and the max over the T positions over each
+    user's recent sequence; the head is ``Dense(K)`` without activation.  ``weights``: the dict of
+    ``weights_io.wavenet_weights`` (or the raw variables it takes, ``synthetic.make_wavenet_weights``), which
+    carries the per-layer dilations: ``2**i`` in layer i of a block, or 1 everywhere for a model built by TF1."""
+
+    NAME = "WaveNet"
+
+    def __init__(self, data_info_or_spec, weights, recent_seqs, recent_seq_lens, norm_embed=False, device=None):
+        from .weights_io import wavenet_weights
+
+        if "conv" not in weights:
+            weights = wavenet_weights(weights)
+        super().__init__(data_info_or_spec, weights, recent_seqs, recent_seq_lens, norm_embed, device)
+
+    def _check_encoder(self, weights):
+        self.F, dil = int(weights["F"]), [int(d) for d in weights["dilations"]]
+        if not 1 <= self.F <= CONV_MAX_F:
+            raise ValueError(f"WaveNet: n_filters {self.F} outside [1, {CONV_MAX_F}]")
+        if not 1 <= len(dil) <= CONV_MAX_LAYERS or min(dil) < 1:
+            raise ValueError(f"WaveNet: dilations {dil}: 1 to {CONV_MAX_LAYERS} causal layers, each dilation >= 1")
+        if np.size(weights["conv"]) != int(_lib.lib.b200_wavenet_weight_floats(self.K, self.F, len(dil))):
+            raise ValueError(f"WaveNet: {np.size(weights['conv'])} packed convolution floats do not match K {self.K}, "
+                             f"F {self.F}, {len(dil)} causal layers")
+        if tuple(np.shape(weights["dense_kernel"])) != (self.F, self.K):
+            raise ValueError(f"WaveNet: `dense_kernel` has shape {np.shape(weights['dense_kernel'])}, expected "
+                             f"({self.F}, {self.K})")
+        self.dilations = dil
+        self.dil = (ctypes.c_int32 * len(dil))(*dil)
+
+    def _encode_into(self, rows_d, seqs, out):
+        _lib.check(_lib.lib.b200_wavenet_encode(
+            _lib.ptr(rows_d), int(rows_d.numel()), _lib.ptr(seqs), seqs.stride(0), self.T, _lib.ptr(self.seq_embeds),
+            self.seq_embeds.stride(0), self.K, len(self.dilations), self.F, self.dil, _lib.ptr(self.conv_w),
+            _lib.ptr(out), out.stride(0), _lib.current_stream()))
 
 
 class _ConsumedOwner:

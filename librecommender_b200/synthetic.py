@@ -267,3 +267,48 @@ def make_rnn4rec_weights(rng, n_items, K, hidden_units=(16,), rnn_type="gru", us
     return dict(rnn_scheme=scheme, rnn_type=rnn_type, use_layer_norm=bool(use_layer_norm and scheme == "keras"),
                 seq_embeds=_glorot(rng, (n_items + 1, hidden_units[0])), item_embeds=_glorot(rng, (n_items, K)),
                 item_biases=small(n_items), rnn_layers=layers, dense_kernel=_glorot(rng, (d, K)), dense_bias=small(K))
+
+
+def _conv_kernel(rng, w, c_in, c_out):
+    lim = np.sqrt(6.0 / (w * c_in + w * c_out))          # Keras glorot_uniform of a Conv1D kernel [w, in, out]
+    return rng.uniform(-lim, lim, size=(w, c_in, c_out)).astype(np.float32)
+
+
+def _conv_model_tables(rng, n_users, n_items, K):
+    """The four embedding-scope tables of Caser / WaveNet: ``user_embeds`` [n_users+1, K] (the last row is the OOV
+    row ``set_embeddings`` overwrites), ``seq_embeds`` [n_items+1, K] (the pad row, an ordinary random row distinct
+    from the others), ``item_embeds`` [n_items, 2K], ``item_biases`` [n_items]."""
+    return dict(user_embeds=_glorot(rng, (n_users + 1, K)), seq_embeds=_glorot(rng, (n_items + 1, K)),
+                item_embeds=_glorot(rng, (n_items, 2 * K)),
+                item_biases=(rng.standard_normal(n_items) * 0.1).astype(np.float32))
+
+
+def make_caser_weights(rng, n_users, n_items, K, max_seq_len=10, nh_filters=2, nv_filters=4):
+    """Caser variables (libreco/algorithms/caser.py:162-221) in their raw shapes: the four tables, ``convs`` = the
+    horizontal Conv1D layers {kernel [h, K, nh], bias [nh]} for h = 1..T, ``vertical`` {kernel [1, T, nv], bias [nv]},
+    the head ``dense_kernel`` [T*nh + K*nv, K], ``dense_bias`` [K].  Biases are non-zero and of both signs, so that
+    ReLU zeros and the max-pool positions are exercised.  ``weights_io.caser_weights`` packs them."""
+    T, nh, nv = int(max_seq_len), int(nh_filters), int(nv_filters)
+    bias = lambda n: (rng.standard_normal(n) * 0.1).astype(np.float32)      # noqa: E731
+    w = _conv_model_tables(rng, n_users, n_items, K)
+    w.update(convs=[dict(kernel=_conv_kernel(rng, h, K, nh), bias=bias(nh)) for h in range(1, T + 1)],
+             vertical=dict(kernel=_conv_kernel(rng, 1, T, nv), bias=bias(nv)),
+             dense_kernel=_glorot(rng, (T * nh + K * nv, K)), dense_bias=bias(K))
+    return w
+
+
+def make_wavenet_weights(rng, n_users, n_items, K, n_filters=16, n_blocks=1, n_layers_per_block=4, dilated=True):
+    """WaveNet variables (libreco/algorithms/wave_net.py:166-222) in their raw shapes: the four tables, ``convs`` =
+    the causal Conv1D layers {kernel [2, C_in, F], bias [F]}, ``out_conv`` {kernel [1, F, F], bias [F]}, the head
+    ``dense_kernel`` [F, K], ``dense_bias`` [K], and ``dilations`` (``weights_io.wavenet_dilations``).  Biases are
+    non-zero and of both signs.  ``weights_io.wavenet_weights`` packs them."""
+    from .weights_io import wavenet_dilations
+
+    F = int(n_filters)
+    dil = wavenet_dilations(n_blocks, n_layers_per_block, dilated)
+    bias = lambda n: (rng.standard_normal(n) * 0.1).astype(np.float32)      # noqa: E731
+    w = _conv_model_tables(rng, n_users, n_items, K)
+    w.update(convs=[dict(kernel=_conv_kernel(rng, 2, K if i == 0 else F, F), bias=bias(F)) for i in range(len(dil))],
+             out_conv=dict(kernel=_conv_kernel(rng, 1, F, F), bias=bias(F)),
+             dense_kernel=_glorot(rng, (F, K)), dense_bias=bias(K), dilations=dil)
+    return w

@@ -192,7 +192,13 @@ def default_tf_names(model_name, n_hidden, use_bn, use_tf_attention=False, n_lay
                      rnn_type="gru", use_layer_norm=False):
     """{engine weight key: TF variable name (or nested dict / list of names)} for the auto-named
     variables of `model_name` in {"FM", "DeepFM", "DIN", "YouTubeRanking", "TwoTower", "AutoInt", "Transformer",
-    "RNN4Rec"}.
+    "RNN4Rec", "Caser", "WaveNet"}.
+
+    Caser (caser.py:194-220; `n_layers` = max_seq_len T): the horizontal ``conv1d[_i]/{kernel,bias}:0`` for
+    i = 0..T-1 under ``convs``, the vertical ``conv1d_T`` under ``vertical``, the head ``dense/{kernel,bias}:0``.
+    WaveNet (wave_net.py:198-221; `n_layers` = n_blocks * n_layers_per_block): the causal ``conv1d[_i]`` under
+    ``convs``, the 1x1 ``conv1d_{n_layers}`` under ``out_conv``, the head ``dense``.  Both also use the four
+    ``CONV_TABLES``.
 
     RNN4Rec (rnn4rec.py:151-237 with layers/recurrent.py:4-63; `n_layers` = len(hidden_units)): "keras" layer i is
     ``{t}[_i]/{t}_cell/{kernel,recurrent_kernel,bias}:0`` (t = gru or lstm) plus, with `use_layer_norm`,
@@ -220,6 +226,8 @@ def default_tf_names(model_name, n_hidden, use_bn, use_tf_attention=False, n_lay
     (per-layer {query, key, value, attention_output | output}), ``out_kernel``, ``out_bias``."""
     if model_name == "RNN4Rec":
         return _rnn4rec_names(scheme, rnn_type, n_layers, use_layer_norm)
+    if model_name in ("Caser", "WaveNet"):
+        return _conv_names(model_name, n_layers)
     if model_name == "Transformer":
         _check_mha_scheme(scheme, "Transformer")
         layers = []
@@ -633,10 +641,137 @@ def _rnn4rec_raw(npz, rnn_type, hidden_units, use_layer_norm, extra_names=None):
     return raw
 
 
+# Caser / WaveNet (caser.py:162-221, wave_net.py:166-222): the four embedding-scope tables, then auto-named Conv1D
+# layers and the Dense head.  The names restate TensorFlow's naming rule and are unverified against a saved model.
+CONV_TABLES = {"user_embeds": "embedding/user_embeds_var:0", "seq_embeds": "embedding/seq_embeds_var:0",
+               "item_embeds": "embedding/item_embeds_var:0", "item_biases": "embedding/item_bias_var:0"}
+
+
+def _conv_names(model_name, n_conv):
+    """Caser: ``n_conv`` = T horizontal layers ``conv1d[_i]`` (i = 0..T-1, kernel size i+1) then the vertical
+    ``conv1d_T``.  WaveNet: ``n_conv`` causal layers ``conv1d[_i]`` then the 1x1 layer ``conv1d_{n_conv}``."""
+    conv = lambda i: {k: f"conv1d{'' if i == 0 else f'_{i}'}/{k}:0" for k in ("kernel", "bias")}   # noqa: E731
+    last = "vertical" if model_name == "Caser" else "out_conv"
+    return {"convs": [conv(i) for i in range(n_conv)], last: conv(n_conv), "dense_kernel": "dense/kernel:0",
+            "dense_bias": "dense/bias:0"}
+
+
+def conv_tf_shapes(model_name, n_users, n_items, K, T=None, nh=None, nv=None, F=None, n_conv=None):
+    """Expected shapes of every Caser / WaveNet variable: the tables ``user_embeds [n_users+1, K]``, ``seq_embeds
+    [n_items+1, K]``, ``item_embeds [n_items, 2K]``, ``item_biases [n_items]``; Caser ``W_h [h, K, nh]``, ``[nh]``
+    (h = 1..T), ``Wv [1, T, nv]``, ``[nv]``, head ``[T*nh + K*nv, K]``; WaveNet ``[2, C_in, F]``, ``[F]`` per causal
+    layer (C_in = K first, then F), ``[1, F, F]``, ``[F]``, head ``[F, K]``.  Keyed like :func:`_conv_names`."""
+    out = {"user_embeds": (n_users + 1, K), "seq_embeds": (n_items + 1, K), "item_embeds": (n_items, 2 * K),
+           "item_biases": (n_items,), "dense_bias": (K,)}
+    if model_name == "Caser":
+        out.update(convs=[{"kernel": (h, K, nh), "bias": (nh,)} for h in range(1, T + 1)],
+                   vertical={"kernel": (1, T, nv), "bias": (nv,)}, dense_kernel=(T * nh + K * nv, K))
+    else:
+        out.update(convs=[{"kernel": (2, K if i == 0 else F, F), "bias": (F,)} for i in range(n_conv)],
+                   out_conv={"kernel": (1, F, F), "bias": (F,)}, dense_kernel=(F, K))
+    return out
+
+
+def wavenet_dilations(n_blocks, n_layers_per_block, dilated=True):
+    """Per-layer dilations of WaveNet's causal stack: ``2**i`` for layer i of each block (wave_net.py:199-208), or 1
+    everywhere for a TF1-trained model, whose ``tf.layers.conv1d`` is built without ``dilation_rate``
+    (layers/convolutional.py:19-27)."""
+    return [2 ** i if dilated else 1 for _ in range(int(n_blocks)) for i in range(int(n_layers_per_block))]
+
+
+def _conv_tables(raw):
+    w = {k: np.asarray(raw[k], dtype=np.float32) for k in CONV_TABLES}
+    w["item_biases"] = w["item_biases"].reshape(-1)
+    w["dense_kernel"] = np.asarray(raw["dense_kernel"], dtype=np.float32)
+    w["dense_bias"] = np.asarray(raw["dense_bias"], dtype=np.float32).reshape(-1)
+    return w
+
+
+def caser_weights(raw):
+    """Engine weight dict of :class:`feat_models.Caser` from the raw variables (the four tables, ``convs`` = the T
+    horizontal layers {kernel [h, K, nh], bias [nh]}, ``vertical`` {kernel [1, T, nv], bias [nv]}, the head):
+    ``conv`` packs them as ``b200_caser_encode`` reads them, W_1 .. W_T, then b_h [T, nh], Wv [T, nv], bv [nv]."""
+    f32 = lambda a: np.asarray(a, dtype=np.float32)      # noqa: E731
+    convs, vert = raw["convs"], raw["vertical"]
+    T, nh, nv = len(convs), int(np.shape(convs[0]["bias"])[-1]), int(np.shape(vert["bias"])[-1])
+    w = _conv_tables(raw)
+    w["conv"] = np.concatenate([f32(c["kernel"]).reshape(-1) for c in convs] +
+                               [f32(c["bias"]).reshape(-1) for c in convs] +
+                               [f32(vert["kernel"]).reshape(-1), f32(vert["bias"]).reshape(-1)])
+    w.update(model="Caser", T=T, nh=nh, nv=nv)
+    return w
+
+
+def wavenet_weights(raw):
+    """Engine weight dict of :class:`feat_models.WaveNet` from the raw variables (the four tables, ``convs`` = the
+    causal layers {kernel [2, C_in, F], bias [F]}, ``out_conv`` {kernel [1, F, F], bias [F]}, ``dilations``, the
+    head): ``conv`` packs them as ``b200_wavenet_encode`` reads them, per layer W then b, then W1, b1."""
+    f32 = lambda a: np.asarray(a, dtype=np.float32).reshape(-1)      # noqa: E731
+    parts = [f32(c[k]) for c in raw["convs"] + [raw["out_conv"]] for k in ("kernel", "bias")]
+    w = _conv_tables(raw)
+    w["conv"] = np.concatenate(parts)
+    dil = [int(d) for d in raw["dilations"]]
+    if len(dil) != len(raw["convs"]):
+        raise ValueError(f"WaveNet: {len(dil)} dilations for {len(raw['convs'])} causal layers")
+    w.update(model="WaveNet", F=int(np.shape(raw["out_conv"]["bias"])[-1]), dilations=dil)
+    return w
+
+
+def _conv_tf_variables(raw):
+    """Raw Caser / WaveNet variables (what :func:`caser_weights` / :func:`wavenet_weights` take) -> ``{TF variable
+    name: array}``: what ``save_tf_variables`` writes, and the inverse of ``load_reference_tf_model``."""
+    model = "Caser" if "vertical" in raw else "WaveNet"
+    names = _conv_names(model, len(raw["convs"]))
+    out = {n: np.asarray(raw[k], dtype=np.float32) for k, n in CONV_TABLES.items()}
+    out[CONV_TABLES["item_biases"]] = out[CONV_TABLES["item_biases"]].reshape(-1)
+    return _put_tf_names(out, names, raw)
+
+
+# the dilations of WaveNet are not variables: the loader takes them as arguments
+caser_tf_variables = wavenet_tf_variables = _conv_tf_variables
+
+
+def _conv_raw(npz, model_name, n_filters=None, n_blocks=None, n_layers_per_block=None, dilated=True,
+              extra_names=None):
+    """Raw Caser / WaveNet variables of a saved model, every name and shape checked.  Caser reads T off the vertical
+    kernel ``conv1d_{T}`` [1, T, nv]: the one layer whose index equals its kernel's T; nh and nv come off the first
+    and the vertical bias.  WaveNet's graph (``n_filters``, ``n_blocks``, ``n_layers_per_block``, ``dilated``) is
+    taken as arguments: the file does not tell the TF1 graph (dilation 1) from the TF2 one."""
+    tab = resolve_tf_names(npz, {"user_embeds": CONV_TABLES["user_embeds"], "item_embeds": CONV_TABLES["item_embeds"]})
+    if tab["user_embeds"].ndim != 2 or tab["item_embeds"].ndim != 2:
+        raise KeyError(f"`{CONV_TABLES['user_embeds']}` / `{CONV_TABLES['item_embeds']}` must be 2-D")
+    (nu1, K), n_items = tab["user_embeds"].shape, tab["item_embeds"].shape[0]
+    if model_name == "Caser":
+        T = None
+        for n in npz.files:
+            parts = n.split("/")
+            if len(parts) == 2 and parts[1] == "kernel:0" and parts[0].startswith("conv1d_"):
+                shp = np.shape(npz[n])
+                if len(shp) == 3 and shp[0] == 1 and parts[0] == f"conv1d_{shp[1]}":
+                    T = int(shp[1])
+        if T is None:
+            raise KeyError("Caser: no vertical kernel `conv1d_{T}/kernel:0` of shape [1, T, nv] in the file")
+        names = _conv_names("Caser", T)
+        nh = int(np.shape(resolve_tf_names(npz, names["convs"][0]["bias"]))[0])
+        nv = int(np.shape(resolve_tf_names(npz, names["vertical"]["bias"]))[0])
+        shapes = conv_tf_shapes("Caser", nu1 - 1, n_items, K, T=T, nh=nh, nv=nv)
+    else:
+        F, dil = int(n_filters), wavenet_dilations(n_blocks, n_layers_per_block, dilated)
+        names = _conv_names("WaveNet", len(dil))
+        shapes = conv_tf_shapes("WaveNet", nu1 - 1, n_items, K, F=F, n_conv=len(dil))
+    names.update(extra_names or {})
+    raw = resolve_tf_names(npz, {k: CONV_TABLES[k] for k in CONV_TABLES}, {k: shapes[k] for k in CONV_TABLES})
+    raw.update(resolve_tf_names(npz, names, {k: shapes[k] for k in names}))
+    if model_name == "WaveNet":
+        raw["dilations"] = dil
+    return raw
+
+
 def load_reference_tf_model(path, model_name, arch, n_hidden, use_bn, use_tf_attention=False, extra_names=None,
                             num_heads=None, att_embed_size=(8, 8, 8), use_residual=True, num_tfm_layers=1,
                             positional_embedding="trainable", use_causal_mask=False, feat_agg_mode="concat",
-                            rnn_type="gru", hidden_units=(16,), use_layer_norm=False):
+                            rnn_type="gru", hidden_units=(16,), use_layer_norm=False, n_filters=16, n_blocks=1,
+                            n_layers_per_block=4, dilated=True):
     """Engine weight dict of a model saved by the reference (``save_tf_variables``,
     utils/save_load.py:70-98) WITHOUT a hand-written name map: the embedding-scope variables by their
     fixed names, the heads / MLPs / batch-norms through :func:`default_tf_names` (override single entries
@@ -647,7 +782,10 @@ def load_reference_tf_model(path, model_name, arch, n_hidden, use_bn, use_tf_att
     for Transformer).  YouTubeRetrieval (``n_hidden`` Dense layers in the user tower) returns the layout of
     ``feat_models.YouTubeRetrieval``, every name and shape checked.  RNN4Rec takes its constructor's ``rnn_type``,
     ``hidden_units`` and ``use_layer_norm`` (``n_hidden`` and ``use_bn`` are unused), reads the graph (keras or
-    legacy) off the names, checks every name and shape and returns the layout of ``feat_models.RNN4Rec``."""
+    legacy) off the names, checks every name and shape and returns the layout of ``feat_models.RNN4Rec``.  Caser
+    reads max_seq_len off the vertical kernel; WaveNet takes ``n_filters``, ``n_blocks``, ``n_layers_per_block`` and
+    ``dilated`` (False for a TF1-trained model, whose causal layers all have dilation 1).  Both check every name and
+    shape and return the layout of ``feat_models.Caser`` / ``feat_models.WaveNet``."""
     from .feat_models import from_tf_variables
 
     npz = np.load(os.path.join(path, f"{model_name}_tf_variables.npz"))
@@ -655,6 +793,10 @@ def load_reference_tf_model(path, model_name, arch, n_hidden, use_bn, use_tf_att
         return _youtube_retrieval_weights(npz, n_hidden, use_bn, extra_names)
     if arch == "RNN4Rec":
         return rnn4rec_weights(_rnn4rec_raw(npz, rnn_type, hidden_units, bool(use_layer_norm), extra_names))
+    if arch == "Caser":
+        return caser_weights(_conv_raw(npz, "Caser", extra_names=extra_names))
+    if arch == "WaveNet":
+        return wavenet_weights(_conv_raw(npz, "WaveNet", n_filters, n_blocks, n_layers_per_block, dilated, extra_names))
     w = from_tf_variables(npz)
     if arch == "Transformer":
         scheme = "keras" if "transformer_layer1/multi_head_attention/query/kernel:0" in npz.files else "legacy"
