@@ -1324,8 +1324,7 @@ class TwoTower:
         torch = self._torch
         outs = []
         for which, n in (("user", self.n_users), ("item", self.n_items)):
-            rows = [self.tower(which, np.arange(i, min(n, i + chunk))) for i in range(0, n, chunk)]
-            E = torch.cat(rows, dim=0)
+            E = _chunked_rows(lambda ids: self.tower(which, ids), n, chunk)
             outs.append(torch.cat([E, E.mean(dim=0, keepdim=True)], dim=0))
         return outs[0], outs[1]
 
@@ -1359,9 +1358,11 @@ class YouTubeRetrieval:
         self.mlp = [(_dev(Wt, self.device, f32), _dev(b, self.device, f32), relu) for Wt, b, relu in fold_mlp(weights["mlp"])]
 
     def user_vectors(self, ids):
-        """[n, H] user embeddings of the given (inner) user ids, before the pseudo bias."""
+        """[n, H] user embeddings of the given (inner) user ids, before the pseudo bias.  ``ValueError`` for an id
+        outside ``[0, n_users]`` or without a cached sequence row."""
         torch = self._torch
-        ids_d = torch.as_tensor(np.asarray(ids, dtype=np.int64)).to(self.device)
+        ids = _check_user_ids("YouTubeRetrieval", ids, self.n_users, self.seqs.shape[0])
+        ids_d = torch.as_tensor(ids).to(self.device)
         n, K = int(ids_d.numel()), self.K
         L, pos = self.base.side("user", with_id=False)      # no id-embedding field: the pooled sequence takes its place
         x = torch.empty((n, (1 + len(pos)) * K), dtype=torch.float32, device=self.device)
@@ -1381,9 +1382,34 @@ class YouTubeRetrieval:
     def set_embeddings(self, chunk=1 << 20):
         """Device tensors ``U [n_users + 1, H + 1]`` (pseudo bias 1 in the last column, last row = mean OOV row) and
         ``I [n_items + 1, H + 1]`` (``[item_embeds | item_biases]`` + the mean row) for :class:`engine.EmbedScorer`."""
-        torch = self._torch
-        rows = [self.user_vectors(np.arange(i, min(self.n_users, i + chunk))) for i in range(0, self.n_users, chunk)]
-        return dyn_embed_tables(torch.cat(rows, dim=0), self.item_embeds, self.item_biases, self.norm_embed)
+        U = _chunked_rows(self.user_vectors, self.n_users, chunk)
+        return dyn_embed_tables(U, self.item_embeds, self.item_biases, self.norm_embed)
+
+
+def _n_users_items(data_info_or_spec):
+    """``(n_users, n_items)`` of a ``DataInfo`` or of a dict holding both."""
+    if isinstance(data_info_or_spec, dict):
+        return int(data_info_or_spec["n_users"]), int(data_info_or_spec["n_items"])
+    return int(data_info_or_spec.n_users), int(data_info_or_spec.n_items)
+
+
+def _check_user_ids(name, ids, n_users, n_rows=None):
+    """``ids`` as a flat host int64 array.  The kernels index the user and sequence tables with them unchecked, so
+    an id outside ``[0, n_users]``, or (with ``n_rows``, the cached sequence rows) at or past ``n_rows``, raises
+    ``ValueError`` here."""
+    ids = np.asarray(ids, dtype=np.int64).reshape(-1)
+    if ids.size and (ids.min() < 0 or ids.max() > n_users):
+        raise ValueError(f"{name}: user ids must lie in [0, {n_users}]")
+    if ids.size and n_rows is not None and ids.max() >= n_rows:
+        raise ValueError(f"{name}: user id {ids.max()} has no cached sequence: {n_rows} recent sequence rows")
+    return ids
+
+
+def _chunked_rows(rows_of, n, chunk):
+    """``rows_of(ids)`` over the ids ``0 .. n-1`` in chunks of ``chunk`` ids, concatenated on the device."""
+    import torch
+
+    return torch.cat([rows_of(np.arange(i, min(n, i + chunk))) for i in range(0, n, chunk)], dim=0)
 
 
 def dyn_embed_tables(U, item_embeds, item_biases, norm_embed):
@@ -1410,35 +1436,153 @@ def _dyn_item_rows(item_embeds, item_biases, norm_embed):
     return torch.cat([I, item_biases[:, None]], dim=1)
 
 
+class _DynEmbedSeqModel:
+    """What the ``DynEmbedBase`` sequence-encoder models share (``bases/dyn_embed_base.py:166-283``,
+    ``recommendation/preprocess.py:26-46``): each user's recent sequence (``recent_sequences``: right-padded with
+    ``n_items``) goes through the subclass's encoder kernel and a Dense head on :func:`linear` into the user vector
+    (L2-normalised as a whole with ``norm_embed``); the item side is ``[item_embeds | item_bias]`` and the user side
+    gets the pseudo bias 1, so all-items retrieval is the embed scorer on d = ``item_embeds`` width + 1.
+
+    A subclass supplies ``_check_weights(weights, recent_seqs)``, which raises ``ValueError`` outside the kernel's
+    envelope before the device lookup and returns ``{attribute: host array}`` of its own float32 device tables, and
+    ``_features(ids_d, rows_d, seqs, lens)``, the [n, d] rows before the normalisation of the users ``ids_d`` over the
+    rows ``rows_d`` of ``seqs`` / ``lens`` (None: the recent sequences).  ``_before_set_embeddings`` may prepare the
+    tables before ``set_embeddings`` encodes."""
+
+    NAME = ""
+    READS_LENS = False      # whether the encoder reads the sequence lengths
+    _I = None               # [I | b] of recommend_dynamic, built on its first call
+
+    def __init__(self, data_info_or_spec, weights, recent_seqs, recent_seq_lens, norm_embed, device):
+        import torch
+
+        self._torch = torch
+        self.n_users, self.n_items = _n_users_items(data_info_or_spec)
+        self.norm_embed = bool(norm_embed)
+        self.T = int(np.shape(recent_seqs)[1])
+        own = self._check_weights(weights, recent_seqs)
+        self.device = torch.device(device) if device is not None else _lib.require_cuda()
+        f32 = torch.float32
+        self.seq_embeds = _dev(weights["seq_embeds"], self.device, f32)          # [n_items + 1, encoder input]
+        self.item_embeds = _dev(weights["item_embeds"], self.device, f32)        # [n_items, d]
+        self.item_biases = _dev(np.asarray(weights["item_biases"]).reshape(-1), self.device, f32)
+        self.dense_Wt = _dev(np.asarray(weights["dense_kernel"]).T, self.device, f32)    # [K, pre-head width]
+        self.dense_b = _dev(np.asarray(weights["dense_bias"]).reshape(-1), self.device, f32)
+        self.seqs = _dev(recent_seqs, self.device, torch.int32)
+        self.lens = _dev(np.asarray(recent_seq_lens).reshape(-1), self.device, torch.int32)
+        for k, a in own.items():
+            setattr(self, k, _dev(a, self.device, f32))
+
+    def _before_set_embeddings(self):
+        pass
+
+    def user_vectors(self, ids, seqs=None, lens=None):
+        """[n, d] user vectors of the users ``ids`` (0..n_users; n_users is the unknown user), L2-normalised with
+        ``norm_embed``.  The sequence of ``ids[i]`` is its recent sequence or, when given, row i of ``seqs`` [n, T]
+        (host or device) with length ``lens[i]``, which only a model that reads lengths reads.  A row's bits depend
+        only on its own user and sequence.  ``ValueError`` before any launch for an id outside ``[0, n_users]``, an id
+        without a cached sequence row (no ``seqs``), or ``seqs`` / ``lens`` that are not ``[n, T]`` / ``[n]``."""
+        torch = self._torch
+        ids = _check_user_ids(self.NAME, ids, self.n_users, self.seqs.shape[0] if seqs is None else None)
+        n = int(ids.size)
+        if self.READS_LENS and (seqs is None) != (lens is None):
+            raise ValueError("give both `seqs` and `lens`, or neither")
+        ids_d = rows_d = torch.as_tensor(ids).to(self.device)
+        if seqs is not None:
+            seqs = _dev(seqs, self.device, torch.int32)
+            if tuple(seqs.shape) != (n, self.T):
+                raise ValueError(f"`seqs` has shape {tuple(seqs.shape)}, expected ({n}, {self.T})")
+            if self.READS_LENS:
+                lens = _dev(lens.reshape(-1) if isinstance(lens, torch.Tensor) else np.asarray(lens).reshape(-1),
+                            self.device, torch.int32)
+                if tuple(lens.shape) != (n,):
+                    raise ValueError(f"`lens` has shape {tuple(lens.shape)}, expected ({n},)")
+            rows_d = torch.arange(n, dtype=torch.int64, device=self.device)
+        if n == 0:
+            return torch.empty((0, self.item_embeds.shape[1]), dtype=torch.float32, device=self.device)
+        x = self._features(ids_d, rows_d, seqs, lens)
+        if self.norm_embed:
+            _lib.check(_lib.lib.b200_l2_normalize_rows(_lib.ptr(x), x.stride(0), n, x.shape[1],
+                                                       _lib.current_stream()))
+        return x
+
+    def set_embeddings(self, chunk=1 << 20):
+        """Device tensors ``U [n_users + 1, d + 1]`` (pseudo bias 1 in the last column, last row = the mean row) and
+        ``I [n_items + 1, d + 1]`` (``[item_embeds | item_biases]`` + the mean row) for :class:`engine.EmbedScorer`."""
+        self._before_set_embeddings()
+        U = _chunked_rows(self.user_vectors, self.n_users, chunk)
+        return dyn_embed_tables(U, self.item_embeds, self.item_biases, self.norm_embed)
+
+    def recommend_dynamic(self, user_id, n_rec, data_info, user_feats=None, seq=None, filter_consumed=True,
+                          inner_id=False, return_scores=False):
+        """``recommend_user`` for ONE user (inner id; ``n_users`` = the unknown user) with an optional behaviour
+        sequence supplied for this call (``dyn_embed_base.py:166-214``, ``recommendation/preprocess.py:26-46``): the
+        sequence is cut to its last ``max_seq_len`` items and unknown original ids become the pad id ``n_items``;
+        without one the user's cached sequence is used.  ``user_feats`` is accepted and ignored (no user features).
+        The vector scores ``I[:n_items]`` with the pseudo bias, then the consumed filter (none for the unknown user)
+        and top-K select.  The model's tables are not touched."""
+        from .dynamic_feats import build_rec_seq
+
+        if n_rec > self.n_items:
+            raise ValueError(f"`n_rec` {n_rec} exceeds num of items {self.n_items}")
+        u = int(user_id)
+        if seq is not None and len(seq) > 0:
+            row, ln = build_rec_seq(seq, self.n_items, self.T, getattr(data_info, "item2id", None), inner_id)
+            v = self.user_vectors([u], row, ln)
+        else:
+            v = self.user_vectors([u])
+        return self._dynamic_topk(v, u, n_rec, data_info, filter_consumed, return_scores)
+
+    def _dynamic_topk(self, v, u, n_rec, data_info, filter_consumed, return_scores):
+        """The scoring tail of ``recommend_dynamic``: the user vector ``v`` [1, d] with the pseudo bias 1 appended
+        scores ``[I | b]`` over ``I[:n_items]``, then the consumed filter of user ``u`` and top-K select."""
+        torch = self._torch
+        dev = self.device
+        if self._I is None:
+            self._I = _dyn_item_rows(self.item_embeds, self.item_biases, self.norm_embed).contiguous()
+        q = torch.cat([v, torch.ones((1, 1), dtype=torch.float32, device=dev)], dim=1).contiguous()
+        N, d = self.n_items, q.shape[1]
+        scores = torch.empty((1, N), dtype=torch.float32, device=dev)
+        zero = torch.zeros(1, dtype=torch.int64, device=dev)
+        _lib.check(_lib.lib.b200_score_rows_f32(_lib.ptr(q), q.stride(0), _lib.ptr(zero), 1, _lib.ptr(self._I),
+                                                self._I.stride(0), N, d, _lib.ptr(scores), scores.stride(0),
+                                                _lib.current_stream()))
+        consumed = getattr(data_info, "user_consumed", None)
+        owner = _ConsumedOwner(consumed, self.n_users, self.n_items, dev)
+        out_ids = torch.empty((1, n_rec), dtype=torch.int64, device=dev)
+        out_sc = torch.empty((1, n_rec), dtype=torch.float32, device=dev)
+        uid = torch.tensor([u], dtype=torch.int64, device=dev)
+        masked_topk(owner, scores, uid, n_rec, filter_consumed, out_ids, out_sc)
+        ids = out_ids.cpu().numpy()
+        return (ids, out_sc.cpu().numpy()) if return_scores else ids
+
+
 RNN_MAX_T, RNN_MAX_DIM, RNN_MAX_LAYERS = 128, 256, 4     # the envelope of b200_rnn_encode
 
 
-class RNN4Rec:
+class RNN4Rec(_DynEmbedSeqModel):
     """libreco/algorithms/rnn4rec.py:151-237 (inference) + the serving step of ``DynEmbedBase``
-    (``bases/dyn_embed_base.py:166-269``).  The user vector is ``tf_dense(embed_size)(rnn(seq_embeds[seq]))``
-    (optionally L2-normalised): ``b200_rnn_encode`` runs the stacked GRU / LSTM over each user's recent sequence
-    (``recent_sequences``: right-padded with ``n_items``, len 0 for no history) and :func:`linear` the head.  The
-    item side is ``[item_embeds | item_bias]`` and the user side gets the pseudo bias 1, so all-items retrieval is
-    the embed scorer on d = embed_size + 1.  ``weights``: the dict of ``weights_io.rnn4rec_weights`` (or the raw
-    variables it takes).  RNN4Rec has no user table and no user features."""
+    (:class:`_DynEmbedSeqModel`).  The user vector is ``tf_dense(embed_size)(rnn(seq_embeds[seq]))`` (optionally
+    L2-normalised): ``b200_rnn_encode`` runs the stacked GRU / LSTM over each user's recent sequence (len 0 for no
+    history) and :func:`linear` the head, so d = embed_size.  ``weights``: the dict of ``weights_io.rnn4rec_weights``
+    (or the raw variables it takes).  RNN4Rec has no user table and no user features: users with the same sequence
+    get the same vector."""
+
+    NAME = "RNN4Rec"
+    READS_LENS = True
 
     def __init__(self, data_info_or_spec, weights, recent_seqs, recent_seq_lens, norm_embed=False, device=None):
-        import torch
-
         from .weights_io import rnn4rec_weights
 
-        self._torch = torch
         if "rnn_scheme" in weights:
             weights = rnn4rec_weights(weights)
-        g = (data_info_or_spec.get if isinstance(data_info_or_spec, dict)
-             else lambda k: getattr(data_info_or_spec, k))
-        self.n_users, self.n_items = int(g("n_users")), int(g("n_items"))
-        self.device = torch.device(device) if device is not None else _lib.require_cuda()
-        self.norm_embed = bool(norm_embed)
+        super().__init__(data_info_or_spec, weights, recent_seqs, recent_seq_lens, norm_embed, device)
+
+    def _check_weights(self, weights, recent_seqs):
         layers = weights["rnn_layers"]
         self.in_dim = int(np.shape(weights["seq_embeds"])[1])
         self.hidden = [int(np.shape(lw["U"])[0]) for lw in layers]
-        self.T = int(np.shape(recent_seqs)[1])
+        self.K = int(np.shape(weights["dense_kernel"])[1])
         if not 1 <= self.T <= RNN_MAX_T:
             raise ValueError(f"RNN4Rec: max_seq_len {self.T} outside [1, {RNN_MAX_T}]")
         if not 1 <= len(layers) <= RNN_MAX_LAYERS:
@@ -1454,19 +1598,10 @@ class RNN4Rec:
                                  "packed floats")
             packed.append(flat)
             d = H
-        f32 = torch.float32
-        self.rnn_w = _dev(np.concatenate(packed), self.device, f32)
         self.kinds = (ctypes.c_int32 * len(layers))(*[int(lw["kind"]) for lw in layers])
         self.hid = (ctypes.c_int32 * len(layers))(*self.hidden)
         self.acts = (ctypes.c_int32 * len(layers))(*[int(lw["act"]) for lw in layers])
-        self.seq_embeds = _dev(weights["seq_embeds"], self.device, f32)          # [n_items + 1, in_dim]
-        self.dense_Wt = _dev(np.asarray(weights["dense_kernel"]).T, self.device, f32)    # [K, H_last]
-        self.dense_b = _dev(np.asarray(weights["dense_bias"]).reshape(-1), self.device, f32)
-        self.K = int(self.dense_Wt.shape[0])
-        self.item_embeds = _dev(weights["item_embeds"], self.device, f32)        # [n_items, K]
-        self.item_biases = _dev(np.asarray(weights["item_biases"]).reshape(-1), self.device, f32)
-        self.seqs = _dev(recent_seqs, self.device, torch.int32)
-        self.lens = _dev(np.asarray(recent_seq_lens).reshape(-1), self.device, torch.int32)
+        return {"rnn_w": np.concatenate(packed)}
 
     def encode(self, ids_d, seqs=None, lens=None):
         """[n, H_last]: ``b200_rnn_encode`` of the rows ``ids_d`` (device int64) of ``seqs`` / ``lens`` (default: the
@@ -1482,105 +1617,23 @@ class RNN4Rec:
             _lib.ptr(self.rnn_w), _lib.ptr(h), h.stride(0), _lib.current_stream()))
         return h
 
-    def user_vectors(self, ids, seqs=None, lens=None):
-        """[n, embed_size] user vectors of the rows ``ids`` of the recent sequences, or of the supplied ``seqs``
-        [*, T] / ``lens`` (host or device) when given: the encoder, the Dense head, then the L2 normalisation with
-        ``norm_embed``.  A row's bits depend only on its own sequence."""
-        torch = self._torch
-        ids_d = torch.as_tensor(np.asarray(ids, dtype=np.int64)).to(self.device)
-        if (seqs is None) != (lens is None):
-            raise ValueError("give both `seqs` and `lens`, or neither")
-        if seqs is not None:
-            seqs = _dev(seqs, self.device, torch.int32)
-            lens = _dev(np.asarray(lens).reshape(-1) if not isinstance(lens, torch.Tensor) else lens.reshape(-1),
-                        self.device, torch.int32)
-            if seqs.shape[1] != self.T:
-                raise ValueError(f"`seqs` has {seqs.shape[1]} columns, the model's max_seq_len is {self.T}")
-        x = linear(self.encode(ids_d, seqs, lens), self.dense_Wt, self.dense_b, ACT_NONE, impl="f32")
-        if self.norm_embed:
-            _lib.check(_lib.lib.b200_l2_normalize_rows(_lib.ptr(x), x.stride(0), x.shape[0], x.shape[1],
-                                                       _lib.current_stream()))
-        return x
-
-    def set_embeddings(self, chunk=1 << 20):
-        """Device tensors ``U [n_users + 1, K + 1]`` (pseudo bias 1 in the last column, last row = mean OOV row) and
-        ``I [n_items + 1, K + 1]`` (``[item_embeds | item_biases]`` + the mean row) for :class:`engine.EmbedScorer`."""
-        torch = self._torch
-        rows = [self.user_vectors(np.arange(i, min(self.n_users, i + chunk))) for i in range(0, self.n_users, chunk)]
-        return dyn_embed_tables(torch.cat(rows, dim=0), self.item_embeds, self.item_biases, self.norm_embed)
-
-    def recommend_dynamic(self, user_id, n_rec, data_info, user_feats=None, seq=None, filter_consumed=True,
-                          inner_id=False, return_scores=False):
-        """``recommend_user`` for ONE user with an optional behaviour sequence supplied for this call
-        (``dyn_embed_base.py:166-214``, ``recommendation/preprocess.py:26-46``): the sequence is cut to its last
-        ``max_seq_len`` items, unknown original ids become the pad id ``n_items``, and it is encoded once; without
-        one the user's cached sequence is used.  ``user_feats`` is accepted and ignored (the model has no user
-        features).  The vector scores ``I[:n_items]`` with the pseudo bias and the consumed filter (none for the
-        unknown user ``n_users``) and top-K select.  The model's sequence table is not touched."""
-        from .dynamic_feats import build_rec_seq
-
-        if n_rec > self.n_items:
-            raise ValueError(f"`n_rec` {n_rec} exceeds num of items {self.n_items}")
-        u = int(user_id)
-        if seq is not None and len(seq) > 0:
-            row, ln = build_rec_seq(seq, self.n_items, self.T, getattr(data_info, "item2id", None), inner_id)
-            v = self.user_vectors([0], row, ln)
-        else:
-            v = self.user_vectors([u])
-        return _dynamic_topk(self, v, u, n_rec, data_info, filter_consumed, return_scores)
-
-
-def _dynamic_topk(model, v, u, n_rec, data_info, filter_consumed, return_scores):
-    """The scoring tail of ``recommend_dynamic`` for the ``DynEmbedBase`` sequence models: the user vector ``v``
-    [1, d] with the pseudo bias 1 appended scores ``[I | b]`` (``model.item_embeds`` / ``item_biases``, normalised
-    with ``model.norm_embed``; cached on the model) over ``I[:n_items]``, then the consumed filter of user ``u``
-    (none for the unknown user ``n_users``) and top-K select."""
-    import torch
-
-    dev = model.device
-    if not hasattr(model, "_I"):
-        model._I = _dyn_item_rows(model.item_embeds, model.item_biases, model.norm_embed).contiguous()
-    q = torch.cat([v, torch.ones((1, 1), dtype=torch.float32, device=dev)], dim=1).contiguous()
-    N, d = model.n_items, q.shape[1]
-    scores = torch.empty((1, N), dtype=torch.float32, device=dev)
-    zero = torch.zeros(1, dtype=torch.int64, device=dev)
-    _lib.check(_lib.lib.b200_score_rows_f32(_lib.ptr(q), q.stride(0), _lib.ptr(zero), 1, _lib.ptr(model._I),
-                                            model._I.stride(0), N, d, _lib.ptr(scores), scores.stride(0),
-                                            _lib.current_stream()))
-    consumed = getattr(data_info, "user_consumed", None)
-    owner = _ConsumedOwner(consumed, model.n_users, model.n_items, dev)
-    out_ids = torch.empty((1, n_rec), dtype=torch.int64, device=dev)
-    out_sc = torch.empty((1, n_rec), dtype=torch.float32, device=dev)
-    uid = torch.tensor([u], dtype=torch.int64, device=dev)
-    masked_topk(owner, scores, uid, n_rec, filter_consumed, out_ids, out_sc)
-    ids = out_ids.cpu().numpy()
-    return (ids, out_sc.cpu().numpy()) if return_scores else ids
+    def _features(self, ids_d, rows_d, seqs, lens):
+        return linear(self.encode(rows_d, seqs, lens), self.dense_Wt, self.dense_b, ACT_NONE, impl="f32")
 
 
 CONV_MAX_T, CONV_MAX_K, CONV_MAX_FILTERS, CONV_MAX_F, CONV_MAX_LAYERS = 64, 128, 32, 128, 16   # b200_*_encode envelope
 
 
-class _ConvSeqModel:
-    """What Caser and WaveNet share (``bases/dyn_embed_base.py:166-283``, ``recommendation/preprocess.py:26-46``):
-    the user vector ``[user_embeds[u] | head(encoder(seq_embeds[seq]))]`` (2K wide, L2-normalised as a whole with
-    ``norm_embed``), where the encoder is the subclass's kernel over the user's recent sequence (right-padded with
-    ``n_items``; the pad positions are ordinary rows, neither model masks by length) and the Dense head runs on
-    :func:`linear`; the item side is ``[item_embeds (2K) | item_bias]`` and the user side gets the pseudo bias 1, so
-    all-items retrieval is the embed scorer on d = 2K + 1.  The user table's last row ``n_users`` is the unknown
-    user's: ``set_embeddings`` first sets it to the mean of the other rows (``_assign_user_oov``)."""
+class _ConvSeqModel(_DynEmbedSeqModel):
+    """What Caser and WaveNet add to :class:`_DynEmbedSeqModel`: a user table.  The user vector is
+    ``[user_embeds[u] | head(encoder(seq_embeds[seq]))]`` (d = 2K), where the encoder is the subclass's kernel (the
+    pad positions are ordinary rows, neither model masks by length).  The user table's last row ``n_users`` is the
+    unknown user's: ``set_embeddings`` first sets it to the mean of the other rows (``_assign_user_oov``), and a cold
+    and a warm user with the same sequence get different vectors."""
 
-    NAME = ""
     HEAD_ACT = ACT_NONE
 
-    def __init__(self, data_info_or_spec, weights, recent_seqs, recent_seq_lens, norm_embed=False, device=None):
-        import torch
-
-        self._torch = torch
-        g = (data_info_or_spec.get if isinstance(data_info_or_spec, dict)
-             else lambda k: getattr(data_info_or_spec, k))
-        self.n_users, self.n_items = int(g("n_users")), int(g("n_items"))
-        self.norm_embed = bool(norm_embed)
-        self.T = int(np.shape(recent_seqs)[1])
+    def _check_weights(self, weights, recent_seqs):
         self.K = int(np.shape(weights["seq_embeds"])[1])
         if not 1 <= self.T <= CONV_MAX_T:
             raise ValueError(f"{self.NAME}: max_seq_len {self.T} outside [1, {CONV_MAX_T}]")
@@ -1595,17 +1648,7 @@ class _ConvSeqModel:
             raise ValueError(f"{self.NAME}: {np.shape(recent_seqs)[0]} recent sequences for {self.n_users} users + "
                              "the OOV row")
         self._check_encoder(weights)
-        self.device = torch.device(device) if device is not None else _lib.require_cuda()
-        f32 = torch.float32
-        self.user_embeds = _dev(weights["user_embeds"], self.device, f32)       # [n_users + 1, K]
-        self.seq_embeds = _dev(weights["seq_embeds"], self.device, f32)         # [n_items + 1, K]
-        self.item_embeds = _dev(weights["item_embeds"], self.device, f32)       # [n_items, 2K]
-        self.item_biases = _dev(np.asarray(weights["item_biases"]).reshape(-1), self.device, f32)
-        self.conv_w = _dev(weights["conv"], self.device, f32)
-        self.dense_Wt = _dev(np.asarray(weights["dense_kernel"]).T, self.device, f32)    # [K, D]
-        self.dense_b = _dev(np.asarray(weights["dense_bias"]).reshape(-1), self.device, f32)
-        self.seqs = _dev(recent_seqs, self.device, torch.int32)
-        self.lens = _dev(np.asarray(recent_seq_lens).reshape(-1), self.device, torch.int32)   # kept, never read
+        return {"user_embeds": weights["user_embeds"], "conv_w": weights["conv"]}
 
     def _check_encoder(self, weights):
         raise NotImplementedError
@@ -1622,67 +1665,19 @@ class _ConvSeqModel:
         self._encode_into(rows_d, seqs, out)
         return out
 
-    def user_vectors(self, ids, seqs=None, lens=None):
-        """[n, 2K] user vectors of the users ``ids`` (0..n_users; n_users is the unknown user): the user table row
-        beside the encoded sequence, which is the user's recent sequence or, when given, row i of ``seqs`` [n, T]
-        (host or device) for ``ids[i]``; then the L2 normalisation with ``norm_embed``.  ``lens`` is accepted and
-        not read: neither graph masks by length.  A row's bits depend only on its own user row and sequence."""
-        torch = self._torch
-        ids = np.asarray(ids, dtype=np.int64).reshape(-1)
-        n, K = int(ids.size), self.K
-        if n and (ids.min() < 0 or ids.max() > self.n_users):
-            raise ValueError(f"{self.NAME}: user ids must lie in [0, {self.n_users}]")
-        ids_d = torch.as_tensor(ids).to(self.device)
-        rows_d = ids_d
-        if seqs is not None:
-            seqs = _dev(seqs, self.device, torch.int32)
-            if tuple(seqs.shape) != (n, self.T):
-                raise ValueError(f"`seqs` has shape {tuple(seqs.shape)}, expected ({n}, {self.T})")
-            rows_d = torch.arange(n, dtype=torch.int64, device=self.device)
-        x = torch.empty((n, 2 * K), dtype=torch.float32, device=self.device)
-        if n == 0:
-            return x
+    def _features(self, ids_d, rows_d, seqs, lens):
+        n, K = int(ids_d.numel()), self.K
+        x = self._torch.empty((n, 2 * K), dtype=self._torch.float32, device=self.device)
         _lib.check(_lib.lib.b200_gather_rows(_lib.ptr(self.user_embeds), self.user_embeds.stride(0), K,
                                              _lib.ptr(ids_d), n, _lib.ptr(x), x.stride(0), _lib.current_stream()))
         x[:, K:] = linear(self.encode(rows_d, seqs), self.dense_Wt, self.dense_b, self.HEAD_ACT, impl="f32")
-        if self.norm_embed:
-            _lib.check(_lib.lib.b200_l2_normalize_rows(_lib.ptr(x), x.stride(0), n, x.shape[1],
-                                                       _lib.current_stream()))
         return x
 
     def assign_user_oov(self):
         """``_assign_user_oov`` (dyn_embed_base.py:271-283): the unknown user's row := mean of the known rows."""
         self.user_embeds[self.n_users] = self.user_embeds[:self.n_users].mean(dim=0)
 
-    def set_embeddings(self, chunk=1 << 20):
-        """Assigns the OOV user row, then returns device tensors ``U [n_users + 1, 2K + 1]`` (pseudo bias 1 in the
-        last column, last row = the mean row) and ``I [n_items + 1, 2K + 1]`` (``[item_embeds | item_biases]`` + the
-        mean row) for :class:`engine.EmbedScorer`."""
-        torch = self._torch
-        self.assign_user_oov()
-        rows = [self.user_vectors(np.arange(i, min(self.n_users, i + chunk))) for i in range(0, self.n_users, chunk)]
-        return dyn_embed_tables(torch.cat(rows, dim=0), self.item_embeds, self.item_biases, self.norm_embed)
-
-    def recommend_dynamic(self, user_id, n_rec, data_info, user_feats=None, seq=None, filter_consumed=True,
-                          inner_id=False, return_scores=False):
-        """``recommend_user`` for ONE user (inner id; ``n_users`` = the unknown user, whose table row is the mean row
-        once ``set_embeddings`` ran) with an optional behaviour sequence supplied for this call
-        (``dyn_embed_base.py:166-214``, ``recommendation/preprocess.py:26-46``): the sequence is cut to its last
-        ``max_seq_len`` items and unknown original ids become the pad id ``n_items``; without one the user's cached
-        sequence is used.  The user's own table row always goes beside it, so a cold and a warm user with the same
-        sequence get different vectors.  ``user_feats`` is accepted and ignored (no user features).  The model's
-        tables are not touched."""
-        from .dynamic_feats import build_rec_seq
-
-        if n_rec > self.n_items:
-            raise ValueError(f"`n_rec` {n_rec} exceeds num of items {self.n_items}")
-        u = int(user_id)
-        if seq is not None and len(seq) > 0:
-            row, _ = build_rec_seq(seq, self.n_items, self.T, getattr(data_info, "item2id", None), inner_id)
-            v = self.user_vectors([u], row)
-        else:
-            v = self.user_vectors([u])
-        return _dynamic_topk(self, v, u, n_rec, data_info, filter_consumed, return_scores)
+    _before_set_embeddings = assign_user_oov
 
 
 class Caser(_ConvSeqModel):

@@ -198,7 +198,7 @@ def default_tf_names(model_name, n_hidden, use_bn, use_tf_attention=False, n_lay
     i = 0..T-1 under ``convs``, the vertical ``conv1d_T`` under ``vertical``, the head ``dense/{kernel,bias}:0``.
     WaveNet (wave_net.py:198-221; `n_layers` = n_blocks * n_layers_per_block): the causal ``conv1d[_i]`` under
     ``convs``, the 1x1 ``conv1d_{n_layers}`` under ``out_conv``, the head ``dense``.  Both also use the four
-    ``CONV_TABLES``.
+    ``CONV_TABLE_KEYS`` of ``DYN_EMBED_TABLES``.
 
     RNN4Rec (rnn4rec.py:151-237 with layers/recurrent.py:4-63; `n_layers` = len(hidden_units)): "keras" layer i is
     ``{t}[_i]/{t}_cell/{kernel,recurrent_kernel,bias}:0`` (t = gru or lstm) plus, with `use_layer_norm`,
@@ -410,11 +410,20 @@ def transformer_tf_variables(raw):
     return out
 
 
-YOUTUBE_RETRIEVAL_TABLES = {
-    "seq_embeds": "embedding/seq_embeds_var:0", "item_embeds": "embedding/item_embeds_var:0",
-    "item_biases": "embedding/item_bias_var:0", "sparse_embeds": "embedding/sparse_embeds_var:0",
-    "dense_embeds": "embedding/dense_embeds_var:0",
-}
+# the embedding-scope tables of the DynEmbedBase models (YouTubeRetrieval, RNN4Rec, Caser, WaveNet)
+DYN_EMBED_TABLES = {"user_embeds": "embedding/user_embeds_var:0", "seq_embeds": "embedding/seq_embeds_var:0",
+                    "item_embeds": "embedding/item_embeds_var:0", "item_biases": "embedding/item_bias_var:0",
+                    "sparse_embeds": "embedding/sparse_embeds_var:0", "dense_embeds": "embedding/dense_embeds_var:0"}
+
+
+def _dyn_embed_tf_variables(w, keys):
+    """``{TF variable name: float32 array}`` of the tables ``keys`` that ``w`` holds; ``item_biases`` written flat."""
+    out = {}
+    for k in keys:
+        if w.get(k) is not None:
+            a = np.asarray(w[k], dtype=np.float32)
+            out[DYN_EMBED_TABLES[k]] = a.reshape(-1) if k == "item_biases" else a
+    return out
 
 
 def youtube_retrieval_tf_variables(w):
@@ -423,9 +432,7 @@ def youtube_retrieval_tf_variables(w):
     of ``youtube_retrieval.py:194-260`` (``seq_embeds_var`` [n_items, K], ``item_embeds_var`` [n_items, H],
     ``item_bias_var`` [n_items], ``sparse_embeds_var``, ``dense_embeds_var``) and the user tower's ``mlp`` dense_nn
     stack.  The inverse of ``load_reference_tf_model(..., "YouTubeRetrieval", ...)``."""
-    out = {name: np.asarray(w[k], dtype=np.float32) for k, name in YOUTUBE_RETRIEVAL_TABLES.items()
-           if w.get(k) is not None}
-    out[YOUTUBE_RETRIEVAL_TABLES["item_biases"]] = out[YOUTUBE_RETRIEVAL_TABLES["item_biases"]].reshape(-1)
+    out = _dyn_embed_tf_variables(w, ("seq_embeds", "item_embeds", "item_biases", "sparse_embeds", "dense_embeds"))
     mlp = w["mlp"]
     return _put_tf_names(out, _mlp_names("mlp", len(mlp["kernels"]), mlp.get("bn_in") is not None), mlp)
 
@@ -433,11 +440,10 @@ def youtube_retrieval_tf_variables(w):
 def _youtube_retrieval_weights(npz, n_hidden, use_bn, extra_names=None):
     """Engine weight dict of a saved YouTubeRetrieval: every name and shape checked (``KeyError`` naming the
     variable and listing what the file holds)."""
-    seq = resolve_tf_names(npz, YOUTUBE_RETRIEVAL_TABLES["seq_embeds"])
+    seq = resolve_tf_names(npz, DYN_EMBED_TABLES["seq_embeds"])
     n_items, K = seq.shape if seq.ndim == 2 else (None, None)
     if n_items is None:
-        raise KeyError(f"TF variable `{YOUTUBE_RETRIEVAL_TABLES['seq_embeds']}` has shape {seq.shape}, expected "
-                       f"[n_items, K]")
+        raise KeyError(f"TF variable `{DYN_EMBED_TABLES['seq_embeds']}` has shape {seq.shape}, expected [n_items, K]")
     names = {"mlp": _mlp_names("mlp", n_hidden, use_bn)}
     names.update(extra_names or {})
     mlp = resolve_tf_names(npz, names)["mlp"]
@@ -452,17 +458,15 @@ def _youtube_retrieval_weights(npz, n_hidden, use_bn, extra_names=None):
     w = resolve_tf_names(npz, names, shapes)
     tables = {"seq_embeds": (n_items, K), "item_embeds": (n_items, H), "item_biases": (n_items,)}
     for k in ("sparse_embeds", "dense_embeds"):
-        if YOUTUBE_RETRIEVAL_TABLES[k] in npz:
+        if DYN_EMBED_TABLES[k] in npz:
             tables[k] = (None, K)
-    w.update(resolve_tf_names(npz, {k: YOUTUBE_RETRIEVAL_TABLES[k] for k in tables}, tables))
+    w.update(resolve_tf_names(npz, {k: DYN_EMBED_TABLES[k] for k in tables}, tables))
     if np.shape(mlp["kernels"][0])[0] % K:
         raise KeyError(f"TF variable `{names['mlp']['kernels'][0]}` has {np.shape(mlp['kernels'][0])[0]} input rows, "
                        f"not a multiple of K = {K}")
     return w
 
 
-RNN4REC_TABLES = {"seq_embeds": "embedding/seq_embeds_var:0", "item_embeds": "embedding/item_embeds_var:0",
-                  "item_biases": "embedding/item_bias_var:0"}
 RNN_CELL_KINDS = {"gru_reset_after": 0, "gru_reset_before": 1, "lstm": 2}   # cell kinds of b200_rnn_encode
 RNN_ACT_TANH, RNN_ACT_LN_TANH = 0, 1
 
@@ -599,10 +603,7 @@ def rnn4rec_weights(raw):
     ``seq_embeds`` [n_items+1, hidden_units[0]], ``item_embeds`` [n_items, K], ``item_biases`` [n_items],
     ``rnn_scheme``, ``rnn_type``, ``use_layer_norm``, ``rnn_layers`` (per layer, as :func:`default_tf_names` names
     them), ``dense_kernel`` [H_last, K] and ``dense_bias`` [K]."""
-    w = {k: np.asarray(raw[k], dtype=np.float32) for k in ("seq_embeds", "item_embeds", "item_biases", "dense_kernel",
-                                                             "dense_bias")}
-    w["item_biases"] = w["item_biases"].reshape(-1)
-    w["dense_bias"] = w["dense_bias"].reshape(-1)
+    w = _seq_model_tables(raw, ("seq_embeds", "item_embeds", "item_biases"))
     w["rnn_layers"] = rnn_layers(raw["rnn_layers"], raw["rnn_scheme"], raw["rnn_type"], w["seq_embeds"].shape[1],
                                  bool(raw.get("use_layer_norm", False)))
     return w
@@ -614,8 +615,7 @@ def rnn4rec_tf_variables(raw):
     the inverse of ``load_reference_tf_model(..., "RNN4Rec", ...)``."""
     names = default_tf_names("RNN4Rec", None, False, n_layers=len(raw["rnn_layers"]), scheme=raw["rnn_scheme"],
                              rnn_type=raw["rnn_type"], use_layer_norm=bool(raw.get("use_layer_norm", False)))
-    out = {name: np.asarray(raw[k], dtype=np.float32) for k, name in RNN4REC_TABLES.items()}
-    out[RNN4REC_TABLES["item_biases"]] = out[RNN4REC_TABLES["item_biases"]].reshape(-1)
+    out = _dyn_embed_tf_variables(raw, ("seq_embeds", "item_embeds", "item_biases"))
     _put_tf_names(out, names["rnn_layers"], raw["rnn_layers"])
     out[names["dense_kernel"]] = np.asarray(raw["dense_kernel"], dtype=np.float32)
     out[names["dense_bias"]] = np.asarray(raw["dense_bias"], dtype=np.float32).reshape(-1)
@@ -629,22 +629,21 @@ def _rnn4rec_raw(npz, rnn_type, hidden_units, use_layer_norm, extra_names=None):
     names = default_tf_names("RNN4Rec", None, False, n_layers=len(hidden_units), scheme=scheme, rnn_type=rnn_type,
                              use_layer_norm=use_layer_norm)
     names.update(extra_names or {})
-    item = resolve_tf_names(npz, RNN4REC_TABLES["item_embeds"])
+    item = resolve_tf_names(npz, DYN_EMBED_TABLES["item_embeds"])
     if item.ndim != 2:
-        raise KeyError(f"TF variable `{RNN4REC_TABLES['item_embeds']}` has shape {item.shape}, expected [n_items, K]")
+        raise KeyError(f"TF variable `{DYN_EMBED_TABLES['item_embeds']}` has shape {item.shape}, expected [n_items, K]")
     n_items, K = item.shape
     tables = {"seq_embeds": (n_items + 1, hidden_units[0]), "item_embeds": (n_items, K), "item_biases": (n_items,)}
-    raw = resolve_tf_names(npz, {k: RNN4REC_TABLES[k] for k in tables}, tables)
+    raw = resolve_tf_names(npz, {k: DYN_EMBED_TABLES[k] for k in tables}, tables)
     raw.update(resolve_tf_names(npz, names, rnn4rec_tf_shapes(scheme, rnn_type, hidden_units[0], hidden_units,
                                                               use_layer_norm, K)))
     raw.update(rnn_scheme=scheme, rnn_type=rnn_type, use_layer_norm=bool(use_layer_norm and scheme == "keras"))
     return raw
 
 
-# Caser / WaveNet (caser.py:162-221, wave_net.py:166-222): the four embedding-scope tables, then auto-named Conv1D
+# Caser / WaveNet (caser.py:162-221, wave_net.py:166-222): four embedding-scope tables, then auto-named Conv1D
 # layers and the Dense head.  The names restate TensorFlow's naming rule and are unverified against a saved model.
-CONV_TABLES = {"user_embeds": "embedding/user_embeds_var:0", "seq_embeds": "embedding/seq_embeds_var:0",
-               "item_embeds": "embedding/item_embeds_var:0", "item_biases": "embedding/item_bias_var:0"}
+CONV_TABLE_KEYS = ("user_embeds", "seq_embeds", "item_embeds", "item_biases")
 
 
 def _conv_names(model_name, n_conv):
@@ -679,8 +678,9 @@ def wavenet_dilations(n_blocks, n_layers_per_block, dilated=True):
     return [2 ** i if dilated else 1 for _ in range(int(n_blocks)) for i in range(int(n_layers_per_block))]
 
 
-def _conv_tables(raw):
-    w = {k: np.asarray(raw[k], dtype=np.float32) for k in CONV_TABLES}
+def _seq_model_tables(raw, keys):
+    """The tables ``keys`` (``item_biases`` flat) and the Dense head of a sequence model's raw variables, float32."""
+    w = {k: np.asarray(raw[k], dtype=np.float32) for k in keys}
     w["item_biases"] = w["item_biases"].reshape(-1)
     w["dense_kernel"] = np.asarray(raw["dense_kernel"], dtype=np.float32)
     w["dense_bias"] = np.asarray(raw["dense_bias"], dtype=np.float32).reshape(-1)
@@ -694,7 +694,7 @@ def caser_weights(raw):
     f32 = lambda a: np.asarray(a, dtype=np.float32)      # noqa: E731
     convs, vert = raw["convs"], raw["vertical"]
     T, nh, nv = len(convs), int(np.shape(convs[0]["bias"])[-1]), int(np.shape(vert["bias"])[-1])
-    w = _conv_tables(raw)
+    w = _seq_model_tables(raw, CONV_TABLE_KEYS)
     w["conv"] = np.concatenate([f32(c["kernel"]).reshape(-1) for c in convs] +
                                [f32(c["bias"]).reshape(-1) for c in convs] +
                                [f32(vert["kernel"]).reshape(-1), f32(vert["bias"]).reshape(-1)])
@@ -708,7 +708,7 @@ def wavenet_weights(raw):
     head): ``conv`` packs them as ``b200_wavenet_encode`` reads them, per layer W then b, then W1, b1."""
     f32 = lambda a: np.asarray(a, dtype=np.float32).reshape(-1)      # noqa: E731
     parts = [f32(c[k]) for c in raw["convs"] + [raw["out_conv"]] for k in ("kernel", "bias")]
-    w = _conv_tables(raw)
+    w = _seq_model_tables(raw, CONV_TABLE_KEYS)
     w["conv"] = np.concatenate(parts)
     dil = [int(d) for d in raw["dilations"]]
     if len(dil) != len(raw["convs"]):
@@ -722,9 +722,7 @@ def _conv_tf_variables(raw):
     name: array}``: what ``save_tf_variables`` writes, and the inverse of ``load_reference_tf_model``."""
     model = "Caser" if "vertical" in raw else "WaveNet"
     names = _conv_names(model, len(raw["convs"]))
-    out = {n: np.asarray(raw[k], dtype=np.float32) for k, n in CONV_TABLES.items()}
-    out[CONV_TABLES["item_biases"]] = out[CONV_TABLES["item_biases"]].reshape(-1)
-    return _put_tf_names(out, names, raw)
+    return _put_tf_names(_dyn_embed_tf_variables(raw, CONV_TABLE_KEYS), names, raw)
 
 
 # the dilations of WaveNet are not variables: the loader takes them as arguments
@@ -737,9 +735,9 @@ def _conv_raw(npz, model_name, n_filters=None, n_blocks=None, n_layers_per_block
     kernel ``conv1d_{T}`` [1, T, nv]: the one layer whose index equals its kernel's T; nh and nv come off the first
     and the vertical bias.  WaveNet's graph (``n_filters``, ``n_blocks``, ``n_layers_per_block``, ``dilated``) is
     taken as arguments: the file does not tell the TF1 graph (dilation 1) from the TF2 one."""
-    tab = resolve_tf_names(npz, {"user_embeds": CONV_TABLES["user_embeds"], "item_embeds": CONV_TABLES["item_embeds"]})
+    tab = resolve_tf_names(npz, {k: DYN_EMBED_TABLES[k] for k in ("user_embeds", "item_embeds")})
     if tab["user_embeds"].ndim != 2 or tab["item_embeds"].ndim != 2:
-        raise KeyError(f"`{CONV_TABLES['user_embeds']}` / `{CONV_TABLES['item_embeds']}` must be 2-D")
+        raise KeyError(f"`{DYN_EMBED_TABLES['user_embeds']}` / `{DYN_EMBED_TABLES['item_embeds']}` must be 2-D")
     (nu1, K), n_items = tab["user_embeds"].shape, tab["item_embeds"].shape[0]
     if model_name == "Caser":
         T = None
@@ -760,7 +758,8 @@ def _conv_raw(npz, model_name, n_filters=None, n_blocks=None, n_layers_per_block
         names = _conv_names("WaveNet", len(dil))
         shapes = conv_tf_shapes("WaveNet", nu1 - 1, n_items, K, F=F, n_conv=len(dil))
     names.update(extra_names or {})
-    raw = resolve_tf_names(npz, {k: CONV_TABLES[k] for k in CONV_TABLES}, {k: shapes[k] for k in CONV_TABLES})
+    raw = resolve_tf_names(npz, {k: DYN_EMBED_TABLES[k] for k in CONV_TABLE_KEYS},
+                           {k: shapes[k] for k in CONV_TABLE_KEYS})
     raw.update(resolve_tf_names(npz, names, {k: shapes[k] for k in names}))
     if model_name == "WaveNet":
         raw["dilations"] = dil

@@ -397,6 +397,7 @@ def test_youtube_retrieval_user_vectors_and_retrieval(norm, n_rows):
     """SURVEY 8f-4 adjacent model: YouTubeRetrieval's user tower (sqrtn-pooled history + user features, K1 without an
     id field, both the small-batch and the pipelined large-batch kernels) against the numpy restatement, then all-items
     retrieval through the embed scorer with the reference's pseudo-bias column."""
+    from librecommender_b200 import _lib
     from librecommender_b200.engine import EmbedScorer
     from librecommender_b200.feat_models import YouTubeRetrieval, recent_sequences
     from librecommender_b200.synthetic import _glorot, make_embeddings, make_mlp
@@ -413,6 +414,11 @@ def test_youtube_retrieval_user_vectors_and_retrieval(norm, n_rows):
     consumed = {u: rng.choice(n_items, size=int(rng.integers(1, 25)), replace=False).tolist() for u in range(n_users - 1)}
     seqs, lens = recent_sequences(consumed, n_users, n_items, T)          # the last user has no history
     model = YouTubeRetrieval(spec, w, seqs, lens, norm_embed=norm)
+    n0 = _lib.launch_count()
+    for bad in ([n_users + 1], [-1], [0, n_users + 7]):
+        with pytest.raises(ValueError, match="user ids"):
+            model.user_vectors(bad)
+    assert _lib.launch_count() == n0
     ids = np.arange(n_users)
     got = model.user_vectors(ids).cpu().numpy()
     ref = tm.youtube_retrieval_user_vectors(w, spec, ids, seqs, lens, norm, dtype=np.float64)

@@ -16,26 +16,17 @@ the data-sheet 3.35 TB/s.  The card name and power limit are read in the same ru
 import argparse
 import json
 import os
-import subprocess
 import sys
-import time
 
 import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
-FP32_PEAK = 67e12
-HBM_PEAK = 3.35e12
+from _profile_common import FP32_PEAK, HBM_PEAK, card, event_seconds, serving_times, write_report  # noqa: E402
 
 CASES = [("Caser", "default", dict(nh_filters=2, nv_filters=4)), ("Caser", "wide", dict(nh_filters=8, nv_filters=8)),
          ("WaveNet", "default", dict(n_filters=16, n_blocks=1, n_layers_per_block=4)),
          ("WaveNet", "wide", dict(n_filters=64, n_blocks=2, n_layers_per_block=4))]
-
-
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True)
-    return q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else "unknown"
 
 
 def algorithmic_flop(model, T, K, cfg):
@@ -52,7 +43,6 @@ def algorithmic_flop(model, T, K, cfg):
 def case(model_name, label, cfg, n_users, n_items, T, K, seqs, lens, chunk, reps):
     import torch
 
-    from librecommender_b200.engine import EmbedScorer
     from librecommender_b200.feat_models import Caser, WaveNet
     from librecommender_b200.synthetic import make_caser_weights, make_wavenet_weights
 
@@ -65,39 +55,19 @@ def case(model_name, label, cfg, n_users, n_items, T, K, seqs, lens, chunk, reps
         model = WaveNet({"n_users": n_users, "n_items": n_items}, raw, seqs, lens)
     del raw
     ids = torch.arange(min(chunk, n_users), dtype=torch.int64, device=model.device)
-    model.encode(ids)
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(reps):
-        model.encode(ids)
-    e1.record()
-    torch.cuda.synchronize()
-    sec = e0.elapsed_time(e1) / 1e3 / reps
+    sec = event_seconds(lambda: model.encode(ids), reps)
     n = ids.numel()
     enc_flop, head_flop, D = algorithmic_flop(model_name, T, K, cfg)
     flop = enc_flop * n
     nbytes = n * (4.0 * T * K + 4.0 * T + 4.0 * D)
-    t0 = time.perf_counter()
-    U, I = model.set_embeddings()
-    torch.cuda.synchronize()
-    set_sec = time.perf_counter() - t0
-    sc = EmbedScorer(U, I, n_items, None, n_users=n_users)
-    users = np.random.default_rng(2).integers(0, n_users, 32768)
-    sc.recommend(users[:1024], 100, False)
-    torch.cuda.synchronize()
-    t0 = time.perf_counter()
-    sc.recommend(users, 100, False)
-    torch.cuda.synchronize()
-    rec_sec = time.perf_counter() - t0
+    serving = serving_times(model, n_users, n_items)
     f_share, b_share = flop / sec / FP32_PEAK, nbytes / sec / HBM_PEAK
-    out = dict(model=model_name, case=label, T=T, config=cfg, pre_head_width=D, serving_width=int(U.shape[1]),
+    out = dict(model=model_name, case=label, T=T, config=cfg, pre_head_width=D,
+               serving_width=int(model.item_embeds.shape[1]) + 1,
                encode_users=n, encode_sec=sec, encode_users_per_s=n / sec, encoder_flop_per_user=enc_flop,
                head_flop_per_user=head_flop, flop_per_s=flop / sec, share_fp32_peak=f_share, bytes_per_s=nbytes / sec,
-               share_hbm_peak=b_share, bound="compute" if f_share >= b_share else "memory",
-               set_embeddings_sec=set_sec, set_embeddings_users_per_s=n_users / set_sec, recommend_users=len(users),
-               recommend_sec=rec_sec, recommend_users_per_s=len(users) / rec_sec)
-    del model, U, I, sc
+               share_hbm_peak=b_share, bound="compute" if f_share >= b_share else "memory", **serving)
+    del model
     torch.cuda.empty_cache()
     return out
 
@@ -125,12 +95,7 @@ def main():
             print(json.dumps(r), flush=True)
             res["cases"].append(r)
         del seqs, lens
-    line = json.dumps(res, indent=1)
-    print(line)
-    if args.out:
-        os.makedirs(os.path.dirname(args.out) or ".", exist_ok=True)
-        with open(args.out, "w") as f:
-            f.write(line)
+    write_report(res, args.out)
 
 
 if __name__ == "__main__":

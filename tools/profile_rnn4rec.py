@@ -12,28 +12,18 @@ against the data-sheet 3.35 TB/s.  The card name and power limit are read in the
 import argparse
 import json
 import os
-import subprocess
 import sys
-import time
 
 import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
-FP32_PEAK = 67e12
-HBM_PEAK = 3.35e12
-
-
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True)
-    return q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else "unknown"
+from _profile_common import FP32_PEAK, HBM_PEAK, card, event_seconds, serving_times, write_report  # noqa: E402
 
 
 def case(rnn_type, hidden, n_users, n_items, T, K, seqs, lens, chunk, reps):
     import torch
 
-    from librecommender_b200.engine import EmbedScorer
     from librecommender_b200.feat_models import RNN4Rec
     from librecommender_b200.synthetic import make_rnn4rec_weights
 
@@ -41,15 +31,7 @@ def case(rnn_type, hidden, n_users, n_items, T, K, seqs, lens, chunk, reps):
     raw = make_rnn4rec_weights(rng, n_items, K, hidden, rnn_type, False, "keras")
     model = RNN4Rec({"n_users": n_users, "n_items": n_items}, raw, seqs, lens)
     ids = torch.arange(min(chunk, n_users), dtype=torch.int64, device=model.device)
-    model.encode(ids)
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(reps):
-        model.encode(ids)
-    e1.record()
-    torch.cuda.synchronize()
-    sec = e0.elapsed_time(e1) / 1e3 / reps
+    sec = event_seconds(lambda: model.encode(ids), reps)
     n = ids.numel()
     valid = float(lens[:n].clip(0, T).sum())
     G = 3 if rnn_type == "gru" else 4
@@ -58,25 +40,12 @@ def case(rnn_type, hidden, n_users, n_items, T, K, seqs, lens, chunk, reps):
         flop += 2.0 * G * H * (d + H) * valid
         d = H
     nbytes = valid * hidden[0] * 4 + n * T * 4 + n * hidden[-1] * 4
-    t0 = time.perf_counter()
-    U, I = model.set_embeddings()
-    torch.cuda.synchronize()
-    set_sec = time.perf_counter() - t0
-    sc = EmbedScorer(U, I, n_items, None, n_users=n_users)
-    users = np.random.default_rng(2).integers(0, n_users, 32768)
-    sc.recommend(users[:1024], 100, False)
-    torch.cuda.synchronize()
-    t0 = time.perf_counter()
-    sc.recommend(users, 100, False)
-    torch.cuda.synchronize()
-    rec_sec = time.perf_counter() - t0
+    serving = serving_times(model, n_users, n_items)
     f_share, b_share = flop / sec / FP32_PEAK, nbytes / sec / HBM_PEAK
     out = dict(rnn_type=rnn_type, hidden_units=list(hidden), encode_users=n, encode_sec=sec, encode_users_per_s=n / sec,
                flop_per_s=flop / sec, share_fp32_peak=f_share, bytes_per_s=nbytes / sec, share_hbm_peak=b_share,
-               bound="compute" if f_share >= b_share else "memory", set_embeddings_sec=set_sec,
-               set_embeddings_users_per_s=n_users / set_sec, recommend_users=len(users), recommend_sec=rec_sec,
-               recommend_users_per_s=len(users) / rec_sec)
-    del model, U, I, sc
+               bound="compute" if f_share >= b_share else "memory", **serving)
+    del model
     torch.cuda.empty_cache()
     return out
 
@@ -103,12 +72,7 @@ def main():
             r = case(rnn_type, hidden, n, args.items, T, args.K, seqs, lens, args.chunk, args.reps)
             print(json.dumps(r), flush=True)
             res["cases"].append(r)
-    line = json.dumps(res, indent=1)
-    print(line)
-    if args.out:
-        os.makedirs(os.path.dirname(args.out) or ".", exist_ok=True)
-        with open(args.out, "w") as f:
-            f.write(line)
+    write_report(res, args.out)
 
 
 if __name__ == "__main__":

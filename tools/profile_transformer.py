@@ -11,7 +11,6 @@ data-sheet FP32 rate (67 TFLOP/s); the card name and power limit are read in the
 import argparse
 import json
 import os
-import subprocess
 import sys
 import time
 
@@ -19,13 +18,7 @@ import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
-FP32_PEAK = 67e12
-
-
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True)
-    return q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else "unknown"
+from _profile_common import FP32_PEAK, card  # noqa: E402
 
 
 def build(n_users, n_items, K, T, item_sparse, hidden, seed=0):
