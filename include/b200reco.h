@@ -711,6 +711,47 @@ int b200_wavenet_encode(const int64_t* users, int64_t n, const int32_t* seqs, in
                         const float* X, int64_t ldx, int32_t K, int32_t n_conv, int32_t F, const int32_t* dilations,
                         const float* weights, float* out, int64_t ldo, void* stream);
 
+/* ---- Caser / WaveNet training (caser.py:135-221, wave_net.py:139-222 in training mode) ---------------------------
+ * b200_caser_train_forward / b200_wavenet_train_forward: b200_caser_encode / b200_wavenet_encode (the same out, bit
+ * for bit) that also save what the backward needs.  argmax is a max-pool's argmax: the LOWEST position reaching the
+ * maximum, or -1 when the maximum is <= 0 (the ReLU then passes no gradient).  Caser: argmax [n, T*nh] (column
+ * (h-1)*nh + f, a window start p in [0, T-h]).  WaveNet: layer_out [n_conv, n * T, F] (causal layer l's output y_l at
+ * row s * T + t of block l) and argmax [n, F] over t of the 1x1 layer.  Same envelope and errors as the encoders.
+ * b200_caser_backward: given dF [n, T*nh + K*nv] (lddf) = d loss / d out, the features feat (ldfe) and argmax of the
+ * training forward, the gathered input rows X [n * T, ldx] (row s * T + t = seq_embeds[seq[s, t]]) and the packed
+ * weights, WRITES dX [n * T, lddx] and dW (b200_caser_weight_floats floats, the packed layout of weights).  A
+ * horizontal column routes g = dF to its argmax window (nothing for -1); a vertical column passes g = dF where
+ * feat > 0.  dX[s, t, k] = sum over (h ascending, f ascending) with p* <= t < p* + h of g W_h[t - p*, k, f], then
+ * sum_f (ascending) gv[k, f] Wv[t, f].  dW: each chunk of rows is summed in row order into workspace
+ * (b200_caser_backward_workspace_floats(n, ...) floats), then the chunks in a fixed order (b200_col_reduce).  No
+ * atomics: a repeated call gives the same bits.
+ * b200_wavenet_pool_backward: dZ [n * T, F] = dF[s, f] at t = argmax[s, f], 0 elsewhere (the 1x1 layer's max).
+ * b200_wavenet_layer_inputs: out [n * T, 2C] = [x[s*T + t - d] (0 for t < d) | x[s*T + t]], so that one dense
+ * product with a causal layer's kernel [2, C, F] seen as [2C, F] gives its pre-activation, and its transpose the
+ * kernel gradient.
+ * b200_wavenet_layer_dx: given P = dpre [2, C, F]^T [n * T, 2C], dx[s*T + t, c] = P[s*T + t, C + c] +
+ * P[s*T + t + d, c] (the second term while t + d < T).
+ * Supported: the encoders' envelope (C <= 128, dilation >= 1 for the layer helpers); anything else returns -2
+ * before launching; n = 0 launches nothing. */
+int b200_caser_train_forward(const int64_t* users, int64_t n, const int32_t* seqs, int64_t ld_seq, int32_t T,
+                             const float* X, int64_t ldx, int32_t K, int32_t nh, int32_t nv, const float* weights,
+                             float* out, int64_t ldo, int32_t* argmax, void* stream);
+int b200_wavenet_train_forward(const int64_t* users, int64_t n, const int32_t* seqs, int64_t ld_seq, int32_t T,
+                               const float* X, int64_t ldx, int32_t K, int32_t n_conv, int32_t F,
+                               const int32_t* dilations, const float* weights, float* out, int64_t ldo,
+                               float* layer_out, int32_t* argmax, void* stream);
+int64_t b200_caser_backward_workspace_floats(int64_t n, int32_t T, int32_t K, int32_t nh, int32_t nv);
+int b200_caser_backward(int64_t n, int32_t T, int32_t K, int32_t nh, int32_t nv, const float* dF, int64_t lddf,
+                        const float* feat, int64_t ldfe, const int32_t* argmax, const float* X, int64_t ldx,
+                        const float* weights, float* dX, int64_t lddx, float* dW, float* workspace,
+                        int64_t workspace_floats, void* stream);
+int b200_wavenet_pool_backward(int64_t n, int32_t T, int32_t F, const float* dF, int64_t lddf, const int32_t* argmax,
+                               float* dZ, void* stream);
+int b200_wavenet_layer_inputs(const float* x, int64_t ldx, int64_t n, int32_t T, int32_t C, int32_t dilation,
+                              float* out, void* stream);
+int b200_wavenet_layer_dx(const float* P, int64_t n, int32_t T, int32_t C, int32_t dilation, float* dx, int64_t lddx,
+                          void* stream);
+
 /* ---- a14: predict_from_embedding (libreco/prediction/predict.py:36-40) -----------------
  * out[r] = sum_k U[users[r],k] * I[items[r],k]; mode 0: raw, 1: expit (ranking),
  * 2: clip to [lo, hi] (rating) — normalize_prediction (:18-23). */

@@ -158,6 +158,16 @@ SIGNATURES = {
                                   c_int64, _P]),
     "b200_wavenet_encode": (c_int, [_P, c_int64, _P, c_int64, c_int32, _P, c_int64, c_int32, c_int32, c_int32, _P, _P,
                                     _P, c_int64, _P]),
+    "b200_caser_train_forward": (c_int, [_P, c_int64, _P, c_int64, c_int32, _P, c_int64, c_int32, c_int32, c_int32, _P,
+                                         _P, c_int64, _P, _P]),
+    "b200_wavenet_train_forward": (c_int, [_P, c_int64, _P, c_int64, c_int32, _P, c_int64, c_int32, c_int32, c_int32,
+                                           _P, _P, _P, c_int64, _P, _P, _P]),
+    "b200_caser_backward_workspace_floats": (c_int64, [c_int64, c_int32, c_int32, c_int32, c_int32]),
+    "b200_caser_backward": (c_int, [c_int64, c_int32, c_int32, c_int32, c_int32, _P, c_int64, _P, c_int64, _P, _P,
+                                    c_int64, _P, _P, c_int64, _P, _P, c_int64, _P]),
+    "b200_wavenet_pool_backward": (c_int, [c_int64, c_int32, c_int32, _P, c_int64, _P, _P, _P]),
+    "b200_wavenet_layer_inputs": (c_int, [_P, c_int64, c_int64, c_int32, c_int32, c_int32, _P, _P]),
+    "b200_wavenet_layer_dx": (c_int, [_P, c_int64, c_int32, c_int32, c_int32, _P, c_int64, _P]),
 }
 
 for _name, (_res, _args) in SIGNATURES.items():

@@ -15,6 +15,7 @@ variable moves, i.e. a dense Adam step with a zero-filled gradient.  torch: memo
 """
 from __future__ import annotations
 
+import ctypes
 import functools
 
 import numpy as np
@@ -206,6 +207,34 @@ class _Trainer:
         # d h = dlogit (x) out_kernel: the Dense(1) transposed, on the library's dense kernel (din = 1)
         dh = linear(dlogit.view(R, 1), p["out_kernel"].view(-1, 1), None, False, cache_split=False)
         return loss, dh
+
+    def _items(self, items_d):
+        """(rows of ``item_embeds`` [B, d] normalised with norm_embed, their pre-normalisation rows or None, biases
+        [B] of ``item_biases``)."""
+        torch = self._torch
+        p, B = self.params, int(items_d.numel())
+        d = int(p["item_embeds"].shape[1])
+        I0 = torch.empty((B, d), dtype=torch.float32, device=self.device)
+        b = torch.empty((B, 1), dtype=torch.float32, device=self.device)
+        st = _lib.current_stream()
+        _lib.check(_lib.lib.b200_gather_rows(_lib.ptr(p["item_embeds"]), d, d, _lib.ptr(items_d), B, _lib.ptr(I0), d,
+                                             st))
+        _lib.check(_lib.lib.b200_gather_rows(_lib.ptr(p["item_biases"]), 1, 1, _lib.ptr(items_d), B, _lib.ptr(b), 1,
+                                             st))
+        I, pre = self._normalize(I0)
+        return I, pre, b.view(-1)
+
+    def _score(self, u, I, b):
+        """<u_r, I_r> + b_r per row."""
+        torch = self._torch
+        B = int(u.shape[0])
+        rows = torch.arange(B, dtype=torch.int64, device=self.device)
+        s = torch.empty(B, dtype=torch.float32, device=self.device)
+        _lib.check(_lib.lib.b200_gather_dot(_lib.ptr(u), u.stride(0), _lib.ptr(rows), _lib.ptr(I), I.stride(0),
+                                            _lib.ptr(rows), B, int(u.shape[1]), 0, 0.0, 0.0, _lib.ptr(s),
+                                            _lib.current_stream()))
+        _lib.check(_lib.lib.b200_axpy(_lib.ptr(s), _lib.ptr(b), 1.0, B, _lib.current_stream()))
+        return s
 
     def _device_counters(self):
         """The Adam step counter and step size live on the device (allocated outside any graph capture)."""
@@ -1619,30 +1648,6 @@ class RNN4RecTrainer(_Trainer):
         c["h"] = h
         return u, c
 
-    def _items(self, items_d):
-        """(item rows [B, K] normalised with norm_embed, their pre-normalisation rows or None, biases [B])."""
-        torch = self._torch
-        p, K, B = self.params, self.K, int(items_d.numel())
-        I0 = torch.empty((B, K), dtype=torch.float32, device=self.device)
-        b = torch.empty((B, 1), dtype=torch.float32, device=self.device)
-        st = _lib.current_stream()
-        _lib.check(_lib.lib.b200_gather_rows(_lib.ptr(p["item_embeds"]), K, K, _lib.ptr(items_d), B, _lib.ptr(I0), K,
-                                             st))
-        _lib.check(_lib.lib.b200_gather_rows(_lib.ptr(p["item_biases"]), 1, 1, _lib.ptr(items_d), B, _lib.ptr(b), 1,
-                                             st))
-        I, pre = self._normalize(I0)
-        return I, pre, b.view(-1)
-
-    def _score(self, u, I, b):
-        torch = self._torch
-        B = int(u.shape[0])
-        rows = torch.arange(B, dtype=torch.int64, device=self.device)
-        s = torch.empty(B, dtype=torch.float32, device=self.device)
-        _lib.check(_lib.lib.b200_gather_dot(_lib.ptr(u), u.stride(0), _lib.ptr(rows), _lib.ptr(I), I.stride(0),
-                                            _lib.ptr(rows), B, self.K, 0, 0.0, 0.0, _lib.ptr(s), _lib.current_stream()))
-        _lib.check(_lib.lib.b200_axpy(_lib.ptr(s), _lib.ptr(b), 1.0, B, _lib.current_stream()))
-        return s
-
     # -- one step ----------------------------------------------------------------------------------------------------
     def forward_backward(self, items_d, seqs_d, lens_d, labels_or_neg):
         """Loss (device scalar) with every gradient buffer filled."""
@@ -1773,6 +1778,376 @@ class RNN4RecTrainer(_Trainer):
                     item_biases=p["item_biases"].cpu().numpy(),
                     rnn_layers=rnn_raw_layers(self.canonical_layers(), self.scheme, self.rnn_type, self.in_dim),
                     dense_kernel=p["dense_Wt"].cpu().numpy().T.copy(), dense_bias=p["dense_b"].cpu().numpy())
+
+CONV_LOSSES = {"cross_entropy": 0, "focal": 1}
+
+
+class _ConvSeqTrainer(_Trainer):
+    """What the Caser and WaveNet training steps share (``caser.py:135-221``, ``wave_net.py:139-222`` in training
+    mode, the losses of ``tfops/loss.py:4-25``, TF-Adam of ``training/tf_trainer.py:103-124``).  The user vector of
+    a row is ``[user_embeds[u] | head(encoder(seq_embeds[seq]))]`` (2K wide), scored against ``item_embeds`` (2K)
+    plus ``item_biases``:
+
+        b200_gather_rows (user rows, the T input rows) -> b200_{caser,wavenet}_train_forward (saving the max-pool
+        argmax, and WaveNet's layer outputs) -> the Dense head on b200_linear_f32 -> [b200_l2_normalize_rows]
+        -> <u, i> + b_i (b200_gather_dot) -> b200_pointwise_loss -> [normalisation backward] -> b200_scatter_add_rows
+        of the item, bias and user-row gradients -> head backward -> encoder backward -> b200_scatter_add_rows of dX
+        into seq_embeds -> b200_adam_dense_dev
+
+    ``weights``: the raw variables (``synthetic.make_caser_weights`` / ``make_wavenet_weights``,
+    ``weights_io._conv_raw``) or the packed dict of ``weights_io.caser_weights`` / ``wavenet_weights``.  The Adam
+    variables are the four tables, the head and every TF convolution variable, the last as views into the packed
+    buffer ``conv_w`` that the kernels read (the packed layout is TensorFlow's, element for element); their gradients
+    are views into ``conv_g``.  ``step(users, items, seqs, lens, labels)``: ``seqs`` [B, T] holds item ids padded with
+    the pad row ``n_items``, which is trained like any other row (neither graph masks by length, so ``lens`` is
+    accepted and not read).  ``users`` must lie in ``[0, n_users]``: they index ``user_embeds`` unchecked (a check
+    would synchronise the host every step and break graph capture).  ``ValueError`` before any launch for ``bpr``
+    (neither graph defines it), an unknown loss, the rating task, a ``seq_embeds`` row count other than
+    ``n_items + 1``, shapes outside the envelope of the encoders and a batch whose saved state does not fit in the
+    free device memory."""
+
+    embed_table = "seq_embeds"
+    reg_vars = ("user_embeds", "seq_embeds", "item_embeds")   # item_bias_var has no regularizer (caser.py:171-175)
+    NAME = ""
+    HEAD_ACT = ACT_NONE
+
+    def __init__(self, spec, weights, loss_type="cross_entropy", norm_embed=False, task="ranking", lr=1e-3,
+                 epsilon=1e-5, device=None):
+        from .feat_models import CONV_MAX_K, _spec_get
+
+        name = type(self).__name__
+        if task != "ranking":
+            raise ValueError(f"{name}: task `{task}` is not supported (ranking only)")
+        if loss_type not in CONV_LOSSES:
+            raise ValueError(f"{name}: loss_type must be one of {sorted(CONV_LOSSES)}, got `{loss_type}` (the graph "
+                             "defines no bpr loss)")
+        w = weights if "conv" in weights else self._pack(weights)
+        g = None if isinstance(spec, FeatSpec) else _spec_get(spec)
+        n_users = int(spec.n_users if g is None else g("n_users"))
+        n_items = int(spec.n_items if g is None else g("n_items"))
+        K = int(np.shape(w["seq_embeds"])[1])
+        if not 1 <= K <= CONV_MAX_K:
+            raise ValueError(f"{name}: embed_size {K} outside [1, {CONV_MAX_K}]")
+        if np.shape(w["seq_embeds"])[0] != n_items + 1:
+            raise ValueError(f"{name}: seq_embeds has {np.shape(w['seq_embeds'])[0]} rows, expected n_items + 1 = "
+                             f"{n_items + 1}")
+        shapes = {"user_embeds": (n_users + 1, K), "item_embeds": (n_items, 2 * K), "item_biases": (n_items,),
+                  "dense_bias": (K,)}
+        for k, shp in shapes.items():
+            if tuple(np.shape(w[k])) != shp:
+                raise ValueError(f"{name}: `{k}` has shape {np.shape(w[k])}, expected {shp}")
+        self._check_encoder(w, K)
+        self.loss_type, self.norm_embed = loss_type, bool(norm_embed)
+        super().__init__(spec, w, False, lr, epsilon, device)
+        torch = self._torch
+        self.conv_g = torch.zeros_like(self.conv_w)
+        for k, (off, shape) in self._views.items():
+            self.grads[k] = self.conv_g[off:off + int(np.prod(shape))].view(shape)
+
+    def _init_params(self, weights):
+        p = self.params
+        p["seq_embeds"] = self._var(weights["seq_embeds"])
+        p["item_biases"] = self._var(weights["item_biases"], -1)
+        p["dense_Wt"] = self._var(np.asarray(weights["dense_kernel"]).T.copy())      # [K, D]
+        p["dense_b"] = self._var(weights["dense_bias"], -1)
+        self.conv_w = self._var(weights["conv"], -1)
+        self._views = self._conv_views()
+        for k, (off, shape) in self._views.items():
+            p[k] = self.conv_w[off:off + int(np.prod(shape))].view(shape)
+
+    # -- memory ------------------------------------------------------------------------------------------------------
+    def _check_batch(self, B, T):
+        from .feat_models import CONV_MAX_T
+
+        torch = self._torch
+        name = type(self).__name__
+        if not 1 <= T <= CONV_MAX_T:
+            raise ValueError(f"{name}: sequence length {T} outside [1, {CONV_MAX_T}]")
+        self._check_T(T)
+        need = B * self.saved_bytes_per_row(T)
+        free = torch.cuda.mem_get_info(self.device)[0] + torch.cuda.memory_reserved(self.device) - \
+            torch.cuda.memory_allocated(self.device)
+        if need > free:
+            raise ValueError(f"{name}: a batch of {B} rows x T = {T} keeps {need} B for the backward, {free} B are "
+                             "free")
+
+    def _check_T(self, T):
+        pass
+
+    # -- forward -----------------------------------------------------------------------------------------------------
+    def user_vectors(self, users_d, seqs_d):
+        """``[user_embeds[users] | head(encoder(seqs))]`` [B, 2K] before any normalisation, and the cache of the
+        backward."""
+        torch = self._torch
+        f32, dev, K = torch.float32, self.device, self.K
+        B, T = int(seqs_d.shape[0]), int(seqs_d.shape[1])
+        p, st = self.params, _lib.current_stream()
+        users_d = users_d.to(torch.int64).contiguous()
+        seqs_d = seqs_d.to(torch.int32).contiguous()
+        rows = torch.arange(B, dtype=torch.int64, device=dev)
+        idx = seqs_d.reshape(-1).to(torch.int64)
+        E = p["seq_embeds"]
+        X0 = torch.empty((B * T, K), dtype=f32, device=dev)
+        _lib.check(_lib.lib.b200_gather_rows(_lib.ptr(E), E.stride(0), K, _lib.ptr(idx), B * T, _lib.ptr(X0), K, st))
+        c = dict(users=users_d, rows=rows, idx=idx, X0=X0, seqs=seqs_d, B=B, T=T)
+        feat = self._encode(c)
+        u = torch.empty((B, 2 * K), dtype=f32, device=dev)
+        U = p["user_embeds"]
+        _lib.check(_lib.lib.b200_gather_rows(_lib.ptr(U), U.stride(0), K, _lib.ptr(users_d), B, _lib.ptr(u), u.stride(0),
+                                             st))
+        head = linear(feat, p["dense_Wt"], p["dense_b"], self.HEAD_ACT, impl="f32")
+        u[:, K:] = head
+        c.update(feat=feat, head=head)
+        return u, c
+
+    # -- one step ----------------------------------------------------------------------------------------------------
+    def forward_backward(self, users_d, items_d, seqs_d, lens_d, labels_d):
+        """Loss (device scalar) with every gradient buffer filled (``lens_d`` is not read)."""
+        torch = self._torch
+        lib, st, p, g, K = _lib.lib, _lib.current_stream(), self.params, self.grads, self.K
+        B = int(seqs_d.shape[0])
+        u0, c = self.user_vectors(users_d, seqs_d)
+        u, u_pre = self._normalize(u0)
+        I, I_pre, b = self._items(items_d)
+        logit = self._score(u, I, b)
+        loss = torch.empty((), dtype=torch.float32, device=self.device)
+        dlogit = torch.empty(B, dtype=torch.float32, device=self.device)
+        _lib.check(lib.b200_pointwise_loss(_lib.ptr(logit), _lib.ptr(labels_d), B, CONV_LOSSES[self.loss_type], 0.25,
+                                           2.0, _lib.ptr(loss), _lib.ptr(dlogit), _lib.ptr(self._lws),
+                                           self._lws.numel(), st))
+        du = self._normalize_backward(dlogit[:, None] * I, u_pre).contiguous()
+        dI = self._normalize_backward(dlogit[:, None] * u, I_pre).contiguous()
+        gI, gb, gU = g["item_embeds"], g["item_biases"], g["user_embeds"]
+        _lib.check(lib.b200_scatter_add_rows(_lib.ptr(gI), 2 * K, 2 * K, _lib.ptr(items_d), B, _lib.ptr(dI), 2 * K,
+                                             st))
+        _lib.check(lib.b200_scatter_add_rows(_lib.ptr(gb), 1, 1, _lib.ptr(items_d), B, _lib.ptr(dlogit), 1, st))
+        _lib.check(lib.b200_scatter_add_rows(_lib.ptr(gU), K, K, _lib.ptr(c["users"]), B, _lib.ptr(du), 2 * K, st))
+        # the Dense head; ReLU's mask is the same read from its output
+        dh = du[:, K:].contiguous()
+        if self.HEAD_ACT == ACT_RELU:
+            _lib.check(lib.b200_activation_backward(_lib.ptr(dh), _lib.ptr(c["head"]), dh.numel(), ACT_RELU,
+                                                    _lib.ptr(dh), st))
+        g["dense_Wt"].copy_(_weight_grad(dh, c["feat"]))
+        self._col_sum(dh, g["dense_b"])
+        dF = linear(dh, p["dense_Wt"].t().contiguous(), None, False, cache_split=False)
+        dX = self._encoder_backward(c, dF)
+        ge = g["seq_embeds"]
+        _lib.check(lib.b200_scatter_add_rows(_lib.ptr(ge), ge.stride(0), K, _lib.ptr(c["idx"]), B * c["T"],
+                                             _lib.ptr(dX), dX.stride(0), st))
+        return loss
+
+    def step(self, users_d, items_d, seqs_d, lens_d, labels_d):
+        """One optimisation step; returns the device loss."""
+        torch = self._torch
+        seqs_d = seqs_d.to(torch.int32).contiguous()
+        self._check_batch(int(seqs_d.shape[0]), int(seqs_d.shape[1]))
+        loss = self.forward_backward(users_d.to(torch.int64).contiguous(), items_d.to(torch.int64).contiguous(),
+                                     seqs_d, lens_d, labels_d.to(torch.float32).contiguous())
+        self._adam_update()
+        return loss
+
+    def _export_common(self):
+        p = self.params
+        out = {k: p[k].cpu().numpy() for k in ("user_embeds", "seq_embeds", "item_embeds", "item_biases")}
+        out.update(dense_kernel=p["dense_Wt"].cpu().numpy().T.copy(), dense_bias=p["dense_b"].cpu().numpy())
+        return out
+
+
+class CaserTrainer(_ConvSeqTrainer):
+    """Caser's training step (``caser.py:135-221``): ``b200_caser_train_forward`` saves each horizontal column's
+    max-pool argmax; ``b200_caser_backward`` routes the head's gradient through it (and through the vertical
+    columns' ReLU) into dX and every convolution variable.  The head is ``Dense(K, relu)``.  See
+    :class:`_ConvSeqTrainer`; the sequence length is the weights' T."""
+
+    HEAD_ACT = ACT_RELU
+
+    @staticmethod
+    def _pack(raw):
+        from .weights_io import caser_weights
+
+        return caser_weights(raw)
+
+    def _check_encoder(self, w, K):
+        from .feat_models import CONV_MAX_FILTERS, CONV_MAX_T
+
+        self.T, self.nh, self.nv = int(w["T"]), int(w["nh"]), int(w["nv"])
+        if not 1 <= self.T <= CONV_MAX_T:
+            raise ValueError(f"CaserTrainer: max_seq_len {self.T} outside [1, {CONV_MAX_T}]")
+        if not (1 <= self.nh <= CONV_MAX_FILTERS and 1 <= self.nv <= CONV_MAX_FILTERS):
+            raise ValueError(f"CaserTrainer: nh_filters {self.nh} / nv_filters {self.nv} outside "
+                             f"[1, {CONV_MAX_FILTERS}]")
+        self.D = self.T * self.nh + K * self.nv
+        if np.size(w["conv"]) != int(_lib.lib.b200_caser_weight_floats(self.T, K, self.nh, self.nv)):
+            raise ValueError(f"CaserTrainer: {np.size(w['conv'])} packed convolution floats do not match T {self.T}, "
+                             f"K {K}, nh {self.nh}, nv {self.nv}")
+        if tuple(np.shape(w["dense_kernel"])) != (self.D, K):
+            raise ValueError(f"CaserTrainer: `dense_kernel` has shape {np.shape(w['dense_kernel'])}, expected "
+                             f"({self.D}, {K})")
+
+    def _check_T(self, T):
+        if T != self.T:
+            raise ValueError(f"CaserTrainer: sequences of length {T}, the model has {self.T} horizontal convolutions")
+
+    def _conv_views(self):
+        """{variable: (offset, TF shape)} in the packed layout: W_1 .. W_T, the T biases, Wv, bv."""
+        T, K, nh, nv = self.T, self.K, self.nh, self.nv
+        out, off = {}, 0
+        for h in range(1, T + 1):
+            out[f"conv{h - 1}_kernel"] = (off, (h, K, nh))
+            off += h * K * nh
+        for h in range(1, T + 1):
+            out[f"conv{h - 1}_bias"] = (off, (nh,))
+            off += nh
+        out["vertical_kernel"] = (off, (1, T, nv))
+        out["vertical_bias"] = (off + T * nv, (nv,))
+        return out
+
+    def saved_bytes_per_row(self, T):
+        """Device bytes one batch row keeps for the backward: the input rows and dX (T x K each), the features and
+        dF (D each), the argmax (T nh), the user vector and its gradient (2K each), the head (K), and the row's
+        share of the weight-gradient partials."""
+        ws = int(_lib.lib.b200_caser_backward_workspace_floats(256, T, self.K, self.nh, self.nv))
+        return 4 * (2 * T * self.K + 2 * self.D + T * self.nh + 5 * self.K) + -(-4 * ws // 256)
+
+    def _encode(self, c):
+        torch = self._torch
+        B, T = c["B"], c["T"]
+        E = self.params["seq_embeds"]
+        feat = torch.empty((B, self.D), dtype=torch.float32, device=self.device)
+        arg = torch.empty((B, T * self.nh), dtype=torch.int32, device=self.device)
+        _lib.check(_lib.lib.b200_caser_train_forward(
+            _lib.ptr(c["rows"]), B, _lib.ptr(c["seqs"]), c["seqs"].stride(0), T, _lib.ptr(E), E.stride(0), self.K,
+            self.nh, self.nv, _lib.ptr(self.conv_w), _lib.ptr(feat), feat.stride(0), _lib.ptr(arg),
+            _lib.current_stream()))
+        c["arg"] = arg
+        return feat
+
+    def _encoder_backward(self, c, dF):
+        torch = self._torch
+        B, T, K = c["B"], c["T"], self.K
+        n_ws = int(_lib.lib.b200_caser_backward_workspace_floats(B, T, K, self.nh, self.nv))
+        ws = torch.empty(max(n_ws, 1), dtype=torch.float32, device=self.device)
+        dX = torch.empty((B * T, K), dtype=torch.float32, device=self.device)
+        _lib.check(_lib.lib.b200_caser_backward(
+            B, T, K, self.nh, self.nv, _lib.ptr(dF), dF.stride(0), _lib.ptr(c["feat"]), c["feat"].stride(0),
+            _lib.ptr(c["arg"]), _lib.ptr(c["X0"]), K, _lib.ptr(self.conv_w), _lib.ptr(dX), K, _lib.ptr(self.conv_g),
+            _lib.ptr(ws), n_ws, _lib.current_stream()))
+        return dX
+
+    def export_weights(self):
+        """The raw variables (``caser_weights``, ``caser_tf_variables`` and ``feat_models.Caser`` take them)."""
+        out = self._export_common()
+        v = {k: self.params[k].cpu().numpy() for k in self._views}
+        out["convs"] = [dict(kernel=v[f"conv{i}_kernel"], bias=v[f"conv{i}_bias"]) for i in range(self.T)]
+        out["vertical"] = dict(kernel=v["vertical_kernel"], bias=v["vertical_bias"])
+        return out
+
+
+class WaveNetTrainer(_ConvSeqTrainer):
+    """WaveNet's training step (``wave_net.py:139-222``): ``b200_wavenet_train_forward`` saves every causal layer's
+    output and the 1x1 layer's argmax over t.  The backward runs on the dense kernels plus three position kernels:
+    ``b200_wavenet_pool_backward`` puts the gradient at each argmax; then the 1x1 layer's products; then, per causal
+    layer from the top, the ReLU mask (``b200_activation_backward`` on the saved output), the kernel gradient
+    ``[x_{t-d} | x_t]^T dpre`` over ``b200_wavenet_layer_inputs``, and ``dx`` from ``dpre [W0; W1]^T`` shifted by
+    ``b200_wavenet_layer_dx``.  The head is ``Dense(K)``.  The dilations come from the weights (1 everywhere for a
+    TF1-trained graph).  See :class:`_ConvSeqTrainer`."""
+
+    @staticmethod
+    def _pack(raw):
+        from .weights_io import wavenet_weights
+
+        return wavenet_weights(raw)
+
+    def _check_encoder(self, w, K):
+        from .feat_models import CONV_MAX_F, CONV_MAX_LAYERS
+
+        self.n_filters, self.dilations = int(w["F"]), [int(d) for d in w["dilations"]]
+        if not 1 <= self.n_filters <= CONV_MAX_F:
+            raise ValueError(f"WaveNetTrainer: n_filters {self.n_filters} outside [1, {CONV_MAX_F}]")
+        if not 1 <= len(self.dilations) <= CONV_MAX_LAYERS or min(self.dilations) < 1:
+            raise ValueError(f"WaveNetTrainer: dilations {self.dilations}: 1 to {CONV_MAX_LAYERS} causal layers, each "
+                             "dilation >= 1")
+        if np.size(w["conv"]) != int(_lib.lib.b200_wavenet_weight_floats(K, self.n_filters, len(self.dilations))):
+            raise ValueError(f"WaveNetTrainer: {np.size(w['conv'])} packed convolution floats do not match K {K}, "
+                             f"F {self.n_filters}, {len(self.dilations)} causal layers")
+        if tuple(np.shape(w["dense_kernel"])) != (self.n_filters, K):
+            raise ValueError(f"WaveNetTrainer: `dense_kernel` has shape {np.shape(w['dense_kernel'])}, expected "
+                             f"({self.n_filters}, {K})")
+        self.D = self.n_filters
+        self._dil = (ctypes.c_int32 * len(self.dilations))(*self.dilations)
+
+    def _conv_views(self):
+        """{variable: (offset, TF shape)} in the packed layout: per causal layer kernel [2, C, F], bias; then the 1x1
+        layer's kernel [1, F, F], bias."""
+        K, F = self.K, self.n_filters
+        out, off = {}, 0
+        for l in range(len(self.dilations)):
+            C = K if l == 0 else F
+            out[f"conv{l}_kernel"] = (off, (2, C, F))
+            out[f"conv{l}_bias"] = (off + 2 * C * F, (F,))
+            off += 2 * C * F + F
+        out["out_conv_kernel"] = (off, (1, F, F))
+        out["out_conv_bias"] = (off + F * F, (F,))
+        return out
+
+    def saved_bytes_per_row(self, T):
+        """Device bytes one batch row keeps for the backward: the input rows (T x K), every causal layer's output
+        (L x T x F), the argmax, features, user vector and head (F + F + 4K + K), dZ / dy (T x F each) and the
+        largest layer's transients (dpre, [x_{t-d} | x_t], the [2C] product, dx)."""
+        K, F, L = self.K, self.n_filters, len(self.dilations)
+        C = max(K, F)
+        return 4 * (T * K + L * T * F + 2 * F + 5 * K + 2 * T * F + T * (F + 5 * C))
+
+    def _encode(self, c):
+        torch = self._torch
+        B, T, F = c["B"], c["T"], self.n_filters
+        E = self.params["seq_embeds"]
+        feat = torch.empty((B, F), dtype=torch.float32, device=self.device)
+        ys = torch.empty((len(self.dilations), B * T, F), dtype=torch.float32, device=self.device)
+        arg = torch.empty((B, F), dtype=torch.int32, device=self.device)
+        _lib.check(_lib.lib.b200_wavenet_train_forward(
+            _lib.ptr(c["rows"]), B, _lib.ptr(c["seqs"]), c["seqs"].stride(0), T, _lib.ptr(E), E.stride(0), self.K,
+            len(self.dilations), F, self._dil, _lib.ptr(self.conv_w), _lib.ptr(feat), feat.stride(0), _lib.ptr(ys),
+            _lib.ptr(arg), _lib.current_stream()))
+        c.update(arg=arg, ys=ys)
+        return feat
+
+    def _encoder_backward(self, c, dF):
+        torch = self._torch
+        lib, st, p, g = _lib.lib, _lib.current_stream(), self.params, self.grads
+        B, T, F, K = c["B"], c["T"], self.n_filters, self.K
+        S, L = B * T, len(self.dilations)
+        f32, dev = torch.float32, self.device
+        dZ = torch.empty((S, F), dtype=f32, device=dev)
+        _lib.check(lib.b200_wavenet_pool_backward(B, T, F, _lib.ptr(dF), dF.stride(0), _lib.ptr(c["arg"]),
+                                                  _lib.ptr(dZ), st))
+        ys = c["ys"]
+        g["out_conv_kernel"][0].copy_(_weight_grad(dZ, ys[L - 1]).t())       # W1[c, f] += y[t, c] dZ[t, f]
+        self._col_sum(dZ, g["out_conv_bias"])
+        dy = linear(dZ, p["out_conv_kernel"][0], None, False, cache_split=False)    # dZ W1^T
+        for l in range(L - 1, -1, -1):
+            C, d = (K if l == 0 else F), self.dilations[l]
+            dpre = torch.empty((S, F), dtype=f32, device=dev)
+            _lib.check(lib.b200_activation_backward(_lib.ptr(dy), _lib.ptr(ys[l]), S * F, ACT_RELU, _lib.ptr(dpre),
+                                                    st))
+            x = c["X0"] if l == 0 else ys[l - 1]
+            xin = torch.empty((S, 2 * C), dtype=f32, device=dev)
+            _lib.check(lib.b200_wavenet_layer_inputs(_lib.ptr(x), x.stride(0), B, T, C, d, _lib.ptr(xin), st))
+            g[f"conv{l}_kernel"].view(2 * C, F).copy_(_weight_grad(dpre, xin).t())
+            self._col_sum(dpre, g[f"conv{l}_bias"])
+            P = linear(dpre, p[f"conv{l}_kernel"].view(2 * C, F), None, False, cache_split=False)   # [S, 2C]
+            dy = torch.empty((S, C), dtype=f32, device=dev)
+            _lib.check(lib.b200_wavenet_layer_dx(_lib.ptr(P), B, T, C, d, _lib.ptr(dy), C, st))
+        return dy
+
+    def export_weights(self):
+        """The raw variables (``wavenet_weights``, ``wavenet_tf_variables`` and ``feat_models.WaveNet`` take them)."""
+        out = self._export_common()
+        v = {k: self.params[k].cpu().numpy() for k in self._views}
+        out["convs"] = [dict(kernel=v[f"conv{i}_kernel"], bias=v[f"conv{i}_bias"]) for i in range(len(self.dilations))]
+        out["out_conv"] = dict(kernel=v["out_conv_kernel"], bias=v["out_conv_bias"])
+        out["dilations"] = list(self.dilations)
+        return out
 
 
 def _ctypes_ptr_array(n):
