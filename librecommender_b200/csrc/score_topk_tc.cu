@@ -626,28 +626,28 @@ sweep_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
               // Slots are visited group by group, row by row, so every list receives its records in
               // column order whichever variant runs.
               if (EPI == 5) {
-                // bit 2 jl + rs: the group reaches tau in that row; OR over the quad, then over the warp
-                uint32_t mask = 0;
+                // one ballot per (group, row) slot: bits 4 q .. 4 q + 3 are the lanes of quad q, so the slot
+                // is live in the warp iff its ballot is non-zero, and quad q stores iff its nibble is
+                uint32_t bal[8][2];
 #pragma unroll
                 for (int jl = 0; jl < 8; ++jl)
 #pragma unroll
-                  for (int rs = 0; rs < 2; ++rs) mask |= (pm[jl][rs] >= tau[rs] ? 1u : 0u) << (2 * jl + rs);
-                mask |= __shfl_xor_sync(0xffffffffu, mask, 1);
-                mask |= __shfl_xor_sync(0xffffffffu, mask, 2);
-                const uint32_t any = __reduce_or_sync(0xffffffffu, mask);
+                  for (int rs = 0; rs < 2; ++rs) bal[jl][rs] = __ballot_sync(0xffffffffu, pm[jl][rs] >= tau[rs]);
+                const uint32_t qmask = 0xfu << (4 * quad);
                 // two-level slot tests: a hot step usually holds one or two slots, so test the four
                 // slots of a group pair only when the pair has one (4 + 4 uniform tests instead of 16)
 #pragma unroll
                 for (int jp = 0; jp < 4; ++jp) {
-                  if (!(any & (0xfu << (4 * jp)))) continue;   // warp-uniform: no slot in groups 2 jp, 2 jp + 1
+                  // warp-uniform: no slot in groups 2 jp, 2 jp + 1
+                  if (!(bal[2 * jp][0] | bal[2 * jp][1] | bal[2 * jp + 1][0] | bal[2 * jp + 1][1])) continue;
 #pragma unroll
                 for (int jl = 2 * jp; jl < 2 * jp + 2; ++jl) {
                   const int jj = 8 * s + jl;
                   const int col = COL0 + 8 * jj;
 #pragma unroll
                   for (int rs = 0; rs < 2; ++rs) {
-                    const uint32_t bit = 1u << (2 * jl + rs);
-                    if (!(any & bit)) continue;   // warp-uniform: no quad of the warp has this slot
+                    if (!bal[jl][rs]) continue;   // warp-uniform: no quad of the warp has this slot
+                    const uint32_t mine = bal[jl][rs] & qmask;
                     float*& r = col >= TN / 2 ? rp[rs][1] : rp[rs][0];
                     // predicated stores (not a branch on the lane's bit, which the compiler would merge
                     // with the uniform test above into one divergent branch per slot)
@@ -657,10 +657,10 @@ sweep_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
                         "setp.eq.and.u32 q, %5, 0, p;\n\t"
                         "@p st.global.v2.f32 [%1], {%2, %3};\n\t"
                         "@q st.global.b32 [%4], %6;\n\t}"
-                        ::"r"(mask & bit), "l"(r + 2 * tq), "f"(d[4 * jj + 2 * rs]), "f"(d[4 * jj + 2 * rs + 1]),
+                        ::"r"(mine), "l"(r + 2 * tq), "f"(d[4 * jj + 2 * rs]), "f"(d[4 * jj + 2 * rs + 1]),
                         "l"(r + 8), "r"(tq), "r"(t * TN + col)
                         : "memory");
-                    r += (mask & bit) ? REC : 0;
+                    r += mine ? REC : 0;
                   }
                 }
                 }
