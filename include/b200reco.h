@@ -593,6 +593,46 @@ int b200_transformer_target_attention(const float* Qi, int64_t ldq, const float*
                                       const int32_t* lens, const int32_t* slot_of_row, const int64_t* items, int64_t n,
                                       int64_t grid_items, int64_t row_offset, float* out, int64_t ldo, void* stream);
 
+/* ---- SIM inference (libreco/algorithms/sim.py:193-304, soft search; the second stage only) --------------------
+ * Gp [N+1, ldg] is the projected item table combine_seq_features(concat) Wp, K columns.  A slot s has the long
+ * sequence long_seqs[s, :L] with length long_lens[s] and the short one short_seqs[s, :S] with short_lens[s] (both
+ * clamped to [0, L] / [0, S]); Kl, Vl [n_slots, L, K] are Gp[long] Wk and Gp[long] Wv (Wv the EFFECTIVE value map).
+ * For a pair (slot s, item n), q = Gp[n]:
+ *   GSU (sim.py:264-286): score_t = q . Gp[long_t] for t < long_len, -1e9 otherwise; the topk largest are selected,
+ *       equal scores resolving to the lower position.  Every score is acc = fmaf(q[d], Gp[long_t][d], acc) over d
+ *       ascending from 0 in both functions, so both select the same positions.
+ *   ESU (sim.py:288-299): per head h of K / H columns, logits (Qp[n]_h . Kl[t]_h) / sqrt(K / H) over the selected t,
+ *       fl32(logit - 1e9) where t >= long_len; o_h = sum p_t Vl[t]_h; long_out = o Wo.
+ *   short (sim.py:301-304): logits q . Gp[short_s], fl32(logit - 1e9) where s >= short_len; short_out =
+ *       (sum_s e_s Gp[short_s]) / sum_s e_s with e_s = exp(logit_s - max).
+ * Supported: 1 <= K <= 64 with H dividing K, 1 <= L <= 256, 1 <= S <= 64, 1 <= topk <= min(32, L); anything else
+ * returns -2 before launching.
+ * b200_sim_attention (rows mode): out[r, :K] = long_out, out[r, K:2K] = short_out for row r, slot = slot_of_row[r]
+ * and item = items[r] (explicit rows) or, both NULL, row g = row_offset + r of the grid: slot g / grid_items, item
+ * g % grid_items.  Qp [N+1, ldq] = Gp Wq, Wo [K, K].  gsu_pos (NULL: not written) [n, topk] receives the selected
+ * positions in ascending order.
+ * b200_sim_pair_scores (grid mode): scores[b * lds + n] for every slot b < B and item n < N:
+ *   h1 = relu(Pu[b] + PiT[:, n] + [o || short_out] W_att),  h2 = h1 W2 + b2,
+ *   H3 > 0: out = <relu(h2) W3 + b3, w_out> + b_out;  H3 = 0: out = <h2, w_out> + b_out.
+ * GpT, QpT [K, ldt] hold Gp and Qp transposed (column n = item n); W_att [2K, H1] = [Wo W1_long ; W1_short],
+ * Pu [B, H1] (first-layer bias included), PiT [H1, ldpi], W2 [H1, H2], W3 [H2, H3] (row-major, BN folded).
+ * Supported: H1 <= 256, H2 <= 128, H3 <= 64, B <= 65535 and b200_sim_pair_smem_bytes(...) within the device's
+ * shared-memory opt-in. */
+int b200_sim_attention(const float* Gp, int64_t ldg, const float* Qp, int64_t ldq, int32_t K, int32_t H,
+                       const int32_t* long_seqs, int64_t ld_long, const int32_t* long_lens, const float* Kl,
+                       const float* Vl, int32_t L, const int32_t* short_seqs, int64_t ld_short,
+                       const int32_t* short_lens, int32_t S, int32_t topk, const float* Wo,
+                       const int32_t* slot_of_row, const int64_t* items, int64_t n, int64_t grid_items,
+                       int64_t row_offset, float* out, int64_t ldo, int32_t* gsu_pos, void* stream);
+int64_t b200_sim_pair_smem_bytes(int32_t K, int32_t L, int32_t S, int32_t topk, int32_t H1, int32_t H2, int32_t H3);
+int b200_sim_pair_scores(const float* GpT, const float* QpT, int64_t ldt, int64_t N, const float* Gp, int64_t ldg,
+                         const int32_t* long_seqs, int64_t ld_long, const int32_t* long_lens,
+                         const int32_t* short_seqs, int64_t ld_short, const int32_t* short_lens, const float* Kl,
+                         const float* Vl, const float* Pu, int64_t B, const float* PiT, int64_t ldpi, int32_t K,
+                         int32_t H, int32_t L, int32_t S, int32_t topk, int32_t H1, int32_t H2, int32_t H3,
+                         const float* W_att, const float* W2, const float* b2, const float* W3, const float* b3,
+                         const float* w_out, float b_out, float* scores, int64_t lds, void* stream);
+
 /* ---- Transformer training (libreco/algorithms/transformer.py:203-339 in training mode) ------------------------
  * The dense products over the R*T sequence rows (Q / K / V / O projections, FFN, MLP and their gradients) run on
  * b200_linear_*; these are the rest.  Every `lens` here is clamped to [1, T] on the device, as the training

@@ -130,6 +130,13 @@ SIGNATURES = {
                                              c_int64, _P]),
     "b200_transformer_target_attention": (c_int, [_P, c_int64, _P, c_int32, c_int32, _P, _P, _P, c_int64, c_int64,
                                                   c_int64, _P, c_int64, _P]),
+    "b200_sim_attention": (c_int, [_P, c_int64, _P, c_int64, c_int32, c_int32, _P, c_int64, _P, _P, _P, c_int32, _P,
+                                   c_int64, _P, c_int32, c_int32, _P, _P, _P, c_int64, c_int64, c_int64, _P, c_int64,
+                                   _P, _P]),
+    "b200_sim_pair_smem_bytes": (c_int64, [c_int32] * 7),
+    "b200_sim_pair_scores": (c_int, [_P, _P, c_int64, c_int64, _P, c_int64, _P, c_int64, _P, _P, c_int64, _P, _P, _P,
+                                     _P, c_int64, _P, c_int64, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32,
+                                     c_int32, c_int32, _P, _P, _P, _P, _P, _P, c_float, _P, c_int64, _P]),
     "b200_autoint_attention_forward": (c_int, [_P, c_int64, _P, c_int64, _P, c_int64, c_int64, c_int32, c_int32,
                                                c_int32, c_float, _P, c_int64, _P, _P]),
     "b200_autoint_attention_backward": (c_int, [_P, c_int64, _P, c_int64, _P, c_int64, _P, c_int64, _P, _P, c_int64,

@@ -115,3 +115,30 @@ def build_rec_seq(seq, n_items, max_seq_len, item2id=None, inner_id=False):
     if seq_len > 0:
         out[0, :seq_len] = np.asarray(seq[-seq_len:], dtype=np.int32)
     return out, np.array([seq_len], dtype=np.int32)
+
+
+def build_dual_seq(seq, n_items, long_max_len, short_max_len, item2id=None, inner_id=False):
+    """(long_seq int32[1, long_max_len], long_len int32[1], short_seq int32[1, short_max_len], short_len int32[1])
+    of a caller-supplied sequence for SIM (``recommendation/preprocess.py:49-76``): the last ``short_max_len`` items
+    and up to ``long_max_len`` items before them, padded with ``n_items``; a sequence of at most ``short_max_len``
+    items gets long length 1 over an all-pad row.  Original ids go through ``item2id`` (unknown -> ``n_items``)."""
+    if not isinstance(seq, (list, np.ndarray)):
+        raise AssertionError("`seq` must be list or numpy.ndarray.")
+    if not inner_id:
+        seq = [item2id.get(i, n_items) for i in seq]
+    seq = np.asarray(seq, dtype=np.int32).reshape(-1)
+    n, L, S = len(seq), int(long_max_len), int(short_max_len)
+    long_seq = np.full((1, L), n_items, dtype=np.int32)
+    if n >= L + S:
+        long_len = L
+        long_seq[0] = seq[n - L - S:n - S]
+    elif n > S:
+        long_len = n - S
+        long_seq[0, :long_len] = seq[:long_len]
+    else:
+        long_len = 1
+    short_seq = np.full((1, S), n_items, dtype=np.int32)
+    short_len = min(S, n)
+    if short_len > 0:
+        short_seq[0, :short_len] = seq[n - short_len:]
+    return long_seq, np.array([long_len], dtype=np.int32), short_seq, np.array([short_len], dtype=np.int32)

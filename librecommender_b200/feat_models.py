@@ -575,7 +575,7 @@ class _FeatModelBase:
         (``dynamic_feats.dynamic_feature_rows``; the device tables are not touched), a sequence model
         reads the supplied sequence instead of the cached one."""
         torch = self._torch
-        from .dynamic_feats import build_rec_seq, dynamic_feature_rows
+        from .dynamic_feats import dynamic_feature_rows
 
         if getattr(self, "has_multi_sparse", False) and user_feats:
             raise NotImplementedError("feature overrides on layouts with multi-sparse fields")
@@ -593,11 +593,8 @@ class _FeatModelBase:
             layout = self.spec.with_rows(sr, dr)
             keep = (sr, dr)
         restore = None
-        if seq is not None and len(seq) > 0 and hasattr(self, "seqs"):
-            row, ln = build_rec_seq(seq, N, self.T, getattr(data_info, "item2id", None), inner_id)
-            restore = (self.seqs[u].clone(), self.lens[u].clone())
-            self.seqs[u] = torch.from_numpy(row[0]).to(self.device)
-            self.lens[u] = int(ln[0])
+        if seq is not None and len(seq) > 0:
+            restore = self._swap_user_seq(u, seq, data_info, inner_id)
         try:
             if user_feats:          # explicit per-row features: the flat (user, item) grid
                 scores = self._forward(layout, uid, None, N, N).view(1, N).contiguous()
@@ -605,12 +602,29 @@ class _FeatModelBase:
                 scores = self.score_all_items(uid).contiguous()
         finally:
             if restore is not None:
-                self.seqs[u], self.lens[u] = restore
+                restore()
         del keep
         out_ids = torch.empty((1, n_rec), dtype=torch.int64, device=self.device)
         out_sc = torch.empty((1, n_rec), dtype=torch.float32, device=self.device)
         masked_topk(self, scores, uid, n_rec, filter_consumed, out_ids, out_sc)
         return self._recs_to_host(out_ids, out_sc, return_scores)
+
+    def _swap_user_seq(self, u, seq, data_info, inner_id):
+        """Put the sequence built from ``seq`` in user ``u``'s row of the device sequence table for one
+        ``recommend_dynamic`` call; returns the callable that restores the row (None: the model reads no sequence)."""
+        from .dynamic_feats import build_rec_seq
+
+        if not hasattr(self, "seqs"):
+            return None
+        torch = self._torch
+        row, ln = build_rec_seq(seq, self.n_items, self.T, getattr(data_info, "item2id", None), inner_id)
+        old = (self.seqs[u].clone(), self.lens[u].clone())
+        self.seqs[u] = torch.from_numpy(row[0]).to(self.device)
+        self.lens[u] = int(ln[0])
+
+        def restore():
+            self.seqs[u], self.lens[u] = old
+        return restore
 
     def assign_oov(self, sparse_oov=None):
         """``assign_tf_variables_oov`` (``bases/tf_base.py:310-353``) on the device tables, in place."""
@@ -1279,6 +1293,250 @@ class Transformer(_SeqModelBase):
         _lib.check(_lib.lib.b200_transformer_target_attention(
             _lib.ptr(self.Qi), self.Qi.stride(0), _lib.ptr(S), self.T, self.D, _lib.ptr(lens), _lib.ptr(slot),
             _lib.ptr(items), n, grid_items, off, _lib.ptr(out_view), out_view.stride(0), _lib.current_stream()))
+
+
+SIM_MAX_L = 256                 # the shapes b200_sim_* accept (include/b200reco.h)
+SIM_MAX_S = 64
+SIM_MAX_TOPK = 32
+SIM_MAX_K = 64
+
+
+def recent_dual_sequences(user_consumed, n_users, n_items, long_max_len, short_max_len):
+    """get_recent_dual_seqs (libreco/batch/sequence.py:150-188): per user the last ``short_max_len`` consumed items
+    (short) and up to ``long_max_len`` items before them (long), padded with n_items.  A user with at most
+    ``short_max_len`` items has long length 1 over an all-pad row; the extra OOV row n_users is all pad with both
+    lengths 1.  Returns (long_seqs, long_lens, short_seqs, short_lens)."""
+    long_seqs = np.full((n_users + 1, long_max_len), n_items, dtype=np.int32)
+    short_seqs = np.full((n_users + 1, short_max_len), n_items, dtype=np.int32)
+    long_lens = np.ones(n_users + 1, dtype=np.int32)
+    short_lens = np.ones(n_users + 1, dtype=np.int32)
+    total = long_max_len + short_max_len
+    for u in range(n_users):
+        items = list(user_consumed[u]) if u in user_consumed else []
+        n = len(items)
+        if n <= short_max_len:
+            short_seqs[u, :n] = items
+            short_lens[u] = n
+            continue
+        if n < total:
+            long_seqs[u, :n - short_max_len] = items[:n - short_max_len]
+            long_lens[u] = n - short_max_len
+        else:
+            long_seqs[u] = items[n - total:n - short_max_len]
+            long_lens[u] = long_max_len
+        short_seqs[u] = items[n - short_max_len:]
+        short_lens[u] = short_max_len
+    return long_seqs, long_lens, short_seqs, short_lens
+
+
+def recent_dual_sequences_csr(consumed, n_items, long_max_len, short_max_len):
+    """Vectorised :func:`recent_dual_sequences` over a ConsumedCSR (arrival order), no per-user Python loop."""
+    indptr, idx = np.asarray(consumed.indptr, dtype=np.int64), consumed.idx
+    n_users = len(indptr) - 1
+    c = np.diff(indptr)
+    slen = np.minimum(c, short_max_len)
+    lreal = np.clip(c - short_max_len, 0, long_max_len)          # items before the short window, capped
+    t_l = np.arange(long_max_len, dtype=np.int64)[None, :]
+    t_s = np.arange(short_max_len, dtype=np.int64)[None, :]
+    long_seqs = np.full((n_users + 1, long_max_len), n_items, dtype=np.int32)
+    short_seqs = np.full((n_users + 1, short_max_len), n_items, dtype=np.int32)
+    src = (indptr[:-1] + c - short_max_len - lreal)[:, None] + t_l
+    valid = t_l < lreal[:, None]
+    long_seqs[:n_users][valid] = idx[src[valid]]
+    src = (indptr[1:] - slen)[:, None] + t_s
+    valid = t_s < slen[:, None]
+    short_seqs[:n_users][valid] = idx[src[valid]]
+    long_lens = np.append(np.where(c <= short_max_len, 1, lreal), 1).astype(np.int32)
+    short_lens = np.append(slen, 1).astype(np.int32)
+    return long_seqs, long_lens, short_seqs, short_lens
+
+
+class SIM(_SeqModelBase):
+    """libreco/algorithms/sim.py:193-304 (inference = the second stage, ``sim.py:206-207``): the item table
+    Gp = combine_seq_features(concat) Wp [n_items+1, K]; for a pair (u, n) with q = Gp[n] the GSU selects the
+    ``search_topk`` positions of the user's long sequence with the largest q . Gp[long_t] (masked positions score -1e9,
+    equal scores resolve to the lower position), the ESU runs ``multi_head_attention`` of q over the selected rows, the
+    short sequence gets Keras dot-product attention, and ``dense_nn`` (relu) runs on [long_out, short_out, user, item,
+    sparse.., dense..], then Dense(1).
+
+    Weights (besides the embedding tables): ``seq_proj`` [K', K], ``sim_attention`` {wq, wk, wv, wo [K, K]} (``wv``
+    the effective value map), ``num_heads``, ``mlp``, ``out_kernel``, ``out_bias`` — :func:`weights_io.sim_weights`
+    makes them from either TensorFlow graph's variables.  ``long_seqs`` / ``short_seqs`` and their lengths are the
+    reference's ``cached_long_seqs`` ... (:func:`recent_dual_sequences`).
+
+    All-items scoring (``b200_sim_pair_scores``) builds Gp, the item queries Qp = Gp Wq and the item part of the first
+    layer once per model and each user's Gp[long] Wk / Wv once per call, then scores every pair without building the
+    [B*N, F*K + 2K] concat.  Rows mode (``predict``, feature rows, ``recommend_dynamic`` with features, an MLP outside
+    the pair kernel's envelope) writes [long_out, short_out] into the concat (``b200_sim_attention``) for the relu MLP
+    on the library's dense layers."""
+
+    def __init__(self, spec, weights, long_seqs, long_lens, short_seqs, short_lens, user_consumed=None,
+                 task="ranking", search_topk=10, device=None):
+        raw_is = None
+        if not isinstance(spec, FeatSpec):
+            g = _spec_get(spec)
+            raw_is = g("item_sparse_unique") if g("item_sparse_col_index") else None
+        super().__init__(spec, weights, short_seqs, short_lens, user_consumed, task, device)
+        torch = self._torch
+        f32 = torch.float32
+        K, F = self.K, self.F
+        self.long_seqs = _dev(long_seqs, self.device, torch.int32)
+        self.long_lens = _dev(long_lens, self.device, torch.int32)
+        self.L, self.S = int(self.long_seqs.shape[1]), self.T
+        self.topk = int(search_topk)
+        H = self.num_heads = int(weights["num_heads"])
+        if K > SIM_MAX_K:
+            raise ValueError(f"SIM: embed size {K} > {SIM_MAX_K} is not supported")
+        if H < 1 or K % H:
+            raise ValueError(f"SIM: embed size {K} must be divisible by num_heads {H}")
+        if not 1 <= self.L <= SIM_MAX_L:
+            raise ValueError(f"SIM: long sequence length {self.L} outside [1, {SIM_MAX_L}]")
+        if not 1 <= self.S <= SIM_MAX_S:
+            raise ValueError(f"SIM: short sequence length {self.S} outside [1, {SIM_MAX_S}]")
+        if not 1 <= self.topk <= min(SIM_MAX_TOPK, self.L):
+            raise ValueError(f"SIM: search_topk {self.topk} outside [1, min({SIM_MAX_TOPK}, long length {self.L})]")
+        # combine_seq_features reads the item sparse columns as they are (multi-sparse sub-columns one by one)
+        self._item_sparse = _dev(raw_is, self.device, torch.int32) if raw_is is not None else self.spec.is_
+        att = weights["sim_attention"]
+        for k in ("wq", "wk", "wv", "wo"):
+            if np.shape(att[k]) != (K, K):
+                raise ValueError(f"SIM: attention {k} has shape {np.shape(att[k])}, expected ({K}, {K})")
+        self._wo64 = np.asarray(att["wo"], dtype=np.float64)
+        tr = lambda a: _dev(np.ascontiguousarray(np.asarray(a, dtype=np.float32).T), self.device, f32)   # noqa: E731
+        self._seq_projT, self._wqT, self._wkT, self._wvT = (tr(weights["seq_proj"]), tr(att["wq"]), tr(att["wk"]),
+                                                             tr(att["wv"]))
+        self.Wo = _dev(np.asarray(att["wo"], dtype=np.float32), self.device, f32)
+        if np.shape(weights["mlp"]["kernels"][0])[0] != (F + 2) * K:
+            raise ValueError(f"SIM: the first MLP layer takes {np.shape(weights['mlp']['kernels'][0])[0]} inputs, "
+                             f"expected (F + 2)*K = ({F} + 2)*{K}")
+        self._rebuild_item_features()
+        self.extra = 2 * K
+        # reference order [long, short, user, item, sparse.., dense..] -> ours [user, item, sparse.., dense.., long, short]
+        perm = np.concatenate([np.arange(2 * K, (F + 2) * K), np.arange(0, 2 * K)])
+        self.mlp = self._upload_mlp(permute_mlp_input(weights["mlp"], perm))
+
+    def _rebuild_item_features(self):
+        """Gp = combine_seq_features(concat) Wp [n_items+1, K] (sim.py:197-199), the item queries Qp = Gp Wq and their
+        transposes for the pair kernel: once per set of tables (again after ``assign_oov``)."""
+        torch = self._torch
+        n = self.n_items + 1
+        parts = [self.t["item_embeds"]]
+        if self._item_sparse is not None:
+            parts.append(self.t["sparse_embeds"][self._item_sparse.long()].reshape(n, -1))
+        if self.spec.id_ is not None:
+            cols = torch.as_tensor(self.spec.item_dense_cols, device=self.device)
+            parts.append((self.spec.id_[:, :, None] * self.t["dense_embeds"][cols][None]).reshape(n, -1))
+        G = torch.cat(parts, dim=1).contiguous()
+        if G.shape[1] != self._seq_projT.shape[1]:
+            raise ValueError(f"SIM: the item feature table has {G.shape[1]} columns, the sequence projection takes "
+                             f"{self._seq_projT.shape[1]}")
+        self.Gp = linear(G, self._seq_projT, None, ACT_NONE, impl="f32")
+        self.Qp = linear(self.Gp, self._wqT, None, ACT_NONE, impl="f32")
+        self.GpT = self.Gp.t().contiguous()
+        self.QpT = self.Qp.t().contiguous()
+
+    def _slots(self, users_d):
+        """The given users' long / short rows and lengths and their keys / values Gp[long] Wk, Gp[long] Wv."""
+        u = users_d.long()
+        ls, ll = self.long_seqs[u].contiguous(), self.long_lens[u].contiguous()
+        ss, sl = self.seqs[u].contiguous(), self.lens[u].contiguous()
+        g = self.Gp[ls.view(-1).long()]
+        Kl = linear(g, self._wkT, None, ACT_NONE, impl="f32")
+        Vl = linear(g, self._wvT, None, ACT_NONE, impl="f32")
+        return ls, ll, ss, sl, Kl, Vl
+
+    def _pair_dims(self):
+        dims = [w.shape[0] for w, _, _ in self.mlp]
+        return dims[0], dims[1], dims[2] if len(dims) == 3 else 0
+
+    def _hoistable(self):
+        """The pair kernel takes 2 or 3 Dense layers of at most 256, 128, 64 units whose shared memory fits."""
+        if len(self.mlp) not in (2, 3):
+            return False
+        need = _lib.lib.b200_sim_pair_smem_bytes(self.K, self.L, self.S, self.topk, *self._pair_dims())
+        return 0 < need <= self._torch.cuda.get_device_properties(self.device).shared_memory_per_block_optin
+
+    def score_all_items(self, user_ids_d):
+        """sim.py:249-304 over (these users) x (every item): per call each user's keys / values, then every pair in
+        ``b200_sim_pair_scores``.  The item part of the first layer and W_att = [Wo W1_long ; W1_short] (multiplied in
+        float64) are made once per model."""
+        torch = self._torch
+        if not self._hoistable():
+            return super().score_all_items(user_ids_d)
+        N, FK, K = self.n_items, self.F * self.K, self.K
+        if "_item_part" not in self.__dict__:
+            xi = self._side_concat("item", torch.arange(N, device=self.device))
+            self._item_part = self._first_layer_partial("item", xi, False).t().contiguous()       # [H1, N]
+            W1 = self.mlp[0][0].double().cpu().numpy()                                             # [H1, FK + 2K]
+            w_att = np.concatenate([self._wo64 @ W1[:, FK:FK + K].T, W1[:, FK + K:FK + 2 * K].T], axis=0)
+            self._w_att = _dev(w_att.astype(np.float32), self.device, torch.float32)              # [2K, H1]
+            three = len(self.mlp) == 3
+            self._sim_tail = (self.mlp[1][0].t().contiguous(), self.mlp[2][0].t().contiguous() if three else None)
+        PiT = self._item_part
+        W2, W3 = self._sim_tail
+        H1, H2, H3 = self._pair_dims()
+        b = int(user_ids_d.numel())
+        scores = torch.empty((b, N), dtype=torch.float32, device=self.device)
+        for r0 in range(0, b, 65535):
+            u = user_ids_d[r0:r0 + 65535]
+            nb = int(u.numel())
+            Pu = self._first_layer_partial("user", self._side_concat("user", u), True)     # [nb, H1] incl. bias
+            ls, ll, ss, sl, Kl, Vl = self._slots(u)
+            out = scores[r0:r0 + nb]
+            _lib.check(_lib.lib.b200_sim_pair_scores(
+                _lib.ptr(self.GpT), _lib.ptr(self.QpT), self.GpT.stride(0), N, _lib.ptr(self.Gp), self.Gp.stride(0),
+                _lib.ptr(ls), ls.stride(0), _lib.ptr(ll), _lib.ptr(ss), ss.stride(0), _lib.ptr(sl), _lib.ptr(Kl),
+                _lib.ptr(Vl), _lib.ptr(Pu), nb, _lib.ptr(PiT), PiT.stride(0), K, self.num_heads, self.L, self.S,
+                self.topk, H1, H2, H3, _lib.ptr(self._w_att), _lib.ptr(W2), _lib.ptr(self.mlp[1][1]), _lib.ptr(W3),
+                _lib.ptr(self.mlp[2][1]) if W3 is not None else None, _lib.ptr(self.out_kernel), self.out_bias,
+                _lib.ptr(out), out.stride(0), _lib.current_stream()))
+        return scores
+
+    def _seq_block(self, users_d, items_d, n, grid_items, row_offset, out_view, gsu_pos=None):
+        """[long_out, short_out] of each row, every distinct user (grid slot) of the chunk prepared once."""
+        torch = self._torch
+        if grid_items > 0:
+            u0 = row_offset // grid_items
+            u1 = (row_offset + n - 1) // grid_items
+            su, slot, items, off = users_d[u0:u1 + 1], None, None, row_offset - u0 * grid_items
+        else:
+            su, inv = torch.unique(users_d, return_inverse=True)
+            slot, items, off = inv.to(torch.int32).contiguous(), items_d.to(torch.int64).contiguous(), 0
+        ls, ll, ss, sl, Kl, Vl = self._slots(su)
+        _lib.check(_lib.lib.b200_sim_attention(
+            _lib.ptr(self.Gp), self.Gp.stride(0), _lib.ptr(self.Qp), self.Qp.stride(0), self.K, self.num_heads,
+            _lib.ptr(ls), ls.stride(0), _lib.ptr(ll), _lib.ptr(Kl), _lib.ptr(Vl), self.L, _lib.ptr(ss), ss.stride(0),
+            _lib.ptr(sl), self.S, self.topk, _lib.ptr(self.Wo), _lib.ptr(slot), _lib.ptr(items), n, grid_items, off,
+            _lib.ptr(out_view), out_view.stride(0), _lib.ptr(gsu_pos), _lib.current_stream()))
+
+    def attention_rows(self, users, items):
+        """([long_out, short_out] [R, 2K], the GSU's selected positions int32 [R, search_topk] in ascending order) of
+        explicit (user, item) rows — the rows-mode kernel on its own."""
+        torch = self._torch
+        u = torch.as_tensor(np.asarray(users, dtype=np.int64)).to(self.device)
+        i = torch.as_tensor(np.asarray(items, dtype=np.int64)).to(self.device)
+        n = int(u.numel())
+        out = torch.empty((n, 2 * self.K), dtype=torch.float32, device=self.device)
+        pos = torch.empty((n, self.topk), dtype=torch.int32, device=self.device)
+        if n:
+            self._seq_block(u, i, n, 0, 0, out, pos)
+        return out, pos
+
+    def _swap_user_seq(self, u, seq, data_info, inner_id):
+        """Both rows of user ``u`` from ``seq`` (``build_dual_seq``, recommendation/preprocess.py:49-76)."""
+        from .dynamic_feats import build_dual_seq
+
+        ls, ll, ss, sl = build_dual_seq(seq, self.n_items, self.L, self.S, getattr(data_info, "item2id", None),
+                                        inner_id)
+        tables = (self.long_seqs, self.long_lens, self.seqs, self.lens)
+        old = [t[u].clone() for t in tables]
+        for t, v in zip(tables, (ls[0], ll[0], ss[0], sl[0])):
+            t[u] = self._torch.as_tensor(v).to(self.device)
+
+        def restore():
+            for t, v in zip(tables, old):
+                t[u] = v
+        return restore
 
 
 class TwoTower:

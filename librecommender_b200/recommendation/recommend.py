@@ -63,10 +63,10 @@ def check_dynamic_rec_feats(model_name, user, user_feats, seq):
 def recommend_tf_feat(model, user_ids, n_rec, user_feats, seq, filter_consumed, random_rec, inner_id=False):
     """recommend.py:81-105 for the feature models.  The reference tiles a B*N-row feed
     (``process_tf_feat``) and runs the TF graph; here ``model.b200_engine`` — a
-    :mod:`librecommender_b200.feat_models` engine (FM / DeepFM / DIN / YouTubeRanking) built from the
+    :mod:`librecommender_b200.feat_models` engine (FM / DeepFM / DIN / YouTubeRanking / AutoInt / Transformer / SIM) built from the
     model's saved variables — scores the implicit (user, item) grid on the GPU and the consumed
     filter + top-K run on the score rows.  A single-user call with ``user_feats`` / ``seq`` goes through
-    ``engine.recommend_dynamic`` (explicit per-row feature matrix / replaced sequence row)."""
+    ``engine.recommend_dynamic`` (explicit per-row feature matrix / replaced sequence row; both of SIM's rows)."""
     from .. import _lib
 
     engine = getattr(model, "b200_engine", None)

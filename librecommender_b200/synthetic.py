@@ -236,6 +236,31 @@ def make_transformer_weights(rng, spec, K, num_heads=1, n_layers=1, max_seq_len=
     return w
 
 
+def make_sim_weights(rng, spec, K, num_heads=2, hidden=(200, 80), use_bn=True, version="keras", combiner="sqrtn"):
+    """SIM variables (libreco/algorithms/sim.py:193-304) in the raw shapes of the graph TensorFlow `version` builds:
+    the sequence projection ``seq_proj`` [K', K] with K' = K (1 + item sparse columns + item dense columns), the
+    attention over width K ("keras" [K, H, hd] / [H, hd, K], "legacy" [K, K], v applied to the projected keys), the
+    first stage (``first_stage_mlp`` on [target, pooled long sequence] and its head) and the second stage ``mlp`` on
+    [long_out, short_out, user, item, sparse.., dense..] with its head.  ``weights_io.sim_weights`` turns them into
+    the engine's dict.  F counts a multi-sparse group as one field unless ``combiner == "normal"``."""
+    from .weights_io import autoint_scheme
+
+    scheme = autoint_scheme(version)
+    w = make_embeddings(rng, spec, K, linear=False)
+    n_sparse = spec["n_sparse"]
+    info = spec.get("multi_sparse_combine_info")
+    if info is not None and combiner != "normal":
+        n_sparse = int(info["field_offset"][0]) + len(info["field_offset"])
+    F = 2 + n_sparse + spec["n_dense"]
+    Kp = K * (1 + len(spec["item_sparse_col_index"]) + len(spec["item_dense_col_index"]))
+    w.update(sim_scheme=scheme, num_heads=int(num_heads), seq_proj=_glorot(rng, (Kp, K)),
+             sim_mha=_mha_raw(rng, scheme, K, K, int(num_heads)),
+             first_stage_mlp=make_mlp(rng, 2 * K, hidden, use_bn), first_stage_out_kernel=_glorot(rng, (hidden[-1], 1)),
+             first_stage_out_bias=np.float32(0.01).reshape(1), mlp=make_mlp(rng, (F + 2) * K, hidden, use_bn),
+             out_kernel=_glorot(rng, (hidden[-1], 1)), out_bias=np.float32(-0.02).reshape(1))
+    return w
+
+
 def make_rnn4rec_weights(rng, n_items, K, hidden_units=(16,), rnn_type="gru", use_layer_norm=False, scheme="keras"):
     """RNN4Rec variables (libreco/algorithms/rnn4rec.py:151-237, layers/recurrent.py:4-63) in the raw shapes of the
     graph `scheme` names: "keras" GRU ``kernel [in, 3H]``, ``recurrent_kernel [H, 3H]``, ``bias [2, 3H]``, keras LSTM

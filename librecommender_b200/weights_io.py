@@ -192,7 +192,14 @@ def default_tf_names(model_name, n_hidden, use_bn, use_tf_attention=False, n_lay
                      rnn_type="gru", use_layer_norm=False):
     """{engine weight key: TF variable name (or nested dict / list of names)} for the auto-named
     variables of `model_name` in {"FM", "DeepFM", "DIN", "YouTubeRanking", "TwoTower", "AutoInt", "Transformer",
-    "RNN4Rec", "Caser", "WaveNet"}.
+    "RNN4Rec", "Caser", "WaveNet", "SIM"}.
+
+    SIM (sim.py:193-304, creation order: the sequence projection, the first stage, the attention, the second stage):
+    ``dense/kernel:0`` (``seq_proj``), the ``first_stage_mlp`` stack and its head ``dense_1``; "keras"
+    ``multi_head_attention/{query,key,value,attention_output}/kernel:0`` and the head ``dense_2``; "legacy" q, k, v,
+    out ``dense_2`` .. ``dense_5`` and the head ``dense_6``; the ``second_stage_mlp`` stack (under ``mlp``).  Returned
+    under ``seq_proj``, ``first_stage_mlp``, ``first_stage_out_kernel`` / ``_bias``, ``sim_mha``, ``mlp``,
+    ``out_kernel`` and ``out_bias``.
 
     Caser (caser.py:194-220; `n_layers` = max_seq_len T): the horizontal ``conv1d[_i]/{kernel,bias}:0`` for
     i = 0..T-1 under ``convs``, the vertical ``conv1d_T`` under ``vertical``, the head ``dense/{kernel,bias}:0``.
@@ -226,6 +233,8 @@ def default_tf_names(model_name, n_hidden, use_bn, use_tf_attention=False, n_lay
     (per-layer {query, key, value, attention_output | output}), ``out_kernel``, ``out_bias``."""
     if model_name == "RNN4Rec":
         return _rnn4rec_names(scheme, rnn_type, n_layers, use_layer_norm)
+    if model_name == "SIM":
+        return _sim_names(scheme, n_hidden, use_bn)
     if model_name in ("Caser", "WaveNet"):
         return _conv_names(model_name, n_layers)
     if model_name == "Transformer":
@@ -407,6 +416,53 @@ def transformer_tf_variables(raw):
     _put_tf_names(out, {k: v for k, v in names.items() if k not in ("out_kernel", "out_bias")}, raw)
     out[names["out_kernel"]] = np.asarray(raw["out_kernel"], dtype=np.float32).reshape(-1, 1)
     out[names["out_bias"]] = np.asarray(raw["out_bias"], dtype=np.float32).reshape(1)
+    return out
+
+
+def _sim_names(scheme, n_hidden, use_bn):
+    _check_mha_scheme(scheme, "SIM")
+    head = _dense_name(2 if scheme == "keras" else 6)
+    return {"seq_proj": "dense/kernel:0", "first_stage_mlp": _mlp_names("first_stage_mlp", n_hidden, use_bn),
+            "first_stage_out_kernel": "dense_1/kernel:0", "first_stage_out_bias": "dense_1/bias:0",
+            "sim_mha": _mha_tf_names(scheme, "", 0, 2), "mlp": _mlp_names("second_stage_mlp", n_hidden, use_bn),
+            "out_kernel": f"{head}/kernel:0", "out_bias": f"{head}/bias:0"}
+
+
+def sim_tf_shapes(scheme, K, num_heads):
+    """Expected shapes for :func:`default_tf_names` ("SIM"): ``seq_proj [K', K]`` (K' not known here), the attention
+    over width K (:func:`_mha_tf_shapes`), the heads ``[H_last, 1]`` and ``[1]``; the MLP stacks are not checked."""
+    return {"seq_proj": (None, K), "first_stage_mlp": None, "first_stage_out_kernel": (None, 1),
+            "first_stage_out_bias": (1,), "sim_mha": _mha_tf_shapes(scheme, K, K, num_heads), "mlp": None,
+            "out_kernel": (None, 1), "out_bias": (1,)}
+
+
+def sim_weights(raw):
+    """Engine weight dict for :class:`feat_models.SIM` from the raw variables of either graph: ``raw`` holds the
+    embedding tables, ``sim_scheme``, ``seq_proj``, ``sim_mha`` (as :func:`default_tf_names` names it), ``num_heads``,
+    ``mlp``, ``out_kernel`` and ``out_bias``; the raw attention, the first-stage variables and other entries pass
+    through (the engine ignores them), so :func:`sim_tf_variables` writes the dict back losslessly.  legacy: the value
+    Dense acts on the PROJECTED keys, so the effective value map Wk Wv' is multiplied in float64 and then cast."""
+    _check_mha_scheme(raw["sim_scheme"], "SIM")
+    w = dict(raw)
+    w["seq_proj"] = np.asarray(raw["seq_proj"], dtype=np.float32)
+    w["sim_attention"] = _mha_engine(raw["sim_mha"], raw["sim_scheme"])
+    w["out_kernel"] = np.asarray(raw["out_kernel"], dtype=np.float32).reshape(-1)
+    w["out_bias"] = np.float32(np.asarray(raw["out_bias"]).reshape(-1)[0])
+    return w
+
+
+def sim_tf_variables(raw):
+    """Raw SIM variables of either graph (the layout :func:`sim_weights` takes) -> ``{TF variable name: array}`` named
+    by :func:`default_tf_names` for the raw dict's scheme: what ``save_tf_variables`` writes as
+    ``<name>_tf_variables.npz``, and the inverse of ``load_reference_tf_model(..., "SIM", ...)``."""
+    mlp = raw["mlp"]
+    names = default_tf_names("SIM", len(mlp["kernels"]), mlp.get("bn_in") is not None, scheme=raw["sim_scheme"])
+    out = to_tf_variables({k: raw[k] for k in EMBEDDING_SCOPE if k in raw})
+    _put_tf_names(out, {k: v for k, v in names.items() if not k.endswith(("out_kernel", "out_bias"))}, raw)
+    for k in ("first_stage_out_kernel", "out_kernel"):
+        out[names[k]] = np.asarray(raw[k], dtype=np.float32).reshape(-1, 1)
+    for k in ("first_stage_out_bias", "out_bias"):
+        out[names[k]] = np.asarray(raw[k], dtype=np.float32).reshape(1)
     return out
 
 
@@ -784,7 +840,9 @@ def load_reference_tf_model(path, model_name, arch, n_hidden, use_bn, use_tf_att
     legacy) off the names, checks every name and shape and returns the layout of ``feat_models.RNN4Rec``.  Caser
     reads max_seq_len off the vertical kernel; WaveNet takes ``n_filters``, ``n_blocks``, ``n_layers_per_block`` and
     ``dilated`` (False for a TF1-trained model, whose causal layers all have dilation 1).  Both check every name and
-    shape and return the layout of ``feat_models.Caser`` / ``feat_models.WaveNet``."""
+    shape and return the layout of ``feat_models.Caser`` / ``feat_models.WaveNet``.  SIM takes ``num_heads`` (default 2),
+    reads its attention graph (keras or legacy) off the names, checks every name and shape and returns the layout of
+    ``feat_models.SIM``; the first-stage variables are read too and carried along."""
     from .feat_models import from_tf_variables
 
     npz = np.load(os.path.join(path, f"{model_name}_tf_variables.npz"))
@@ -817,6 +875,16 @@ def load_reference_tf_model(path, model_name, arch, n_hidden, use_bn, use_tf_att
         return transformer_weights(w)
     if num_heads is None:
         num_heads = 2
+    if arch == "SIM":
+        scheme = "keras" if "multi_head_attention/query/kernel:0" in npz.files else "legacy"
+        names = default_tf_names(arch, n_hidden, use_bn, scheme=scheme)
+        names.update(extra_names or {})
+        K = int(np.shape(npz[EMBEDDING_SCOPE["user_embeds"]])[1])
+        if K % int(num_heads):
+            raise ValueError(f"SIM: embed size {K} must be divisible by num_heads {num_heads}")
+        w.update(resolve_tf_names(npz, names, sim_tf_shapes(scheme, K, int(num_heads))), sim_scheme=scheme,
+                 num_heads=int(num_heads))
+        return sim_weights(w)
     if arch == "AutoInt":
         hds = autoint_head_dims(att_embed_size)
         scheme = "keras" if "multi_head_attention/query/kernel:0" in npz.files else "legacy"
