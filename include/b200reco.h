@@ -83,15 +83,25 @@ int b200_score_rows_f32(const float* U, int64_t ldu, const int64_t* user_ids, in
  * per split, out[3] user tiles, out[4] sampled tiles per split, out[5] TMA stages, out[6] = 10 x CTAs
  * per cluster (2: every item tile is fetched from L2 once per pair of user tiles and TMA-multicast to
  * both CTAs) + MMA organisation actually used (1, 2 or 3 as in the tune code; 3 runs as 1 when
- * d > 128), out[7] records per candidate list (n_out >= 8).  Without a device the plan is the one
- * of a 132-SM H100.
+ * d > 128), out[7] records per candidate list (n_out >= 8); out[8] pre-pass stride and out[9] item
+ * tiles the pre-pass visits (sampled fraction f = out[9] / item tiles) when n_out >= 10; out[10 + k]
+ * = the speculative rank pre_k of k_row = k, k = 0 .. 288, when n_out >= 299.  Without a device the
+ * plan is the one of a 132-SM H100.
  * b200_recommend_embed_tune (process-wide, not thread-safe; 0 keeps a value): organisation code =
  * 100 x cluster size (1|2) + 10 x MMA organisation (1: one N=256 group per item tile; 2: two N=128
  * groups; 3: two N=128 groups pipelined across item tiles, each half-tile epilogue running under the
  * MMAs of the other half; d > 128 falls back to 1) + epilogue variant (3: divergent per-lane group
  * tests, 5: one warp vote per 64-column step + quad-mask record stores; default 215), and the rank
- * coefficient c of the speculative threshold (about c * k_row items are expected above it). */
+ * coefficient c in [1, 16] of the linear speculative rule pre_k = margin + ceil(c * f * k_row)
+ * (about c * k_row items are expected above the threshold; a non-zero c selects that rule, the
+ * margin is set by b200_recommend_embed_debug(-margin), default 12). */
 int b200_recommend_embed_tune(int32_t organisation_code, float pre_rank_coef);
+/* speculative threshold of b200_recommend_embed (process-wide, not thread-safe): the pre-pass visits
+ * every pre_stride-th item tile (2 .. 32; 0 = default 8) and pre_k is the smallest r with
+ * P[Binomial(k_row + 16, f) >= r] <= delta, the failure budget per row (1e-9 .. 1e-2; 0 = default
+ * 1e-5).  Selects this rule (the default) again after a non-zero rank coefficient of
+ * b200_recommend_embed_tune. */
+int b200_recommend_embed_speculation(int32_t pre_stride, float delta);
 /* profiling diagnostics only (results are wrong while level > 0): ablate parts of the main pass
  * (1: nothing is collected, cold epilogue steps only; 2: no epilogue at all, MMAs and stage releases only) */
 int b200_recommend_embed_debug(int32_t ablate_level);

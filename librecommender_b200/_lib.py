@@ -34,6 +34,7 @@ SIGNATURES = {
     "b200_embed_catalog_bytes": (c_int, [c_int64, c_int32, POINTER(c_size_t)]),
     "b200_embed_catalog_prepare": (c_int, [_P, c_int64, c_int64, c_int32, _P, c_size_t, _P]),
     "b200_recommend_embed_tune": (c_int, [c_int32, c_float]),
+    "b200_recommend_embed_speculation": (c_int, [c_int32, c_float]),
     "b200_recommend_embed_debug": (c_int, [c_int32]),
     "b200_recommend_embed_plan": (c_int, [c_int64, c_int64, c_int32, c_int32, _P, c_int32]),
     "b200_recommend_embed_workspace_bytes": (c_int, [c_int64, c_int64, c_int32, c_int32, POINTER(c_size_t)]),

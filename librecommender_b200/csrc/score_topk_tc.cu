@@ -9,10 +9,10 @@
 //                                        scaled by a power of two so that max ||I_i|| is in [64,128)
 //   prep_users   gather U[user_ids] -> fp16 [B_pad, d_pad], every row scaled by its own power of
 //                two (row norm in [64,128)); per-row error bound eps, k_row
-//   sweep<PRE>   tensor-core pass over every 16th item tile that only records, per user row, the
+//   sweep<PRE>   tensor-core pass over every pre_stride-th item tile that only records, per user row, the
 //                maximum coarse score of each sampled 128-item block (one coalesced store per
 //                tile, no divergence); guess_kernel turns the block maxima into a SPECULATIVE
-//                per-row threshold (the pre_k-th largest block maximum).
+//                per-row threshold (the pre_k-th largest block maximum, pre_k from a failure budget).
 //   sweep<MAIN>  persistent wgmma kernel over all item tiles: TMA -> smem (SWIZZLE_128B, multi-stage
 //                ring, item tiles shared by a 2-CTA cluster through TMA multicast) -> wgmma (fp16 in,
 //                fp32 accumulate in registers, 128x256 tile = two warpgroups x 64 user rows) -> the
@@ -40,6 +40,7 @@
 // reference's filter rule applies (ranking.py:38), so removing consumed candidates still leaves
 // the exact top-K.  Rows that cannot be bounded (k_row too large, failed speculation, too many
 // near-ties) are flagged in row_status and re-run by the caller on the exact materialised path.
+#include <cmath>
 #include <type_traits>
 #include "common.cuh"
 #include "ptx_sm90.cuh"
@@ -62,7 +63,12 @@ constexpr int STEP = 64;       // accumulator columns per epilogue vote
 constexpr int W_PRE = 2;
 constexpr int KROW_MAX = 288;  // fast-path limit for k_row = K + c_u
 constexpr int MAX_KB = 4;      // d_pad <= 256
-constexpr int PRE_STRIDE = 16; // the pre-pass visits every 16th item tile of a split
+// Speculation defaults (b200_recommend_embed_speculation): the pre-pass visits every PRE_STRIDE-th item
+// tile of a split, and a row's speculative threshold fails with probability at most PRE_DELTA (DESIGN §4).
+constexpr int PRE_STRIDE = 8;
+constexpr double PRE_DELTA = 1e-5;
+// items allowed for inside the 2 eps band below c_k when the speculative rank is chosen (DESIGN §4)
+constexpr int PRE_TIE_ALLOWANCE = 16;
 constexpr int A_KB_BYTES = TM * KBLK * 2;   // 16 KB
 constexpr int B_KB_BYTES = TN * KBLK * 2;   // 32 KB
 constexpr int MAXU = 3072;                  // finalize: collected elements per row (union of the lists)
@@ -104,6 +110,7 @@ struct SweepParams {
   int32_t B_pad, m_tiles, n_splits, tiles_per_split, total_tiles, KB, nstage;
   int32_t kb_stages;          // 1: a ring stage holds ONE 64-wide k-block of an item tile (d_pad > 128), 0: the whole tile
   int32_t n_pre_tiles;        // sampled tiles per split in the pre-pass
+  int32_t pre_stride;         // the pre-pass visits every pre_stride-th tile of a split
   int32_t capg, trig;         // records per list / uncounted records that trigger a compaction
   int32_t ablate;             // diagnostics only (b200_recommend_embed_debug): 0 = normal operation
   uint32_t hint_ns;           // suspend-time hint of the mbarrier waits
@@ -165,9 +172,13 @@ __global__ void prep_items_kernel(const float* __restrict__ I, int64_t ldi, int6
   }
 }
 
+struct PreRank {   // speculative rank pre_k of every k_row (rank_table on the host)
+  int32_t k[KROW_MAX + 1];
+};
+
 __global__ void prep_users_kernel(const float* __restrict__ U, int64_t ldu,
                                   const int64_t* __restrict__ user_ids, int64_t B, int B_pad, int d,
-                                  int d_pad, int K, int64_t N, int filter, float pre_scale, int pre_margin,
+                                  int d_pad, int K, int64_t N, int filter, const __grid_constant__ PreRank pre_rank,
                                   const int64_t* __restrict__ indptr, int64_t n_users,
                                   const CatalogHeader* __restrict__ hdr,
                                   __half* __restrict__ A, RowMeta* __restrict__ meta,
@@ -212,10 +223,8 @@ __global__ void prep_users_kernel(const float* __restrict__ U, int64_t ldu,
     m.apply = apply;
     m.capped = k_row < k_full;
     m.k_row = (int32_t)k_row;
-    // speculative threshold = pre_k-th largest SAMPLED block maximum: about pre_k / f items of the
-    // whole catalogue lie above it (f = sampled fraction); pre_scale = c * f keeps that at
-    // >= c * k_row + 16 / f
-    m.pre_k = pre_margin + (int32_t)ceilf(pre_scale * (float)m.k_row);
+    // speculative threshold = pre_k-th largest SAMPLED block maximum
+    m.pre_k = pre_rank.k[m.k_row];
     m.active = real;
     meta[row] = m;
     row_tau_key[row] = 0u;  // below every finite float
@@ -377,7 +386,7 @@ sweep_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
   const int cid = (int)blockIdx.x / CL, n_clusters = (int)gridDim.x / CL;
   const int m_groups = p.m_tiles / CL;                    // host guarantees m_tiles % CL == 0
   const int n_units = m_groups * p.n_splits;              // units per cluster-rank
-  constexpr int STRIDE = PRE ? PRE_STRIDE : 1;
+  const int STRIDE = PRE ? p.pre_stride : 1;
   constexpr uint16_t CL_MASK = (uint16_t)((1u << CL) - 1u);
 
   if (threadIdx.x == 0) {
@@ -1267,15 +1276,18 @@ static int g_nh = 1;               // MMA organisation of an item tile (1 x N=25
                                    // the first overlaps the second; 3 = 2 x N=128 pipelined across tiles)
 static int g_ablate = 0;           // b200_recommend_embed_debug
 static int g_hint_ns = 20000;      // suspend-time hint of the mbarrier waits in the sweep kernels
-static int g_pre_margin = 12;      // additive part of the speculative rank: pre_k = margin + coef * f * k_row sampled block maxima
-static float g_pre_coef = 2.0f;    // speculative rank target = g_pre_coef * k_row (+ 16 / sampled fraction)
+static int g_pre_stride = PRE_STRIDE;   // b200_recommend_embed_speculation
+static double g_pre_delta = PRE_DELTA;
+static float g_pre_coef = 0.f;     // non-zero: linear speculative rank pre_k = margin + coef * f * k_row (A/B runs, tests)
+static int g_pre_margin = 12;      // its additive part (b200_recommend_embed_debug)
 
 struct Plan {
   int B_pad, d_pad, KB, m_tiles, total_tiles, n_splits, tiles_per_split, nstage, n_pre_tiles, kb_stages;
   int W, n_lists, capg, trig;
   int CL, NH;        // CTAs per cluster (TMA multicast of the item tiles), MMA groups per item tile
   bool use_pre;
-  float pre_scale;   // g_pre_coef x sampled fraction of the item tiles (see prep_users_kernel)
+  int pre_stride;    // the pre-pass visits every pre_stride-th item tile of a split
+  int pre_sampled;   // item tiles the pre-pass visits (f = pre_sampled / total_tiles)
   int64_t N_pad;
   size_t smem_bytes;
   // workspace offsets
@@ -1315,22 +1327,20 @@ static int make_plan(int64_t B, int64_t N, int d, Plan* pl) {
   }
   pl->tiles_per_split = (pl->total_tiles + bestS - 1) / bestS;
   pl->n_splits = (pl->total_tiles + pl->tiles_per_split - 1) / pl->tiles_per_split;
-  pl->n_pre_tiles = (pl->tiles_per_split + PRE_STRIDE - 1) / PRE_STRIDE;
+  pl->pre_stride = g_pre_stride;
+  pl->n_pre_tiles = (pl->tiles_per_split + pl->pre_stride - 1) / pl->pre_stride;
   pl->n_lists = pl->W * pl->n_splits;
   // speculation needs enough sampled blocks per row to take a stable order statistic
   pl->use_pre = (long)W_PRE * pl->n_splits * pl->n_pre_tiles >= 256;
-  {   // sampled fraction of the item tiles (every PRE_STRIDE-th tile of every split)
-    long sampled = 0;
-    for (int sp = 0; sp < pl->n_splits; ++sp) {
-      const int t0 = sp * pl->tiles_per_split;
-      const int t1 = t0 + pl->tiles_per_split < pl->total_tiles ? t0 + pl->tiles_per_split : pl->total_tiles;
-      sampled += (t1 - t0 + PRE_STRIDE - 1) / PRE_STRIDE;
-    }
-    pl->pre_scale = g_pre_coef * (float)sampled / (float)pl->total_tiles;
+  pl->pre_sampled = 0;   // every pre_stride-th tile of every split
+  for (int sp = 0; sp < pl->n_splits; ++sp) {
+    const int t0 = sp * pl->tiles_per_split;
+    const int t1 = t0 + pl->tiles_per_split < pl->total_tiles ? t0 + pl->tiles_per_split : pl->total_tiles;
+    pl->pre_sampled += (t1 - t0 + pl->pre_stride - 1) / pl->pre_stride;
   }
-  // With the speculative threshold about g_pre_coef * k_row + 16 / f candidates per row (<= ~1500
-  // at k_row = 288) are spread over the lists; the lists are sized for that and the compaction runs
-  // only when a list is about to overflow (the speculation was far off).
+  // With the speculative threshold a few times k_row candidates per row (<= ~1500 at k_row = 288 under
+  // the linear rule's defaults) are spread over the lists; the lists are sized for that and the
+  // compaction runs only when a list is about to overflow (the speculation was far off).
   pl->capg = (pl->use_pre && pl->n_lists >= 16) ? 128 : CAPG_MAX;
   pl->trig = pl->use_pre ? pl->capg : 96;
   const size_t budget = 227 * 1024 - 1024 /*align*/ - sizeof(SweepSmem) - (size_t)pl->KB * A_KB_BYTES;
@@ -1353,6 +1363,44 @@ static int make_plan(int64_t B, int64_t N, int d, Plan* pl) {
   pl->off_bm = off; off += al256((size_t)W_PRE * pl->n_splits * pl->n_pre_tiles * pl->B_pad * 4);
   pl->total = off + 256;
   return 0;
+}
+
+// Smallest r with P[Binomial(n, f) >= r] <= delta (n + 1 when no r <= n qualifies).
+static int binomial_rank(int n, double f, double delta) {
+  if (f >= 1.0) return n + 1;
+  const double log_odds = std::log(f) - std::log1p(-f);
+  double log_pmf = n * std::log1p(-f);   // log P[X = 0]
+  double cdf = 0.0;
+  for (int r = 0; r < n; ++r) {
+    cdf += std::exp(log_pmf);
+    if (1.0 - cdf <= delta) return r + 1;   // P[X >= r + 1] = 1 - P[X <= r]
+    log_pmf += std::log((double)(n - r) / (double)(r + 1)) + log_odds;
+  }
+  return n + 1;
+}
+
+// Speculative rank pre_k of every k_row for the plan's sampled fraction f, under the active rule.
+// Failure budget (default): speculation fails exactly when at least pre_k sampled block maxima exceed
+// c_k - 2 eps, and each such block holds a sampled item with coarse >= c_k - 2 eps.  About
+// n = k_row + PRE_TIE_ALLOWANCE items lie that high; when the item order does not depend on the scores,
+// the number of them in the sampled tiles is about Binomial(n, f), so pre_k = the smallest r with
+// P[Binomial(n, f) >= r] <= delta keeps the rate of failed rows (status 3, repaired on the exact path)
+// near delta.  Linear rule (a non-zero rank coefficient): pre_k = margin + ceil(coef * f * k_row).
+static void rank_table(const Plan& pl, int32_t* out) {
+  thread_local int32_t tab[KROW_MAX + 1];
+  thread_local double key_f = -1.0, key_delta = -1.0;
+  const double f = (double)pl.pre_sampled / (double)pl.total_tiles;
+  if (g_pre_coef != 0.f) {
+    const float pre_scale = g_pre_coef * (float)pl.pre_sampled / (float)pl.total_tiles;
+    for (int k = 0; k <= KROW_MAX; ++k) out[k] = g_pre_margin + (int32_t)ceilf(pre_scale * (float)k);
+    return;
+  }
+  if (f != key_f || g_pre_delta != key_delta) {   // recomputed only when the plan's f or delta changes
+    for (int k = 0; k <= KROW_MAX; ++k) tab[k] = binomial_rank(k + PRE_TIE_ALLOWANCE, f, g_pre_delta);
+    key_f = f;
+    key_delta = g_pre_delta;
+  }
+  memcpy(out, tab, sizeof(tab));
 }
 
 template <bool PRE, int EPI, int CL, int NH>
@@ -1465,11 +1513,21 @@ extern "C" int b200_recommend_embed_tune(int32_t epilogue_warps_per_quadrant, fl
   return 0;
 }
 
+extern "C" int b200_recommend_embed_speculation(int32_t pre_stride, float delta) {
+  B200_REQUIRE((pre_stride == 0 || (pre_stride >= 2 && pre_stride <= 32)) &&
+                   (delta == 0.f || (delta >= 1e-9f && delta <= 1e-2f)),
+               "b200_recommend_embed_speculation: stride 0 or 2..32, failure budget 0 or [1e-9, 1e-2]");
+  g_pre_stride = pre_stride ? pre_stride : PRE_STRIDE;
+  g_pre_delta = delta != 0.f ? (double)delta : PRE_DELTA;
+  g_pre_coef = 0.f;   // the failure-budget rule
+  return 0;
+}
+
 // Diagnostics (profiling only; results are WRONG while level 1 or 2 is set): 1 = the main pass collects
 // nothing (cold epilogue steps only), 2 = the main pass runs no epilogue at all (wait, MMA, release).
 extern "C" int b200_recommend_embed_debug(int32_t ablate_level) {
   // levels >= 100: suspend-time hint (ns) of the mbarrier waits of the sweep kernels = level - 100
-  // levels -1 .. -64: additive margin of the speculative rank (pre_k = margin + coef * f * k_row) = -level
+  // levels -1 .. -64: additive margin of the linear speculative rank (pre_k = margin + coef * f * k_row) = -level
   if (ablate_level < 0 && ablate_level >= -64) { g_pre_margin = -ablate_level; return 0; }
   if (ablate_level >= 100) { g_hint_ns = ablate_level - 100; return 0; }
   B200_REQUIRE(ablate_level >= 0 && ablate_level <= 2, "b200_recommend_embed_debug: level 0..2 (or 100 + hint ns)");
@@ -1485,6 +1543,8 @@ extern "C" int b200_recommend_embed_plan(int64_t B, int64_t N, int32_t d, int32_
   if (int rc = make_plan(B, N, d, &pl)) return rc;
   out[0] = pl.use_pre ? 1 : 0; out[1] = pl.n_splits; out[2] = pl.tiles_per_split; out[3] = pl.m_tiles;
   out[4] = pl.n_pre_tiles; out[5] = pl.nstage; out[6] = pl.CL * 10 + pl.NH; out[7] = pl.capg;
+  if (n_out >= 10) { out[8] = pl.pre_stride; out[9] = pl.pre_sampled; }
+  if (n_out >= 10 + KROW_MAX + 1) rank_table(pl, out + 10);
   return 0;
 }
 
@@ -1527,8 +1587,10 @@ extern "C" int b200_recommend_embed(const float* U, int64_t ldu, const int64_t* 
   const CatalogHeader* hdr = (const CatalogHeader*)catalog;
   const __half* Ih = (const __half*)((const char*)catalog + 256);
 
+  PreRank pre_rank;
+  rank_table(pl, pre_rank.k);
   prep_users_kernel<<<(unsigned)ceil_div64((int64_t)pl.B_pad * 32, 256), 256, 0, stream>>>(
-      U, ldu, user_ids, B, pl.B_pad, d, pl.d_pad, K, N, filter, pl.pre_scale, g_pre_margin, indptr, n_users, hdr, A, meta,
+      U, ldu, user_ids, B, pl.B_pad, d, pl.d_pad, K, N, filter, pre_rank, indptr, n_users, hdr, A, meta,
       tau, status);
   count_launch();
   // cnt and ghist are adjacent in the workspace: one memset
@@ -1542,7 +1604,8 @@ extern "C" int b200_recommend_embed(const float* U, int64_t ldu, const int64_t* 
   SweepParams sp;
   sp.N = N; sp.B_pad = pl.B_pad; sp.m_tiles = pl.m_tiles; sp.n_splits = pl.n_splits;
   sp.tiles_per_split = pl.tiles_per_split; sp.total_tiles = pl.total_tiles; sp.KB = pl.KB;
-  sp.nstage = pl.nstage; sp.kb_stages = pl.kb_stages; sp.n_pre_tiles = pl.n_pre_tiles; sp.capg = pl.capg; sp.trig = pl.trig;
+  sp.nstage = pl.nstage; sp.kb_stages = pl.kb_stages; sp.n_pre_tiles = pl.n_pre_tiles;
+  sp.pre_stride = pl.pre_stride; sp.capg = pl.capg; sp.trig = pl.trig;
   sp.meta = meta; sp.row_tau_key = tau;
   sp.row_status = status; sp.ghist = ghist; sp.cand_r = cand_r; sp.cand_cnt = cnt;
   sp.blockmax = bm; sp.ablate = g_ablate; sp.hint_ns = (uint32_t)g_hint_ns;
