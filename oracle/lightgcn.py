@@ -6,6 +6,10 @@ Follows ``libreco/algorithms/torch_modules/lightgcn_module.py`` (reference @ 746
 * ``embedding_propagation`` (:66-88): E^{l+1} = L E^l, output = mean over the n_layers+1 terms,
   split into users / items.
 
+* ``propagate64`` / ``propagate64_grad``: the same layer mean in float64 for any value array
+  (including the non-symmetric values edge dropout leaves, :90-96), and its gradient
+  ``mean_l (L^T)^l G``.
+
 Pinned against the unmodified reference module run in the build container
 (``tests/golden/gen_lightgcn.py`` -> ``tests/golden/lightgcn_*.npz``).
 """
@@ -43,3 +47,19 @@ def propagate(L, user_embeds, item_embeds, n_layers):
         layers.append((L @ layers[-1]).astype(np.float32))
     out = np.mean(np.stack(layers, axis=1), axis=1, dtype=np.float32)
     return out[: len(user_embeds)], out[len(user_embeds):]
+
+
+def propagate64(L, E0, n_layers):
+    """mean over l = 0..n_layers of L^l E0 in float64; ``L`` is any scipy sparse matrix."""
+    L = sp.csr_matrix(L, dtype=np.float64)
+    cur = np.asarray(E0, dtype=np.float64)
+    total = cur.copy()
+    for _ in range(n_layers):
+        cur = L @ cur
+        total += cur
+    return total / (n_layers + 1)
+
+
+def propagate64_grad(L, G, n_layers):
+    """Gradient of ``(propagate64(L, E0, n_layers) * G).sum()`` w.r.t. E0: mean_l (L^T)^l G."""
+    return propagate64(sp.csr_matrix(L, dtype=np.float64).T, G, n_layers)

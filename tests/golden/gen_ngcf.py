@@ -19,7 +19,9 @@ from libreco.algorithms.torch_modules.ngcf_module import NGCFModel  # noqa: E402
 OUT = os.path.dirname(os.path.abspath(__file__))
 
 
-def case(seed, n_users, n_items, d, layers, mean_deg, name):
+def case(seed, n_users, n_items, d, layers, mean_deg, name, head_users=0):
+    """``head_users > 0``: those users also consume item 0 and nobody consumes item n_items - 1, so
+    the graph has a row above the SpMM's long-row threshold and an item with only its self loop."""
     rng = np.random.default_rng(seed)
     consumed = {}
     w = 1.0 / np.arange(1, n_items + 1)
@@ -29,6 +31,10 @@ def case(seed, n_users, n_items, d, layers, mean_deg, name):
         items = rng.choice(n_items, size=c, replace=False, p=w).tolist()
         if c > 3:
             items.append(items[0])
+        if head_users:
+            items = [i for i in items if i != n_items - 1]
+            if u < head_users:
+                items.append(0)
         consumed[u] = items
     consumed[n_users - 1] = []               # isolated user: only its self loop
     torch.manual_seed(seed)
@@ -54,6 +60,15 @@ def case(seed, n_users, n_items, d, layers, mean_deg, name):
     print(name, ue.shape, ie.shape, lap._nnz())
 
 
+CASES = {
+    "d16": lambda: case(41, 120, 90, 16, (16, 16, 16), 7, "d16"),
+    "d64": lambda: case(42, 80, 150, 64, (64, 32), 12, "d64"),
+    # layer-input widths 10 / 24 / 36 / 132 cover the scalar (lpr 16), vec4 (LPR 8, 16) and scalar T = 5
+    # SpMM paths; the head item's row (over 1 024 users + self loop) takes the long-row chunk kernels
+    "d10": lambda: case(43, 1200, 150, 10, (24, 7), 4, "d10", head_users=1100),
+    "d36": lambda: case(44, 1060, 60, 36, (132, 20), 4, "d36", head_users=1040),
+}
+
 if __name__ == "__main__":
-    case(41, 120, 90, 16, (16, 16, 16), 7, "d16")
-    case(42, 80, 150, 64, (64, 32), 12, "d64")
+    for key in sys.argv[1:] or CASES:
+        CASES[key]()
