@@ -524,6 +524,15 @@ int b200_interacted_seqs(const int64_t* indptr, const int32_t* idx, int64_t n_us
                          const int64_t* items, int64_t n, int32_t max_seq_len, int32_t pad_index,
                          const int64_t* rand_pos, uint64_t seed, uint64_t step, int32_t* seqs,
                          int32_t* lens, void* stream);
+/* SIM's dual sequences (libreco/batch/sequence.py:94-147, get_dual_seqs; batch/collators.py:114-116) with the same
+ * position rule p and the same draw stream: short = the s = min(p, S) items before p, long = the up to L items before
+ * those (none when p <= S), each padded with pad_index, lengths max(count, 1).  A user with no items gets p = 0 (two
+ * all-pad rows of length 1), where the reference raises. */
+int b200_interacted_dual_seqs(const int64_t* indptr, const int32_t* idx, int64_t n_users, const int64_t* users,
+                              const int64_t* items, int64_t n, int32_t long_max_len, int32_t short_max_len,
+                              int32_t pad_index, const int64_t* rand_pos, uint64_t seed, uint64_t step,
+                              int32_t* long_seqs, int32_t* long_lens, int32_t* short_seqs, int32_t* short_lens,
+                              void* stream);
 
 /* ---- AutoInt inference (libreco/algorithms/autoint.py:146-168, layers/attention.py:67-138) -------
  * X [F, K] = the pair's field embeddings [user, item, sparse.., dense..] (the b200_feat_forward concat).
@@ -642,6 +651,36 @@ int b200_sim_pair_scores(const float* GpT, const float* QpT, int64_t ldt, int64_
                          int32_t H, int32_t L, int32_t S, int32_t topk, int32_t H1, int32_t H2, int32_t H3,
                          const float* W_att, const float* W2, const float* b2, const float* W3, const float* b3,
                          const float* w_out, float b_out, float* scores, int64_t lds, void* stream);
+
+/* ---- SIM training (libreco/algorithms/sim.py:193-304, training mode) -------------------------------------------
+ * Row r carries its own long sequence long_seqs[r, :L] (length long_lens[r]) and target item items[r]; Gp as above.
+ * b200_sim_gsu_forward: one warp per row.  sel_pos [R, topk] receives the GSU positions in ascending order, selected
+ *   by the very code of b200_sim_attention (same scores, same tie rule: the same positions bit for bit on the same
+ *   Gp and sequence), pooled [R, ldp] (K columns) the first stage's sum_{t < long_len} Gp[long_t] over t ascending
+ *   (long_len clamped to [0, L]; pad ids inside the length are summed).
+ * b200_sim_esu_forward: per head h of hd = K / H columns, one query Q[r] over its topk selected keys
+ *   Ksel / Vsel [R * topk, ldkv] (row r * topk + i = the i-th selected position): logits (Q_h . Ksel_h) / sqrt(hd) as
+ *   one fmaf chain, p = softmax over the visible keys, O[r]_h = sum_i p_i Vsel_h (i ascending).  Key i is visible when
+ *   sel_pos[r, i] < max(long_lens[r], 1); a hidden key gets probability exactly 0.  P [R, H, topk] is saved.
+ * b200_sim_esu_backward: WRITES dQ [R, lddq], dKsel and dVsel [R * topk, lddkv] from dO and the saved P; hidden keys'
+ *   rows are exact zeros.  Both: one warp per (row, head), no atomics, bit-identical repeats.
+ * b200_sim_long_backward: ADDS (float atomics) dpooled[r] into dGp[long_seqs[r, t]] for t < long_len and
+ *   dXsel[r * topk + i] into dGp[long_seqs[r, sel_pos[r, i]]].
+ * Supported: 1 <= K <= 64 (H dividing K), 1 <= L <= 256, 1 <= topk <= min(32, L); anything else returns -2 before
+ * launching. */
+int b200_sim_gsu_forward(const float* Gp, int64_t ldg, int32_t K, const int64_t* items, const int32_t* long_seqs,
+                         int64_t ld_long, const int32_t* long_lens, int32_t L, int32_t topk, int64_t R,
+                         int32_t* sel_pos, float* pooled, int64_t ldp, void* stream);
+int b200_sim_esu_forward(const float* Q, int64_t ldq, const float* Ksel, const float* Vsel, int64_t ldkv,
+                         const int32_t* sel_pos, const int32_t* long_lens, int64_t R, int32_t K, int32_t H,
+                         int32_t topk, float* O, int64_t ldo, float* P, void* stream);
+int b200_sim_esu_backward(const float* Q, int64_t ldq, const float* Ksel, const float* Vsel, int64_t ldkv,
+                          const int32_t* sel_pos, const int32_t* long_lens, int64_t R, int32_t K, int32_t H,
+                          int32_t topk, const float* P, const float* dO, int64_t lddo, float* dQ, int64_t lddq,
+                          float* dKsel, float* dVsel, int64_t lddkv, void* stream);
+int b200_sim_long_backward(const int32_t* long_seqs, int64_t ld_long, const int32_t* long_lens, int32_t L,
+                           const int32_t* sel_pos, int32_t topk, int64_t R, int32_t K, const float* dpooled,
+                           int64_t ldp, const float* dXsel, int64_t ldx, float* dGp, int64_t ldg, void* stream);
 
 /* ---- Transformer training (libreco/algorithms/transformer.py:203-339 in training mode) ------------------------
  * The dense products over the R*T sequence rows (Q / K / V / O projections, FFN, MLP and their gradients) run on

@@ -118,6 +118,8 @@ SIGNATURES = {
                                       _P, _P, c_int64, _P, _P, _P]),
     "b200_interacted_seqs": (c_int, [_P, _P, c_int64, _P, _P, c_int64, c_int32, c_int32, _P, c_uint64, c_uint64,
                                      _P, _P, _P]),
+    "b200_interacted_dual_seqs": (c_int, [_P, _P, c_int64, _P, _P, c_int64, c_int32, c_int32, c_int32, _P, c_uint64,
+                                          c_uint64, _P, _P, _P, _P, _P]),
     "b200_gather_dot": (c_int, [_P, c_int64, _P, _P, c_int64, _P, c_int64, c_int32, c_int32, c_float, c_float, _P, _P]),
     "b200_autoint_rows": (c_int, [_P, c_int64, c_int64, c_int32, c_int32, c_int32, c_int32, _P, _P, _P, c_float, c_int32,
                                   _P, _P]),
@@ -138,7 +140,15 @@ SIGNATURES = {
     "b200_sim_pair_scores": (c_int, [_P, _P, c_int64, c_int64, _P, c_int64, _P, c_int64, _P, _P, c_int64, _P, _P, _P,
                                      _P, c_int64, _P, c_int64, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32,
                                      c_int32, c_int32, _P, _P, _P, _P, _P, _P, c_float, _P, c_int64, _P]),
-    "b200_autoint_attention_forward": (c_int, [_P, c_int64, _P, c_int64, _P, c_int64, c_int64, c_int32, c_int32,
+    "b200_sim_gsu_forward": (c_int, [_P, c_int64, c_int32, _P, _P, c_int64, _P, c_int32, c_int32, c_int64, _P, _P,
+                                     c_int64, _P]),
+    "b200_sim_esu_forward": (c_int, [_P, c_int64, _P, _P, c_int64, _P, _P, c_int64, c_int32, c_int32, c_int32, _P,
+                                     c_int64, _P, _P]),
+    "b200_sim_esu_backward": (c_int, [_P, c_int64, _P, _P, c_int64, _P, _P, c_int64, c_int32, c_int32, c_int32, _P,
+                                      _P, c_int64, _P, c_int64, _P, _P, c_int64, _P]),
+    "b200_sim_long_backward": (c_int, [_P, c_int64, _P, c_int32, _P, c_int32, c_int64, c_int32, _P, c_int64, _P,
+                                       c_int64, _P, c_int64, _P]),
+    "b200_autoint_attention_forward":(c_int, [_P, c_int64, _P, c_int64, _P, c_int64, c_int64, c_int32, c_int32,
                                                c_int32, c_float, _P, c_int64, _P, _P]),
     "b200_autoint_attention_backward": (c_int, [_P, c_int64, _P, c_int64, _P, c_int64, _P, c_int64, _P, _P, c_int64,
                                                 c_int64, c_int32, c_int32, c_int32, c_float, _P, _P, _P, c_int64, _P]),

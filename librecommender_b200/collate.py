@@ -105,3 +105,40 @@ class DeviceSequenceBuilder:
             _lib.ptr(lens), _lib.current_stream()))
         self.step += 1
         return seqs, lens
+
+
+class DeviceDualSequenceBuilder:
+    """``get_dual_seqs`` (libreco/batch/sequence.py:94-147) on the device: SIM's per-sample long and short windows
+    (``batch/collators.py:114-116``), the dual counterpart of :class:`DeviceSequenceBuilder` with the same position
+    rule and draw stream.  Parity mode passes the positions of :func:`interacted_positions_host`: ``get_dual_seqs``
+    draws from the same ``random.randrange`` stream.  A user with no items gets position 0 (two all-pad rows of length
+    1) where the reference raises.  Returns (long_seqs [n, L], long_lens, short_seqs [n, S], short_lens), int32."""
+
+    def __init__(self, consumed, long_max_len: int, short_max_len: int, pad_index: int, seed: int = 42,
+                 device="cuda"):
+        self.consumed, self.pad_index = consumed, int(pad_index)
+        self.long_max_len, self.short_max_len = int(long_max_len), int(short_max_len)
+        self.seed, self.step, self.device = int(seed), 0, device
+
+    def __call__(self, users_d, items_d, rand_pos_d=None):
+        import torch
+
+        from . import _lib
+
+        indptr, idx = self.consumed.device(users_d.device)
+        n, L, S = users_d.numel(), self.long_max_len, self.short_max_len
+        dev = users_d.device
+        long_seqs = torch.empty((n, L), dtype=torch.int32, device=dev)
+        short_seqs = torch.empty((n, S), dtype=torch.int32, device=dev)
+        long_lens = torch.empty(n, dtype=torch.int32, device=dev)
+        short_lens = torch.empty(n, dtype=torch.int32, device=dev)
+        users_d = users_d.to(torch.int64).contiguous()
+        items_d = items_d.to(torch.int64).contiguous()
+        if rand_pos_d is not None:
+            rand_pos_d = rand_pos_d.to(torch.int64).contiguous()
+        _lib.check(_lib.lib.b200_interacted_dual_seqs(
+            _lib.ptr(indptr), _lib.ptr(idx), self.consumed.n_users, _lib.ptr(users_d), _lib.ptr(items_d), n, L, S,
+            self.pad_index, _lib.ptr(rand_pos_d), self.seed, self.step, _lib.ptr(long_seqs), _lib.ptr(long_lens),
+            _lib.ptr(short_seqs), _lib.ptr(short_lens), _lib.current_stream()))
+        self.step += 1
+        return long_seqs, long_lens, short_seqs, short_lens

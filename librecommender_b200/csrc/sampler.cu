@@ -17,8 +17,8 @@
 //   mode 2 "popular"    (negatives.py:34-43): inverse-CDF draw from p ~ freq^0.75 (cdf given),
 //                        one re-draw when equal to the positive.
 // Layout: negatives of positive j are out[j*num_neg : (j+1)*num_neg] (collators.py:231-232).
-// Also here: the per-sample history windows (b200_interacted_seqs) and the unique candidate sampler of the
-// sampled-class losses (b200_unique_candidates, training/tf_trainer.py:162-245).
+// Also here: the per-sample history windows (b200_interacted_seqs, SIM's b200_interacted_dual_seqs) and the unique
+// candidate sampler of the sampled-class losses (b200_unique_candidates, training/tf_trainer.py:162-245).
 #include "common.cuh"
 #include "../../include/b200reco.h"
 
@@ -128,16 +128,16 @@ __global__ void sample_negatives_kernel(const int64_t* __restrict__ users,
 // (random.randrange(0, len) in the reference: `rand_pos` carries that stream in parity mode, else
 // Philox(seed, step, j)).  seq = consumed[max(0, position - L) : position], padded with pad_index;
 // len = min(position, L), 1 when position == 0 (reference :56-58).
-__global__ void interacted_seqs_kernel(const int64_t* __restrict__ indptr, const int32_t* __restrict__ idx,
-                                       int64_t n_users, const int64_t* __restrict__ users,
-                                       const int64_t* __restrict__ items, int64_t n, int L, int32_t pad_index,
-                                       const int64_t* __restrict__ rand_pos, uint64_t seed, uint64_t step,
-                                       int32_t* __restrict__ seqs, int32_t* __restrict__ lens) {
-  const int64_t j = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int lane = threadIdx.x & 31;
-  if (j >= n) return;
+// One warp per sample: the sample's position in its user's list and the list's bounds [beg, beg + clen).
+__device__ __forceinline__ int64_t interacted_position(const int64_t* __restrict__ indptr,
+                                                       const int32_t* __restrict__ idx, int64_t n_users,
+                                                       const int64_t* __restrict__ users,
+                                                       const int64_t* __restrict__ items, int64_t j,
+                                                       const int64_t* __restrict__ rand_pos, uint64_t seed,
+                                                       uint64_t step, int lane, int64_t& beg) {
   const int64_t u = users[j];
-  int64_t beg = 0, end = 0;
+  int64_t end = 0;
+  beg = 0;
   if (u >= 0 && u < n_users) { beg = indptr[u]; end = indptr[u + 1]; }
   const int64_t clen = end - beg;
   const int64_t item = items[j];
@@ -158,11 +158,54 @@ __global__ void interacted_seqs_kernel(const int64_t* __restrict__ indptr, const
       pos = bounded(r.x, r.y, clen);
     }
   }
+  return pos;
+}
+
+__global__ void interacted_seqs_kernel(const int64_t* __restrict__ indptr, const int32_t* __restrict__ idx,
+                                       int64_t n_users, const int64_t* __restrict__ users,
+                                       const int64_t* __restrict__ items, int64_t n, int L, int32_t pad_index,
+                                       const int64_t* __restrict__ rand_pos, uint64_t seed, uint64_t step,
+                                       int32_t* __restrict__ seqs, int32_t* __restrict__ lens) {
+  const int64_t j = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (j >= n) return;
+  int64_t beg;
+  const int64_t pos = interacted_position(indptr, idx, n_users, users, items, j, rand_pos, seed, step, lane, beg);
   const int64_t count = pos < L ? pos : L;
   const int64_t start = pos - count;
   for (int t = lane; t < L; t += 32)
     seqs[j * L + t] = t < count ? __ldg(idx + beg + start + t) : pad_index;
   if (lane == 0) lens[j] = pos == 0 ? 1 : (int32_t)count;
+}
+
+// ---- SIM's per-sample dual sequences at collate time (libreco/batch/sequence.py:94-147, called from
+// batch/collators.py:114-116).  Same position rule as above.  With p the position: short = consumed[p - s : p],
+// s = min(p, S); long = the up to L items before the short window, consumed[p - s - l : p - s], l = min(p - S, L)
+// when p > S and 0 otherwise.  Both padded with pad_index; each length is max(count, 1) (position 0 gives two
+// all-pad rows of length 1, 1 <= p <= S an all-pad long row of length 1).
+__global__ void interacted_dual_seqs_kernel(const int64_t* __restrict__ indptr, const int32_t* __restrict__ idx,
+                                            int64_t n_users, const int64_t* __restrict__ users,
+                                            const int64_t* __restrict__ items, int64_t n, int L, int S,
+                                            int32_t pad_index, const int64_t* __restrict__ rand_pos, uint64_t seed,
+                                            uint64_t step, int32_t* __restrict__ long_seqs,
+                                            int32_t* __restrict__ long_lens, int32_t* __restrict__ short_seqs,
+                                            int32_t* __restrict__ short_lens) {
+  const int64_t j = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (j >= n) return;
+  int64_t beg;
+  const int64_t pos = interacted_position(indptr, idx, n_users, users, items, j, rand_pos, seed, step, lane, beg);
+  const int64_t s_cnt = pos < S ? pos : S;
+  const int64_t l_cnt = pos <= S ? 0 : (pos - S < L ? pos - S : L);
+  const int64_t s_start = pos - s_cnt, l_start = s_start - l_cnt;
+  for (int t = lane; t < L; t += 32)
+    long_seqs[j * L + t] = t < l_cnt ? __ldg(idx + beg + l_start + t) : pad_index;
+  for (int t = lane; t < S; t += 32)
+    short_seqs[j * S + t] = t < s_cnt ? __ldg(idx + beg + s_start + t) : pad_index;
+  if (lane == 0) {
+    long_lens[j] = l_cnt > 0 ? (int32_t)l_cnt : 1;
+    short_lens[j] = s_cnt > 0 ? (int32_t)s_cnt : 1;
+  }
 }
 
 // ---- unique candidate sampler of the sampled-class losses (YouTubeRetrieval training): TensorFlow's
@@ -271,6 +314,23 @@ extern "C" int b200_interacted_seqs(const int64_t* indptr, const int32_t* idx, i
   if (n == 0) return 0;
   sampler::interacted_seqs_kernel<<<(unsigned)ceil_div64(n * 32, 256), 256, 0, (cudaStream_t)stream>>>(
       indptr, idx, n_users, users, items, n, max_seq_len, pad_index, rand_pos, seed, step, seqs, lens);
+  count_launch();
+  B200_CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int b200_interacted_dual_seqs(const int64_t* indptr, const int32_t* idx, int64_t n_users,
+                                         const int64_t* users, const int64_t* items, int64_t n, int32_t long_max_len,
+                                         int32_t short_max_len, int32_t pad_index, const int64_t* rand_pos,
+                                         uint64_t seed, uint64_t step, int32_t* long_seqs, int32_t* long_lens,
+                                         int32_t* short_seqs, int32_t* short_lens, void* stream) {
+  B200_REQUIRE(indptr && idx && users && items && long_seqs && long_lens && short_seqs && short_lens,
+               "b200_interacted_dual_seqs: null pointer");
+  B200_REQUIRE(long_max_len >= 1 && short_max_len >= 1, "b200_interacted_dual_seqs: lengths must be positive");
+  if (n == 0) return 0;
+  sampler::interacted_dual_seqs_kernel<<<(unsigned)ceil_div64(n * 32, 256), 256, 0, (cudaStream_t)stream>>>(
+      indptr, idx, n_users, users, items, n, long_max_len, short_max_len, pad_index, rand_pos, seed, step, long_seqs,
+      long_lens, short_seqs, short_lens);
   count_launch();
   B200_CUDA_OK(cudaGetLastError());
   return 0;

@@ -11,8 +11,9 @@
 // Hidden logits are fl32(logit - 1e9), as Keras adds the mask; with no valid key the weights are the softmax of those
 // rounded values, uniform whenever |logit| < 32.
 //
-// Both modes compute the GSU scores with the same chain, acc = fmaf(q[d], Gp[t][d], acc) over d ascending from 0, on
-// the same Gp, so they select the same positions.
+// The rows kernel's GSU (scores, warp top-k, compaction) is sim::gsu_select of sim_gsu.cuh, which the training GSU
+// kernel (sim_train.cu) calls too.  Both modes compute the GSU scores with the same chain,
+// acc = fmaf(q[d], Gp[t][d], acc) over d ascending from 0, on the same Gp, so they select the same positions.
 //   * b200_sim_attention (rows mode): one warp per (slot, item) row writes [long_out || short_out] into the sequence
 //     block of the concat the library's dense layers read.
 //   * b200_sim_pair_scores (grid mode): one thread per (slot, item) pair, the first MLP layer re-associated as
@@ -24,15 +25,16 @@
 
 #include "../../include/b200reco.h"
 #include "common.cuh"
+#include "sim_gsu.cuh"
 
 namespace b200 {
 namespace {
 
-constexpr int SIM_MAX_L = 256;
-constexpr int SIM_MAX_S = 64;
-constexpr int SIM_MAX_TOPK = 32;
-constexpr int SIM_MAX_K = 64;
-constexpr float MASK_NEG = 1.0e9f;
+constexpr int SIM_MAX_L = sim::MAX_L;
+constexpr int SIM_MAX_S = sim::MAX_S;
+constexpr int SIM_MAX_TOPK = sim::MAX_TOPK;
+constexpr int SIM_MAX_K = sim::MAX_K;
+constexpr float MASK_NEG = sim::MASK_NEG;
 
 __host__ __device__ inline int64_t round_up64(int64_t n, int64_t m) { return (n + m - 1) / m * m; }
 
@@ -71,56 +73,7 @@ __global__ void __launch_bounds__(ROWS_THREADS) sim_attention_kernel(const __gri
     const int llen = min(max(a.long_lens[slot], 0), L), slen = min(max(a.short_lens[slot], 0), S);
     const float* kl = a.Kl + slot * L * K;
     const float* vl = a.Vl + slot * L * K;
-    // GSU scores: lane owns positions t = lane + 32 j
-    float sc[SIM_MAX_L / 32];
-#pragma unroll
-    for (int j = 0; j < SIM_MAX_L / 32; ++j) {
-      const int t = lane + 32 * j;
-      float s = -MASK_NEG;
-      if (t < llen) {
-        const float* g = a.Gp + (int64_t)__ldg(ls + t) * a.ldg;
-        float acc = 0.f;
-        for (int d = 0; d < K; ++d) acc = fmaf(__ldg(q + d), __ldg(g + d), acc);
-        s = acc != acc ? -INFINITY : acc;
-      }
-      sc[j] = s;
-    }
-    // top-k: k rounds of a warp arg-max over (score desc, position asc) among the positions not yet taken
-    uint32_t selm = 0;
-    for (int i = 0; i < k; ++i) {
-      float bv = -INFINITY;
-      int bt = INT_MAX;
-#pragma unroll
-      for (int j = 0; j < SIM_MAX_L / 32; ++j) {
-        const int t = lane + 32 * j;
-        if (t < L && !((selm >> j) & 1u) && (sc[j] > bv || (sc[j] == bv && t < bt))) {
-          bv = sc[j];
-          bt = t;
-        }
-      }
-#pragma unroll
-      for (int off = 16; off > 0; off >>= 1) {
-        const float ov = __shfl_xor_sync(0xffffffffu, bv, off);
-        const int ot = __shfl_xor_sync(0xffffffffu, bt, off);
-        if (ov > bv || (ov == bv && ot < bt)) {
-          bv = ov;
-          bt = ot;
-        }
-      }
-      if ((bt & 31) == lane) selm |= 1u << (bt >> 5);
-    }
-    // the selected positions in ascending order
-    int cnt = 0;
-#pragma unroll
-    for (int j = 0; j < SIM_MAX_L / 32; ++j) {
-      const bool mine = (selm >> j) & 1u;
-      const uint32_t ball = __ballot_sync(0xffffffffu, mine);
-      if (mine) sel_sm[wib][cnt + __popc(ball & ((1u << lane) - 1u))] = lane + 32 * j;
-      cnt += __popc(ball);
-    }
-    __syncwarp();
-    const int pi = lane < k ? sel_sm[wib][lane] : 0;
-    __syncwarp();
+    const int pi = sim::gsu_select(a.Gp, a.ldg, q, ls, llen, K, L, k, sel_sm[wib], lane);
     if (a.gsu_pos && lane < k) a.gsu_pos[r * k + lane] = pi;
     // ESU: lane i owns the i-th selected key for the logits, lanes own columns d = lane, lane + 32 for the mix
     float o[2] = {0.f, 0.f};

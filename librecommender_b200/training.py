@@ -152,20 +152,25 @@ class _Trainer:
         for n, shp in _mha_2d(self.scheme, d_in, D).items():
             self.params[prefix + n] = self._var(lw[n], shp)
 
-    def _mha_forward(self, prefix, X, core):
-        """q = X Wq, k = X Wk, v = (k if legacy else X) Wv, (o, lse) = core(q, k, v), then o Wo; returns (o Wo, cache)."""
+    def _mha_forward(self, prefix, X, core, kv=None):
+        """q = X Wq, k = S Wk, v = (k if legacy else S) Wv with S = ``kv`` (cross attention) or X, (o, lse) =
+        core(q, k, v), then o Wo; returns (o Wo, cache)."""
         wq, wk, wv, wo = (self.params[prefix + n] for n in _MHA_VARS[self.scheme])
+        src = X if kv is None else kv
         q = linear(X, wq.t().contiguous(), None, ACT_NONE, cache_split=False)
-        k = linear(X, wk.t().contiguous(), None, ACT_NONE, cache_split=False)
-        v = linear(k if self.scheme == "legacy" else X, wv.t().contiguous(), None, ACT_NONE, cache_split=False)
+        k = linear(src, wk.t().contiguous(), None, ACT_NONE, cache_split=False)
+        v = linear(k if self.scheme == "legacy" else src, wv.t().contiguous(), None, ACT_NONE, cache_split=False)
         o, lse = core(q, k, v)
-        return linear(o, wo.t().contiguous(), None, ACT_NONE, cache_split=False), dict(x=X, q=q, k=k, v=v, o=o, lse=lse)
+        return (linear(o, wo.t().contiguous(), None, ACT_NONE, cache_split=False),
+                dict(x=X, kv=kv, q=q, k=k, v=v, o=o, lse=lse))
 
     def _mha_backward(self, prefix, c, dY, core_backward):
         """Backward of ``_mha_forward`` given dY = d loss / d (o Wo): the four weight gradients ADDED into ``grads``;
-        returns d loss / d X.  ``core_backward(c, dO)`` returns (dq, dk, dv)."""
+        returns d loss / d X, or (d loss / d X, d loss / d kv) for cross attention.  ``core_backward(c, dO)`` returns
+        (dq, dk, dv)."""
         p, g = self.params, self.grads
         nq, nk, nv, no = (prefix + n for n in _MHA_VARS[self.scheme])
+        src = c["x"] if c["kv"] is None else c["kv"]
         g[no] += _weight_grad(dY, c["o"]).t()                     # dWo = O^T dY
         dO = linear(dY, p[no], None, ACT_NONE, cache_split=False)  # dO = dY Wo^T
         dq, dk, dv = core_backward(c, dO)
@@ -173,39 +178,47 @@ class _Trainer:
             g[nv] += _weight_grad(dv, c["k"]).t()                 # dWv' = Kproj^T dV
             self._axpy(dk, linear(dv, p[nv], None, ACT_NONE, cache_split=False))
         g[nq] += _weight_grad(dq, c["x"]).t()
-        g[nk] += _weight_grad(dk, c["x"]).t()
+        g[nk] += _weight_grad(dk, src).t()
         dX = linear(dq, p[nq], None, ACT_NONE, cache_split=False)
-        self._axpy(dX, linear(dk, p[nk], None, ACT_NONE, cache_split=False))
+        dS = dX if c["kv"] is None else None
+        if dS is None:
+            dS = linear(dk, p[nk], None, ACT_NONE, cache_split=False)
+        else:
+            self._axpy(dS, linear(dk, p[nk], None, ACT_NONE, cache_split=False))
         if self.scheme == "keras":
-            g[nv] += _weight_grad(dv, c["x"]).t()
-            self._axpy(dX, linear(dv, p[nv], None, ACT_NONE, cache_split=False))
-        return dX
+            g[nv] += _weight_grad(dv, src).t()
+            self._axpy(dS, linear(dv, p[nv], None, ACT_NONE, cache_split=False))
+        return dX if c["kv"] is None else (dX, dS)
 
     def _export_mha(self, prefix, d_in, D):
         """One layer's variables in their raw shapes (the inverse of ``_init_mha``)."""
         return {n: self.params[prefix + n].cpu().numpy().reshape(shp)
                 for n, shp in _mha_tf_shapes(self.scheme, d_in, D, self.H).items()}
 
-    def _dense1_forward(self, h):
-        """Logits of the Dense(1) head (variables ``out_kernel`` [C], ``out_bias`` [1]) on ``h`` [R, C]."""
+    def _dense1_forward(self, h, prefix="out_"):
+        """Logits of the Dense(1) head (variables ``{prefix}kernel`` [C], ``{prefix}bias`` [1]) on ``h`` [R, C]."""
         torch = self._torch
         p = self.params
         R = int(h.shape[0])
         logit = torch.empty(R, dtype=torch.float32, device=self.device)
         _lib.check(_lib.lib.b200_concat_dense(_lib.ptr(h), h.stride(0), h.shape[1], None, 0, 0, None, 0, 0,
-                                              _lib.ptr(p["out_kernel"]), 0.0, R, _lib.ptr(logit), _lib.current_stream()))
-        logit += p["out_bias"]                      # device scalar add (the bias is a trainable variable)
+                                              _lib.ptr(p[prefix + "kernel"]), 0.0, R, _lib.ptr(logit),
+                                              _lib.current_stream()))
+        logit += p[prefix + "bias"]                 # device scalar add (the bias is a trainable variable)
         return logit
 
-    def _dense1_backward(self, h, logit, labels_d):
-        """Loss and the Dense(1) head's gradients (written into ``grads``); returns (loss, d loss / d h)."""
+    def _dense1_backward(self, h, logit, labels_d, prefix="out_", dlogit=None):
+        """Loss and the Dense(1) head's gradients (written into ``grads``); returns (loss, d loss / d h).  Given
+        ``dlogit`` (d loss / d logit of a loss taken elsewhere) only the gradients are formed and the loss is None."""
         p, g = self.params, self.grads
         R = int(h.shape[0])
-        loss, dlogit = self._loss(logit, labels_d)
-        self._col_sum(h, g["out_kernel"], dlogit)
-        self._col_sum(dlogit, g["out_bias"])
-        # d h = dlogit (x) out_kernel: the Dense(1) transposed, on the library's dense kernel (din = 1)
-        dh = linear(dlogit.view(R, 1), p["out_kernel"].view(-1, 1), None, False, cache_split=False)
+        loss = None
+        if dlogit is None:
+            loss, dlogit = self._loss(logit, labels_d)
+        self._col_sum(h, g[prefix + "kernel"], dlogit)
+        self._col_sum(dlogit, g[prefix + "bias"])
+        # d h = dlogit (x) kernel: the Dense(1) transposed, on the library's dense kernel (din = 1)
+        dh = linear(dlogit.view(R, 1), p[prefix + "kernel"].view(-1, 1), None, False, cache_split=False)
         return loss, dh
 
     def _items(self, items_d):
@@ -2154,3 +2167,244 @@ def _ctypes_ptr_array(n):
     import ctypes
 
     return ctypes.c_void_p * n
+
+
+SIM_LOSSES = {"cross_entropy": 0, "focal": 1}
+
+
+class SIMTrainer(_SeqTrainer):
+    """SIM training step on the device: ``libreco/algorithms/sim.py:193-304`` in training mode (no dropout), mean
+    sigmoid cross entropy or focal loss on ``alpha * z1 + beta * z2``, TF-Adam.  Every row carries its own dual
+    sequences (``collate.DeviceDualSequenceBuilder``): ``long_seqs`` [R, L], ``short_seqs`` [R, S] and their lengths,
+    clamped to [1, L] / [1, S] as the collator gives them.
+
+        G (the item feature table, concat mode, from the CURRENT tables) -> Gp = G Wp (b200_linear_f32, the bits the
+        inference engine selects from) -> q = Gp[item] (b200_gather_rows)
+        first stage: b200_sim_gsu_forward also sums pooled = sum_{t < long_len} Gp[long_t] -> dense_nn "fs_" on
+            [q, pooled] -> Dense(1) = z1
+        second stage: the GSU selection (b200_sim_gsu_forward) -> Gp of the selected rows -> multi_head_attention
+            of q over them (projections on the dense kernels, b200_sim_esu_forward) -> short attention
+            (b200_transformer_target_attention) -> K1 gather -> dense_nn on [fields.., long_out, short_out] ->
+            Dense(1) = z2
+        -> b200_pointwise_loss -> the reverse (b200_sim_esu_backward, b200_transformer_target_attention_backward,
+        the dense kernels) -> dGp: query and short-key rows through b200_scatter_add_rows, the selected and pooled
+        rows through b200_sim_long_backward -> dWp = G^T dGp, dG = dGp Wp^T folded into the tables ->
+        b200_feat_backward -> b200_adam_dense_dev
+
+    ``weights``: the RAW variables of either attention graph, as ``synthetic.make_sim_weights`` and
+    ``weights_io.load_reference_tf_model(..., "SIM", ...)`` give them.  The second stage's first kernel is held with
+    the sequence block after the field blocks (the inference engine's layout) and permuted back on export.
+    ``export_weights`` returns the same raw layout (``weights_io.sim_weights`` makes the serving dict,
+    ``weights_io.sim_tf_variables`` the reference's variable names).  ``reg`` applies to the embedding tables only.
+
+    Raises ``ValueError`` before anything is launched for alpha or beta outside [0, 1], an unknown ``loss_type``, the
+    rating task, shapes outside the kernels' envelope (K <= 64 with heads dividing K, L <= 256, S <= 64,
+    search_topk <= min(32, L)), multi-sparse fields with a combiner other than "normal" (the pooling backward is not
+    built) and first layers whose width disagrees with the fields."""
+
+    def __init__(self, spec, weights, search_topk=10, alpha=1.0, beta=1.0, loss_type="cross_entropy", use_bn=True,
+                 lr=1e-3, epsilon=1e-5, device=None, task="ranking"):
+        from .feat_models import _spec_get
+
+        if not (0.0 <= float(alpha) <= 1.0 and 0.0 <= float(beta) <= 1.0):
+            raise ValueError(f"SIMTrainer: alpha {alpha} and beta {beta} must lie in [0, 1]")
+        if task != "ranking":
+            raise ValueError(f"SIMTrainer: task {task!r} is not supported, SIM trains the ranking task only")
+        if loss_type not in SIM_LOSSES:
+            raise ValueError(f"SIMTrainer: unsupported loss_type {loss_type!r}, expected one of {sorted(SIM_LOSSES)}")
+        g = _spec_get(spec) if not isinstance(spec, FeatSpec) else (lambda k, d=None: d)
+        if g("multi_sparse_combine_info") is not None and weights.get("multi_sparse_combiner", "sqrtn") != "normal":
+            raise ValueError("SIMTrainer: multi-sparse fields need the combiner \"normal\"; the pooling backward is "
+                             "not built")
+        self._combiner = weights.get("multi_sparse_combiner")
+        self.alpha, self.beta, self.loss_type = float(alpha), float(beta), loss_type
+        self.topk = int(search_topk)
+        super().__init__(spec, weights, use_bn, lr, epsilon, device)
+
+    def _init_params(self, weights):
+        from .feat_models import SIM_MAX_K, SIM_MAX_TOPK
+
+        K, F = self.K, self.F
+        H = self.H = int(weights["num_heads"])
+        self.scheme = weights["sim_scheme"]
+        _check_mha_scheme(self.scheme, "SIMTrainer")
+        if K > SIM_MAX_K or H < 1 or K % H:
+            raise ValueError(f"SIMTrainer: embed size {K} with {H} heads outside K <= {SIM_MAX_K}, heads dividing K")
+        if not 1 <= self.topk <= SIM_MAX_TOPK:
+            raise ValueError(f"SIMTrainer: search_topk {self.topk} outside [1, {SIM_MAX_TOPK}]")
+        for name, want in (("mlp", (F + 2) * K), ("first_stage_mlp", 2 * K)):
+            n_in = np.shape(weights[name]["kernels"][0])[0]
+            if n_in != want:
+                raise ValueError(f"SIMTrainer: the first layer of {name} takes {n_in} inputs, expected {want} "
+                                 f"(F = {F}, K = {K})")
+        # reference order [long, short, user, item, sparse.., dense..] -> ours [user, item, sparse.., dense.., long, short]
+        self.perm = np.concatenate([np.arange(2 * K, (F + 2) * K), np.arange(0, 2 * K)])
+        super()._init_params(dict(weights, mlp=permute_mlp_input(weights["mlp"], self.perm)))
+        p = self.params
+        self.n_fs = self._init_stack("fs_", weights["first_stage_mlp"])
+        p["first_stage_out_kernel"] = self._var(weights["first_stage_out_kernel"], -1)
+        p["first_stage_out_bias"] = self._var(weights["first_stage_out_bias"], 1)
+        self._init_item_table()
+        if np.shape(weights["seq_proj"]) != (self.Kp, K):
+            raise ValueError(f"SIMTrainer: seq_proj has shape {np.shape(weights['seq_proj'])}, expected "
+                             f"({self.Kp}, {K})")
+        p["seq_projT"] = self._var(np.ascontiguousarray(np.asarray(weights["seq_proj"]).T))
+        self._init_mha("sim_", weights["sim_mha"], K, K, 0)
+
+    def _check_batch(self, L, S):
+        from .feat_models import SIM_MAX_L, SIM_MAX_S
+
+        if not 1 <= L <= SIM_MAX_L or not 1 <= S <= SIM_MAX_S or self.topk > L:
+            raise ValueError(f"SIMTrainer: long length {L}, short length {S}, search_topk {self.topk} outside "
+                             f"L <= {SIM_MAX_L}, S <= {SIM_MAX_S}, search_topk <= L")
+
+    def forward(self, users_d, items_d, long_seqs, long_lens, short_seqs, short_lens):
+        """Training-mode logits alpha z1 + beta z2 of the batch (batch statistics in the BN); caches what the backward
+        needs."""
+        torch = self._torch
+        lib, st, p = _lib.lib, _lib.current_stream(), self.params
+        K, F, H, k = self.K, self.F, self.H, self.topk
+        R, L, S = int(users_d.numel()), int(long_seqs.shape[1]), int(short_seqs.shape[1])
+        f32, dev = torch.float32, self.device
+        G = self._build_G()
+        Gp = linear(G, p["seq_projT"], None, ACT_NONE, impl="f32")
+        q = torch.empty((R, K), dtype=f32, device=dev)
+        _lib.check(lib.b200_gather_rows(_lib.ptr(Gp), Gp.stride(0), K, _lib.ptr(items_d), R, _lib.ptr(q), K, st))
+        # first-stage input [q || pooled]; the GSU kernel writes the pooled block
+        xf = torch.empty((R, 2 * K), dtype=f32, device=dev)
+        xf[:, :K] = q
+        sel = torch.empty((R, k), dtype=torch.int32, device=dev)
+        pooled = xf[:, K:]
+        _lib.check(lib.b200_sim_gsu_forward(_lib.ptr(Gp), Gp.stride(0), K, _lib.ptr(items_d), _lib.ptr(long_seqs),
+                                            long_seqs.stride(0), _lib.ptr(long_lens), L, k, R, _lib.ptr(sel),
+                                            _lib.ptr(pooled), xf.stride(0), st))
+        sel_idx = torch.gather(long_seqs, 1, sel.to(torch.int64)).reshape(-1).to(torch.int64)
+        Xsel = torch.empty((R * k, K), dtype=f32, device=dev)
+        _lib.check(lib.b200_gather_rows(_lib.ptr(Gp), Gp.stride(0), K, _lib.ptr(sel_idx), R * k, _lib.ptr(Xsel), K,
+                                        st))
+
+        def core(qq, kk, vv):
+            o = torch.empty((R, K), dtype=f32, device=dev)
+            P = torch.empty(R * H * k, dtype=f32, device=dev)
+            _lib.check(lib.b200_sim_esu_forward(_lib.ptr(qq), qq.stride(0), _lib.ptr(kk), _lib.ptr(vv), K,
+                                                _lib.ptr(sel), _lib.ptr(long_lens), R, K, H, k, _lib.ptr(o), K,
+                                                _lib.ptr(P), st))
+            return o, P
+
+        long_out, mha = self._mha_forward("sim_", q, core, kv=Xsel)
+        x = torch.empty((R, F * K + 2 * K), dtype=f32, device=dev)
+        feat_forward(self.spec.layout, self.tables, users_d, items_d, R, concat=x)
+        x[:, F * K:F * K + K] = long_out
+        short_idx = short_seqs.reshape(-1).to(torch.int64)
+        Sg = torch.empty((R * S, K), dtype=f32, device=dev)
+        _lib.check(lib.b200_gather_rows(_lib.ptr(Gp), Gp.stride(0), K, _lib.ptr(short_idx), R * S, _lib.ptr(Sg), K,
+                                        st))
+        so = x[:, F * K + K:]
+        rows = torch.arange(R, dtype=torch.int64, device=dev)
+        slots = rows.to(torch.int32)
+        _lib.check(lib.b200_transformer_target_attention(_lib.ptr(q), K, _lib.ptr(Sg), S, K, _lib.ptr(short_lens),
+                                                         _lib.ptr(slots), _lib.ptr(rows), R, 0, 0, _lib.ptr(so),
+                                                         x.stride(0), st))
+        h2, c2 = self._stack_forward("", self.n_layers, x)
+        z2 = self._dense1_forward(h2)
+        h1, c1 = self._stack_forward("fs_", self.n_fs, xf)
+        z1 = self._dense1_forward(h1, "first_stage_out_")
+        logit = torch.zeros(R, dtype=f32, device=dev)
+        _lib.check(lib.b200_axpy(_lib.ptr(logit), _lib.ptr(z1), self.alpha, R, st))
+        _lib.check(lib.b200_axpy(_lib.ptr(logit), _lib.ptr(z2), self.beta, R, st))
+        self._cache = dict(R=R, L=L, S=S, users=users_d, items=items_d, long_seqs=long_seqs, long_lens=long_lens,
+                           short_idx=short_idx, short_lens=short_lens, G=G, q=q, sel=sel, Sg=Sg, mha=mha, c2=c2,
+                           h2=h2, c1=c1, h1=h1, logit=logit)
+        return logit
+
+    def backward(self, labels_d):
+        """Loss + every gradient buffer filled (before the optimiser); returns the device loss."""
+        torch = self._torch
+        lib, st, p, g = _lib.lib, _lib.current_stream(), self.params, self.grads
+        K, F, H, k = self.K, self.F, self.H, self.topk
+        c = self._cache
+        R, L, S = c["R"], c["L"], c["S"]
+        f32, dev = torch.float32, self.device
+        loss = torch.empty((), dtype=f32, device=dev)
+        dlogit = torch.empty(R, dtype=f32, device=dev)
+        _lib.check(lib.b200_pointwise_loss(_lib.ptr(c["logit"]), _lib.ptr(labels_d), R, SIM_LOSSES[self.loss_type],
+                                           0.25, 2.0, _lib.ptr(loss), _lib.ptr(dlogit), _lib.ptr(self._lws),
+                                           self._lws.numel(), st))
+        dz1 = torch.zeros(R, dtype=f32, device=dev)
+        dz2 = torch.zeros(R, dtype=f32, device=dev)
+        _lib.check(lib.b200_axpy(_lib.ptr(dz1), _lib.ptr(dlogit), self.alpha, R, st))
+        _lib.check(lib.b200_axpy(_lib.ptr(dz2), _lib.ptr(dlogit), self.beta, R, st))
+        # second stage
+        _, dh2 = self._dense1_backward(c["h2"], None, None, dlogit=dz2)
+        dx = self._stack_backward("", self.n_layers, c["c2"], dh2)
+        feat_backward(self.spec.layout, self.tables, c["users"], c["items"], R, g, dconcat=dx)
+        q, sel, ll = c["q"], c["sel"], c["long_lens"]
+        dq = torch.empty((R, K), dtype=f32, device=dev)
+        dSg = torch.empty((R * S, K), dtype=f32, device=dev)
+        dso = dx[:, F * K + K:]
+        _lib.check(lib.b200_transformer_target_attention_backward(
+            _lib.ptr(q), K, _lib.ptr(c["Sg"]), S, K, _lib.ptr(c["short_lens"]), _lib.ptr(dso), dx.stride(0), R,
+            _lib.ptr(dq), K, _lib.ptr(dSg), st))
+
+        def core_backward(m, dO):
+            dqh = torch.empty((R, K), dtype=f32, device=dev)
+            dk, dv = (torch.empty((R * k, K), dtype=f32, device=dev) for _ in range(2))
+            _lib.check(lib.b200_sim_esu_backward(_lib.ptr(m["q"]), m["q"].stride(0), _lib.ptr(m["k"]),
+                                                 _lib.ptr(m["v"]), K, _lib.ptr(sel), _lib.ptr(ll), R, K, H, k, _lib.ptr(m["lse"]),
+                                                 _lib.ptr(dO), dO.stride(0), _lib.ptr(dqh), K, _lib.ptr(dk),
+                                                 _lib.ptr(dv), K, st))
+            return dqh, dk, dv
+
+        dq_esu, dXsel = self._mha_backward("sim_", c["mha"], dx[:, F * K:F * K + K].contiguous(), core_backward)
+        # first stage
+        _, dh1 = self._dense1_backward(c["h1"], None, None, "first_stage_out_", dlogit=dz1)
+        dxf = self._stack_backward("fs_", self.n_fs, c["c1"], dh1)
+        self._axpy(dq, dq_esu)
+        self._axpy(dq, dxf[:, :K].contiguous())
+        # dGp: the query rows, the short keys, the selected and the pooled rows
+        n = self.n_items + 1
+        dGp = torch.zeros((n, K), dtype=f32, device=dev)
+        _lib.check(lib.b200_scatter_add_rows(_lib.ptr(dGp), K, K, _lib.ptr(c["items"]), R, _lib.ptr(dq), K, st))
+        _lib.check(lib.b200_scatter_add_rows(_lib.ptr(dGp), K, K, _lib.ptr(c["short_idx"]), R * S, _lib.ptr(dSg), K,
+                                             st))
+        dpooled = dxf[:, K:]
+        _lib.check(lib.b200_sim_long_backward(_lib.ptr(c["long_seqs"]), c["long_seqs"].stride(0), _lib.ptr(ll), L,
+                                              _lib.ptr(sel), k, R, K, _lib.ptr(dpooled), dxf.stride(0),
+                                              _lib.ptr(dXsel), dXsel.stride(0), _lib.ptr(dGp), K, st))
+        # Gp = G Wp
+        G = c["G"]
+        g["seq_projT"] += _weight_grad(dGp, G)
+        self._fold_dG(linear(dGp, p["seq_projT"].t().contiguous(), None, ACT_NONE, cache_split=False))
+        return loss
+
+    def step(self, users_d, items_d, long_seqs, long_lens, short_seqs, short_lens, labels_d):
+        """One optimisation step; returns the device loss."""
+        torch = self._torch
+        L, S = int(long_seqs.shape[1]), int(short_seqs.shape[1])
+        self._check_batch(L, S)
+        i32 = torch.int32
+        self.forward(users_d.to(torch.int64).contiguous(), items_d.to(torch.int64).contiguous(),
+                     long_seqs.to(i32).contiguous(), long_lens.to(i32).clamp(1, L).contiguous(),
+                     short_seqs.to(i32).contiguous(), short_lens.to(i32).clamp(1, S).contiguous())
+        loss = self.backward(labels_d.to(torch.float32).contiguous())
+        self._adam_update()
+        self._cache = None
+        return loss
+
+    def export_weights(self):
+        """The raw variables in the scheme they came in, both stages."""
+        p, K = self.params, self.K
+        w = super().export_weights()
+        inv = np.argsort(self.perm)
+        w["mlp"]["kernels"][0] = w["mlp"]["kernels"][0][inv]
+        if self.use_bn:
+            w["mlp"]["bn_in"] = {k: v[inv] for k, v in w["mlp"]["bn_in"].items()}
+        w.update(sim_scheme=self.scheme, num_heads=self.H,
+                 seq_proj=np.ascontiguousarray(p["seq_projT"].cpu().numpy().T), sim_mha=self._export_mha("sim_", K, K), first_stage_mlp=self._export_stack("fs_", self.n_fs),
+                 first_stage_out_kernel=p["first_stage_out_kernel"].cpu().numpy().reshape(-1, 1),
+                 first_stage_out_bias=p["first_stage_out_bias"].cpu().numpy().reshape(1),
+                 out_kernel=w["out_kernel"].reshape(-1, 1),
+                 out_bias=np.asarray(w["out_bias"], dtype=np.float32).reshape(1))
+        if self._combiner is not None:
+            w["multi_sparse_combiner"] = self._combiner
+        return w
