@@ -148,6 +148,38 @@ int b200_spmm_csr(const int64_t* indptr, const int32_t* col, const float* val, i
                   const int64_t* long_chunk_ptr, int64_t n_long, const int32_t* chunk_row,
                   const int32_t* chunk_k, int64_t n_chunks, float* partials, void* stream);
 
+/* ---- ALS training: one half-epoch of libreco/algorithms/_als.pyx als_update (:47-93) ---------
+ * Solves every row m of X [n_x, d] in place against the fixed table Y [n_y, d] (both contiguous) given that
+ * side's CSR (indptr int64 [n_x+1], indices int32, data float32).  A0 [d, d] is the base matrix: Y^T Y + reg I
+ * (implicit, task "ranking") or reg I (explicit, "rating"), float32, built by the caller.
+ * Row plan (built once per CSR): rows with at most b200_als_long_row_threshold() nnz are listed in
+ * short_rows; the others in long_rows, split into chunks of b200_als_chunk() nnz: chunk c covers nnz
+ * [indptr[row] + chunk_k[c] * chunk, ...) of row long_rows[chunk_long[c]], and long_chunk_ptr[n_long+1]
+ * delimits each long row's chunks.  n_short + n_long == n_x.  workspace: b200_als_workspace_bytes(),
+ * 16-byte aligned.  Supported: 1 <= d <= 128, any nnz per row; anything else returns -2 before a launch.
+ * Deterministic (no float atomics).
+ *   b200_als_cg      _least_squares_cg (:167-268): cg_steps >= 0 CG iterations warm-started from X[m], with the
+ *                    reference's exits (rsold < 1e-10 leaves X[m] untouched; rsnew < 1e-10 breaks).  Rows of
+ *                    at most b200_als_stage_rows(d) nnz read their Y slice from shared memory.
+ *   b200_als_direct  _least_squares (:96-164): A = A0 + sum w y y^T, b = sum c y, Cholesky solve.  A row whose
+ *                    pivot at column j is <= 0 or NaN is not written; *fail_row / *fail_info receive the
+ *                    smallest such row and its LAPACK info j+1 (-1 / 0: none).  Synchronises the stream. */
+int b200_als_long_row_threshold(void);
+int b200_als_chunk(void);
+int b200_als_stage_rows(int32_t d);
+int b200_als_workspace_bytes(int32_t d, int32_t use_cg, int64_t n_long, int64_t n_chunks, size_t* bytes);
+int b200_als_cg(const int64_t* indptr, const int32_t* indices, const float* data, int64_t n_x, float* X,
+                const float* Y, int64_t n_y, int32_t d, const float* A0, int32_t implicit, int32_t cg_steps,
+                const int32_t* short_rows, int64_t n_short, const int32_t* long_rows, const int64_t* long_chunk_ptr,
+                int64_t n_long, const int32_t* chunk_long, const int32_t* chunk_k, int64_t n_chunks,
+                void* workspace, size_t workspace_bytes, void* stream);
+int b200_als_direct(const int64_t* indptr, const int32_t* indices, const float* data, int64_t n_x, float* X,
+                    const float* Y, int64_t n_y, int32_t d, const float* A0, int32_t implicit,
+                    const int32_t* short_rows, int64_t n_short, const int32_t* long_rows,
+                    const int64_t* long_chunk_ptr, int64_t n_long, const int32_t* chunk_long,
+                    const int32_t* chunk_k, int64_t n_chunks, void* workspace, size_t workspace_bytes,
+                    int64_t* fail_row, int32_t* fail_info, void* stream);
+
 /* ---- a4/a5/a6: feature models (FM, DeepFM, towers) -------------------------------------
  * Layout of the per-row features, as the reference's DataInfo provides them
  * (libreco/data/data_info.py:107-158, libreco/prediction/preprocess.py:15-57):

@@ -44,6 +44,14 @@ SIGNATURES = {
     "b200_spmm_chunk": (c_int, []),
     "b200_spmm_csr": (c_int, [_P, _P, _P, c_int64, _P, c_int64, c_int32, _P, c_int64, _P, c_int64, c_int32,
                               c_float, _P, _P, c_int64, _P, _P, c_int64, _P, _P]),
+    "b200_als_long_row_threshold": (c_int, []),
+    "b200_als_chunk": (c_int, []),
+    "b200_als_stage_rows": (c_int, [c_int32]),
+    "b200_als_workspace_bytes": (c_int, [c_int32, c_int32, c_int64, c_int64, POINTER(c_size_t)]),
+    "b200_als_cg": (c_int, [_P, _P, _P, c_int64, _P, _P, c_int64, c_int32, _P, c_int32, c_int32, _P, c_int64, _P, _P,
+                            c_int64, _P, _P, c_int64, _P, c_size_t, _P]),
+    "b200_als_direct": (c_int, [_P, _P, _P, c_int64, _P, _P, c_int64, c_int32, _P, c_int32, _P, c_int64, _P, _P,
+                                c_int64, _P, _P, c_int64, _P, c_size_t, POINTER(c_int64), POINTER(c_int32), _P]),
     "b200_feat_forward_tune": (c_int, [c_int32]),
     "b200_feat_forward": (c_int, [_P, _P, _P, _P, c_int64, c_int64, c_int64, _P, c_int64, _P, c_int64, _P, _P, _P, c_float,
                                   _P, _P, _P, c_float, _P, _P, c_int64, _P]),

@@ -15,13 +15,20 @@ What is patched (seams of SURVEY.md §8b; nothing else of the reference changes)
 * ``libreco.algorithms.lightgcn.LightGCNModel`` (``algorithms/lightgcn.py:4,117-127``) → the
   differentiable K6 module with the reference's constructor / ``forward(use_dropout)`` contract;
 * optionally the loss functions ``TorchTrainer._compute_loss`` uses
-  (``training/torch_trainer.py:15-23,140-161``).
+  (``training/torch_trainer.py:15-23,140-161``);
+* optionally (``als=True``) the Cython extension ``libreco.algorithms._als``: a module whose ``als_update``
+  is ``librecommender_b200.als.als_update`` is registered in ``sys.modules`` and as the package attribute,
+  so ``ALS.fit``'s ``from ._als import als_update`` (``algorithms/als.py:135``) resolves to the GPU solver
+  whether or not a Cython build exists.
 """
 from __future__ import annotations
 
 import importlib
+import sys
+import types
 
 _saved: list = []
+_MISSING = object()
 
 
 def _patch(mod, name, value):
@@ -30,7 +37,21 @@ def _patch(mod, name, value):
         setattr(mod, name, value)
 
 
-def install(libreco=None, losses: bool = True, lightgcn: bool = True) -> None:
+def _register_als(base):
+    """Put a GPU ``_als`` module at ``{base}.algorithms._als``; remember what was there (or that nothing was)."""
+    from . import als as gpu_als
+
+    name = f"{base}.algorithms._als"
+    pkg = importlib.import_module(f"{base}.algorithms")
+    mod = types.ModuleType(name, "librecommender_b200.als.als_update registered as the reference's _als")
+    mod.als_update = gpu_als.als_update
+    _saved.append((sys.modules, name, sys.modules.get(name, _MISSING)))
+    sys.modules[name] = mod
+    _saved.append((pkg, "_als", getattr(pkg, "_als", _MISSING)))
+    pkg._als = mod
+
+
+def install(libreco=None, losses: bool = True, lightgcn: bool = True, als: bool = False) -> None:
     """Patch the reference package in place (idempotent: a second call re-installs)."""
     from . import recommendation as rec
 
@@ -67,13 +88,24 @@ def install(libreco=None, losses: bool = True, lightgcn: bool = True) -> None:
                          "max_margin_loss", "pairwise_bce_loss", "pairwise_focal_loss"):
                 if hasattr(L, name):
                     _patch(m, name, getattr(L, name))
+    if als:
+        _register_als(base)
 
 
 def uninstall() -> None:
     """Restore every patched name."""
     while _saved:
         mod, name, old = _saved.pop()
-        setattr(mod, name, old)
+        if mod is sys.modules:
+            if old is _MISSING:
+                sys.modules.pop(name, None)
+            else:
+                sys.modules[name] = old
+        elif old is _MISSING:
+            if hasattr(mod, name):
+                delattr(mod, name)
+        else:
+            setattr(mod, name, old)
 
 
 def installed() -> bool:
