@@ -180,6 +180,28 @@ int b200_als_direct(const int64_t* indptr, const int32_t* indices, const float* 
                     const int32_t* chunk_k, int64_t n_chunks, void* workspace, size_t workspace_bytes,
                     int64_t* fail_row, int32_t* fail_info, void* stream);
 
+/* ---- BPR training: one epoch of libreco/algorithms/_bpr.pyx bpr_update (:30-110, :116-399) ---------------
+ * Tables U [n_users, D], I [n_items, D], D = embed_size + 1 (bias last; U[:, D-1] == 1 is never written), all
+ * contiguous float32.  For each of the n samples (users[s], items_pos[s]) in order: a negative, then the
+ * reference's update, diff = U[u] . (I[p] - I[n]) over all D columns, g = 1 / (1 + exp(diff)), gradient ascent with
+ * reg on every updated element.  optimizer: 0 sgd (_bpr_update_sgd :116-190), 1 momentum (:196-280; state1 =
+ * velocity tables), 2 adam (:286-399; state1 / state2 = first / second moment tables, bias correction
+ * 1 - rho^epoch from the caller's epoch >= 1).  State tables not used by the optimizer may be NULL.
+ * Negatives: items_neg[s] when items_neg is given; otherwise uniform over the items not in the user's CSR row
+ * (indptr int64 [n_users+1], indices int32, rows sorted and duplicate-free), one Philox4x32-10 draw keyed by
+ * (seed, epoch, s) and rank selection.  A user whose row holds every item is skipped.  neg_out (optional)
+ * receives the negatives used (-1: skipped).  Updates are atomic adds of deltas; max_inflight bounds the
+ * samples in flight (1: serial, deterministic, the sequential reference semantics; 0: the library default,
+ * b200_bpr_default_inflight()).  embed_size outside 1..128, null required pointers, an unknown optimizer or
+ * missing state return -2 before a launch. */
+int64_t b200_bpr_default_inflight(int32_t embed_size);
+int b200_bpr_update(int32_t optimizer, const int32_t* users, const int32_t* items_pos, int64_t n,
+                    const int64_t* indptr, const int32_t* indices, int64_t n_users, int64_t n_items, float* U,
+                    float* I, int32_t embed_size, float* u_state1, float* i_state1, float* u_state2,
+                    float* i_state2, float lr, float reg, float momentum, float rho1, float rho2, int32_t epoch,
+                    uint64_t seed, const int32_t* items_neg, int32_t* neg_out, int64_t max_inflight,
+                    void* stream);
+
 /* ---- a4/a5/a6: feature models (FM, DeepFM, towers) -------------------------------------
  * Layout of the per-row features, as the reference's DataInfo provides them
  * (libreco/data/data_info.py:107-158, libreco/prediction/preprocess.py:15-57):

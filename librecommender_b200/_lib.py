@@ -52,6 +52,9 @@ SIGNATURES = {
                             c_int64, _P, _P, c_int64, _P, c_size_t, _P]),
     "b200_als_direct": (c_int, [_P, _P, _P, c_int64, _P, _P, c_int64, c_int32, _P, c_int32, _P, c_int64, _P, _P,
                                 c_int64, _P, _P, c_int64, _P, c_size_t, POINTER(c_int64), POINTER(c_int32), _P]),
+    "b200_bpr_default_inflight": (c_int64, [c_int32]),
+    "b200_bpr_update": (c_int, [c_int32, _P, _P, c_int64, _P, _P, c_int64, c_int64, _P, _P, c_int32, _P, _P, _P, _P,
+                                c_float, c_float, c_float, c_float, c_float, c_int32, c_uint64, _P, _P, c_int64, _P]),
     "b200_feat_forward_tune": (c_int, [c_int32]),
     "b200_feat_forward": (c_int, [_P, _P, _P, _P, c_int64, c_int64, c_int64, _P, c_int64, _P, c_int64, _P, _P, _P, c_float,
                                   _P, _P, _P, c_float, _P, _P, c_int64, _P]),

@@ -19,7 +19,10 @@ What is patched (seams of SURVEY.md §8b; nothing else of the reference changes)
 * optionally (``als=True``) the Cython extension ``libreco.algorithms._als``: a module whose ``als_update``
   is ``librecommender_b200.als.als_update`` is registered in ``sys.modules`` and as the package attribute,
   so ``ALS.fit``'s ``from ._als import als_update`` (``algorithms/als.py:135``) resolves to the GPU solver
-  whether or not a Cython build exists.
+  whether or not a Cython build exists;
+* optionally (``bpr=True``) the Cython extension ``libreco.algorithms._bpr`` in the same way, with
+  ``librecommender_b200.bpr.bpr_update``, so ``BPR(use_tf=False).fit``'s ``from ._bpr import bpr_update``
+  (``algorithms/bpr.py:309``) trains on the GPU.
 """
 from __future__ import annotations
 
@@ -37,21 +40,21 @@ def _patch(mod, name, value):
         setattr(mod, name, value)
 
 
-def _register_als(base):
-    """Put a GPU ``_als`` module at ``{base}.algorithms._als``; remember what was there (or that nothing was)."""
-    from . import als as gpu_als
-
-    name = f"{base}.algorithms._als"
+def _register_cython(base, name, func):
+    """Put a module holding the GPU ``func`` at ``{base}.algorithms.{name}`` in place of the reference's Cython
+    extension; remember what was there (or that nothing was)."""
+    full = f"{base}.algorithms.{name}"
     pkg = importlib.import_module(f"{base}.algorithms")
-    mod = types.ModuleType(name, "librecommender_b200.als.als_update registered as the reference's _als")
-    mod.als_update = gpu_als.als_update
-    _saved.append((sys.modules, name, sys.modules.get(name, _MISSING)))
-    sys.modules[name] = mod
-    _saved.append((pkg, "_als", getattr(pkg, "_als", _MISSING)))
-    pkg._als = mod
+    mod = types.ModuleType(full, f"{func.__module__}.{func.__name__} registered as the reference's {name}")
+    setattr(mod, func.__name__, func)
+    _saved.append((sys.modules, full, sys.modules.get(full, _MISSING)))
+    sys.modules[full] = mod
+    _saved.append((pkg, name, getattr(pkg, name, _MISSING)))
+    setattr(pkg, name, mod)
 
 
-def install(libreco=None, losses: bool = True, lightgcn: bool = True, als: bool = False) -> None:
+def install(libreco=None, losses: bool = True, lightgcn: bool = True, als: bool = False,
+            bpr: bool = False) -> None:
     """Patch the reference package in place (idempotent: a second call re-installs)."""
     from . import recommendation as rec
 
@@ -89,7 +92,13 @@ def install(libreco=None, losses: bool = True, lightgcn: bool = True, als: bool 
                 if hasattr(L, name):
                     _patch(m, name, getattr(L, name))
     if als:
-        _register_als(base)
+        from .als import als_update
+
+        _register_cython(base, "_als", als_update)
+    if bpr:
+        from .bpr import bpr_update
+
+        _register_cython(base, "_bpr", bpr_update)
 
 
 def uninstall() -> None:
