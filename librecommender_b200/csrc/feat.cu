@@ -1224,6 +1224,10 @@ extern "C" int b200_linear_f32(const float* X, int64_t ldx, int64_t R, const flo
                                int64_t ldy, void* stream) {
   B200_REQUIRE(X && Wt && Y, "b200_linear_f32: null pointer");
   B200_REQUIRE(act >= 0 && act <= 2, "b200_linear_f32: activation code %d outside [0, 2]", act);
+  B200_REQUIRE(R >= 0 && din > 0 && dout > 0, "b200_linear_f32: bad shape (R %lld, din %d, dout %d)", (long long)R,
+               din, dout);
+  // ldy < dout would overlap output rows; ldx / ldw < din would read the next row's elements
+  B200_REQUIRE(ldx >= din && ldw >= din && ldy >= dout, "b200_linear_f32: leading dimension too small");
   if (R == 0) return 0;
   const int64_t gy = ceil_div64(R, LM);
   B200_REQUIRE(gy <= 65535 * 32ll, "b200_linear_f32: too many rows");

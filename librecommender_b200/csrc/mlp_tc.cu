@@ -12,6 +12,8 @@
 // treats the 13 low mantissa bits of an fp32 container.  The dominant hi*hi products and the
 // 2^-11-times smaller cross products go to SEPARATE wgmma accumulators, and both are promoted to
 // fp32 registers (round-to-nearest adds) every GC k-chunks, so no accumulator runs over many MMAs.
+// Unlike b200_linear_f32 it does not carry +-inf inputs through: the lo part of +-inf is inf - inf = NaN, so
+// an output that b200_linear_f32 gives as +-inf comes out NaN here (finite inputs only).
 //
 // One persistent CTA per SM, warp-specialised:
 //   warpgroups 0-1  split the landed tiles into hi / lo, issue the wgmma of rows [64 g, 64 g + 64) of

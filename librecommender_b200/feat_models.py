@@ -123,13 +123,14 @@ def split_weights(Wt):
     (keyed by storage pointer + shape + version counter, so in-place updates re-split)."""
     import torch
 
-    key = (Wt.data_ptr(), tuple(Wt.shape), Wt.stride(0), Wt._version)
+    dout, din = Wt.shape
+    ldw = Wt.stride(0) if dout > 1 else din      # one row: torch's row stride is arbitrary
+    key = (Wt.data_ptr(), tuple(Wt.shape), ldw, Wt._version)
     hit = _SPLIT_CACHE.get(key)
     if hit is None:
-        dout, din = Wt.shape
         ld = int(_lib.lib.b200_linear_tf32x3_split_ld(din))
         buf = torch.empty(2 * dout * ld, dtype=torch.float32, device=Wt.device)
-        _lib.check(_lib.lib.b200_linear_tf32x3_split_weights(_lib.ptr(Wt), Wt.stride(0), din, dout, _lib.ptr(buf),
+        _lib.check(_lib.lib.b200_linear_tf32x3_split_weights(_lib.ptr(Wt), ldw, din, dout, _lib.ptr(buf),
                                                              _lib.current_stream()))
         if len(_SPLIT_CACHE) > 256:
             _SPLIT_CACHE.clear()
@@ -141,22 +142,48 @@ ACT_NONE, ACT_RELU, ACT_SWISH = 0, 1, 2     # activation codes of b200_linear_* 
 ACT_GELU = 3                                # b200_activation_* only: the erf gelu
 
 
+def _row_major(t, name):
+    """``t`` as the dense kernels read a matrix operand — float32 CUDA rows with unit inner stride, a copy when the
+    view is transposed or its rows overlap (a broadcast) — and its leading dimension.  Torch gives a single row an
+    arbitrary row stride (``y.t()`` of an [n, 1] column has stride 1), so one row reads as ``ld`` = its width."""
+    import torch
+
+    if not isinstance(t, torch.Tensor) or t.dtype != torch.float32 or not t.is_cuda or t.dim() != 2:
+        raise ValueError(f"linear: {name} must be a 2-D float32 CUDA tensor, got "
+                         f"{getattr(t, 'dtype', type(t).__name__)} {tuple(getattr(t, 'shape', ()))} on "
+                         f"{getattr(t, 'device', 'host')}")
+    if (t.shape[1] > 1 and t.stride(1) != 1) or (t.shape[0] > 1 and t.stride(0) < t.shape[1]):
+        t = t.contiguous()
+    return t, (t.stride(0) if t.shape[0] > 1 else t.shape[1])
+
+
 def linear(x, Wt, b, act, cache_split=True, impl=None):
     """tf_dense (libreco/layers/dense.py:52-80) with BN folded: act(x Wt^T + b), fp32 device tensors.  ``act`` is an
     activation code (a bool reads as relu on / off): 0 none, 1 relu, 2 swish.  ``impl`` overrides ``LINEAR_IMPL``
-    for this call ("f32": one fmaf chain per output, so a row's bits do not depend on how many rows come with it)."""
+    for this call ("f32": one fmaf chain per output, so a row's bits do not depend on how many rows come with it).
+    Any strided view works (a transposed ``x`` or ``Wt`` is copied); another dtype or a host tensor raises
+    ``ValueError``."""
     import torch
 
     impl = LINEAR_IMPL if impl is None else impl
+    x, ldx = _row_major(x, "x")
+    Wt_in = Wt
+    Wt, ldw = _row_major(Wt, "Wt")
+    cache_split = cache_split and Wt is Wt_in      # a fresh copy would only fill the split cache
+    if b is not None:
+        if not isinstance(b, torch.Tensor) or b.dtype != torch.float32 or not b.is_cuda:
+            raise ValueError(f"linear: b must be a float32 CUDA tensor, got {getattr(b, 'dtype', type(b).__name__)} "
+                             f"on {getattr(b, 'device', 'host')}")
+        b = b.contiguous()
     R, din, dout = x.shape[0], Wt.shape[1], Wt.shape[0]
     y = torch.empty((R, dout), dtype=torch.float32, device=x.device)
     bp = _lib.ptr(b) if b is not None else None
-    aligned = x.stride(0) % 4 == 0 and x.data_ptr() % 16 == 0 and x.stride(1) == 1 and Wt.stride(1) == 1
+    aligned = ldx % 4 == 0 and x.data_ptr() % 16 == 0
     # few output rows but a long reduction (the weight gradients dWt = dY^T X of the training steps: 128 x 1792
     # outputs over 8192 rows) would run on a handful of SIMT CTAs: send those to the tensor-core kernel too
     use_tc = impl == "tf32x3" or (impl == "auto" and din >= TC_MIN_DIN and
                                   (R >= TC_MIN_ROWS or din >= TC_LONG_K or R * din * dout >= TC_MIN_MACS))
-    w_ok = cache_split or (Wt.stride(0) % 4 == 0 and Wt.data_ptr() % 16 == 0)
+    w_ok = cache_split or (ldw % 4 == 0 and Wt.data_ptr() % 16 == 0)
     if use_tc and aligned and w_ok and not cache_split and din >= TC_LONG_K:
         # few output tiles, long reduction: split the reduction over enough CTAs to fill the SMs
         tiles = -(-R // 128) * -(-dout // 128)
@@ -164,18 +191,18 @@ def linear(x, Wt, b, act, cache_split=True, impl=None):
         splits = max(1, min(16, sms // tiles, din // 256))
         if splits > 1:
             part = torch.empty(splits * R * dout, dtype=torch.float32, device=x.device)
-            _lib.check(_lib.lib.b200_linear_tf32x3_splitk(_lib.ptr(x), x.stride(0), R, _lib.ptr(Wt), Wt.stride(0), bp, din,
+            _lib.check(_lib.lib.b200_linear_tf32x3_splitk(_lib.ptr(x), ldx, R, _lib.ptr(Wt), ldw, bp, din,
                                                           dout, int(act), splits, _lib.ptr(part),
                                                           part.numel() * 4, _lib.ptr(y), y.stride(0),
                                                           _lib.current_stream()))
             return y
     if use_tc and aligned and w_ok:
         ws = split_weights(Wt) if cache_split else None
-        _lib.check(_lib.lib.b200_linear_tf32x3(_lib.ptr(x), x.stride(0), R, _lib.ptr(Wt), Wt.stride(0), _lib.ptr(ws), bp,
+        _lib.check(_lib.lib.b200_linear_tf32x3(_lib.ptr(x), ldx, R, _lib.ptr(Wt), ldw, _lib.ptr(ws), bp,
                                                din, dout, int(act), _lib.ptr(y), y.stride(0),
                                                _lib.current_stream()))
     else:
-        _lib.check(_lib.lib.b200_linear_f32(_lib.ptr(x), x.stride(0), R, _lib.ptr(Wt), Wt.stride(0), bp, din, dout,
+        _lib.check(_lib.lib.b200_linear_f32(_lib.ptr(x), ldx, R, _lib.ptr(Wt), ldw, bp, din, dout,
                                             int(act), _lib.ptr(y), y.stride(0), _lib.current_stream()))
     return y
 
