@@ -240,7 +240,8 @@ typedef struct {       /* TF scope "embedding" (SURVEY.md Appendix C), fp32, row
 
 /* One pass over R rows: row r = (users[r], items[r]), or with grid_items > 0 the implicit grid
  * (users[(r + row_offset) / grid_items], item (r + row_offset) % grid_items) used by all-items
- * scoring (outputs are indexed by the local r).  Any output may be NULL:
+ * scoring (outputs are indexed by the local r).  R = 0 launches nothing (users / items may then be NULL).
+ * Any output may be NULL:
  *   concat [R, (2+F_s+F_d)*K]  concatenated field embeddings (deep / tower input)
  *   pw     [R, K]              0.5((sum_f e)^2 - sum_f e^2)            (fm.py:158-161)
  *   lin    [R]                 Dense1(concat of linear features) + bias (fm.py:156)

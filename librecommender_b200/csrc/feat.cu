@@ -1019,8 +1019,9 @@ extern "C" int b200_feat_forward(const b200_feat_layout* L, const b200_feat_tabl
                                  float lin_bias, const float* bn_scale, const float* bn_shift,
                                  const float* pw_kernel, float pw_bias, float* ssum, float* sqsum,
                                  int64_t ld_s, void* stream) {
-  B200_REQUIRE(L && T && users, "b200_feat_forward: null pointer");
-  B200_REQUIRE(grid_items > 0 || items, "b200_feat_forward: item ids missing");
+  // an empty batch may come with null id arrays (an empty torch tensor has no storage)
+  B200_REQUIRE(L && T && (users || R == 0), "b200_feat_forward: null pointer");
+  B200_REQUIRE(grid_items > 0 || items || R == 0, "b200_feat_forward: item ids missing");
   B200_REQUIRE(L->embed_size >= 1 && L->embed_size <= 32 * MAX_T, "embed size %d outside [1, %d]",
                L->embed_size, 32 * MAX_T);
   B200_REQUIRE(L->n_sparse <= B200_MAX_FIELDS && L->n_dense <= B200_MAX_FIELDS, "too many feature fields");

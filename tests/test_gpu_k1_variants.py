@@ -1,7 +1,8 @@
 """K1 (b200_feat_forward) kernel variants against the oracle's field embeddings: the software-pipelined field-group
-kernel (default for >= 4096 rows), its cp.async staged variant, the plain field-group kernel, the lane-per-field kernel and — for a K the fast
-paths do not take — the generic kernel.  Concatenated rows must be bit-exact (pure copies / one multiply), the FM
-sums agree to fp32 summation order; the three fast variants must agree with each other bit-for-bit on the copies.
+kernel (default for >= 4096 rows), its cp.async staged variant, the plain field-group kernel and the lane-per-field
+kernel (K = 12 takes the lane-per-field kernel under every switch setting; the generic kernel and the bulk-copy kernel
+are covered by tests/test_gpu_feat_gather.py).  Concatenated rows must be bit-exact (pure copies / one multiply), the
+FM sums agree to fp32 summation order; the three fast variants must agree with each other bit-for-bit on the copies.
 Covers K in {4, 8, 16, 32, 12}, row counts that are no multiple of anything, tower layouts (one id field),
 the all-items grid mode and more fields than one 8-step batch."""
 import numpy as np
