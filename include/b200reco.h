@@ -102,8 +102,10 @@ int b200_recommend_embed_tune(int32_t organisation_code, float pre_rank_coef);
  * 1e-5).  Selects this rule (the default) again after a non-zero rank coefficient of
  * b200_recommend_embed_tune. */
 int b200_recommend_embed_speculation(int32_t pre_stride, float delta);
-/* profiling diagnostics only (results are wrong while level > 0): ablate parts of the main pass
- * (1: nothing is collected, cold epilogue steps only; 2: no epilogue at all, MMAs and stage releases only) */
+/* profiling diagnostics only (results are wrong while level 1 or 2 is set): ablate parts of the main pass
+ * (1: nothing is collected, cold epilogue steps only; 2: no epilogue at all, MMAs and stage releases only);
+ * 3 (results unchanged): every row is finalized by the one-CTA-per-row kernel instead of the one-warp-per-row
+ * kernel, so that tests can compare the two paths on the same inputs */
 int b200_recommend_embed_debug(int32_t ablate_level);
 int b200_recommend_embed_plan(int64_t B, int64_t N, int32_t d, int32_t K, int32_t* out, int32_t n_out);
 int b200_embed_catalog_bytes(int64_t N, int32_t d, size_t* bytes);

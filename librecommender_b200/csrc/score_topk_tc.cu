@@ -23,7 +23,8 @@
 //                the speculative threshold did not exceed c_k - 2*eps (otherwise the row is
 //                flagged); cuts at c_k - 2*eps, drops consumed items, EXACT fp32 re-score
 //                (sequential fma = the library's exact-score definition), sorts by
-//                (score desc, id asc), emits K ids.
+//                (score desc, id asc), emits K ids.  One warp per row (finalize_warp_kernel); rows
+//                outside its envelope are deferred to one CTA per row (finalize_kernel).
 //
 // Coarse scores live in a SCALED domain: coarse(u, i) ~ s_u * s_i * <u, i> with s_u, s_i powers of
 // two (exact scalings), so the fp16 operands keep 11 significant bits whatever the magnitude of the
@@ -879,13 +880,18 @@ guess_kernel(const float* __restrict__ blockmax, int n_vals /* lists * n_pre_til
 }
 
 // ------------------------------------------------------------------------------------------
-// finalize kernel: one CTA per user row
+// finalize: one warp per user row (finalize_warp_kernel), rows outside its envelope deferred to
+// one CTA per row (finalize_kernel)
 // ------------------------------------------------------------------------------------------
 struct FinalizeParams {
   int64_t B, N;
   int32_t B_pad, n_lists, K, d, capg;
+  int32_t defer_all;               // diagnostics (b200_recommend_embed_debug level 3): every row takes finalize_kernel
   const RowMeta* meta;
-  int32_t* row_status;
+  const int32_t* row_status;       // [B_pad] status after the sweep (0, or 1 = list overflow)
+  int32_t* out_status;             // [B] final row_status of the call, written once per row by one of the kernels
+  int32_t* defer_count;            // rows handed from finalize_warp_kernel to finalize_kernel ...
+  int32_t* defer_rows;             // ... and their indices [B_pad]
   const uint32_t* row_tau_key;     // [B_pad] final threshold of the row (speculative start or rigorous raises)
   const uint32_t* tau_guess_key;   // [B_pad] speculative threshold used by the main pass (0 = none)
   const float* cand_r;
@@ -898,8 +904,8 @@ struct FinalizeParams {
   float* out_scores;   // [B, K] or null
 };
 
-__global__ void __launch_bounds__(FIN_THREADS, 5)
-finalize_kernel(const FinalizeParams p) {
+// not inlined: inside finalize_kernel's row loop ptxas spills it
+__device__ __noinline__ void finalize_row(const FinalizeParams& p, const int64_t row) {
   __shared__ uint32_t hist[256];
   __shared__ uint32_t s_prefix, s_krem;
   __shared__ uint32_t s_wtot[FIN_THREADS / 32];
@@ -910,14 +916,13 @@ finalize_kernel(const FinalizeParams p) {
   __shared__ float urow[MAX_KB * KBLK];
   int32_t* htab = reinterpret_cast<int32_t*>(c_sort);
   const int tid = threadIdx.x;
-  const int64_t row = blockIdx.x;
   int64_t* oid = p.out_ids + row * p.K;
   float* osc = p.out_scores ? p.out_scores + row * p.K : nullptr;
   const RowMeta meta = p.meta[row];
   // row_status codes (non-zero = re-run on the exact path): 1 sweep overflow, 2 too few collected,
   // 3 failed speculation, 4 candidate set outside [K, MAXC], 5 capped row not provable
   auto give_up = [&](int code) {
-    if (code && tid == 0) p.row_status[row] = code;
+    if (tid == 0) p.out_status[row] = code ? code : p.row_status[row];
     for (int i = tid; i < p.K; i += FIN_THREADS) { oid[i] = -1; if (osc) osc[i] = 0.f; }
   };
   if (p.row_status[row] != 0) { give_up(0); return; }
@@ -1228,6 +1233,254 @@ finalize_kernel(const FinalizeParams p) {
     oid[i] = (int64_t)(~(uint32_t)(c & 0xffffffffull));
     if (osc) osc[i] = key_to_float((uint32_t)(c >> 32));
   }
+  if (tid == 0) p.out_status[row] = 0;
+}
+
+// The rows finalize_warp_kernel deferred (rare at the bench shape), over a fixed grid: the count is
+// only known on the device.
+constexpr int FIN_CTAS_PER_SM = 3;
+__global__ void __launch_bounds__(FIN_THREADS)
+finalize_kernel(const FinalizeParams p) {
+  const int n = *p.defer_count;
+#pragma unroll 1
+  for (int i = blockIdx.x; i < n; i += gridDim.x) {
+    finalize_row(p, p.defer_rows[i]);
+    __syncthreads();   // the next row reuses the shared memory
+  }
+}
+
+// One warp per row, no block barriers: the same steps as finalize_row on a per-warp buffer, for the
+// rows that fit it (at the bench shape all but a handful).  It only ever completes rows with status 0:
+// a row that would give up, or does not fit (more than WCAP collected elements, more than WSORT
+// candidates, a capped k_row), is appended to the deferred list and finalize_kernel redoes it from
+// scratch, so every give-up code and output comes from the block kernel.
+constexpr int FINW_WARPS = 4;      // warps (rows) per CTA
+constexpr int FINW_CTAS_PER_SM = 8;
+constexpr int WCAP = 512;          // collected elements per row (measured at the bench shape: DESIGN §4)
+constexpr int WSORT = 256;         // candidates per row (sort keys in FinWarpSmem::s)
+struct FinWarpSmem {
+  float4 urow[MAX_KB * KBLK / 4];  // the user row (fp32, unscaled)
+  float s[WCAP];                   // collected coarse scores; after the cut: the hash set, then the sort keys
+  int32_t id[WCAP];                // collected item ids; after the cut: candidate ids (~id = consumed)
+  uint32_t hist[256];
+};
+static_assert(WCAP >= 2 * WSORT, "the hash set (2 WSORT slots) and the sort keys live in FinWarpSmem::s");
+
+__global__ void __launch_bounds__(FINW_WARPS * 32, FINW_CTAS_PER_SM)
+finalize_warp_kernel(const FinalizeParams p) {
+  __shared__ FinWarpSmem smem[FINW_WARPS];
+  const int lane = threadIdx.x & 31;
+  const int64_t row = (int64_t)blockIdx.x * FINW_WARPS + (threadIdx.x >> 5);
+  if (row >= p.B) return;
+  FinWarpSmem& sm = smem[threadIdx.x >> 5];
+  const unsigned lt = (1u << lane) - 1u;
+  // ---- every independent load of the row at once
+  const int32_t st = p.row_status[row];
+  const RowMeta meta = p.meta[row];
+  const uint32_t tk = p.row_tau_key[row], gk = p.tau_guess_key[row];
+  const int64_t u = p.user_ids[row];
+  auto defer = [&]() { if (lane == 0) p.defer_rows[atomicAdd(p.defer_count, 1)] = (int32_t)row; };
+  if (st != 0 || meta.capped || p.defer_all) { defer(); return; }
+  int64_t beg = 0, end = 0;
+  if (meta.apply) { beg = p.indptr[u]; end = p.indptr[u + 1]; }
+  float* urow = reinterpret_cast<float*>(sm.urow);
+  for (int k = lane; k < p.d; k += 32) urow[k] = __ldg(p.U + u * p.ldu + k);   // needed only by the re-score
+  // ---- gather every element >= the row's final threshold (ids < N) into the warp's buffer
+  const float low = tk ? key_to_float(tk) : __int_as_float(0xff800000);
+  int nu = 0;
+  for (int s0 = 0; s0 < p.n_lists; s0 += 32) {
+    const int c = s0 + lane < p.n_lists ? p.cand_cnt[(int64_t)(s0 + lane) * p.B_pad + row] : 0;
+    int incl = c;   // records of lists s0 .. s0 + lane
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const int t = __shfl_up_sync(0xffffffffu, incl, o);
+      if (lane >= o) incl += t;
+    }
+    const int total = __shfl_sync(0xffffffffu, incl, 31);
+    constexpr int UN = 4;   // records in flight per lane
+    for (int g0 = 0; g0 < total; g0 += 32 * UN) {
+      float4 a[UN], b[UN];
+      int base[UN];
+#pragma unroll
+      for (int q = 0; q < UN; ++q) {
+        const int g = g0 + q * 32 + lane;
+        int lo = 0, hi = 31;   // first lane (list) whose inclusive count exceeds g
+#pragma unroll
+        for (int it = 0; it < 5; ++it) {
+          const int mid = (lo + hi) >> 1;
+          if (__shfl_sync(0xffffffffu, incl, mid) <= g) lo = mid + 1; else hi = mid;
+        }
+        const int j = g - (__shfl_sync(0xffffffffu, incl, lo) - __shfl_sync(0xffffffffu, c, lo));
+        a[q] = b[q] = make_float4(0.f, 0.f, 0.f, 0.f);
+        base[q] = 0;
+        if (g < total) {
+          const int64_t slot = (int64_t)(s0 + lo) * p.B_pad + row;
+          const float4* ls = reinterpret_cast<const float4*>(p.cand_r + (slot * (int64_t)p.capg + j) * REC);
+          a[q] = __ldcs(ls);
+          b[q] = __ldcs(ls + 1);
+          base[q] = __ldcs(reinterpret_cast<const int32_t*>(ls + 2));
+        }
+      }
+#pragma unroll
+      for (int q = 0; q < UN; ++q) {
+        const bool ok = g0 + q * 32 + lane < total;
+        const float v[8] = {a[q].x, a[q].y, a[q].z, a[q].w, b[q].x, b[q].y, b[q].z, b[q].w};
+#pragma unroll
+        for (int e = 0; e < 8; ++e) {
+          const bool hit = ok && v[e] >= low && (int64_t)(base[q] + e) < p.N;   // never a zero-padded item row
+          const unsigned m = __ballot_sync(0xffffffffu, hit);
+          const int pos = nu + __popc(m & lt);
+          if (hit && pos < WCAP) { sm.s[pos] = v[e]; sm.id[pos] = base[q] + e; }
+          nu += __popc(m);
+        }
+      }
+    }
+  }
+  if (nu < meta.k_row || nu > WCAP) { defer(); return; }
+  __syncwarp();
+  // ---- exact k_row-th largest coarse score of the buffer: 4 x 8-bit radix select, per-warp histogram
+  uint32_t prefix = 0, krem = (uint32_t)meta.k_row;
+  for (int pass = 0; pass < 4; ++pass) {
+    const int shift = 24 - 8 * pass;
+    reinterpret_cast<uint4*>(sm.hist)[2 * lane] = make_uint4(0u, 0u, 0u, 0u);
+    reinterpret_cast<uint4*>(sm.hist)[2 * lane + 1] = make_uint4(0u, 0u, 0u, 0u);
+    __syncwarp();
+    for (int i = lane; i < nu; i += 32) {
+      const uint32_t key = float_to_key(sm.s[i]);
+      if (pass == 0 || (key >> (shift + 8)) == prefix) atomicAdd(&sm.hist[(key >> shift) & 255u], 1u);
+    }
+    __syncwarp();
+    // lane l owns bins [8 l, 8 l + 8); suffix counts over the lanes above
+    uint32_t mine[8], tot = 0;
+    const uint4 h0 = reinterpret_cast<const uint4*>(sm.hist)[2 * lane];
+    const uint4 h1 = reinterpret_cast<const uint4*>(sm.hist)[2 * lane + 1];
+    mine[0] = h0.x; mine[1] = h0.y; mine[2] = h0.z; mine[3] = h0.w;
+    mine[4] = h1.x; mine[5] = h1.y; mine[6] = h1.z; mine[7] = h1.w;
+#pragma unroll
+    for (int b = 0; b < 8; ++b) tot += mine[b];
+    uint32_t incl = tot;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const uint32_t t = __shfl_down_sync(0xffffffffu, incl, o);
+      if (lane + o < 32) incl += t;
+    }
+    const uint32_t excl = incl - tot;   // count in the bins of the lanes above
+    uint32_t np = 0, nk = 0;
+    const bool owner = excl < krem && krem <= incl;
+    if (owner) {
+      uint32_t c = excl;
+#pragma unroll
+      for (int b = 7; b >= 0; --b) {
+        if (c + mine[b] >= krem) { np = (prefix << 8) | (uint32_t)(lane * 8 + b); nk = krem - c; break; }
+        c += mine[b];
+      }
+    }
+    const int src = __ffs(__ballot_sync(0xffffffffu, owner)) - 1;
+    prefix = __shfl_sync(0xffffffffu, np, src);
+    krem = __shfl_sync(0xffffffffu, nk, src);
+    __syncwarp();   // every lane has read the histogram before the next pass clears it
+  }
+  const float thr = key_to_float(prefix) - meta.eps2;
+  // the speculative threshold must not exceed thr (see finalize_row)
+  if (gk != 0u && key_to_float(gk) > thr) { defer(); return; }
+  // ---- candidates: elements >= thr, compacted in place (a chunk is read before any of it is written)
+  int nc = 0;
+  for (int i0 = 0; i0 < nu; i0 += 32) {
+    const int i = i0 + lane;
+    const bool keep = i < nu && sm.s[i] >= thr;
+    const int32_t id = i < nu ? sm.id[i] : 0;
+    const unsigned m = __ballot_sync(0xffffffffu, keep);
+    __syncwarp();
+    const int pos = nc + __popc(m & lt);
+    if (keep && pos < WSORT) sm.id[pos] = id;
+    nc += __popc(m);
+  }
+  if (nc > WSORT || nc < p.K) { defer(); return; }
+  int32_t* c_id = sm.id;
+  // ---- consumed filter through a hash set of candidate slots (in s, dead after the cut)
+  if (meta.apply) {
+    int32_t* htab = reinterpret_cast<int32_t*>(sm.s);
+    for (int i = lane; i < 2 * WSORT; i += 32) htab[i] = -1;
+    __syncwarp();
+    for (int i = lane; i < nc; i += 32) {
+      uint32_t h = ((uint32_t)c_id[i] * 2654435761u) & (2 * WSORT - 1);
+      while (atomicCAS(&htab[h], -1, i) != -1) h = (h + 1) & (2 * WSORT - 1);
+    }
+    __syncwarp();
+    for (int64_t j = beg + lane; j < end; j += 32) {
+      const int32_t it = p.idx[j];
+      uint32_t h = ((uint32_t)it * 2654435761u) & (2 * WSORT - 1);
+      while (true) {
+        const int32_t e = htab[h];
+        if (e < 0) break;
+        if (c_id[e] == it || c_id[e] == ~it) { c_id[e] = ~it; break; }  // mark removed (negative)
+        h = (h + 1) & (2 * WSORT - 1);
+      }
+    }
+  }
+  __syncwarp();   // the hash set is dead from here on: its storage holds the sort keys
+  // ---- exact fp32 re-score, one lane per candidate: acc = fma(u[k], i[k], acc), k ascending
+  unsigned long long* skey = reinterpret_cast<unsigned long long*>(sm.s);
+  const bool vec4 = (p.d % 4 == 0) && (p.ldi % 4 == 0) && ((reinterpret_cast<uintptr_t>(p.I) & 15) == 0);
+#pragma unroll 1
+  for (int i = lane; i < WSORT; i += 32) {
+    unsigned long long comp = 0ull;
+    if (i < nc && c_id[i] >= 0) {
+      const float* it = p.I + (int64_t)c_id[i] * p.ldi;
+      float acc = 0.f;
+      if (vec4) {   // 16-byte loads; the fma chain stays sequential in k (exact-score definition)
+        const float4* it4 = reinterpret_cast<const float4*>(it);
+#pragma unroll 8
+        for (int k4 = 0; k4 < p.d / 4; ++k4) {
+          const float4 x = __ldg(it4 + k4);
+          const float4 w = sm.urow[k4];
+          acc = fmaf(w.x, x.x, acc);
+          acc = fmaf(w.y, x.y, acc);
+          acc = fmaf(w.z, x.z, acc);
+          acc = fmaf(w.w, x.w, acc);
+        }
+      } else {
+        for (int k = 0; k < p.d; ++k) acc = fmaf(urow[k], __ldg(it + k), acc);
+      }
+      comp = ((unsigned long long)float_to_key(acc) << 32) | (unsigned long long)(~(uint32_t)c_id[i]);
+    }
+    skey[i] = comp;
+  }
+  __syncwarp();
+  // ---- bitonic sort (descending) of the first P keys in shared memory: stages with j >= 32 pair
+  // elements of one lane, stages with j < 32 run on shuffles, one element per lane at a time
+  int P = 32;
+  while (P < nc) P <<= 1;
+  for (int k = 2; k <= P; k <<= 1) {
+    for (int j = k >> 1; j >= 32; j >>= 1) {
+      for (int q = lane; q < P / 2; q += 32) {
+        const int e = ((q & ~(j - 1)) << 1) | (q & (j - 1));   // the pair (e, e + j), bit j of e clear
+        const unsigned long long a = skey[e], b = skey[e + j];
+        if ((e & k) == 0 ? a < b : a > b) { skey[e] = b; skey[e + j] = a; }
+      }
+      __syncwarp();
+    }
+    for (int e = lane; e < P; e += 32) {
+      unsigned long long x = skey[e];
+      for (int j = min(k >> 1, 16); j > 0; j >>= 1) {
+        const unsigned long long y = __shfl_xor_sync(0xffffffffu, x, j);
+        const bool take_max = ((e & k) == 0) == ((e & j) == 0);
+        x = take_max ? (x > y ? x : y) : (x < y ? x : y);
+      }
+      skey[e] = x;
+    }
+    __syncwarp();
+  }
+  // fewer than K survivors: finalize_kernel flags the row (code 5)
+  if (skey[p.K - 1] == 0ull) { defer(); return; }
+  int64_t* oid = p.out_ids + row * p.K;
+  float* osc = p.out_scores ? p.out_scores + row * p.K : nullptr;
+  for (int e = lane; e < p.K; e += 32) {
+    const unsigned long long c = skey[e];
+    oid[e] = (int64_t)(~(uint32_t)(c & 0xffffffffull));
+    if (osc) osc[e] = key_to_float((uint32_t)(c >> 32));
+  }
+  if (lane == 0) p.out_status[row] = 0;
 }
 
 // ------------------------------------------------------------------------------------------
@@ -1275,6 +1528,7 @@ static int g_cluster = 2;          // 2 = pairs of user tiles share every item t
 static int g_nh = 1;               // MMA organisation of an item tile (1 x N=256, measured best on H100; 2 x N=128, epilogue of
                                    // the first overlaps the second; 3 = 2 x N=128 pipelined across tiles)
 static int g_ablate = 0;           // b200_recommend_embed_debug
+static int g_defer_all = 0;        // b200_recommend_embed_debug level 3
 static int g_hint_ns = 20000;      // suspend-time hint of the mbarrier waits in the sweep kernels
 static int g_pre_stride = PRE_STRIDE;   // b200_recommend_embed_speculation
 static double g_pre_delta = PRE_DELTA;
@@ -1291,7 +1545,7 @@ struct Plan {
   int64_t N_pad;
   size_t smem_bytes;
   // workspace offsets
-  size_t off_A, off_meta, off_tau, off_guess, off_status, off_cnt, off_hist, off_cs, off_bm, total;
+  size_t off_A, off_meta, off_tau, off_guess, off_status, off_cnt, off_defer, off_hist, off_cs, off_bm, total;
 };
 
 static int make_plan(int64_t B, int64_t N, int d, Plan* pl) {
@@ -1358,6 +1612,7 @@ static int make_plan(int64_t B, int64_t N, int d, Plan* pl) {
   pl->off_guess = off; off += al256((size_t)pl->B_pad * 4);
   pl->off_status = off; off += al256((size_t)pl->B_pad * 4);
   pl->off_cnt = off; off += al256((size_t)pl->n_lists * pl->B_pad * 4);
+  pl->off_defer = off; off += al256((size_t)(1 + pl->B_pad) * 4);   // count, then the rows finalize_kernel redoes
   pl->off_hist = off; off += al256((size_t)pl->B_pad * NB * 4);
   pl->off_cs = off; off += al256((size_t)pl->n_lists * pl->B_pad * pl->capg * REC * 4);
   pl->off_bm = off; off += al256((size_t)W_PRE * pl->n_splits * pl->n_pre_tiles * pl->B_pad * 4);
@@ -1525,13 +1780,16 @@ extern "C" int b200_recommend_embed_speculation(int32_t pre_stride, float delta)
 
 // Diagnostics (profiling only; results are WRONG while level 1 or 2 is set): 1 = the main pass collects
 // nothing (cold epilogue steps only), 2 = the main pass runs no epilogue at all (wait, MMA, release).
+// Level 3 (results unchanged) = finalize_warp_kernel defers every row to finalize_kernel, so that both
+// finalize paths can be run and compared on the same sweep output.
 extern "C" int b200_recommend_embed_debug(int32_t ablate_level) {
   // levels >= 100: suspend-time hint (ns) of the mbarrier waits of the sweep kernels = level - 100
   // levels -1 .. -64: additive margin of the linear speculative rank (pre_k = margin + coef * f * k_row) = -level
   if (ablate_level < 0 && ablate_level >= -64) { g_pre_margin = -ablate_level; return 0; }
   if (ablate_level >= 100) { g_hint_ns = ablate_level - 100; return 0; }
-  B200_REQUIRE(ablate_level >= 0 && ablate_level <= 2, "b200_recommend_embed_debug: level 0..2 (or 100 + hint ns)");
-  g_ablate = ablate_level;
+  B200_REQUIRE(ablate_level >= 0 && ablate_level <= 3, "b200_recommend_embed_debug: level 0..3 (or 100 + hint ns)");
+  g_ablate = ablate_level <= 2 ? ablate_level : 0;
+  g_defer_all = ablate_level == 3;
   return 0;
 }
 
@@ -1581,6 +1839,7 @@ extern "C" int b200_recommend_embed(const float* U, int64_t ldu, const int64_t* 
   uint32_t* guess = (uint32_t*)(ws + pl.off_guess);
   int32_t* status = (int32_t*)(ws + pl.off_status);
   int32_t* cnt = (int32_t*)(ws + pl.off_cnt);
+  int32_t* defer = (int32_t*)(ws + pl.off_defer);
   uint32_t* ghist = (uint32_t*)(ws + pl.off_hist);
   float* cand_r = (float*)(ws + pl.off_cs);
   float* bm = (float*)(ws + pl.off_bm);
@@ -1593,7 +1852,7 @@ extern "C" int b200_recommend_embed(const float* U, int64_t ldu, const int64_t* 
       U, ldu, user_ids, B, pl.B_pad, d, pl.d_pad, K, N, filter, pre_rank, indptr, n_users, hdr, A, meta,
       tau, status);
   count_launch();
-  // cnt and ghist are adjacent in the workspace: one memset
+  // cnt, the deferred-row list and ghist are adjacent in the workspace: one memset
   B200_CUDA_OK(cudaMemsetAsync(cnt, 0, (pl.off_cs - pl.off_cnt), stream));
 
   CUtensorMap tmA, tmB, tmBh;
@@ -1628,13 +1887,17 @@ extern "C" int b200_recommend_embed(const float* U, int64_t ldu, const int64_t* 
 
   FinalizeParams fp;
   fp.B = B; fp.N = N; fp.B_pad = pl.B_pad; fp.n_lists = pl.n_lists; fp.K = K; fp.d = d; fp.capg = pl.capg;
-  fp.meta = meta; fp.row_status = status; fp.row_tau_key = tau; fp.tau_guess_key = guess;
+  fp.defer_all = g_defer_all;
+  fp.meta = meta; fp.row_status = status; fp.out_status = row_status; fp.defer_count = defer;
+  fp.defer_rows = defer + 1; fp.row_tau_key = tau; fp.tau_guess_key = guess;
   fp.cand_r = cand_r; fp.cand_cnt = cnt;
   fp.U = U; fp.ldu = ldu; fp.I = I; fp.ldi = ldi; fp.user_ids = user_ids; fp.indptr = indptr;
   fp.idx = idx; fp.out_ids = out_ids; fp.out_scores = out_scores;
-  finalize_kernel<<<(unsigned)B, FIN_THREADS, 0, stream>>>(fp);
-  count_launch();
-  B200_CUDA_OK(cudaMemcpyAsync(row_status, status, (size_t)B * 4, cudaMemcpyDeviceToDevice, stream));
+  // every row writes its row_status once: 0 from the warp kernel, or any code from the block kernel
+  finalize_warp_kernel<<<(unsigned)ceil_div64(B, FINW_WARPS), FINW_WARPS * 32, 0, stream>>>(fp);
+  const int64_t fin_grid = (int64_t)FIN_CTAS_PER_SM * (sm_count > 0 ? sm_count : 132);
+  finalize_kernel<<<(unsigned)(B < fin_grid ? B : fin_grid), FIN_THREADS, 0, stream>>>(fp);
+  count_launch(2);
   B200_CUDA_OK(cudaGetLastError());
   return 0;
 }

@@ -3,7 +3,8 @@
 
 * sweep (PRE + guess + MAIN) and whole-call times from CUDA events, and the sweep at the per-phase levels
   0 (normal), 1 (cold epilogue steps only) and 2 (no epilogue) of b200_recommend_embed_debug;
-* per-kernel times (pre-pass, guess, main pass, finalize) from torch.profiler, in a run of their own;
+* per-kernel times (pre-pass, guess, main pass, finalize: the warp kernel and the deferred rows' block
+  kernel) from torch.profiler, in a run of their own;
 * candidate records per row (sum of the row's list lengths, cand_cnt) and rows per row_status code.
 
     python tools/profile_speculation.py [--settings legacy,16:1e-5,8:1e-5,4:1e-5] [--steps 10] [--out F]
@@ -25,7 +26,7 @@ import bench  # noqa: E402
 from _profile_common import card  # noqa: E402
 
 KERNELS = {"pre": "sweep_kernel<true", "guess": "guess_kernel", "main": "sweep_kernel<false",
-           "finalize": "finalize_kernel", "prep_users": "prep_users_kernel"}
+           "finalize_warp": "finalize_warp_kernel", "finalize": "finalize_kernel", "prep_users": "prep_users_kernel"}
 
 
 def select(setting):
