@@ -204,6 +204,51 @@ int b200_bpr_update(int32_t optimizer, const int32_t* users, const int32_t* item
                     uint64_t seed, const int32_t* items_neg, int32_t* neg_out, int64_t max_inflight,
                     void* stream);
 
+/* ---- Skip-gram training: gensim Word2Vec(sg=1) as Item2Vec / DeepWalk call it -----------------------------
+ * (libreco/bases/gensim_base.py:65-70 training, algorithms/item2vec.py:70-83 hs=0 negative=5,
+ * algorithms/deepwalk.py:96-126 hs=1 negative=5 and the Python random walks).  A corpus is a sentence CSR
+ * (indptr int64 [S+1], tokens int32 item ids, at most 10 000 tokens per sentence).  Every random draw is one
+ * Philox4x32-10 keyed by (seed, pass, position) only, never by the launch shape: pass 0 is DeepWalk's vocabulary
+ * walk set, training epoch e (from 1) is pass e.
+ *   b200_skipgram_subsample  replaces gensim's per-token downsampling: raw token t of item w is kept when the
+ *                            draw's first word is < keep_thr[w] (uint64 per item, 2^32 = always).  The kept tokens
+ *                            of sentence s are compacted in place: kept_tokens[indptr[s] + k], k < kept_len[s];
+ *                            kept_sent[q] is the sentence of slot q or -1 for an empty slot.  keep_out (optional,
+ *                            uint8 [T]) records every decision.
+ *   b200_skipgram_epoch      one epoch of skip-gram SGD over the compacted corpus (n_tokens = indptr[S] slots)
+ *                            into syn0 / syn1neg [n_items, d] and, with hs = 1, syn1 [V-1, d] along each item's
+ *                            Huffman path (hs_ptr int64 [n_items+1] into hs_points int32 / hs_codes int8, root
+ *                            first).  Negatives: bisect_left(neg_cum, r) for r uniform in [0, cum_last), cum_last =
+ *                            neg_cum[vocab_size-1], mapped to an item by neg_items; neg_guide [guide_buckets+1]
+ *                            holds bisect_left(neg_cum, k * ceil(cum_last / guide_buckets)).  alpha of sentence s
+ *                            = alpha0 - (alpha0 - min_alpha) min(1, (words_before + indptr[s]) / words_total).
+ *                            window_out (optional, int32 [T]) records each centre's reduced window b; neg_out
+ *                            (optional, int32 [T, 2 window + 1, negative]) each negative draw by (slot, context
+ *                            offset + window, draw).  max_inflight bounds the centres in flight (1: serial,
+ *                            deterministic, the sequential semantics; 0: b200_skipgram_default_inflight(d), but at most
+ *                            n_tokens / 256, at least 1).
+ *   b200_item_walks          replaces deepwalk.py:116-126: walk w = round * n_items + start item, each step
+ *                            uniform over the node's out-edges (graph CSR with multiplicity), stopping at
+ *                            walk_length tokens or a sink.  Call it twice: with lengths (int64 [n_walks n_items])
+ *                            to size the walks, then with their prefix sum in indptr to write tokens.
+ * d outside 1..128, window outside 1..4096, negative outside 1..16, bad sizes or null required pointers return -2
+ * before a launch. */
+int64_t b200_skipgram_default_inflight(int32_t d);
+int b200_skipgram_subsample(const int64_t* indptr, const int32_t* tokens, int64_t n_sentences, int64_t n_items,
+                            const uint64_t* keep_thr, uint64_t seed, int64_t pass, int32_t* kept_tokens,
+                            int32_t* kept_sent, int32_t* kept_len, uint8_t* keep_out, void* stream);
+int b200_skipgram_epoch(const int64_t* indptr, int64_t n_sentences, const int32_t* kept_tokens,
+                        const int32_t* kept_sent, const int32_t* kept_len, int64_t n_tokens, int64_t n_items,
+                        float* syn0, float* syn1neg, float* syn1, int32_t d, int32_t hs, const int64_t* hs_ptr,
+                        const int32_t* hs_points, const int8_t* hs_codes, const uint32_t* neg_cum,
+                        const int32_t* neg_items, int64_t vocab_size, uint32_t cum_last, const int32_t* neg_guide,
+                        int64_t guide_buckets, int32_t window, int32_t negative, double alpha0, double min_alpha,
+                        double words_before, double words_total, uint64_t seed, int64_t pass, int32_t* window_out,
+                        int32_t* neg_out, int64_t max_inflight, void* stream);
+int b200_item_walks(const int64_t* graph_indptr, const int32_t* graph_dst, int64_t n_items, int32_t n_walks,
+                    int32_t walk_length, uint64_t seed, int64_t pass, int64_t* lengths, const int64_t* indptr,
+                    int32_t* tokens, void* stream);
+
 /* ---- a4/a5/a6: feature models (FM, DeepFM, towers) -------------------------------------
  * Layout of the per-row features, as the reference's DataInfo provides them
  * (libreco/data/data_info.py:107-158, libreco/prediction/preprocess.py:15-57):

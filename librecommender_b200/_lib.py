@@ -7,7 +7,8 @@ from __future__ import annotations
 
 import ctypes
 import os
-from ctypes import c_char_p, c_float, c_int, c_int32, c_int64, c_size_t, c_uint64, c_ulonglong, c_void_p, POINTER
+from ctypes import (c_char_p, c_double, c_float, c_int, c_int32, c_int64, c_size_t, c_uint32, c_uint64, c_ulonglong,
+                    c_void_p, POINTER)
 
 _PKG_DIR = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_PKG_DIR, "libb200reco.so")
@@ -55,6 +56,12 @@ SIGNATURES = {
     "b200_bpr_default_inflight": (c_int64, [c_int32]),
     "b200_bpr_update": (c_int, [c_int32, _P, _P, c_int64, _P, _P, c_int64, c_int64, _P, _P, c_int32, _P, _P, _P, _P,
                                 c_float, c_float, c_float, c_float, c_float, c_int32, c_uint64, _P, _P, c_int64, _P]),
+    "b200_skipgram_default_inflight": (c_int64, [c_int32]),
+    "b200_skipgram_subsample": (c_int, [_P, _P, c_int64, c_int64, _P, c_uint64, c_int64, _P, _P, _P, _P, _P]),
+    "b200_skipgram_epoch": (c_int, [_P, c_int64, _P, _P, _P, c_int64, c_int64, _P, _P, _P, c_int32, c_int32, _P, _P,
+                                    _P, _P, _P, c_int64, c_uint32, _P, c_int64, c_int32, c_int32, c_double, c_double,
+                                    c_double, c_double, c_uint64, c_int64, _P, _P, c_int64, _P]),
+    "b200_item_walks": (c_int, [_P, _P, c_int64, c_int32, c_int32, c_uint64, c_int64, _P, _P, _P, _P]),
     "b200_feat_forward_tune": (c_int, [c_int32]),
     "b200_feat_forward": (c_int, [_P, _P, _P, _P, c_int64, c_int64, c_int64, _P, c_int64, _P, c_int64, _P, _P, _P, c_float,
                                   _P, _P, _P, c_float, _P, _P, c_int64, _P]),

@@ -22,7 +22,11 @@ What is patched (seams of SURVEY.md §8b; nothing else of the reference changes)
   whether or not a Cython build exists;
 * optionally (``bpr=True``) the Cython extension ``libreco.algorithms._bpr`` in the same way, with
   ``librecommender_b200.bpr.bpr_update``, so ``BPR(use_tf=False).fit``'s ``from ._bpr import bpr_update``
-  (``algorithms/bpr.py:309``) trains on the GPU.
+  (``algorithms/bpr.py:309``) trains on the GPU;
+* optionally (``gensim=True``) the ``Word2Vec`` name that ``bases/gensim_base.py:5``, ``algorithms/item2vec.py:2``
+  and ``algorithms/deepwalk.py:6`` bound at import → ``librecommender_b200.skipgram.Word2Vec``, and
+  ``GensimBase.set_embeddings`` (``gensim_base.py:96-108``, a per-user Python loop) → the device pooling, so
+  ``Item2Vec(...).fit`` / ``DeepWalk(...).fit`` train on the GPU whether or not gensim is installed.
 """
 from __future__ import annotations
 
@@ -54,7 +58,7 @@ def _register_cython(base, name, func):
 
 
 def install(libreco=None, losses: bool = True, lightgcn: bool = True, als: bool = False,
-            bpr: bool = False) -> None:
+            bpr: bool = False, gensim: bool = False) -> None:
     """Patch the reference package in place (idempotent: a second call re-installs)."""
     from . import recommendation as rec
 
@@ -99,6 +103,14 @@ def install(libreco=None, losses: bool = True, lightgcn: bool = True, als: bool 
         from .bpr import bpr_update
 
         _register_cython(base, "_bpr", bpr_update)
+    if gensim:
+        from . import skipgram
+
+        for sub in ("bases.gensim_base", "algorithms.item2vec", "algorithms.deepwalk"):
+            m = importlib.import_module(f"{base}.{sub}")
+            _patch(m, "Word2Vec", skipgram.Word2Vec)
+        gb = importlib.import_module(f"{base}.bases.gensim_base")
+        _patch(gb.GensimBase, "set_embeddings", skipgram.set_embeddings)
 
 
 def uninstall() -> None:
