@@ -249,6 +249,43 @@ int b200_item_walks(const int64_t* graph_indptr, const int32_t* graph_dst, int64
                     int32_t walk_length, uint64_t seed, int64_t pass, int64_t* lengths, const int64_t* indptr,
                     int32_t* tokens, void* stream);
 
+/* ---- GraphSage / PinSage inference (libreco/bases/sage_base.py:136-173, non-DGL) --------------------------
+ * The graph is two CSRs built from the reference's dicts with list order and multiplicity kept: item_consumed
+ * (item_ptr int64 [n_items+1], item_users int32) and user_consumed (user_ptr int64 [n_users+1], user_items int32).
+ * A sampling call covers one level: nodes int32 [n] (n = n_roots * per_root, node r belongs to roots[r / per_root]
+ * at path r % per_root; level 0: the roots themselves, per_root 1); level l+1 is the flattened output of level l with
+ * per_root * num_neighbors.  Every draw is Philox4x32-10 keyed by (seed, root, path, level, draw index), never by the
+ * batch.  A node id < 0 gives an empty row (-1 ids, weight 0, length 0).
+ *   b200_sage_neighbors     replaces bipartite_neighbors (libreco/sampling/random_walks.py:48-76): out int32
+ *                           [n, num_neighbors], each slot one-walks item -> consumer -> item with the reference's
+ *                           rejection rules (5 redraws while self or taken, 5 while self, then accept).
+ *   b200_pinsage_neighbors  replaces bipartite_neighbors_with_weights (random_walks.py:79-147) with items_pos =
+ *                           None: num_walks walks of at most walk_len one-walks, step s > 0 taken when the draw's
+ *                           word is >= cont_threshold (ceil(termination_prob 2^32)); the target removed, the top
+ *                           num_neighbors visits by count (ties: first visit), weight count / kept total.  out_ids
+ *                           int32 / out_weights float [n, num_neighbors], padded with -1 / 0; out_lens int32 [n].
+ *   b200_sage_aggregate     the per-layer input of the w_linears (graphsage_module.py:136-149,
+ *                           pinsage_module.py:79-97): out[r] = [S[self_idx ? self_idx[r] : r] (zeros for an index < 0),
+ *                           sum_j w_j N[nb_idx ? nb_idx[j] : j]] over row r's neighbour rows j = start .. start + len:
+ *                           start = nb_offsets[r] (or r * nb_stride), len = nb_lens[r] when given, else
+ *                           nb_offsets[r+1] - start (or nb_stride).  w_j = nb_weights[j], or 1 / len without weights
+ *                           (embedding_bag "mean"; an empty bag gives zeros).  out [n_rows, ldo >= 2 d].
+ * num_neighbors outside 1..32, num_walks * walk_len outside 1..256, d outside 1..128, bad sizes or null required
+ * pointers return -2 before a launch. */
+int b200_sage_neighbors(const int64_t* item_ptr, const int32_t* item_users, const int64_t* user_ptr,
+                        const int32_t* user_items, const int32_t* roots, const int32_t* nodes, int64_t n,
+                        int64_t per_root, int32_t level, int32_t num_neighbors, uint64_t seed, int32_t* out,
+                        void* stream);
+int b200_pinsage_neighbors(const int64_t* item_ptr, const int32_t* item_users, const int64_t* user_ptr,
+                           const int32_t* user_items, const int32_t* roots, const int32_t* nodes, int64_t n,
+                           int64_t per_root, int32_t level, int32_t num_neighbors, int32_t num_walks,
+                           int32_t walk_len, uint64_t cont_threshold, uint64_t seed, int32_t* out_ids,
+                           float* out_weights, int32_t* out_lens, void* stream);
+int b200_sage_aggregate(const float* S, int64_t lds, const int32_t* self_idx, int64_t n_rows, const float* N,
+                        int64_t ldn, const int32_t* nb_idx, const int64_t* nb_offsets, const int32_t* nb_lens,
+                        int32_t nb_stride, const float* nb_weights, int32_t d, float* out, int64_t ldo,
+                        void* stream);
+
 /* ---- a4/a5/a6: feature models (FM, DeepFM, towers) -------------------------------------
  * Layout of the per-row features, as the reference's DataInfo provides them
  * (libreco/data/data_info.py:107-158, libreco/prediction/preprocess.py:15-57):

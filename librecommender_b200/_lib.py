@@ -62,6 +62,11 @@ SIGNATURES = {
                                     _P, _P, _P, c_int64, c_uint32, _P, c_int64, c_int32, c_int32, c_double, c_double,
                                     c_double, c_double, c_uint64, c_int64, _P, _P, c_int64, _P]),
     "b200_item_walks": (c_int, [_P, _P, c_int64, c_int32, c_int32, c_uint64, c_int64, _P, _P, _P, _P]),
+    "b200_sage_neighbors": (c_int, [_P, _P, _P, _P, _P, _P, c_int64, c_int64, c_int32, c_int32, c_uint64, _P, _P]),
+    "b200_pinsage_neighbors": (c_int, [_P, _P, _P, _P, _P, _P, c_int64, c_int64, c_int32, c_int32, c_int32, c_int32,
+                                       c_uint64, c_uint64, _P, _P, _P, _P]),
+    "b200_sage_aggregate": (c_int, [_P, c_int64, _P, c_int64, _P, c_int64, _P, _P, _P, c_int32, _P, c_int32, _P,
+                                    c_int64, _P]),
     "b200_feat_forward_tune": (c_int, [c_int32]),
     "b200_feat_forward": (c_int, [_P, _P, _P, _P, c_int64, c_int64, c_int64, _P, c_int64, _P, c_int64, _P, _P, _P, c_float,
                                   _P, _P, _P, c_float, _P, _P, c_int64, _P]),

@@ -26,7 +26,10 @@ What is patched (seams of SURVEY.md §8b; nothing else of the reference changes)
 * optionally (``gensim=True``) the ``Word2Vec`` name that ``bases/gensim_base.py:5``, ``algorithms/item2vec.py:2``
   and ``algorithms/deepwalk.py:6`` bound at import → ``librecommender_b200.skipgram.Word2Vec``, and
   ``GensimBase.set_embeddings`` (``gensim_base.py:96-108``, a per-user Python loop) → the device pooling, so
-  ``Item2Vec(...).fit`` / ``DeepWalk(...).fit`` train on the GPU whether or not gensim is installed.
+  ``Item2Vec(...).fit`` / ``DeepWalk(...).fit`` train on the GPU whether or not gensim is installed;
+* optionally (``sage=True``) ``SageBase.set_embeddings`` (``bases/sage_base.py:136-173``, a Python neighbour walk
+  and a torch encoder per batch) → ``librecommender_b200.sage.set_embeddings`` for the non-DGL ``GraphSage`` /
+  ``PinSage``; the DGL classes keep the reference's method.
 """
 from __future__ import annotations
 
@@ -58,7 +61,7 @@ def _register_cython(base, name, func):
 
 
 def install(libreco=None, losses: bool = True, lightgcn: bool = True, als: bool = False,
-            bpr: bool = False, gensim: bool = False) -> None:
+            bpr: bool = False, gensim: bool = False, sage: bool = False) -> None:
     """Patch the reference package in place (idempotent: a second call re-installs)."""
     from . import recommendation as rec
 
@@ -111,6 +114,18 @@ def install(libreco=None, losses: bool = True, lightgcn: bool = True, als: bool 
             _patch(m, "Word2Vec", skipgram.Word2Vec)
         gb = importlib.import_module(f"{base}.bases.gensim_base")
         _patch(gb.GensimBase, "set_embeddings", skipgram.set_embeddings)
+    if sage:
+        from . import sage as sage_engine
+
+        sb = importlib.import_module(f"{base}.bases.sage_base")
+        reference_set_embeddings = sb.SageBase.set_embeddings
+
+        def set_embeddings(model):
+            if model.use_dgl:
+                return reference_set_embeddings(model)
+            return sage_engine.set_embeddings(model)
+
+        _patch(sb.SageBase, "set_embeddings", set_embeddings)
 
 
 def uninstall() -> None:
