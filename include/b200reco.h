@@ -118,7 +118,9 @@ int b200_recommend_embed(const float* U, int64_t ldu, const int64_t* user_ids, i
                          int32_t K, int64_t* out_ids, float* out_scores, int32_t* row_status,
                          void* workspace, size_t workspace_bytes, void* stream,
                          void* ev_sweep_start /* cudaEvent_t or NULL: recorded on `stream` */,
-                         void* ev_sweep_stop  /* just before / after the wgmma sweep kernels */);
+                         void* ev_sweep_stop  /* just before / after the wgmma sweep kernels */,
+                         int32_t* n_flagged   /* NULL, or one int32 (pinned host or device): the call's count of
+                                                 rows with a non-zero row_status, copied on `stream` after them */);
 
 /* ---- 8e row 2: row-sharded embedding table over NVLink peer memory ------------------------
  * (the reference has ONE table, libreco/layers/embedding.py:16-23; here row r lives on GPU r % G at

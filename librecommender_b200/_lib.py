@@ -40,7 +40,7 @@ SIGNATURES = {
     "b200_recommend_embed_plan": (c_int, [c_int64, c_int64, c_int32, c_int32, _P, c_int32]),
     "b200_recommend_embed_workspace_bytes": (c_int, [c_int64, c_int64, c_int32, c_int32, POINTER(c_size_t)]),
     "b200_recommend_embed": (c_int, [_P, c_int64, _P, c_int64, _P, c_int64, c_int64, c_int32, _P, _P, _P,
-                                     c_int64, c_int32, c_int32, _P, _P, _P, _P, c_size_t, _P, _P, _P]),
+                                     c_int64, c_int32, c_int32, _P, _P, _P, _P, c_size_t, _P, _P, _P, _P]),
     "b200_spmm_long_row_threshold": (c_int, []),
     "b200_spmm_chunk": (c_int, []),
     "b200_spmm_csr": (c_int, [_P, _P, _P, c_int64, _P, c_int64, c_int32, _P, c_int64, _P, c_int64, c_int32,

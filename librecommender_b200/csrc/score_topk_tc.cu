@@ -892,6 +892,7 @@ struct FinalizeParams {
   int32_t* out_status;             // [B] final row_status of the call, written once per row by one of the kernels
   int32_t* defer_count;            // rows handed from finalize_warp_kernel to finalize_kernel ...
   int32_t* defer_rows;             // ... and their indices [B_pad]
+  int32_t* flagged;                // rows of the call whose final status is not 0 (only finalize_kernel flags)
   const uint32_t* row_tau_key;     // [B_pad] final threshold of the row (speculative start or rigorous raises)
   const uint32_t* tau_guess_key;   // [B_pad] speculative threshold used by the main pass (0 = none)
   const float* cand_r;
@@ -921,8 +922,11 @@ __device__ __noinline__ void finalize_row(const FinalizeParams& p, const int64_t
   const RowMeta meta = p.meta[row];
   // row_status codes (non-zero = re-run on the exact path): 1 sweep overflow, 2 too few collected,
   // 3 failed speculation, 4 candidate set outside [K, MAXC], 5 capped row not provable
-  auto give_up = [&](int code) {
-    if (tid == 0) p.out_status[row] = code ? code : p.row_status[row];
+  auto give_up = [&](int code) {   // code 0 only for a row the sweep flagged: the status is never 0
+    if (tid == 0) {
+      p.out_status[row] = code ? code : p.row_status[row];
+      atomicAdd(p.flagged, 1);
+    }
     for (int i = tid; i < p.K; i += FIN_THREADS) { oid[i] = -1; if (osc) osc[i] = 0.f; }
   };
   if (p.row_status[row] != 0) { give_up(0); return; }
@@ -1545,7 +1549,7 @@ struct Plan {
   int64_t N_pad;
   size_t smem_bytes;
   // workspace offsets
-  size_t off_A, off_meta, off_tau, off_guess, off_status, off_cnt, off_defer, off_hist, off_cs, off_bm, total;
+  size_t off_A, off_meta, off_tau, off_guess, off_status, off_cnt, off_defer, off_flag, off_hist, off_cs, off_bm, total;
 };
 
 static int make_plan(int64_t B, int64_t N, int d, Plan* pl) {
@@ -1613,6 +1617,7 @@ static int make_plan(int64_t B, int64_t N, int d, Plan* pl) {
   pl->off_status = off; off += al256((size_t)pl->B_pad * 4);
   pl->off_cnt = off; off += al256((size_t)pl->n_lists * pl->B_pad * 4);
   pl->off_defer = off; off += al256((size_t)(1 + pl->B_pad) * 4);   // count, then the rows finalize_kernel redoes
+  pl->off_flag = off; off += al256(4);                              // rows with a non-zero status
   pl->off_hist = off; off += al256((size_t)pl->B_pad * NB * 4);
   pl->off_cs = off; off += al256((size_t)pl->n_lists * pl->B_pad * pl->capg * REC * 4);
   pl->off_bm = off; off += al256((size_t)W_PRE * pl->n_splits * pl->n_pre_tiles * pl->B_pad * 4);
@@ -1821,7 +1826,7 @@ extern "C" int b200_recommend_embed(const float* U, int64_t ldu, const int64_t* 
                                     int64_t n_users, int32_t filter, int32_t K, int64_t* out_ids,
                                     float* out_scores, int32_t* row_status, void* workspace,
                                     size_t workspace_bytes, void* stream_, void* ev_sweep_start,
-                                    void* ev_sweep_stop) {
+                                    void* ev_sweep_stop, int32_t* n_flagged) {
   B200_REQUIRE(U && user_ids && I && catalog && out_ids && row_status && workspace,
                "b200_recommend_embed: null pointer");
   B200_REQUIRE((int64_t)K <= N, "`n_rec` %d exceeds num of items %lld", K, (long long)N);
@@ -1840,6 +1845,7 @@ extern "C" int b200_recommend_embed(const float* U, int64_t ldu, const int64_t* 
   int32_t* status = (int32_t*)(ws + pl.off_status);
   int32_t* cnt = (int32_t*)(ws + pl.off_cnt);
   int32_t* defer = (int32_t*)(ws + pl.off_defer);
+  int32_t* flagged = (int32_t*)(ws + pl.off_flag);
   uint32_t* ghist = (uint32_t*)(ws + pl.off_hist);
   float* cand_r = (float*)(ws + pl.off_cs);
   float* bm = (float*)(ws + pl.off_bm);
@@ -1852,7 +1858,7 @@ extern "C" int b200_recommend_embed(const float* U, int64_t ldu, const int64_t* 
       U, ldu, user_ids, B, pl.B_pad, d, pl.d_pad, K, N, filter, pre_rank, indptr, n_users, hdr, A, meta,
       tau, status);
   count_launch();
-  // cnt, the deferred-row list and ghist are adjacent in the workspace: one memset
+  // cnt, the deferred-row list, the flagged-row count and ghist are adjacent in the workspace: one memset
   B200_CUDA_OK(cudaMemsetAsync(cnt, 0, (pl.off_cs - pl.off_cnt), stream));
 
   CUtensorMap tmA, tmB, tmBh;
@@ -1889,7 +1895,7 @@ extern "C" int b200_recommend_embed(const float* U, int64_t ldu, const int64_t* 
   fp.B = B; fp.N = N; fp.B_pad = pl.B_pad; fp.n_lists = pl.n_lists; fp.K = K; fp.d = d; fp.capg = pl.capg;
   fp.defer_all = g_defer_all;
   fp.meta = meta; fp.row_status = status; fp.out_status = row_status; fp.defer_count = defer;
-  fp.defer_rows = defer + 1; fp.row_tau_key = tau; fp.tau_guess_key = guess;
+  fp.defer_rows = defer + 1; fp.flagged = flagged; fp.row_tau_key = tau; fp.tau_guess_key = guess;
   fp.cand_r = cand_r; fp.cand_cnt = cnt;
   fp.U = U; fp.ldu = ldu; fp.I = I; fp.ldi = ldi; fp.user_ids = user_ids; fp.indptr = indptr;
   fp.idx = idx; fp.out_ids = out_ids; fp.out_scores = out_scores;
@@ -1898,6 +1904,8 @@ extern "C" int b200_recommend_embed(const float* U, int64_t ldu, const int64_t* 
   const int64_t fin_grid = (int64_t)FIN_CTAS_PER_SM * (sm_count > 0 ? sm_count : 132);
   finalize_kernel<<<(unsigned)(B < fin_grid ? B : fin_grid), FIN_THREADS, 0, stream>>>(fp);
   count_launch(2);
+  if (n_flagged)   // stream-ordered: a caller can wait for this call alone, not for what it enqueues next
+    B200_CUDA_OK(cudaMemcpyAsync(n_flagged, flagged, sizeof(int32_t), cudaMemcpyDefault, stream));
   B200_CUDA_OK(cudaGetLastError());
   return 0;
 }

@@ -164,8 +164,9 @@ class EmbedScorer:
                 "cluster_x10_plus_mma_groups", "records_per_list")
         return dict(zip(keys, [int(v) for v in out]))
 
-    def _fused_chunk(self, uid_chunk, n_rec, use_filter, out_ids, out_scores, status):
-        """One ``b200_recommend_embed`` call (<= FUSED_ROWS_PER_CALL rows) on the current stream."""
+    def _fused_chunk(self, uid_chunk, n_rec, use_filter, out_ids, out_scores, status, n_flagged=None):
+        """One ``b200_recommend_embed`` call (<= FUSED_ROWS_PER_CALL rows) on the current stream; ``n_flagged``:
+        address of an int32 that receives the chunk's count of rows with a non-zero status, or None."""
         torch = self._torch
         b = int(uid_chunk.numel())
         nbytes = ctypes.c_size_t(0)
@@ -183,17 +184,18 @@ class EmbedScorer:
             _lib.ptr(self.I), self.I.stride(0), self.n_items, self.d, _lib.ptr(self.catalog),
             _lib.ptr(self.indptr_d), _lib.ptr(self.idx_d), self.csr.n_users, use_filter, n_rec,
             _lib.ptr(out_ids), _lib.ptr(out_scores) if out_scores is not None else None,
-            _lib.ptr(status), _lib.ptr(ws), nbytes.value, _lib.current_stream(), ev0, ev1))
+            _lib.ptr(status), _lib.ptr(ws), nbytes.value, _lib.current_stream(), ev0, ev1, n_flagged))
         if self.events is not None:
             self.events.append((e0, e1))
 
     def recommend_fused(self, user_ids_d, n_rec, filter_consumed=True, return_scores=False, on_chunk=None,
-                        before_chunk=None, rows_per_call=None):
+                        before_chunk=None, rows_per_call=None, n_flagged=None):
         """Tensor-core path (b200_recommend_embed).  Returns (ids, scores|None, status):
         rows with status != 0 hold -1 ids and must be re-run on the exact path.  ``on_chunk(r0, r1)``
         is called after the kernels of rows [r0, r1) have been enqueued, ``before_chunk(r0, r1)`` just before
         (the host seam fills ``user_ids_d[r0:r1]`` there, so converting the ids of chunk i+1 overlaps the kernels
-        of chunk i)."""
+        of chunk i).  ``n_flagged``: pinned host int32 tensor with a word per chunk, which receives the chunk's
+        count of rows with a non-zero status in stream order."""
         torch = self._torch
         B = int(user_ids_d.numel())
         N = self.n_items
@@ -209,7 +211,8 @@ class EmbedScorer:
             if before_chunk is not None:
                 before_chunk(r0, r1)
             self._fused_chunk(user_ids_d[r0:r1], n_rec, use_filter, out_ids[r0:r1],
-                              out_scores[r0:r1] if return_scores else None, status[r0:r1])
+                              out_scores[r0:r1] if return_scores else None, status[r0:r1],
+                              None if n_flagged is None else n_flagged[r0 // step].data_ptr())
             if on_chunk is not None:
                 on_chunk(r0, r1)
         return out_ids, out_scores, status
@@ -232,9 +235,18 @@ class EmbedScorer:
         if path == "exact" or (path == "auto" and not self.fused_ok(n_rec)):
             return _Pending(self, user_ids_d, n_rec, filter_consumed, return_scores,
                             self.recommend_exact(user_ids_d, n_rec, filter_consumed, return_scores), None)
-        ids, scores, status = self.recommend_fused(user_ids_d, n_rec, filter_consumed, return_scores)
+        # the flagged-row count of every chunk lands in a pinned word right after the chunk's kernels, so that
+        # result() waits for this call only and not for a call enqueued after it
+        torch = self._torch
+        step = FUSED_ROWS_PER_CALL
+        slot = self._pinned("flagged", (max(1, -(-int(user_ids_d.numel()) // step)),), torch.int32)
+        slot[0].zero_()
+        ids, scores, status = self.recommend_fused(user_ids_d, n_rec, filter_consumed, return_scores,
+                                                   rows_per_call=step, n_flagged=slot[0])
+        done = torch.cuda.Event()
+        done.record()
         return _Pending(self, user_ids_d, n_rec, filter_consumed, return_scores,
-                        (ids, scores) if return_scores else ids, status)
+                        (ids, scores) if return_scores else ids, status, (self._export(slot), done))
 
     def recommend_device(self, user_ids_d, n_rec, filter_consumed=True, return_scores=False,
                          path="auto"):
@@ -378,24 +390,27 @@ class EmbedScorer:
 class _Pending:
     """Result handle of :meth:`EmbedScorer.recommend_device_async`."""
 
-    def __init__(self, scorer, uid_d, n_rec, filter_consumed, return_scores, res, status):
+    def __init__(self, scorer, uid_d, n_rec, filter_consumed, return_scores, res, status, flagged=None):
         self.scorer, self.uid_d, self.n_rec = scorer, uid_d, n_rec
         self.filter_consumed, self.return_scores = filter_consumed, return_scores
         self.res, self.status = res, status
+        self.flagged = flagged     # (pinned per-chunk counts of flagged rows, event recorded after the call)
 
     def result(self):
         if self.status is not None:
             torch = self.scorer._torch
-            bad = torch.nonzero(self.status).flatten()          # the only synchronisation
-            self.scorer.last_fallback_rows = int(bad.numel())
-            if bad.numel():
+            counts, done = self.flagged
+            done.synchronize()            # this call's kernels only; the only synchronisation unless a row is flagged
+            self.scorer.last_fallback_rows = int(counts.sum())
+            if self.scorer.last_fallback_rows:
+                bad = torch.nonzero(self.status).flatten()
                 fix = self.scorer.recommend_exact(self.uid_d[bad], self.n_rec, self.filter_consumed,
                                                   self.return_scores)
                 if self.return_scores:
                     self.res[0][bad], self.res[1][bad] = fix[0], fix[1]
                 else:
                     self.res[bad] = fix
-            self.status = None
+            self.status = self.flagged = None
         return self.res
 
 
