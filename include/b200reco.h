@@ -517,6 +517,8 @@ int b200_pointwise_loss(const float* logits, const float* labels, int64_t n, int
 /* kind 0 bpr = -mean log sigmoid(pos - neg) (torchops/loss.py:22-24), 1 max-margin
  * mean relu(margin - (pos - neg)) (:27-30, tfops/loss.py:61-64): n_neg must be a multiple of n_pos,
  * negatives of positive j are neg[j*f .. (j+1)*f) (compute_pair_scores, :63-90), dpos has n_pos entries.
+ * Max-margin ties follow torch's clamp_min: a pair exactly on the hinge (margin == pos - neg) has loss 0
+ * and gradient -1/n_neg w.r.t. pos (TF's relu would give 0 there).
  * kind 2 / 3 = sigmoid CE / focal over [pos (label 1), neg (label 0)] (:33-60), mean or sum. */
 int b200_pairwise_loss(const float* pos, int64_t n_pos, const float* neg, int64_t n_neg, int32_t kind,
                        float margin, float alpha, float gamma, int32_t mean, float* loss_out, float* dpos,

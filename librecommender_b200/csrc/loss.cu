@@ -90,10 +90,10 @@ pair_rank_kernel(const float* __restrict__ pos, int64_t n_pos, const float* __re
       if (kind == 0) {   // -log sigmoid(d)
         v = fmaxf(-d, 0.f) + softplus_neg_abs(d);
         gp = -sigmoidf(-d);
-      } else {           // relu(margin - d)
+      } else {           // relu(margin - d); torch's clamp_min passes the gradient at the hinge t == 0
         const float t = margin - d;
         v = fmaxf(t, 0.f);
-        gp = t > 0.f ? -1.f : 0.f;
+        gp = t >= 0.f ? -1.f : 0.f;
       }
       acc += v;
       if (dneg) dneg[e] = -gp * inv_n;

@@ -145,7 +145,10 @@ def bpr_loss(pos_scores, neg_scores):
 
 
 def max_margin_loss(pos_scores, neg_scores, margin):
-    """torchops/loss.py:27-30 (margin_ranking_loss with target 1) = tfops/loss.py:61-64 + reduce_mean."""
+    """torchops/loss.py:27-30 (margin_ranking_loss with target 1) = tfops/loss.py:61-64 + reduce_mean.
+
+    The value is the same for both.  The gradient follows torch: a pair exactly on the hinge
+    (``pos - neg == margin``) passes gradient -1/n to ``pos`` and 1/n to ``neg``, where TF's relu gives 0."""
     return _fns()[1].apply(pos_scores, neg_scores, 1, float(margin), 0.25, 2.0, True)
 
 
