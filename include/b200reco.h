@@ -991,6 +991,49 @@ int b200_gather_dot(const float* U, int64_t ldu, const int64_t* users, const flo
                     int64_t ldi, const int64_t* items, int64_t n, int32_t d, int32_t mode,
                     float lo, float hi, float* out, void* stream);
 
+/* ---- Swing (libreco/algorithms/swing.py; recfarm rust/src/graph.rs, swing.rs, inference.rs) -------------------
+ * The graph: R, the user x item CSR of train_data.sparse_interaction (user_ptr int64 [n_users+1], user_items int32,
+ * user_labels float), and R^T (item_ptr int64 [n_items+1], item_users int32); rows sorted and duplicate-free.
+ *   b200_swing_scores   replaces compute_swing_scores (graph.rs:147-234): w_u = 1 / sqrt(|I_u|); for each item i and
+ *                       users u < v of row i of R^T, C = I_u ∩ I_v, the term (w_u * w_v) * (alpha + |C| - 1)^-1 (fp32,
+ *                       the reference's rounding) is added to score_i[j] for every j in C, j != i.  Out: nbr_ids int32 /
+ *                       nbr_scores float [n_items, top_k], item i's top_k nonzero scores by (score desc, id asc),
+ *                       padded with -1 / 0, and nbr_count int64 [n_items], its number of nonzero scores (what
+ *                       swing.rs:150-151 sums).  Sums run in atomic order: repeated calls may differ in the last
+ *                       bits.  Synchronises `stream` (the task plan is built on the host from item_ptr).  top_k
+ *                       outside 1..4096, a catalogue whose bitmap does not fit in shared memory (n_items above
+ *                       about 1.8 M at top_k 20, 1.6 M at top_k 4096), a negative or non-finite alpha return -2 before a launch.
+ *   b200_swing_plan     which accumulator the scores kernel uses for n_items (1: shared memory, 0: one global row
+ *                       per resident CTA) and how many CTAs it keeps resident.
+ *   b200_swing_recommend  the accumulation of swing.rs:187-240: row r (user users[r]) of scores [B, ld] gets, for
+ *                       every (i, label) of row u of R and each of i's first min(top_k, nbr_count[i]) neighbours
+ *                       (j, s), s * label added at j, unless filter_consumed and j is in the consumed CSR's row u
+ *                       (always, not b200_mask_consumed's rule).  Items that got no term hold REMOVED, so
+ *                       b200_topk_rows ranks them last; counts[r] is the number that got one (the candidates).  A user
+ *                       outside [0, n_users) gets an all-REMOVED row and count 0.
+ *   b200_swing_random_keys  random_rec (inference.rs:78-86): a row with more than n_rec candidates gets a uniform
+ *                       key in [1, 2) at each candidate, Philox4x32-10 keyed by (seed, user, item); b200_topk_rows then
+ *                       draws n_rec distinct candidates.
+ *   b200_swing_predict  swing.rs:153-185 with compute_pred "ranking" (inference.rs:48-71): out[r] is the mean of
+ *                       the scores of item i's first top_k neighbours that row u of R holds; default_pred for an
+ *                       id outside range, an item without neighbours, an empty row or an empty intersection. */
+int b200_swing_scores_workspace_bytes(int64_t n_users, int64_t n_items, int32_t top_k, size_t* bytes);
+int b200_swing_scores(const int64_t* user_ptr, const int32_t* user_items, int64_t n_users, const int64_t* item_ptr,
+                      const int32_t* item_users, int64_t n_items, float alpha, int32_t top_k, int32_t* nbr_ids,
+                      float* nbr_scores, int64_t* nbr_count, void* workspace, size_t workspace_bytes, void* stream);
+int b200_swing_plan(int64_t n_items, int32_t top_k, int32_t* smem_acc, int32_t* ctas);
+int b200_swing_recommend(const int64_t* user_ptr, const int32_t* user_items, const float* user_labels,
+                         int64_t n_users, const int32_t* nbr_ids, const float* nbr_scores, const int64_t* nbr_count,
+                         int64_t n_items, int32_t top_k, const int64_t* consumed_ptr, const int32_t* consumed_idx,
+                         int32_t filter_consumed, const int64_t* users, int64_t B, float* scores, int64_t ld,
+                         int64_t* counts, void* stream);
+int b200_swing_random_keys(float* scores, int64_t ld, int64_t B, int64_t n_items, const int64_t* users,
+                           const int64_t* counts, int32_t n_rec, uint64_t seed, void* stream);
+int b200_swing_predict(const int64_t* user_ptr, const int32_t* user_items, int64_t n_users, const int32_t* nbr_ids,
+                       const float* nbr_scores, const int64_t* nbr_count, int64_t n_items, int32_t top_k,
+                       const int64_t* users, const int64_t* items, int64_t n, float default_pred, float* out,
+                       void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -29,7 +29,11 @@ What is patched (seams of SURVEY.md §8b; nothing else of the reference changes)
   ``Item2Vec(...).fit`` / ``DeepWalk(...).fit`` train on the GPU whether or not gensim is installed;
 * optionally (``sage=True``) ``SageBase.set_embeddings`` (``bases/sage_base.py:136-173``, a Python neighbour walk
   and a torch encoder per batch) → ``librecommender_b200.sage.set_embeddings`` for the non-DGL ``GraphSage`` /
-  ``PinSage``; the DGL classes keep the reference's method.
+  ``PinSage``; the DGL classes keep the reference's method;
+* optionally (``swing=True``) ``Swing.fit`` (``algorithms/swing.py:65-116``, which imports ``recfarm``) → a ``fit``
+  that builds ``librecommender_b200.swing.Swing`` into ``self.rs_model``, so the reference's own ``predict`` and
+  ``recommend_user`` run on the device engine whether or not ``recfarm`` is installed.  No ``recfarm`` module is
+  registered: ``data/consumed.py`` catches only ``ModuleNotFoundError`` on ``from recfarm import ...``.
 """
 from __future__ import annotations
 
@@ -61,7 +65,7 @@ def _register_cython(base, name, func):
 
 
 def install(libreco=None, losses: bool = True, lightgcn: bool = True, als: bool = False,
-            bpr: bool = False, gensim: bool = False, sage: bool = False) -> None:
+            bpr: bool = False, gensim: bool = False, sage: bool = False, swing: bool = False) -> None:
     """Patch the reference package in place (idempotent: a second call re-installs)."""
     from . import recommendation as rec
 
@@ -126,6 +130,17 @@ def install(libreco=None, losses: bool = True, lightgcn: bool = True, als: bool 
             return sage_engine.set_embeddings(model)
 
         _patch(sb.SageBase, "set_embeddings", set_embeddings)
+    if swing:
+        from . import swing as swing_engine
+
+        sw = importlib.import_module(f"{base}.algorithms.swing")
+
+        def fit(model, train_data, neg_sampling, verbose=1, eval_data=None, metrics=None, k=10, eval_batch_size=8192,
+                eval_user_num=None):
+            return swing_engine.fit_reference_model(model, sw, train_data, neg_sampling, verbose, eval_data, metrics,
+                                                    k, eval_batch_size, eval_user_num)
+
+        _patch(sw.Swing, "fit", fit)
 
 
 def uninstall() -> None:
