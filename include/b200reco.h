@@ -1034,6 +1034,51 @@ int b200_swing_predict(const int64_t* user_ptr, const int32_t* user_items, int64
                        const int64_t* users, const int64_t* items, int64_t n, float default_pred, float* out,
                        void* stream);
 
+/* ---- UserCF / ItemCF (libreco/bases/cf_base_rs.py; recfarm rust/src/similarities.rs, item_cf.rs, user_cf.rs,
+ * inference.rs) ---------------------------------------------------------------------------------------------------
+ * The "sim side" S (sim_ptr int64 [n_x+1], sim_idx int32, sim_val float) is the CSR whose rows are compared:
+ * item_interactions (R^T) for ItemCF, user_interactions (R) for UserCF; the "middle" M (mid_*) is its transpose.  Rows
+ * sorted and duplicate-free.
+ *   b200_cf_cosine      replaces compute_similarities (similarities.rs): sq[x] = sum of r^2 over row x of S (fp32, row
+ *                       order); for each x1 and x2 != x1 sharing count >= min_common middle rows p, cosine =
+ *                       prod / (sqrt(sq1) * sqrt(sq2)) with prod = sum of r[x1,p] * r[x2,p], or 0 if prod, sq1 or sq2
+ *                       is 0 (fp32, the reference's expression; only the order of the prod sum differs).  Zero and
+ *                       negative cosines are kept.  Out: nbr_ids int32 / nbr_scores float [n_x, k_sim], row x1's
+ *                       first k_sim kept entries by (cosine desc, id asc), padded with -1 / 0, and nbr_count int64
+ *                       [n_x], its kept count (what num_sim_elements sums).  Synchronises `stream` (the task plan is
+ *                       built on the host).  k_sim outside 1..4096 or min_common < 1 return -2 before a launch.
+ *   b200_cf_cosine_workspace_bytes  its workspace: (4 + 8) n_x bytes of row state, 4 n_x bytes per resident CTA
+ *                       (touched lists), 8 n_x more per resident CTA when the accumulator rows do not fit in shared
+ *                       memory (n_x above about 28.7 k at k_sim 20), and 12 n_x per split slot (64 slots).
+ *   b200_cf_plan        which accumulator b200_cf_cosine uses for n_x (1: shared memory, 0: one global row per
+ *                       resident CTA) and how many CTAs it keeps resident.
+ *   ItemCF's recommend (item_cf.rs:156-209) is b200_swing_recommend on the ItemCF neighbour table (top_k = k_sim).
+ *   b200_user_cf_recommend  user_cf.rs:151-205 with b200_swing_recommend's output contract: row r (user u = users[r])
+ *                       of scores [B, ld] gets, for each of u's first min(k_sim, nbr_count[u]) neighbours (v, sim) and
+ *                       each (i, label) of row v of R, sim * label added at i, unless filter_consumed and i is in the
+ *                       consumed CSR's row u.  Untouched items hold REMOVED; counts[r] is the number of candidates.
+ *   b200_cf_predict     item_cf.rs / user_cf.rs predict with compute_pred (inference.rs:48-71): the query's first
+ *                       min(k_sim, nbr_count[q]) neighbours intersected with row r of the CSR (ptr, idx, labels); task
+ *                       0 (rating) gives sum(label * sim / sum(sims)) per term (a zero sum of sims gives NaN or inf, as
+ *                       in the reference), task 1 (ranking) sum(sims) / n.  ItemCF: rows = users over R, queries =
+ *                       items; UserCF: rows = items over R^T, queries = users.  default_pred for an id outside range
+ *                       or an empty intersection. */
+int b200_cf_cosine_workspace_bytes(int64_t n_x, int32_t k_sim, size_t* bytes);
+int b200_cf_plan(int64_t n_x, int32_t k_sim, int32_t* smem_acc, int32_t* ctas);
+int b200_cf_cosine(const int64_t* sim_ptr, const int32_t* sim_idx, const float* sim_val, int64_t n_x,
+                   const int64_t* mid_ptr, const int32_t* mid_idx, const float* mid_val, int64_t n_y,
+                   int64_t min_common, int32_t k_sim, int32_t* nbr_ids, float* nbr_scores, int64_t* nbr_count,
+                   void* workspace, size_t workspace_bytes, void* stream);
+int b200_user_cf_recommend(const int64_t* user_ptr, const int32_t* user_items, const float* user_labels,
+                           int64_t n_users, const int32_t* nbr_ids, const float* nbr_scores, const int64_t* nbr_count,
+                           int64_t n_items, int32_t k_sim, const int64_t* consumed_ptr, const int32_t* consumed_idx,
+                           int32_t filter_consumed, const int64_t* users, int64_t B, float* scores, int64_t ld,
+                           int64_t* counts, void* stream);
+int b200_cf_predict(const int64_t* ptr, const int32_t* idx, const float* labels, int64_t n_rows,
+                    const int32_t* nbr_ids, const float* nbr_scores, const int64_t* nbr_count, int64_t n_queries,
+                    int32_t k_sim, const int64_t* rows, const int64_t* queries, int64_t n, int32_t task,
+                    float default_pred, float* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -21,10 +21,10 @@
 // finalize kernel selects from that row.  At most kSlots split items are in flight per round; rounds run back to
 // back, each with an even share of the unsplit items.
 //
-// Selection.  Per item the nonzero count is the touched count.  The top top_k entries by (score desc, id asc) are an
-// exact 64-bit radix select on (score bits << 32 | ~id) (scores are positive, so their bits order as floats), then a
-// bitonic sort in shared memory of at most top_k keys.
+// Selection.  Per item the nonzero count is the touched count.  The top top_k entries by (score desc, id asc) are
+// neighbours.cuh's exact radix select on (score bits << 32 | ~id) (scores are positive, so their bits order as floats).
 #include "common.cuh"
+#include "neighbours.cuh"
 #include "philox.cuh"
 #include "../../include/b200reco.h"
 
@@ -34,16 +34,9 @@
 namespace b200 {
 namespace swing {
 
-constexpr int THREADS = 256;
-constexpr int WARPS = THREADS / 32;
-constexpr int kMaxTopK = 4096;
-constexpr int kSlots = 64;                    // split items in flight per round
-constexpr int kMaxPieces = 1024;              // pieces per split item
-constexpr int64_t kMinPiecePairs = 1 << 15;   // an item with more pairs than max(this, total / (8 CTAs)) is split
-constexpr int kMaxGlobalCtasPerSm = 4;        // global accumulator rows: bound their number
-constexpr uint32_t kFiltered = 0xfffffffeu;   // recommend: a consumed item while filtering (restored to REMOVED)
+using namespace nbr;
 
-struct Task { int32_t item, pb, pe, slot; };
+constexpr int64_t kMinPiecePairs = 1 << 15;   // an item with more pairs than max(this, total / (8 CTAs)) is split
 
 struct Graph {
   const int64_t* user_ptr; const int32_t* user_items;
@@ -57,8 +50,6 @@ struct Plan {
   int sort_cap;      // power of two >= top_k
   int64_t bm_words;
 };
-
-__host__ __device__ inline int pow2_ceil(int x) { int p = 1; while (p < x) p <<= 1; return p; }
 
 // shared memory: [sort keys u64 sort_cap][bitmap u32 bm_words][acc f32 n_items (smem path)]
 __host__ inline size_t smem_bytes(int64_t n_items, int sort_cap, bool smem_acc) {
@@ -87,81 +78,6 @@ __device__ __forceinline__ bool add_first_touch(float* p, float v) {
 __global__ void user_weights_kernel(const int64_t* __restrict__ user_ptr, int64_t n_users, float* __restrict__ w) {
   const int64_t u = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (u < n_users) w[u] = __frcp_rn(__fsqrt_rn((float)(user_ptr[u + 1] - user_ptr[u])));
-}
-
-// Top min(T, top_k) of the T touched entries `tl` of row `acc` into out_ids / out_scores (padded with -1 / 0), sorted
-// by (score desc, id asc).  Every thread of the CTA calls it; ends with a __syncthreads.
-template <typename AccPtr>
-__device__ void select_topk(AccPtr acc, const int32_t* tl, int64_t T, int top_k, int sort_cap,
-                            unsigned long long* keys, int32_t* out_ids, float* out_scores) {
-  __shared__ int hist[256];
-  __shared__ unsigned long long s_prefix;
-  __shared__ int s_need, s_n;
-  const int tid = threadIdx.x;
-  auto key_of = [acc](int32_t j) -> unsigned long long {
-    return ((unsigned long long)__float_as_uint(acc[j]) << 32) | (unsigned long long)(~(uint32_t)j);
-  };
-  unsigned long long thr = 0;
-  if (T > top_k) {
-    unsigned long long prefix = 0, mask = 0;
-    int need = top_k;
-    for (int shift = 56; shift >= 0; shift -= 8) {
-      for (int b = tid; b < 256; b += blockDim.x) hist[b] = 0;
-      __syncthreads();
-      for (int64_t e = tid; e < T; e += blockDim.x) {
-        const unsigned long long k = key_of(tl[e]);
-        if ((k & mask) == prefix) atomicAdd(&hist[(k >> shift) & 255], 1);
-      }
-      __syncthreads();
-      if (tid == 0) {
-        int cum = 0, b = 255;
-        for (; b > 0; --b) {
-          if (cum + hist[b] >= need) break;
-          cum += hist[b];
-        }
-        s_need = need - cum;
-        s_prefix = prefix | ((unsigned long long)b << shift);
-      }
-      __syncthreads();
-      need = s_need;
-      prefix = s_prefix;
-      mask |= 255ull << shift;
-      __syncthreads();
-    }
-    thr = prefix;   // the top_k-th key itself: keys are distinct, so exactly top_k are >= thr
-  }
-  if (tid == 0) s_n = 0;
-  for (int e = tid; e < sort_cap; e += blockDim.x) keys[e] = 0ull;
-  __syncthreads();
-  for (int64_t e = tid; e < T; e += blockDim.x) {
-    const unsigned long long k = key_of(tl[e]);
-    if (k >= thr) keys[atomicAdd(&s_n, 1)] = k;
-  }
-  __syncthreads();
-  const int n = s_n;
-  const int len = pow2_ceil(n);
-  for (int k = 2; k <= len; k <<= 1) {
-    for (int j = k >> 1; j > 0; j >>= 1) {
-      for (int t = tid; t < len; t += blockDim.x) {
-        const int p = t ^ j;
-        if (p > t) {
-          const unsigned long long a = keys[t], b = keys[p];
-          if (((t & k) == 0) ? (a < b) : (a > b)) { keys[t] = b; keys[p] = a; }
-        }
-      }
-      __syncthreads();
-    }
-  }
-  for (int s = tid; s < top_k; s += blockDim.x) {
-    if (s < n) {
-      out_ids[s] = (int32_t)~(uint32_t)(keys[s] & 0xffffffffull);
-      out_scores[s] = __uint_as_float((uint32_t)(keys[s] >> 32));
-    } else {
-      out_ids[s] = -1;
-      out_scores[s] = 0.f;
-    }
-  }
-  __syncthreads();
 }
 
 __global__ void __launch_bounds__(THREADS) swing_scores_kernel(
@@ -232,7 +148,8 @@ __global__ void __launch_bounds__(THREADS) swing_scores_kernel(
     const int64_t T = (int64_t)s_ntl;
     if (task.slot < 0) {
       if (tid == 0) nbr_count[i] = T;
-      select_topk(acc, tl, T, top_k, sort_cap, keys, nbr_ids + (int64_t)i * top_k, nbr_scores + (int64_t)i * top_k);
+      select_topk<false>([acc](int32_t j) { return acc[j]; }, tl, T, top_k, sort_cap, keys,
+                         nbr_ids + (int64_t)i * top_k, nbr_scores + (int64_t)i * top_k);
     } else {
       float* row = split_rows + (int64_t)task.slot * n_items;
       int32_t* stl = split_tl + (int64_t)task.slot * n_items;
@@ -261,7 +178,8 @@ __global__ void __launch_bounds__(THREADS) swing_split_finalize_kernel(
   const int32_t* stl = split_tl + (int64_t)s * n_items;
   const int64_t T = (int64_t)split_n[s];
   if (threadIdx.x == 0) nbr_count[i] = T;
-  select_topk(row, stl, T, top_k, sort_cap, keys, nbr_ids + (int64_t)i * top_k, nbr_scores + (int64_t)i * top_k);
+  select_topk<false>([row](int32_t j) { return row[j]; }, stl, T, top_k, sort_cap, keys,
+                     nbr_ids + (int64_t)i * top_k, nbr_scores + (int64_t)i * top_k);
   for (int64_t e = threadIdx.x; e < T; e += THREADS) row[stl[e]] = 0.f;
   if (threadIdx.x == 0) split_n[s] = 0;
 }
@@ -272,23 +190,10 @@ __global__ void __launch_bounds__(THREADS) swing_recommend_kernel(
     const int64_t* __restrict__ nbr_count, int64_t n_items, int top_k, const int64_t* __restrict__ cons_ptr,
     const int32_t* __restrict__ cons_idx, int filter, const int64_t* __restrict__ users, float* __restrict__ scores,
     int64_t ld, int64_t* __restrict__ counts) {
-  __shared__ unsigned long long s_cand;
   const int64_t r = blockIdx.x;
   const int64_t u = users[r];
-  uint32_t* row = reinterpret_cast<uint32_t*>(scores + r * ld);
-  for (int64_t n = threadIdx.x; n < n_items; n += THREADS) row[n] = kRemovedBits;
-  if (threadIdx.x == 0) s_cand = 0;
-  const bool known = u >= 0 && u < n_users;
-  const bool filt = known && filter && cons_ptr != nullptr;
-  __syncthreads();
-  if (filt) {
-    for (int64_t e = cons_ptr[u] + threadIdx.x; e < cons_ptr[u + 1]; e += THREADS) {
-      const int32_t c = cons_idx[e];
-      if (c >= 0 && c < n_items) row[c] = kFiltered;
-    }
-    __syncthreads();
-  }
-  if (known) {
+  recommend_row(u, n_users, n_items, cons_ptr, cons_idx, filter, scores + r * ld, counts + r,
+                [&](uint32_t* row, unsigned long long* cand) {
     const int64_t a0 = user_ptr[u], len = user_ptr[u + 1] - a0;
     for (int64_t t = threadIdx.x; t < len * top_k; t += THREADS) {
       const int64_t e = a0 + t / top_k;
@@ -297,28 +202,9 @@ __global__ void __launch_bounds__(THREADS) swing_recommend_kernel(
       if (s >= nbr_count[i]) continue;
       const int32_t j = nbr_ids[(int64_t)i * top_k + s];
       // swing.rs:213-218: item_scores[j] += i_j_swing_score * i_label
-      const float v = __fmul_rn(nbr_scores[(int64_t)i * top_k + s], labels[e]);
-      uint32_t old = row[j];
-      for (;;) {
-        if (old == kFiltered) break;
-        const float nv = old == kRemovedBits ? v : __fadd_rn(__uint_as_float(old), v);
-        const uint32_t prev = atomicCAS(&row[j], old, __float_as_uint(nv));
-        if (prev == old) {
-          if (old == kRemovedBits) atomicAdd(&s_cand, 1ull);
-          break;
-        }
-        old = prev;
-      }
+      add_candidate(row, j, __fmul_rn(nbr_scores[(int64_t)i * top_k + s], labels[e]), cand);
     }
-  }
-  __syncthreads();
-  if (filt) {
-    for (int64_t e = cons_ptr[u] + threadIdx.x; e < cons_ptr[u + 1]; e += THREADS) {
-      const int32_t c = cons_idx[e];
-      if (c >= 0 && c < n_items) row[c] = kRemovedBits;
-    }
-  }
-  if (threadIdx.x == 0) counts[r] = (int64_t)s_cand;
+  });
 }
 
 // random_rec: a row with more than n_rec candidates gets a uniform key in [1, 2) per candidate, keyed by
@@ -337,43 +223,6 @@ __global__ void __launch_bounds__(THREADS) swing_random_keys_kernel(float* __res
     c.x = (uint32_t)n; c.y = (uint32_t)u; c.z = (uint32_t)(u >> 32); c.w = 0x53574e47u;
     row[n] = 0x3f800000u | (philox4x32_10(c, k0, k1).x >> 9);
   }
-}
-
-// one warp per (user, item) row: the mean swing score of the item's first top_k neighbours that row u of R holds
-__global__ void __launch_bounds__(THREADS) swing_predict_kernel(
-    const int64_t* __restrict__ user_ptr, const int32_t* __restrict__ user_items, int64_t n_users,
-    const int32_t* __restrict__ nbr_ids, const float* __restrict__ nbr_scores, const int64_t* __restrict__ nbr_count,
-    int64_t n_items, int top_k, const int64_t* __restrict__ users, const int64_t* __restrict__ items, int64_t n,
-    float default_pred, float* __restrict__ out) {
-  const int64_t r = ((int64_t)blockIdx.x * THREADS + threadIdx.x) >> 5;
-  const int lane = threadIdx.x & 31;
-  if (r >= n) return;
-  const int64_t u = users[r], i = items[r];
-  if (u < 0 || u >= n_users || i < 0 || i >= n_items) {
-    if (lane == 0) out[r] = default_pred;
-    return;
-  }
-  const int kk = (int)min((int64_t)top_k, nbr_count[i]);
-  const int64_t a0 = user_ptr[u], a1 = user_ptr[u + 1];
-  float sum = 0.f;
-  int hits = 0;
-  for (int s = lane; s < kk && a1 > a0; s += 32) {
-    const int32_t j = nbr_ids[i * top_k + s];
-    int64_t lo = a0, hi = a1;          // row u of R is sorted: lower bound of j
-    while (lo < hi) {
-      const int64_t mid = (lo + hi) >> 1;
-      if (user_items[mid] < j) lo = mid + 1; else hi = mid;
-    }
-    if (lo < a1 && user_items[lo] == j) {
-      sum += nbr_scores[i * top_k + s];
-      ++hits;
-    }
-  }
-  sum = warp_sum(sum);
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) hits += __shfl_xor_sync(0xffffffffu, hits, o);
-  // inference.rs:56-59 (ranking): sum of the intersected neighbours' scores / their number
-  if (lane == 0) out[r] = hits ? __fdiv_rn(sum, (float)hits) : default_pred;
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -600,9 +449,10 @@ extern "C" int b200_swing_predict(const int64_t* user_ptr, const int32_t* user_i
   B200_REQUIRE(n >= 0 && n_items >= 1 && n_users >= 0 && top_k >= 1 && top_k <= kMaxTopK,
                "b200_swing_predict: bad shape");
   if (n == 0) return 0;
-  swing_predict_kernel<<<(unsigned)ceil_div64(n, WARPS), THREADS, 0, (cudaStream_t)stream>>>(
-      user_ptr, user_items, n_users, nbr_ids, nbr_scores, nbr_count, n_items, top_k, users, items, n, default_pred,
-      out);
+  // the mean swing score of the item's first top_k neighbours that row u of R holds: compute_pred "ranking"
+  neighbour_predict_kernel<false><<<(unsigned)ceil_div64(n, WARPS), THREADS, 0, (cudaStream_t)stream>>>(
+      user_ptr, user_items, nullptr, n_users, nbr_ids, nbr_scores, nbr_count, n_items, top_k, users, items, n,
+      default_pred, out);
   count_launch();
-  return check_cuda(cudaGetLastError(), "swing_predict_kernel");
+  return check_cuda(cudaGetLastError(), "neighbour_predict_kernel");
 }

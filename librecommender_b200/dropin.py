@@ -33,7 +33,11 @@ What is patched (seams of SURVEY.md §8b; nothing else of the reference changes)
 * optionally (``swing=True``) ``Swing.fit`` (``algorithms/swing.py:65-116``, which imports ``recfarm``) → a ``fit``
   that builds ``librecommender_b200.swing.Swing`` into ``self.rs_model``, so the reference's own ``predict`` and
   ``recommend_user`` run on the device engine whether or not ``recfarm`` is installed.  No ``recfarm`` module is
-  registered: ``data/consumed.py`` catches only ``ModuleNotFoundError`` on ``from recfarm import ...``.
+  registered: ``data/consumed.py`` catches only ``ModuleNotFoundError`` on ``from recfarm import ...``;
+* optionally (``cf=True``) ``RsCfBase.fit`` (``bases/cf_base_rs.py:64-122``, which imports ``recfarm``) → a ``fit``
+  that builds ``librecommender_b200.cf.UserCF`` / ``ItemCF`` into ``self.rs_model``, so the reference's own
+  ``RsUserCF`` / ``RsItemCF`` ``predict``, ``recommend_user`` and ``evaluate`` run on the device engines; again no
+  ``recfarm`` module is registered.
 """
 from __future__ import annotations
 
@@ -65,7 +69,8 @@ def _register_cython(base, name, func):
 
 
 def install(libreco=None, losses: bool = True, lightgcn: bool = True, als: bool = False,
-            bpr: bool = False, gensim: bool = False, sage: bool = False, swing: bool = False) -> None:
+            bpr: bool = False, gensim: bool = False, sage: bool = False, swing: bool = False,
+            cf: bool = False) -> None:
     """Patch the reference package in place (idempotent: a second call re-installs)."""
     from . import recommendation as rec
 
@@ -141,6 +146,17 @@ def install(libreco=None, losses: bool = True, lightgcn: bool = True, als: bool 
                                                     k, eval_batch_size, eval_user_num)
 
         _patch(sw.Swing, "fit", fit)
+    if cf:
+        from . import cf as cf_engine
+
+        cb = importlib.import_module(f"{base}.bases.cf_base_rs")
+
+        def cf_fit(model, train_data, neg_sampling, verbose=1, eval_data=None, metrics=None, k=10,
+                   eval_batch_size=8192, eval_user_num=None):
+            return cf_engine.fit_reference_model(model, cb, train_data, neg_sampling, verbose, eval_data, metrics, k,
+                                                 eval_batch_size, eval_user_num)
+
+        _patch(cb.RsCfBase, "fit", cf_fit)
 
 
 def uninstall() -> None:

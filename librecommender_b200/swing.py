@@ -169,43 +169,16 @@ class Swing:
         """``(ids int64 [B, k], n int64 [B])`` for an int64 device tensor ``users``, k = min(n_rec, n_items): row r's
         first ``n[r]`` ids are its recommendations, the rest -1.  ``seed`` keys the ``random_rec`` draw (default: the
         engine's seed and a call counter)."""
-        import torch
-
-        from .engine import masked_topk
-
         self._require()
-        n_rec = int(n_rec)
-        if n_rec < 1:
-            raise ValueError("n_rec must be >= 1")
-        k = min(n_rec, self.n_items)
-        if k > MAX_TOP_K:
-            raise ValueError(f"n_rec above {MAX_TOP_K} is not supported for a catalogue of {self.n_items} items")
-        users = users.to(self.device, torch.int64).contiguous()
-        B = users.numel()
-        ids = torch.empty((B, k), dtype=torch.int64, device=self.device)
-        counts = torch.empty(B, dtype=torch.int64, device=self.device)
-        if random_rec and seed is None:
-            seed = (self.seed << 20) + self._draws
-            self._draws += 1
-        chunk = max(1, _ROW_BYTES // (4 * self.n_items))
-        stream = _lib.current_stream()
-        for r0 in range(0, B, chunk):
-            ub = users[r0:r0 + chunk]
-            b = ub.numel()
-            rows = torch.empty((b, self.n_items), dtype=torch.float32, device=self.device)
+
+        def accumulate(ub, rows, counts, stream):
             _lib.check(_lib.lib.b200_swing_recommend(
                 _lib.ptr(self.user_ptr), _lib.ptr(self.user_items), _lib.ptr(self.user_labels), self.n_users,
                 _lib.ptr(self.nbr_ids), _lib.ptr(self.nbr_scores), _lib.ptr(self.nbr_count), self.n_items, self.top_k,
-                _lib.ptr(self.cons_ptr), _lib.ptr(self.cons_idx), 1 if filter_consumed else 0, _lib.ptr(ub), b,
-                _lib.ptr(rows), self.n_items, _lib.ptr(counts[r0:r0 + b]), stream))
-            if random_rec:
-                _lib.check(_lib.lib.b200_swing_random_keys(_lib.ptr(rows), self.n_items, b, self.n_items, _lib.ptr(ub),
-                                                           _lib.ptr(counts[r0:r0 + b]), n_rec,
-                                                           int(seed) & 0xFFFFFFFFFFFFFFFF, stream))
-            masked_topk(self, rows, ub, k, False, ids[r0:r0 + b], None)
-        n = torch.clamp(counts, max=k)
-        ids[torch.arange(k, device=self.device)[None, :] >= n[:, None]] = -1
-        return ids, n
+                _lib.ptr(self.cons_ptr), _lib.ptr(self.cons_idx), 1 if filter_consumed else 0, _lib.ptr(ub),
+                ub.numel(), _lib.ptr(rows), self.n_items, _lib.ptr(counts), stream))
+
+        return recommend_rows(self, accumulate, users, n_rec, random_rec, seed)
 
     def recommend(self, users, n_rec, filter_consumed=True, random_rec=False):
         """recfarm's ``recommend``: ``(recs, additional counts)``, ``recs[r]`` the ids of user r as a list and
@@ -225,10 +198,53 @@ class Swing:
         return self.nbr_ids, self.nbr_scores, self.nbr_count
 
 
-def _transposed_cols(indptr, indices):
-    """Column ids of the transpose's entries in its CSR order (rows of the transpose sorted)."""
+def _transposed_cols(indptr, indices, data=None):
+    """Column ids of the transpose's entries in its CSR order (rows of the transpose sorted); with ``data``, also the
+    entries' values in that order."""
     rows = np.repeat(np.arange(len(indptr) - 1, dtype=np.int64), np.diff(indptr))
-    return rows[np.lexsort((rows, indices))].astype(np.int32)
+    order = np.lexsort((rows, indices))
+    cols = rows[order].astype(np.int32)
+    return cols if data is None else (cols, data[order])
+
+
+def recommend_rows(eng, accumulate, users, n_rec, random_rec=False, seed=None):
+    """Batched recommend of a neighbourhood engine ``eng`` (``n_items``, ``device``, ``seed``, the consumed CSR):
+    ``accumulate(ub, rows, counts, stream)`` fills the dense score rows [b, n_items] of the users ``ub`` (REMOVED where
+    untouched) and their candidate counts; ``random_rec`` rows with more than ``n_rec`` candidates then get
+    ``b200_swing_random_keys``, and ``masked_topk`` ranks every row.  Returns ``(ids int64 [B, k], n int64 [B])``,
+    k = min(n_rec, n_items), row r's first ``n[r]`` ids its recommendations and the rest -1."""
+    import torch
+
+    from .engine import masked_topk
+
+    n_rec = int(n_rec)
+    if n_rec < 1:
+        raise ValueError("n_rec must be >= 1")
+    k = min(n_rec, eng.n_items)
+    if k > MAX_TOP_K:
+        raise ValueError(f"n_rec above {MAX_TOP_K} is not supported for a catalogue of {eng.n_items} items")
+    users = users.to(eng.device, torch.int64).contiguous()
+    B = users.numel()
+    ids = torch.empty((B, k), dtype=torch.int64, device=eng.device)
+    counts = torch.empty(B, dtype=torch.int64, device=eng.device)
+    if random_rec and seed is None:
+        seed = (eng.seed << 20) + eng._draws
+        eng._draws += 1
+    chunk = max(1, _ROW_BYTES // (4 * eng.n_items))
+    stream = _lib.current_stream()
+    for r0 in range(0, B, chunk):
+        ub = users[r0:r0 + chunk]
+        b = ub.numel()
+        rows = torch.empty((b, eng.n_items), dtype=torch.float32, device=eng.device)
+        accumulate(ub, rows, counts[r0:r0 + b], stream)
+        if random_rec:
+            _lib.check(_lib.lib.b200_swing_random_keys(_lib.ptr(rows), eng.n_items, b, eng.n_items, _lib.ptr(ub),
+                                                       _lib.ptr(counts[r0:r0 + b]), n_rec,
+                                                       int(seed) & 0xFFFFFFFFFFFFFFFF, stream))
+        masked_topk(eng, rows, ub, k, False, ids[r0:r0 + b], None)
+    n = torch.clamp(counts, max=k)
+    ids[torch.arange(k, device=eng.device)[None, :] >= n[:, None]] = -1
+    return ids, n
 
 
 def plan(n_items, top_k):
