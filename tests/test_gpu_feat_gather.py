@@ -393,11 +393,19 @@ def test_misaligned_pointers_take_the_generic_kernel(what, code, tune):
     ud, itd = cuda_ids(u, it)
     kw = dict(concat_off=1) if what == "concat_ptr" else dict(pad=(5, 3, 5)) if what == "ld_concat" else {}
     tune(code)
-    torch.cuda.synchronize()
-    with profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA]) as prof:
-        got = run(dev, ud, itd, R, **kw)
-    assert _k1_kernels(prof) == [("generic", None)]
-    check(got, fr.ref(case, u, it), R, f"misaligned {what}")
+    want = fr.ref(case, u, it)
+    # torch.profiler occasionally delivers no CUDA kernel record at all for a window this short; such a window says
+    # nothing about the dispatch, so it is profiled again.  Any window that records a K1 kernel must show exactly
+    # the generic one.
+    for _ in range(3):
+        torch.cuda.synchronize()
+        with profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA]) as prof:
+            got = run(dev, ud, itd, R, **kw)
+        check(got, want, R, f"misaligned {what}")
+        ran = _k1_kernels(prof)
+        if ran:
+            break
+    assert ran == [("generic", None)]
 
 
 def test_concat_identical_across_families(tune):
