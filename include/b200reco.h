@@ -962,7 +962,7 @@ int b200_wavenet_encode(const int64_t* users, int64_t n, const int32_t* seqs, in
  * product with a causal layer's kernel [2, C, F] seen as [2C, F] gives its pre-activation, and its transpose the
  * kernel gradient.
  * b200_wavenet_layer_dx: given P = dpre [2, C, F]^T [n * T, 2C], dx[s*T + t, c] = P[s*T + t, C + c] +
- * P[s*T + t + d, c] (the second term while t + d < T).
+ * P[s*T + t + d, c] (the second term while t + d < T, for every dilation up to INT32_MAX).
  * Supported: the encoders' envelope (C <= 128, dilation >= 1 for the layer helpers); anything else returns -2
  * before launching; n = 0 launches nothing. */
 int b200_caser_train_forward(const int64_t* users, int64_t n, const int32_t* seqs, int64_t ld_seq, int32_t T,

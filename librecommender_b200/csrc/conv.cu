@@ -381,7 +381,8 @@ __global__ void wavenet_layer_inputs_kernel(const float* __restrict__ x, int64_t
   }
 }
 
-// dx[s * T + t, c] = P[s * T + t, C + c] + P[s * T + t + d, c] (the second term while t + d < T)
+// dx[s * T + t, c] = P[s * T + t, C + c] + P[s * T + t + d, c] (the second term while t + d < T, tested as
+// d < T - t so that a dilation near INT32_MAX cannot overflow into a read past the slot)
 __global__ void wavenet_layer_dx_kernel(const float* __restrict__ P, int64_t n, int T, int C, int d,
                                         float* __restrict__ dx, int64_t lddx) {
   const int64_t total = n * T * C;
@@ -389,7 +390,7 @@ __global__ void wavenet_layer_dx_kernel(const float* __restrict__ P, int64_t n, 
     const int64_t row = i / C;
     const int c = (int)(i - row * C), t = (int)(row % T);
     float v = __ldg(P + row * 2 * C + C + c);
-    if (t + d < T) v += __ldg(P + (row + d) * 2 * C + c);
+    if (d < T - t) v += __ldg(P + (row + d) * 2 * C + c);
     dx[row * lddx + c] = v;
   }
 }
