@@ -288,6 +288,42 @@ int b200_sage_aggregate(const float* S, int64_t lds, const int32_t* self_idx, in
                         int32_t nb_stride, const float* nb_weights, int32_t d, float* out, int64_t ldo,
                         void* stream);
 
+/* GraphSage training (the non-DGL GraphSageModel, libreco/algorithms/torch_modules/graphsage_module.py:82-140, and
+ * GraphCollator, libreco/batch/collators.py:338-386):
+ *   b200_sage_aggregate_backward  backward of b200_sage_aggregate in mean mode (no weights), the bags read as there:
+ *                           dout [n_rows, ldo >= 2 d] is d loss / d [self | mean] of each row; dout[r, :d] is ADDED
+ *                           into dS[self_idx ? self_idx[r] : r] (skipped for an index < 0) and dout[r, d:] / len into
+ *                           dN[nb_idx ? nb_idx[j] : j] for each neighbour j of row r (ids < 0 and empty bags add
+ *                           nothing).  Both buffers accumulate (+=): zero them first.  A hidden level gets gradient as
+ *                           the self input of one layer and as the neighbours of the level above it, so the caller
+ *                           adds both calls into one buffer.  No float atomics: the self rows must be distinct over r,
+ *                           and so must the neighbour rows (the sampler's layout: num_neighbors consecutive rows per
+ *                           node, one parent each).  The result is then bit-identical from run to run.
+ *   b200_sage_walk_pairs    pairs_from_random_walk (libreco/sampling/random_walks.py:21-41) for n_starts start items
+ *                           drawn uniformly on the device (starts int32 [n_starts]): per start, the (v, v) pair when no
+ *                           consumer of v has another item (has_no_neighbor), then num_walks walks of walk_length
+ *                           one-walks; one-walk cur -> next gives (cur, next) when next != cur, or with focus_start
+ *                           (v, next) when next != v.  Order: start, walk, step.  Draws: Philox4x32-10 keyed by
+ *                           (seed, step, start index, walk * walk_length + step in walk).  Two calls: the count pass
+ *                           (items == NULL) writes starts, counts int64 [n_starts (num_walks + 1)] and their exclusive
+ *                           prefix sum offsets int64 [n_starts (num_walks + 1) + 1] (the last entry: the number of
+ *                           pairs); the fill pass (same arguments, items / items_pos int32 [total]) writes the pairs.
+ *                           Every item must have a consumer.  num_walks / walk_length outside 1..1024 return -2.
+ *   b200_sage_i2i_negatives negatives_from_random with items (libreco/sampling/negatives.py:17-31): out int32 [n num_neg],
+ *                           negatives of pair j at out[j num_neg ..]; uniform over n_items, a draw equal to items[j] or
+ *                           items_pos[j] is drawn again up to `tolerance` times; keyed by (seed, step, slot, attempt).
+ * d outside 1..128, bad sizes or null required pointers return -2 before a launch. */
+int b200_sage_aggregate_backward(const float* dout, int64_t ldo, const int32_t* self_idx, int64_t n_rows, float* dS,
+                                 int64_t lds, const int32_t* nb_idx, const int64_t* nb_offsets, const int32_t* nb_lens,
+                                 int32_t nb_stride, int32_t d, float* dN, int64_t ldn, void* stream);
+int b200_sage_walk_pairs(const int64_t* item_ptr, const int32_t* item_users, const int64_t* user_ptr,
+                         const int32_t* user_items, int64_t n_items, int64_t n_starts, int32_t num_walks,
+                         int32_t walk_length, int32_t focus_start, uint64_t seed, uint64_t step, int32_t* starts,
+                         int64_t* counts, int64_t* offsets, int32_t* items, int32_t* items_pos, void* stream);
+int b200_sage_i2i_negatives(const int32_t* items, const int32_t* items_pos, int64_t n, int32_t num_neg,
+                            int64_t n_items, int32_t tolerance, uint64_t seed, uint64_t step, int32_t* out,
+                            void* stream);
+
 /* ---- a4/a5/a6: feature models (FM, DeepFM, towers) -------------------------------------
  * Layout of the per-row features, as the reference's DataInfo provides them
  * (libreco/data/data_info.py:107-158, libreco/prediction/preprocess.py:15-57):

@@ -67,6 +67,11 @@ SIGNATURES = {
                                        c_uint64, c_uint64, _P, _P, _P, _P]),
     "b200_sage_aggregate": (c_int, [_P, c_int64, _P, c_int64, _P, c_int64, _P, _P, _P, c_int32, _P, c_int32, _P,
                                     c_int64, _P]),
+    "b200_sage_aggregate_backward": (c_int, [_P, c_int64, _P, c_int64, _P, c_int64, _P, _P, _P, c_int32, c_int32, _P,
+                                             c_int64, _P]),
+    "b200_sage_walk_pairs": (c_int, [_P, _P, _P, _P, c_int64, c_int64, c_int32, c_int32, c_int32, c_uint64, c_uint64,
+                                     _P, _P, _P, _P, _P, _P]),
+    "b200_sage_i2i_negatives": (c_int, [_P, _P, c_int64, c_int32, c_int64, c_int32, c_uint64, c_uint64, _P, _P]),
     "b200_swing_scores_workspace_bytes": (c_int, [c_int64, c_int64, c_int32, POINTER(c_size_t)]),
     "b200_swing_scores": (c_int, [_P, _P, c_int64, _P, _P, c_int64, c_float, c_int32, _P, _P, _P, _P, c_size_t, _P]),
     "b200_swing_plan": (c_int, [c_int64, c_int32, POINTER(c_int32), POINTER(c_int32)]),

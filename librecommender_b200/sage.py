@@ -14,6 +14,9 @@ gather and dense-layer kernels.
 * User rows: i2i, the mean of the consumed item rows with multiplicity (``b200_spmm_csr``); u2i, ``user_proj`` of
   the raw user features (PinSage: then ``U2(relu(U1(.)))``).  Both tables get the mean OOV row
   (``assign_embedding_oov``) and serve through :class:`engine.EmbedScorer`.
+* Training (:class:`GraphSageTrainer`, GraphSage only): ``GraphTrainer`` + ``GraphCollator`` on the device, i2i walk
+  pairs and negatives from ``csrc/sage_train.cu``, the encoder's backward through ``b200_sage_aggregate_backward``,
+  ``torch.optim.Adam`` as TF-Adam; :meth:`GraphSageTrainer.state_dict` loads into :class:`GraphSage`.
 """
 from __future__ import annotations
 
@@ -23,7 +26,9 @@ import numpy as np
 
 from . import _lib
 from .consumed import ConsumedCSR
-from .feat_models import ACT_NONE, ACT_RELU, FeatSpec, _dev, _spec_get, feat_forward, linear, tables_struct
+from .feat_models import (ACT_NONE, ACT_RELU, FeatSpec, _dev, _spec_get, feat_backward, feat_forward, linear,
+                          tables_struct)
+from .training import _weight_grad
 
 MAX_LAYERS = 3
 MAX_NEIGHBORS = 32
@@ -430,3 +435,426 @@ def set_embeddings(model):
     U = eng.user_embeddings(I)
     model.item_embeds_np = I.cpu().numpy()
     model.user_embeds_np = U.cpu().numpy()
+
+
+# ---- GraphSage training ---------------------------------------------------------------------------------------------
+BETA1, BETA2 = 0.9, 0.999                    # torch.optim.Adam defaults (training/torch_trainer.py:63-68)
+LOSS_KINDS = {"bpr": 0, "max_margin": 1, "cross_entropy": 2, "focal": 3}    # b200_pairwise_loss kinds
+NEG_TOLERANCE = 10                           # negatives_from_random's tolerance
+_M64 = (1 << 64) - 1
+
+
+def adam_step_constants(lr, epsilon, t):
+    """``torch.optim.Adam`` step t (from 1) as TF-Adam: ``p -= lr_t m / (sqrt(v) + eps_hat)`` with ``lr_t = lr
+    sqrt(1 - beta2^t) / (1 - beta1^t)`` and ``eps_hat = eps sqrt(1 - beta2^t)``.  torch divides sqrt(v) by
+    sqrt(1 - beta2^t) before adding eps; multiplying through by that factor gives the TF form exactly."""
+    c2 = math.sqrt(1.0 - BETA2 ** t)
+    return lr * c2 / (1.0 - BETA1 ** t), epsilon * c2
+
+
+def _mix(seed, step, role):
+    """splitmix64 of (seed, step, role): one sampler seed per step and use, so each step draws fresh neighbours."""
+    x = (int(seed) + 0x9E3779B97F4A7C15 * (2 * int(step) + 1) + 0xD1B54A32D192ED03 * (int(role) + 1)) & _M64
+    x = ((x ^ (x >> 30)) * 0xBF58476D1CE4E5B9) & _M64
+    x = ((x ^ (x >> 27)) * 0x94D049BB133111EB) & _M64
+    return x ^ (x >> 31)
+
+
+def _xavier(rng, shape, gain=1.0):
+    """nn.init.xavier_uniform_ of a 2-D weight (fan_in = shape[1], fan_out = shape[0])."""
+    bound = gain * math.sqrt(6.0 / (shape[0] + shape[1]))
+    return rng.uniform(-bound, bound, size=shape).astype(np.float32)
+
+
+def init_state_dict(data_info, paradigm="i2i", embed_size=16, num_layers=2, seed=42):
+    """A fresh ``GraphSageModel`` state dict as ``init_parameters`` draws it (graphsage_module.py:38-49, 91-99):
+    xavier-uniform tables and projections, ``w_linears`` with the relu gain on every layer but the last, zero biases.
+    The shapes are the reference's; the values come from numpy's generator seeded by ``seed``."""
+    g = _spec_get(data_info)
+    d = int(embed_size)
+    rng = np.random.default_rng(seed)
+    n_users, n_items = int(g("n_users")), int(g("n_items"))
+    sides = ("user", "item") if paradigm == "u2i" else ("item",)
+    width = {s: len(list(g(f"{s}_sparse_col_index") or [])) + len(list(g(f"{s}_dense_col_index") or []))
+             for s in ("user", "item")}
+    sd = {}
+    for s in sides:
+        sd[f"{s}_embeds.weight"] = _xavier(rng, ((n_users if s == "user" else n_items), d))
+        sd[f"{s}_proj.weight"] = _xavier(rng, (d, (width[s] + 1) * d))
+        sd[f"{s}_proj.bias"] = np.zeros(d, np.float32)
+    uniq = [np.asarray(g(f"{s}_sparse_unique")) for s in ("user", "item")
+            if list(g(f"{s}_sparse_col_index") or []) and g(f"{s}_sparse_unique") is not None]
+    if uniq:                                  # sparse_feat_size: the largest index + 1
+        sd["sparse_embeds.weight"] = _xavier(rng, (int(max(int(u.max()) for u in uniq)) + 1, d))
+    n_dense = len(list(g("user_dense_col_index") or [])) + len(list(g("item_dense_col_index") or []))
+    if n_dense:
+        sd["dense_embeds"] = _xavier(rng, (n_dense, d))
+    relu_gain = math.sqrt(2.0)
+    for layer in range(num_layers):
+        sd[f"w_linears.{layer}.weight"] = _xavier(rng, (d, 2 * d), relu_gain if layer != num_layers - 1 else 1.0)
+        sd[f"w_linears.{layer}.bias"] = np.zeros(d, np.float32)
+    return sd
+
+
+def _check_train_options(paradigm, loss_type, sampler, start_node, lr_decay, amsgrad, dropout_rate, remove_edges):
+    if paradigm not in ("i2i", "u2i"):
+        raise ValueError("`paradigm` must either be `u2i` or `i2i`")
+    if loss_type not in LOSS_KINDS:
+        raise ValueError(f"unsupported `loss_type` {loss_type!r}, expected one of {sorted(LOSS_KINDS)}")
+    if lr_decay:
+        raise ValueError("lr_decay (CosineAnnealingWarmRestarts) is not supported by GraphSageTrainer")
+    if amsgrad:
+        raise ValueError("amsgrad is not supported by GraphSageTrainer")
+    if dropout_rate:
+        raise ValueError("dropout_rate > 0 is not supported by GraphSageTrainer")
+    if remove_edges:
+        raise ValueError("remove_edges is not supported by GraphSageTrainer")
+    if sampler in ("popular", "out-batch"):
+        raise ValueError(f"the {sampler!r} sampler is not supported by GraphSageTrainer")
+    allowed = ("random", "unconsumed") if paradigm == "u2i" else ("random",)
+    if sampler not in allowed:
+        raise ValueError(f"`sampler` must be one of {allowed} for {paradigm}, got {sampler!r}")
+    if start_node == "unpopular":
+        raise ValueError("start_node='unpopular' is not supported by GraphSageTrainer")
+    if start_node != "random":
+        raise ValueError(f"`start_node` must be 'random', got {start_node!r}")
+
+
+class GraphSageTrainer:
+    """Device training of the non-DGL ``GraphSage`` (``GraphSageModel``, graphsage_module.py:82-140) with
+    ``GraphTrainer`` (training/torch_trainer.py:170-282) and ``GraphCollator`` (batch/collators.py:338-386).
+
+    One :meth:`step` per mini-batch, every piece on the device:
+
+        i2i: b200_sage_walk_pairs (start items, walk pairs) -> b200_sage_i2i_negatives;  u2i: the batch's (user, item)
+        pairs -> b200_sample_negatives -> b200_sage_neighbors per level for the query, positive and negative items
+        (one encoder pass over all three) -> K1 gather + item_proj -> per layer b200_sage_aggregate + w_linears ->
+        pair scores -> b200_pairwise_loss -> the same chain backward (b200_sage_aggregate_backward, the dense-layer
+        kernel for dX / dW, b200_feat_backward into the tables) -> torch.optim.Adam as TF-Adam (b200_adam_dense_dev
+        with eps_hat = eps sqrt(1 - beta2^t), weight_decay = reg added to the gradient by b200_axpy).
+
+    The only device-to-host copy inside a step is the number of i2i walk pairs, which sizes the batch.  Neighbour
+    draws are keyed by (seed, step, encoder row, path, level), so every occurrence of an item in a batch draws its
+    own neighbours, as the reference's per-call ``random.choice`` does; the streams themselves are not the
+    reference's.
+
+    ``state_dict``: a ``GraphSageModel`` state dict to start from, else :func:`init_state_dict`.  The options are the
+    reference's; ``lr_decay``, ``amsgrad``, ``dropout_rate > 0``, ``remove_edges``, the ``popular`` / ``out-batch``
+    samplers and ``start_node='unpopular'`` raise ``ValueError``."""
+
+    def __init__(self, data_info, state_dict=None, paradigm="i2i", loss_type="cross_entropy", embed_size=16,
+                 num_layers=2, num_neighbors=3, num_neg=1, lr=1e-3, epsilon=1e-8, reg=None, margin=1.0,
+                 sampler="random", num_walks=10, sample_walk_len=5, start_node="random", focus_start=False,
+                 lr_decay=False, amsgrad=False, dropout_rate=0.0, remove_edges=False, seed=42, device=None):
+        _check_train_options(paradigm, loss_type, sampler, start_node, lr_decay, amsgrad, dropout_rate, remove_edges)
+        g = _spec_get(data_info)
+        n_items = int(g("n_items"))
+        if not 0 < int(num_neg) < n_items:
+            raise ValueError(f"`num_neg` should be positive and smaller than total items, got {num_neg}, {n_items}")
+        if not (1 <= int(num_walks) <= 1024 and 1 <= int(sample_walk_len) <= 1024):
+            raise ValueError("num_walks and sample_walk_len must lie in [1, 1024]")
+        if reg is not None and not (isinstance(reg, float) and reg > 0.0):
+            raise ValueError("reg must be float and positive...")
+        import torch
+
+        self._torch = torch
+        if state_dict is None:
+            state_dict = init_state_dict(data_info, paradigm, embed_size, num_layers, seed)
+        self.data_info = data_info
+        self.eng = GraphSage(data_info, state_dict, paradigm, num_layers, num_neighbors, seed, device)
+        e = self.eng
+        if paradigm == "i2i" and np.any(e.item_deg == 0):
+            raise ValueError(f"item {int(np.flatnonzero(e.item_deg == 0)[0])} has no consumer to walk from")
+        self.device, self.d, self.paradigm = e.device, e.d, paradigm
+        self.n_users, self.n_items = e.n_users, e.n_items
+        self.num_layers, self.num_neighbors, self.seed = e.num_layers, e.num_neighbors, e.seed
+        self.loss_type, self.kind = loss_type, LOSS_KINDS[loss_type]
+        self.num_neg, self.margin, self.sampler = int(num_neg), float(margin), sampler
+        self.num_walks, self.walk_len, self.focus_start = int(num_walks), int(sample_walk_len), bool(focus_start)
+        self.lr, self.epsilon, self.reg = float(lr), float(epsilon), float(reg or 0.0)
+        # the trainable tensors are the engine's own device copies, updated in place
+        self.params = {k: v for k, v in e.t.items() if v is not None}
+        self.params.update(e.w)
+        self.grads = {k: torch.zeros_like(v) for k, v in self.params.items()}
+        self.m = {k: torch.zeros_like(v) for k, v in self.params.items()}
+        self.v = {k: torch.zeros_like(v) for k, v in self.params.items()}
+        # torch's Adam skips a parameter without a gradient: the feature tables no side of the paradigm reads
+        sides = ("user", "item") if paradigm == "u2i" else ("item",)
+        reads = {"sparse_embeds": any(getattr(e.spec, f"{s}_sparse_cols") for s in sides),
+                 "dense_embeds": any(getattr(e.spec, f"{s}_dense_cols") for s in sides)}
+        self.frozen = {k for k, used in reads.items() if k in self.params and not used}
+        self.t = 0
+        self._step_dev = torch.zeros(1, dtype=torch.int64, device=self.device)
+        self._lr_t = torch.zeros(1, dtype=torch.float32, device=self.device)
+        self._lws = torch.empty(int(_lib.lib.b200_loss_workspace_bytes()), dtype=torch.uint8, device=self.device)
+        self._sorted = None
+        if sampler == "unconsumed":          # b200_sample_negatives reads each user's items sorted
+            row = np.repeat(np.arange(self.n_users), np.diff(e.user_ptr))
+            idx = e.user_items[np.lexsort((e.user_items, row))]
+            self._sorted = (torch.as_tensor(e.user_ptr).to(self.device),
+                            torch.as_tensor(np.ascontiguousarray(idx)).to(self.device))
+        self.last = None
+
+    # ---- sampling ---------------------------------------------------------------------------------------------------
+    def walk_pairs(self, n_starts, step=None):
+        """(starts, items, items_pos) int32 device tensors of one i2i batch: ``n_starts`` start items and their
+        random-walk pairs.  The pair count is the one device-to-host copy of a step."""
+        torch = self._torch
+        step = self.t if step is None else int(step)
+        dev, n = self.device, int(n_starts)
+        slots = n * (self.num_walks + 1)
+        starts = torch.empty(n, dtype=torch.int32, device=dev)
+        counts = torch.empty(slots, dtype=torch.int64, device=dev)
+        offsets = torch.empty(slots + 1, dtype=torch.int64, device=dev)
+        args = [_lib.ptr(a) for a in self.eng.graph] + [self.n_items, n, self.num_walks, self.walk_len,
+                                                         int(self.focus_start), self.seed, step, _lib.ptr(starts)]
+        _lib.check(_lib.lib.b200_sage_walk_pairs(*args, _lib.ptr(counts), _lib.ptr(offsets), None, None,
+                                                 _lib.current_stream()))
+        total = int(offsets[slots].item())
+        items = torch.empty(total, dtype=torch.int32, device=dev)
+        items_pos = torch.empty(total, dtype=torch.int32, device=dev)
+        if total:
+            _lib.check(_lib.lib.b200_sage_walk_pairs(*args, None, _lib.ptr(offsets), _lib.ptr(items),
+                                                     _lib.ptr(items_pos), _lib.current_stream()))
+        return starts, items, items_pos
+
+    def negatives(self, items_pos, items=None, users=None, step=None):
+        """int32 device [n * num_neg]: i2i (``items`` given) excludes each pair's item and positive; u2i draws
+        with the ``random`` or ``unconsumed`` rule of b200_sample_negatives."""
+        torch = self._torch
+        step = self.t if step is None else int(step)
+        n, f = int(items_pos.numel()), self.num_neg
+        if items is not None:
+            out = torch.empty(n * f, dtype=torch.int32, device=self.device)
+            _lib.check(_lib.lib.b200_sage_i2i_negatives(_lib.ptr(items), _lib.ptr(items_pos), n, f, self.n_items,
+                                                        NEG_TOLERANCE, self.seed, step, _lib.ptr(out),
+                                                        _lib.current_stream()))
+            return out
+        out = torch.empty(n * f, dtype=torch.int64, device=self.device)
+        pos64 = items_pos.to(torch.int64)
+        users64 = users.to(torch.int64)
+        mode = 1 if self.sampler == "unconsumed" else 0
+        indptr, idx = self._sorted if mode == 1 else (None, None)
+        _lib.check(_lib.lib.b200_sample_negatives(_lib.ptr(users64), _lib.ptr(pos64), n, f, self.n_items, mode,
+                                                  NEG_TOLERANCE, self.seed, step, _lib.ptr(indptr), _lib.ptr(idx),
+                                                  self.n_users, None, _lib.ptr(out), _lib.current_stream()))
+        return out.to(torch.int32)
+
+    def levels(self, items, step=None):
+        """Node ids per level (int32 device): level 0 the items, level l+1 ``num_neighbors`` per node of level l.
+        Each row of ``items`` roots its own draws (keyed by its position), so a repeated item draws anew."""
+        torch = self._torch
+        step = self.t if step is None else int(step)
+        nn, seed = self.num_neighbors, _mix(self.seed, step, 0)
+        keys = torch.arange(int(items.numel()), dtype=torch.int32, device=self.device)
+        ids, nodes, per_root = [items], items, 1
+        for level in range(self.num_layers):
+            n = int(nodes.numel())
+            out = torch.empty(n * nn, dtype=torch.int32, device=self.device)
+            _lib.check(_lib.lib.b200_sage_neighbors(*[_lib.ptr(a) for a in self.eng.graph], _lib.ptr(keys),
+                                                    _lib.ptr(nodes), n, per_root, level, nn, seed, _lib.ptr(out),
+                                                    _lib.current_stream()))
+            ids.append(out)
+            nodes, per_root = out, per_root * nn
+        return ids
+
+    # ---- encoder ----------------------------------------------------------------------------------------------------
+    def _project(self, which, ids64):
+        torch = self._torch
+        L, pos = self.eng.spec.side(which)
+        n = int(ids64.numel())
+        x = torch.empty((n, len(pos) * self.d), dtype=torch.float32, device=self.device)
+        feat_forward(L, self.eng.tables, ids64, ids64, n, concat=x)
+        p = self.params
+        return x, linear(x, p[f"{which}_proj.weight"], p[f"{which}_proj.bias"], ACT_NONE, cache_split=False)
+
+    def _project_backward(self, which, ids64, x, dy):
+        p, g = self.params, self.grads
+        g[f"{which}_proj.weight"] += _weight_grad(dy, x)
+        _col_sum(dy, g[f"{which}_proj.bias"])
+        dx = linear(dy, p[f"{which}_proj.weight"].t().contiguous(), None, ACT_NONE, cache_split=False)
+        feat_backward(self.eng.spec.side(which)[0], self.eng.tables, ids64, ids64, int(ids64.numel()), g, dconcat=dx)
+
+    def encode(self, ids):
+        """GraphSageModel.forward over the levels ``ids`` (from :meth:`levels`): (rows [n_0, d], cache).  Every level
+        is projected in one gather and one GEMM; the levels of a layer are aggregated into one buffer and go through
+        one GEMM."""
+        torch = self._torch
+        d, L, nn = self.d, self.num_layers, self.num_neighbors
+        sizes = [int(a.numel()) for a in ids]
+        offs = np.concatenate([[0], np.cumsum(sizes)]).tolist()
+        ids64 = torch.cat(ids).to(torch.int64)
+        x, H = self._project("item", ids64)
+        c = dict(ids64=ids64, x=x, offs=offs, aggs=[], outs=[])
+        for layer in range(L):
+            depth = L - layer
+            agg = torch.empty((offs[depth], 2 * d), dtype=torch.float32, device=self.device)
+            for k in range(depth):
+                S, N, out = H[offs[k]:offs[k + 1]], H[offs[k + 1]:offs[k + 2]], agg[offs[k]:offs[k + 1]]
+                _lib.check(_lib.lib.b200_sage_aggregate(
+                    _lib.ptr(S), d, None, sizes[k], _lib.ptr(N), d, None, None, None, nn, None, d, _lib.ptr(out),
+                    2 * d, _lib.current_stream()))
+            H = linear(agg, self.params[f"w_linears.{layer}.weight"], self.params[f"w_linears.{layer}.bias"],
+                       ACT_RELU if layer != L - 1 else ACT_NONE, cache_split=False)
+            c["aggs"].append(agg)
+            c["outs"].append(H)
+        return H, c
+
+    def encode_backward(self, c, dH):
+        """Gradients of :meth:`encode`'s parameters ADDED into ``grads`` given d loss / d rows."""
+        torch = self._torch
+        lib, st = _lib.lib, _lib.current_stream()
+        d, L, nn, offs = self.d, self.num_layers, self.num_neighbors, c["offs"]
+        p, g = self.params, self.grads
+        G = dH.contiguous()
+        for layer in range(L - 1, -1, -1):
+            depth = L - layer
+            if layer != L - 1:
+                dz = torch.empty_like(G)
+                _lib.check(lib.b200_relu_backward(_lib.ptr(G), _lib.ptr(c["outs"][layer]), G.numel(), _lib.ptr(dz),
+                                                  st))
+                G = dz
+            g[f"w_linears.{layer}.weight"] += _weight_grad(G, c["aggs"][layer])
+            _col_sum(G, g[f"w_linears.{layer}.bias"])
+            dagg = linear(G, p[f"w_linears.{layer}.weight"].t().contiguous(), None, ACT_NONE, cache_split=False)
+            dprev = torch.zeros((offs[depth + 1], d), dtype=torch.float32, device=self.device)
+            for k in range(depth):
+                dA, dS, dN = dagg[offs[k]:offs[k + 1]], dprev[offs[k]:offs[k + 1]], dprev[offs[k + 1]:offs[k + 2]]
+                _lib.check(lib.b200_sage_aggregate_backward(
+                    _lib.ptr(dA), 2 * d, None, offs[k + 1] - offs[k], _lib.ptr(dS), d, None, None, None, nn, d,
+                    _lib.ptr(dN), d, st))
+            G = dprev
+        self._project_backward("item", c["ids64"], c["x"], G)
+
+    # ---- step -------------------------------------------------------------------------------------------------------
+    def _scores(self, Q, P, N):
+        """compute_pair_scores (torchops/loss.py:67-90): pos [n], neg [n num_neg] with negatives of row i at
+        i num_neg ..; the positives are repeated by the loss kernel for bpr / max-margin."""
+        torch = self._torch
+        n, f, d = int(Q.shape[0]), self.num_neg, self.d
+        rows = torch.arange(n * f, dtype=torch.int64, device=self.device)
+        pos = torch.empty(n, dtype=torch.float32, device=self.device)
+        neg = torch.empty(n * f, dtype=torch.float32, device=self.device)
+        st = _lib.current_stream()
+        _lib.check(_lib.lib.b200_gather_dot(_lib.ptr(Q), d, _lib.ptr(rows), _lib.ptr(P), d, _lib.ptr(rows), n, d, 0,
+                                            0.0, 0.0, _lib.ptr(pos), st))
+        qrows = torch.div(rows, f, rounding_mode="floor")
+        _lib.check(_lib.lib.b200_gather_dot(_lib.ptr(Q), d, _lib.ptr(qrows), _lib.ptr(N), d, _lib.ptr(rows), n * f, d,
+                                            0, 0.0, 0.0, _lib.ptr(neg), st))
+        return pos, neg
+
+    def forward_backward(self, users=None, items=None, batch_size=None):
+        """One batch's loss (device scalar) with every gradient buffer filled, no optimizer step.  u2i: ``users`` /
+        ``items`` the batch's pairs; i2i: ``batch_size`` start items (or ``len(items)``).  The sampled batch is kept
+        in ``last`` (device tensors).  None when an i2i batch yields no pair."""
+        torch = self._torch
+        dev, f = self.device, self.num_neg
+        if self.paradigm == "u2i":
+            users = torch.as_tensor(users).to(dev).to(torch.int64).reshape(-1)
+            q_items = None
+            pos_items = torch.as_tensor(items).to(dev).to(torch.int32).reshape(-1)
+            if users.numel() != pos_items.numel():
+                raise ValueError("users and items differ in length")
+            neg_items = self.negatives(pos_items, users=users)
+            roots = torch.cat([pos_items, neg_items])
+        else:
+            n_starts = int(batch_size if batch_size is not None else len(items))
+            _, q_items, pos_items = self.walk_pairs(n_starts)
+            if q_items.numel() == 0:
+                self.last = None
+                return None
+            neg_items = self.negatives(pos_items, items=q_items)
+            roots = torch.cat([q_items, pos_items, neg_items])
+        n = int(pos_items.numel())
+        ids = self.levels(roots)
+        R, c = self.encode(ids)
+        if self.paradigm == "u2i":
+            xu, Q = self._project("user", users)
+            P, N = R[:n], R[n:]
+        else:
+            Q, P, N = R[:n], R[n:2 * n], R[2 * n:]
+        pos, neg = self._scores(Q, P, N)
+        loss = torch.empty((), dtype=torch.float32, device=dev)
+        dpos, dneg = torch.empty_like(pos), torch.empty_like(neg)
+        mean = 1 if self.paradigm == "u2i" else 0
+        _lib.check(_lib.lib.b200_pairwise_loss(_lib.ptr(pos), n, _lib.ptr(neg), n * f, self.kind, self.margin, 0.25,
+                                               2.0, mean, _lib.ptr(loss), _lib.ptr(dpos), _lib.ptr(dneg),
+                                               _lib.ptr(self._lws), self._lws.numel(), _lib.current_stream()))
+        # d loss / d rows of the pair scores (elementwise; the reductions over the batch happen in the GEMMs above)
+        dneg3 = dneg.view(n, f, 1)
+        dQ = dpos[:, None] * P + (dneg3 * N.view(n, f, self.d)).sum(1)
+        dR = torch.cat([dpos[:, None] * Q, (dneg3 * Q[:, None, :]).reshape(n * f, self.d)])
+        if self.paradigm == "u2i":
+            self._project_backward("user", users, xu, dQ)
+        else:
+            dR = torch.cat([dQ, dR])
+        self.encode_backward(c, dR)
+        self.last = dict(users=users, items=q_items, items_pos=pos_items, items_neg=neg_items, levels=ids, pos=pos,
+                         neg=neg)
+        return loss
+
+    def adam_update(self):
+        """torch.optim.Adam(lr, eps=epsilon, weight_decay=reg) over every parameter; zeroes the gradients."""
+        lib, st = _lib.lib, _lib.current_stream()
+        self.t += 1
+        _, eps_hat = adam_step_constants(self.lr, self.epsilon, self.t)
+        _lib.check(lib.b200_adam_begin_step(_lib.ptr(self._step_dev), self.lr, BETA1, BETA2, 1.0, 0,
+                                            _lib.ptr(self._lr_t), st))
+        for k, p in self.params.items():
+            if k in self.frozen:
+                continue
+            if self.reg:
+                _lib.check(lib.b200_axpy(_lib.ptr(self.grads[k]), _lib.ptr(p), self.reg, p.numel(), st))
+            _lib.check(lib.b200_adam_dense_dev(_lib.ptr(p), _lib.ptr(self.m[k]), _lib.ptr(self.v[k]),
+                                               _lib.ptr(self.grads[k]), p.numel(), _lib.ptr(self._lr_t), BETA1, BETA2,
+                                               eps_hat, st))
+
+    def step(self, users=None, items=None, batch_size=None):
+        """One mini-batch: sampling, forward, backward and the Adam update.  Returns the device loss (None for an
+        i2i batch without pairs, which leaves the parameters and the step count alone)."""
+        loss = self.forward_backward(users, items, batch_size)
+        if loss is not None:
+            self.adam_update()
+        return loss
+
+    def fit(self, users, items, n_epochs=1, batch_size=256, shuffle=True):
+        """Epochs over the training pairs in mini-batches of ``batch_size`` (shuffled per epoch as the reference's
+        DataLoader does); an i2i batch takes its size from the pairs.  Returns the mean batch loss per epoch."""
+        torch = self._torch
+        users, items = np.asarray(users).reshape(-1), np.asarray(items).reshape(-1)
+        rng = np.random.default_rng(self.seed)
+        means = []
+        for _ in range(int(n_epochs)):
+            order = rng.permutation(users.size) if shuffle else np.arange(users.size)
+            losses = []
+            for b0 in range(0, users.size, int(batch_size)):
+                sel = order[b0:b0 + int(batch_size)]
+                loss = self.step(users[sel], items[sel]) if self.paradigm == "u2i" else self.step(batch_size=sel.size)
+                if loss is not None:
+                    losses.append(loss)
+            means.append(float(torch.stack(losses).mean().item()) if losses else float("nan"))
+        return means
+
+    # ---- export -----------------------------------------------------------------------------------------------------
+    def state_dict(self):
+        """The parameters as ``GraphSageModel.state_dict()`` holds them: the reference's keys, shapes and column
+        order, float32 CPU tensors."""
+        out = {}
+        for k, v in self.params.items():
+            a = v.detach().cpu()
+            if k in ("item_proj.weight", "user_proj.weight"):       # the side gather's [id, ...] back to [..., id]
+                a = self._torch.cat([a[:, self.d:], a[:, :self.d]], dim=1)
+            key = k if k in ("dense_embeds",) or "." in k else f"{k}.weight"
+            out[key] = a.contiguous()
+        return out
+
+    def engine(self):
+        """A :class:`GraphSage` inference engine on the current parameters."""
+        return GraphSage(self.data_info, self.state_dict(), self.paradigm, self.num_layers, self.num_neighbors,
+                         self.seed, self.device)
+
+
+def _col_sum(X, out):
+    """out += the column sums of X (b200_col_reduce, deterministic)."""
+    _lib.check(_lib.lib.b200_col_reduce(_lib.ptr(X), X.stride(0), X.shape[0], X.shape[1], None, None, 0, _lib.ptr(out),
+                                        _lib.current_stream()))
