@@ -1041,34 +1041,13 @@ int b200_gather_dot(const float* U, int64_t ldu, const int64_t* users, const flo
  *                       about 1.8 M at top_k 20, 1.6 M at top_k 4096), a negative or non-finite alpha return -2 before a launch.
  *   b200_swing_plan     which accumulator the scores kernel uses for n_items (1: shared memory, 0: one global row
  *                       per resident CTA) and how many CTAs it keeps resident.
- *   b200_swing_recommend  the accumulation of swing.rs:187-240: row r (user users[r]) of scores [B, ld] gets, for
- *                       every (i, label) of row u of R and each of i's first min(top_k, nbr_count[i]) neighbours
- *                       (j, s), s * label added at j, unless filter_consumed and j is in the consumed CSR's row u
- *                       (always, not b200_mask_consumed's rule).  Items that got no term hold REMOVED, so
- *                       b200_topk_rows ranks them last; counts[r] is the number that got one (the candidates).  A user
- *                       outside [0, n_users) gets an all-REMOVED row and count 0.
- *   b200_swing_random_keys  random_rec (inference.rs:78-86): a row with more than n_rec candidates gets a uniform
- *                       key in [1, 2) at each candidate, Philox4x32-10 keyed by (seed, user, item); b200_topk_rows then
- *                       draws n_rec distinct candidates.
- *   b200_swing_predict  swing.rs:153-185 with compute_pred "ranking" (inference.rs:48-71): out[r] is the mean of
- *                       the scores of item i's first top_k neighbours that row u of R holds; default_pred for an
- *                       id outside range, an item without neighbours, an empty row or an empty intersection. */
+ *   Recommend and predict are b200_nbr_recommend (item-based), b200_nbr_random_keys and b200_nbr_predict (task 1,
+ *                       ranking: swing.rs:153-185) on the Swing neighbour table over R. */
 int b200_swing_scores_workspace_bytes(int64_t n_users, int64_t n_items, int32_t top_k, size_t* bytes);
 int b200_swing_scores(const int64_t* user_ptr, const int32_t* user_items, int64_t n_users, const int64_t* item_ptr,
                       const int32_t* item_users, int64_t n_items, float alpha, int32_t top_k, int32_t* nbr_ids,
                       float* nbr_scores, int64_t* nbr_count, void* workspace, size_t workspace_bytes, void* stream);
 int b200_swing_plan(int64_t n_items, int32_t top_k, int32_t* smem_acc, int32_t* ctas);
-int b200_swing_recommend(const int64_t* user_ptr, const int32_t* user_items, const float* user_labels,
-                         int64_t n_users, const int32_t* nbr_ids, const float* nbr_scores, const int64_t* nbr_count,
-                         int64_t n_items, int32_t top_k, const int64_t* consumed_ptr, const int32_t* consumed_idx,
-                         int32_t filter_consumed, const int64_t* users, int64_t B, float* scores, int64_t ld,
-                         int64_t* counts, void* stream);
-int b200_swing_random_keys(float* scores, int64_t ld, int64_t B, int64_t n_items, const int64_t* users,
-                           const int64_t* counts, int32_t n_rec, uint64_t seed, void* stream);
-int b200_swing_predict(const int64_t* user_ptr, const int32_t* user_items, int64_t n_users, const int32_t* nbr_ids,
-                       const float* nbr_scores, const int64_t* nbr_count, int64_t n_items, int32_t top_k,
-                       const int64_t* users, const int64_t* items, int64_t n, float default_pred, float* out,
-                       void* stream);
 
 /* ---- UserCF / ItemCF (libreco/bases/cf_base_rs.py; recfarm rust/src/similarities.rs, item_cf.rs, user_cf.rs,
  * inference.rs) ---------------------------------------------------------------------------------------------------
@@ -1088,32 +1067,48 @@ int b200_swing_predict(const int64_t* user_ptr, const int32_t* user_items, int64
  *                       memory (n_x above about 28.7 k at k_sim 20), and 12 n_x per split slot (64 slots).
  *   b200_cf_plan        which accumulator b200_cf_cosine uses for n_x (1: shared memory, 0: one global row per
  *                       resident CTA) and how many CTAs it keeps resident.
- *   ItemCF's recommend (item_cf.rs:156-209) is b200_swing_recommend on the ItemCF neighbour table (top_k = k_sim).
- *   b200_user_cf_recommend  user_cf.rs:151-205 with b200_swing_recommend's output contract: row r (user u = users[r])
- *                       of scores [B, ld] gets, for each of u's first min(k_sim, nbr_count[u]) neighbours (v, sim) and
- *                       each (i, label) of row v of R, sim * label added at i, unless filter_consumed and i is in the
- *                       consumed CSR's row u.  Untouched items hold REMOVED; counts[r] is the number of candidates.
- *   b200_cf_predict     item_cf.rs / user_cf.rs predict with compute_pred (inference.rs:48-71): the query's first
- *                       min(k_sim, nbr_count[q]) neighbours intersected with row r of the CSR (ptr, idx, labels); task
- *                       0 (rating) gives sum(label * sim / sum(sims)) per term (a zero sum of sims gives NaN or inf, as
- *                       in the reference), task 1 (ranking) sum(sims) / n.  ItemCF: rows = users over R, queries =
- *                       items; UserCF: rows = items over R^T, queries = users.  default_pred for an id outside range
- *                       or an empty intersection. */
+ *   Recommend and predict are b200_nbr_recommend (ItemCF item-based: item_cf.rs:156-209; UserCF
+ *                       user-based: user_cf.rs:151-205), b200_nbr_random_keys and b200_nbr_predict (the engine's
+ *                       task; ItemCF: rows = users over R, queries = items; UserCF: rows = items over R^T, queries =
+ *                       users) on the neighbour table, with top_k = k_sim. */
 int b200_cf_cosine_workspace_bytes(int64_t n_x, int32_t k_sim, size_t* bytes);
 int b200_cf_plan(int64_t n_x, int32_t k_sim, int32_t* smem_acc, int32_t* ctas);
 int b200_cf_cosine(const int64_t* sim_ptr, const int32_t* sim_idx, const float* sim_val, int64_t n_x,
                    const int64_t* mid_ptr, const int32_t* mid_idx, const float* mid_val, int64_t n_y,
                    int64_t min_common, int32_t k_sim, int32_t* nbr_ids, float* nbr_scores, int64_t* nbr_count,
                    void* workspace, size_t workspace_bytes, void* stream);
-int b200_user_cf_recommend(const int64_t* user_ptr, const int32_t* user_items, const float* user_labels,
-                           int64_t n_users, const int32_t* nbr_ids, const float* nbr_scores, const int64_t* nbr_count,
-                           int64_t n_items, int32_t k_sim, const int64_t* consumed_ptr, const int32_t* consumed_idx,
-                           int32_t filter_consumed, const int64_t* users, int64_t B, float* scores, int64_t ld,
-                           int64_t* counts, void* stream);
-int b200_cf_predict(const int64_t* ptr, const int32_t* idx, const float* labels, int64_t n_rows,
-                    const int32_t* nbr_ids, const float* nbr_scores, const int64_t* nbr_count, int64_t n_queries,
-                    int32_t k_sim, const int64_t* rows, const int64_t* queries, int64_t n, int32_t task,
-                    float default_pred, float* out, void* stream);
+
+/* ---- Neighbourhood serving (recfarm rust/src/swing.rs, item_cf.rs, user_cf.rs, inference.rs) ----------------------
+ * A neighbour table is nbr_ids int32 / nbr_scores float [n, top_k] and nbr_count int64 [n] (b200_swing_scores,
+ * b200_cf_cosine): row q's first min(top_k, nbr_count[q]) entries are its neighbours.
+ *   b200_nbr_recommend  row r (user u = users[r]) of scores [B, ld] gets, unless filter_consumed and the item is in
+ *                       the consumed CSR's row u (always, not b200_mask_consumed's rule):
+ *                       user_based 0 (Swing, ItemCF: the table is over items): for every (i, label) of row u of R and
+ *                       each of i's neighbours (j, s), s * label added at j;
+ *                       user_based 1 (UserCF: the table is over users): for each of u's neighbours (v, sim) and each
+ *                       (i, label) of row v of R, sim * label added at i.
+ *                       Items that got no term hold REMOVED, so b200_topk_rows ranks them last; counts[r] is the
+ *                       number that got one (the candidates).  A user outside [0, n_users) gets an all-REMOVED row
+ *                       and count 0.
+ *   b200_nbr_random_keys  random_rec (inference.rs:78-86): a row with more than n_rec candidates gets a uniform
+ *                       key in [1, 2) at each candidate, Philox4x32-10 keyed by (seed, user, item); b200_topk_rows
+ *                       then draws n_rec distinct candidates.
+ *   b200_nbr_predict    predict with compute_pred (inference.rs:48-71): query q's neighbours intersected with row r of
+ *                       the sorted CSR (ptr, idx, labels); task 0 (rating) gives sum(label * sim / sum(sims)) per
+ *                       term (a zero sum of sims gives NaN or inf, as in the reference), task 1 (ranking)
+ *                       sum(sims) / n and reads no labels (labels may be null).  default_pred for an id outside range or an empty
+ *                       intersection. */
+int b200_nbr_recommend(const int64_t* user_ptr, const int32_t* user_items, const float* user_labels, int64_t n_users,
+                       const int32_t* nbr_ids, const float* nbr_scores, const int64_t* nbr_count, int64_t n_items,
+                       int32_t top_k, int32_t user_based, const int64_t* consumed_ptr, const int32_t* consumed_idx,
+                       int32_t filter_consumed, const int64_t* users, int64_t B, float* scores, int64_t ld,
+                       int64_t* counts, void* stream);
+int b200_nbr_random_keys(float* scores, int64_t ld, int64_t B, int64_t n_items, const int64_t* users,
+                         const int64_t* counts, int32_t n_rec, uint64_t seed, void* stream);
+int b200_nbr_predict(const int64_t* ptr, const int32_t* idx, const float* labels, int64_t n_rows,
+                     const int32_t* nbr_ids, const float* nbr_scores, const int64_t* nbr_count, int64_t n_queries,
+                     int32_t top_k, const int64_t* rows, const int64_t* queries, int64_t n, int32_t task,
+                     float default_pred, float* out, void* stream);
 
 #ifdef __cplusplus
 }

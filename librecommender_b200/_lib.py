@@ -75,18 +75,15 @@ SIGNATURES = {
     "b200_swing_scores_workspace_bytes": (c_int, [c_int64, c_int64, c_int32, POINTER(c_size_t)]),
     "b200_swing_scores": (c_int, [_P, _P, c_int64, _P, _P, c_int64, c_float, c_int32, _P, _P, _P, _P, c_size_t, _P]),
     "b200_swing_plan": (c_int, [c_int64, c_int32, POINTER(c_int32), POINTER(c_int32)]),
-    "b200_swing_recommend": (c_int, [_P, _P, _P, c_int64, _P, _P, _P, c_int64, c_int32, _P, _P, c_int32, _P, c_int64,
-                                     _P, c_int64, _P, _P]),
-    "b200_swing_random_keys": (c_int, [_P, c_int64, c_int64, c_int64, _P, _P, c_int32, c_uint64, _P]),
-    "b200_swing_predict": (c_int, [_P, _P, c_int64, _P, _P, _P, c_int64, c_int32, _P, _P, c_int64, c_float, _P, _P]),
     "b200_cf_cosine_workspace_bytes": (c_int, [c_int64, c_int32, POINTER(c_size_t)]),
     "b200_cf_plan": (c_int, [c_int64, c_int32, POINTER(c_int32), POINTER(c_int32)]),
     "b200_cf_cosine": (c_int, [_P, _P, _P, c_int64, _P, _P, _P, c_int64, c_int64, c_int32, _P, _P, _P, _P, c_size_t,
                                _P]),
-    "b200_user_cf_recommend": (c_int, [_P, _P, _P, c_int64, _P, _P, _P, c_int64, c_int32, _P, _P, c_int32, _P,
-                                       c_int64, _P, c_int64, _P, _P]),
-    "b200_cf_predict": (c_int, [_P, _P, _P, c_int64, _P, _P, _P, c_int64, c_int32, _P, _P, c_int64, c_int32, c_float,
-                                _P, _P]),
+    "b200_nbr_recommend": (c_int, [_P, _P, _P, c_int64, _P, _P, _P, c_int64, c_int32, c_int32, _P, _P, c_int32, _P,
+                                   c_int64, _P, c_int64, _P, _P]),
+    "b200_nbr_random_keys": (c_int, [_P, c_int64, c_int64, c_int64, _P, _P, c_int32, c_uint64, _P]),
+    "b200_nbr_predict": (c_int, [_P, _P, _P, c_int64, _P, _P, _P, c_int64, c_int32, _P, _P, c_int64, c_int32, c_float,
+                                 _P, _P]),
     "b200_feat_forward_tune": (c_int, [c_int32]),
     "b200_feat_forward": (c_int, [_P, _P, _P, _P, c_int64, c_int64, c_int64, _P, c_int64, _P, c_int64, _P, _P, _P, c_float,
                                   _P, _P, _P, c_float, _P, _P, c_int64, _P]),

@@ -1,5 +1,5 @@
-// UserCF / ItemCF — recfarm's cosine similarities (rust/src/similarities.rs) and the neighbourhood recommend / predict
-// of rust/src/item_cf.rs, user_cf.rs and inference.rs, on the device.
+// UserCF / ItemCF — recfarm's cosine similarities (rust/src/similarities.rs) on the device.  The neighbourhood
+// recommend / predict of rust/src/item_cf.rs and user_cf.rs over the resulting table is neighbours.cu's.
 //
 // Similarities.  The "sim side" S is the n_x x n_y CSR whose rows are compared (item_interactions for ItemCF,
 // user_interactions for UserCF) and the "middle" M = S^T.  sq[x] = sum of r^2 over row x of S in fp32, in row order
@@ -23,7 +23,6 @@
 #include "neighbours.cuh"
 #include "../../include/b200reco.h"
 
-#include <algorithm>
 #include <vector>
 
 namespace b200 {
@@ -35,18 +34,6 @@ constexpr int kLongRow = 256;                 // a middle row longer than this i
 constexpr int64_t kMinPieceWork = 1 << 16;    // a target with more work than max(this, total / (8 CTAs)) is split
 
 struct Csr { const int64_t* ptr; const int32_t* idx; const float* val; };
-
-struct Plan {
-  bool smem_acc;
-  int ctas;
-  size_t smem;       // dynamic shared memory of the cosine kernel
-  int sort_cap;      // power of two >= k_sim
-};
-
-// shared memory: [sort keys u64 sort_cap][acc u64 n_x (smem path)]
-__host__ inline size_t smem_bytes(int64_t n_x, int sort_cap, bool smem_acc) {
-  return (size_t)sort_cap * 8 + (smem_acc ? (size_t)n_x * 8 : 0);
-}
 
 // *p += (c, v) on a packed (count << 32 | prod bits) entry with a plain fp32 add; true for the add that found 0
 __device__ __forceinline__ bool add_packed(unsigned long long* p, uint32_t c, float v) {
@@ -201,70 +188,15 @@ __global__ void __launch_bounds__(THREADS, 1) cf_split_finalize_kernel(
   if (threadIdx.x == 0) split_n[s] = 0;
 }
 
-// user_cf.rs:168-187: user u's first min(top_k, nbr_count[u]) neighbours v, each (i, label) of row v of R adds
-// sim * label at i; one warp per neighbour
-__global__ void __launch_bounds__(THREADS) user_cf_recommend_kernel(
-    const int64_t* __restrict__ user_ptr, const int32_t* __restrict__ user_items, const float* __restrict__ labels,
-    int64_t n_users, const int32_t* __restrict__ nbr_ids, const float* __restrict__ nbr_scores,
-    const int64_t* __restrict__ nbr_count, int64_t n_items, int top_k, const int64_t* __restrict__ cons_ptr,
-    const int32_t* __restrict__ cons_idx, int filter, const int64_t* __restrict__ users, float* __restrict__ scores,
-    int64_t ld, int64_t* __restrict__ counts) {
-  const int64_t r = blockIdx.x;
-  const int64_t u = users[r];
-  recommend_row(u, n_users, n_items, cons_ptr, cons_idx, filter, scores + r * ld, counts + r,
-                [&](uint32_t* row, unsigned long long* cand) {
-    const int kk = (int)min((int64_t)top_k, nbr_count[u]);
-    const int lane = threadIdx.x & 31;
-    for (int s = threadIdx.x >> 5; s < kk; s += WARPS) {
-      const int32_t v = nbr_ids[u * top_k + s];
-      const float sim = nbr_scores[u * top_k + s];
-      for (int64_t e = user_ptr[v] + lane; e < user_ptr[v + 1]; e += 32)
-        add_candidate(row, user_items[e], __fmul_rn(sim, labels[e]), cand);   // u_v_sim * v_i_score
-    }
-  });
-}
-
 // ---------------------------------------------------------------------------------------------------------------
+// shared memory: [sort keys u64 sort_cap][acc u64 n_x (shared path)]
 Plan make_plan(int64_t n_x, int k_sim) {
-  Plan p;
-  p.sort_cap = pow2_ceil(k_sim);
-  int dev = 0, optin = 0;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
-  const size_t reserve = 2048;     // the kernel's static shared memory
-  p.smem_acc = smem_bytes(n_x, p.sort_cap, true) + reserve <= (size_t)optin;
-  p.smem = smem_bytes(n_x, p.sort_cap, p.smem_acc);
-  p.ctas = 0;
-  if (cudaFuncSetAttribute(cf_cosine_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem) != cudaSuccess)
-    return p;
-  int per_sm = 0;
-  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, cf_cosine_kernel, THREADS, p.smem) != cudaSuccess)
-    return p;
-  if (!p.smem_acc) per_sm = std::min(per_sm, kMaxGlobalCtasPerSm);
-  p.ctas = per_sm * num_sms();
-  return p;
+  return nbr::make_plan(cf_cosine_kernel, n_x, k_sim, sizeof(unsigned long long), 0);
 }
 
-struct Layout {
-  size_t sq, work, counter, tasks, slot_item, tl, acc, split_rows, split_tl, split_n, total;
-};
-
-Layout layout(int64_t n_x, const Plan& p) {
-  Layout L;
-  size_t off = 0;
-  auto take = [&](size_t bytes) { const size_t at = off; off += (bytes + 255) & ~(size_t)255; return at; };
-  L.sq = take((size_t)n_x * 4);
-  L.work = take((size_t)n_x * 8);
-  L.counter = take(4);
-  L.tasks = take(((size_t)n_x + (size_t)kSlots * kMaxPieces) * sizeof(Task));
-  L.slot_item = take((size_t)kSlots * 4);
-  L.tl = take((size_t)p.ctas * n_x * 4);
-  L.acc = take(p.smem_acc ? 0 : (size_t)p.ctas * n_x * 8);
-  L.split_rows = take((size_t)kSlots * n_x * 8);
-  L.split_tl = take((size_t)kSlots * n_x * 4);
-  L.split_n = take((size_t)kSlots * 8);
-  L.total = off;
-  return L;
+// the workspace: sq and the per-target work, then the scheduler's pieces
+Workspace<unsigned long long> carve(unsigned char* ws, int64_t n_x, const Plan& p) {
+  return Workspace<unsigned long long>(ws, round256((size_t)n_x * 4) + round256((size_t)n_x * 8), n_x, p);
 }
 
 }  // namespace cf
@@ -279,7 +211,7 @@ extern "C" int b200_cf_cosine_workspace_bytes(int64_t n_x, int32_t k_sim, size_t
   B200_REQUIRE(k_sim >= 1 && k_sim <= kMaxTopK, "b200_cf_cosine: k_sim %d outside [1, %d]", k_sim, kMaxTopK);
   const Plan p = make_plan(n_x, k_sim);
   B200_REQUIRE(p.ctas > 0, "b200_cf_cosine: no resident CTA for %lld rows", (long long)n_x);
-  *bytes = layout(n_x, p).total;
+  *bytes = carve(nullptr, n_x, p).bytes;
   return 0;
 }
 
@@ -304,18 +236,10 @@ extern "C" int b200_cf_cosine(const int64_t* sim_ptr, const int32_t* sim_idx, co
   B200_REQUIRE(min_common >= 1, "b200_cf_cosine: min_common must be >= 1");
   cudaStream_t stream = (cudaStream_t)stream_;
   const Plan p = make_plan(n_x, k_sim);
-  const Layout L = layout(n_x, p);
   unsigned char* ws = static_cast<unsigned char*>(workspace);
-  float* sq = reinterpret_cast<float*>(ws + L.sq);
-  int64_t* work_d = reinterpret_cast<int64_t*>(ws + L.work);
-  unsigned* counter = reinterpret_cast<unsigned*>(ws + L.counter);
-  Task* tasks_d = reinterpret_cast<Task*>(ws + L.tasks);
-  int32_t* slot_item_d = reinterpret_cast<int32_t*>(ws + L.slot_item);
-  int32_t* tl = reinterpret_cast<int32_t*>(ws + L.tl);
-  unsigned long long* acc = p.smem_acc ? nullptr : reinterpret_cast<unsigned long long*>(ws + L.acc);
-  unsigned long long* split_rows = reinterpret_cast<unsigned long long*>(ws + L.split_rows);
-  int32_t* split_tl = reinterpret_cast<int32_t*>(ws + L.split_tl);
-  unsigned long long* split_n = reinterpret_cast<unsigned long long*>(ws + L.split_n);
+  const Workspace<unsigned long long> W = carve(ws, n_x, p);
+  float* sq = reinterpret_cast<float*>(ws);
+  int64_t* work_d = reinterpret_cast<int64_t*>(ws + round256((size_t)n_x * 4));
 
   B200_CUDA_OK(cudaMemsetAsync(nbr_ids, 0xff, (size_t)n_x * k_sim * 4, stream));
   B200_CUDA_OK(cudaMemsetAsync(nbr_scores, 0, (size_t)n_x * k_sim * 4, stream));
@@ -332,109 +256,25 @@ extern "C" int b200_cf_cosine(const int64_t* sim_ptr, const int32_t* sim_idx, co
   B200_CUDA_OK(cudaMemcpyAsync(work.data(), work_d, n_x * 8, cudaMemcpyDeviceToHost, stream));
   B200_CUDA_OK(cudaStreamSynchronize(stream));
   B200_REQUIRE(sptr[0] == 0, "b200_cf_cosine: sim_ptr[0] != 0");
-  int64_t total = 0;
   for (int64_t x = 0; x < n_x; ++x) {
     const int64_t d = sptr[x + 1] - sptr[x];
     B200_REQUIRE(d >= 0 && d <= n_y, "b200_cf_cosine: row %lld has a bad length", (long long)x);
-    total += work[x];
   }
-  if (total == 0) return 0;
-  const int64_t piece = std::max(kMinPieceWork, total / ((int64_t)p.ctas * 8));
-  std::vector<int32_t> whole, split;
-  for (int64_t x = 0; x < n_x; ++x) {
-    if (work[x] == 0) continue;
-    (work[x] > piece && sptr[x + 1] - sptr[x] > 1 ? split : whole).push_back((int32_t)x);
-  }
-  auto heavier = [&](int32_t a, int32_t b) { return work[a] != work[b] ? work[a] > work[b] : a < b; };
-  std::sort(whole.begin(), whole.end(), heavier);
-  std::sort(split.begin(), split.end(), heavier);
 
-  if (!p.smem_acc) B200_CUDA_OK(cudaMemsetAsync(acc, 0, (size_t)p.ctas * n_x * 8, stream));
-  B200_CUDA_OK(cudaMemsetAsync(split_rows, 0, (size_t)kSlots * n_x * 8, stream));
-  B200_CUDA_OK(cudaMemsetAsync(split_n, 0, (size_t)kSlots * 8, stream));
-
-  const int64_t rounds = std::max<int64_t>(1, ceil_div64((int64_t)split.size(), kSlots));
-  std::vector<Task> tasks;
-  std::vector<int32_t> slot_item;
-  for (int64_t r = 0; r < rounds; ++r) {
-    tasks.clear();
-    slot_item.clear();
-    for (int64_t k = r * kSlots; k < (int64_t)split.size() && k < (r + 1) * kSlots; ++k) {
-      const int32_t x = split[k];
-      const int64_t d = sptr[x + 1] - sptr[x];
-      const int64_t n_pieces = std::min<int64_t>({kMaxPieces, ceil_div64(work[x], piece), d});
-      const int32_t slot = (int32_t)slot_item.size();
-      slot_item.push_back(x);
-      for (int64_t q = 0; q < n_pieces; ++q)      // equal entry counts
-        tasks.push_back(Task{x, (int32_t)(d * q / n_pieces), (int32_t)(d * (q + 1) / n_pieces), slot});
-    }
-    for (size_t t = (size_t)r; t < whole.size(); t += (size_t)rounds)
-      tasks.push_back(Task{whole[t], 0, (int32_t)(sptr[whole[t] + 1] - sptr[whole[t]]), -1});
-    if (tasks.empty()) continue;
-    B200_CUDA_OK(cudaMemcpyAsync(tasks_d, tasks.data(), tasks.size() * sizeof(Task), cudaMemcpyHostToDevice, stream));
-    B200_CUDA_OK(cudaMemsetAsync(counter, 0, 4, stream));
+  auto cut = [](int32_t x, int64_t d, int64_t n_pieces, int32_t slot, std::vector<Task>& tasks) {
+    n_pieces = std::min(n_pieces, d);
+    for (int64_t q = 0; q < n_pieces; ++q)      // equal entry counts
+      tasks.push_back(Task{x, (int32_t)(d * q / n_pieces), (int32_t)(d * (q + 1) / n_pieces), slot});
+  };
+  auto scores = [&](int n_tasks) {
     cf_cosine_kernel<<<p.ctas, THREADS, p.smem, stream>>>(
-        s, m, sq, n_x, min_common, k_sim, p.sort_cap, p.smem_acc ? 1 : 0, tasks_d, (int)tasks.size(), counter, acc, tl,
-        split_rows, split_tl, split_n, nbr_ids, nbr_scores, nbr_count);
-    count_launch();
-    B200_CUDA_OK(cudaGetLastError());
-    if (!slot_item.empty()) {
-      B200_CUDA_OK(cudaMemcpyAsync(slot_item_d, slot_item.data(), slot_item.size() * 4, cudaMemcpyHostToDevice,
-                                   stream));
-      const size_t fsmem = (size_t)p.sort_cap * 8;
-      B200_CUDA_OK(cudaFuncSetAttribute(cf_split_finalize_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                        (int)fsmem));
-      cf_split_finalize_kernel<<<(unsigned)slot_item.size(), THREADS, fsmem, stream>>>(
-          slot_item_d, sq, min_common, k_sim, p.sort_cap, n_x, split_rows, split_tl, split_n, nbr_ids, nbr_scores,
-          nbr_count);
-      count_launch();
-      B200_CUDA_OK(cudaGetLastError());
-    }
-  }
-  // the host task vectors are released on return: wait for the last upload to have been read
-  B200_CUDA_OK(cudaStreamSynchronize(stream));
-  return 0;
-}
-
-extern "C" int b200_user_cf_recommend(const int64_t* user_ptr, const int32_t* user_items, const float* user_labels,
-                                      int64_t n_users, const int32_t* nbr_ids, const float* nbr_scores,
-                                      const int64_t* nbr_count, int64_t n_items, int32_t k_sim,
-                                      const int64_t* consumed_ptr, const int32_t* consumed_idx,
-                                      int32_t filter_consumed, const int64_t* users, int64_t B, float* scores,
-                                      int64_t ld, int64_t* counts, void* stream) {
-  B200_REQUIRE(user_ptr && user_items && user_labels && nbr_ids && nbr_scores && nbr_count && users && scores &&
-               counts, "b200_user_cf_recommend: null pointer");
-  B200_REQUIRE(!filter_consumed || consumed_ptr, "b200_user_cf_recommend: filtering needs the consumed CSR");
-  B200_REQUIRE(B >= 0 && B <= 0x7fffffff && n_items >= 1 && ld >= n_items && n_users >= 0,
-               "b200_user_cf_recommend: bad shape");
-  B200_REQUIRE(k_sim >= 1 && k_sim <= kMaxTopK, "b200_user_cf_recommend: bad k_sim");
-  if (B == 0) return 0;
-  user_cf_recommend_kernel<<<(unsigned)B, THREADS, 0, (cudaStream_t)stream>>>(
-      user_ptr, user_items, user_labels, n_users, nbr_ids, nbr_scores, nbr_count, n_items, k_sim, consumed_ptr,
-      consumed_idx, filter_consumed, users, scores, ld, counts);
-  count_launch();
-  return check_cuda(cudaGetLastError(), "user_cf_recommend_kernel");
-}
-
-extern "C" int b200_cf_predict(const int64_t* ptr, const int32_t* idx, const float* labels, int64_t n_rows,
-                               const int32_t* nbr_ids, const float* nbr_scores, const int64_t* nbr_count,
-                               int64_t n_queries, int32_t k_sim, const int64_t* rows, const int64_t* queries,
-                               int64_t n, int32_t task, float default_pred, float* out, void* stream) {
-  B200_REQUIRE(ptr && labels && nbr_ids && nbr_scores && nbr_count && rows && queries && out,
-               "b200_cf_predict: null pointer");
-  B200_REQUIRE(n >= 0 && n_queries >= 1 && n_rows >= 0 && k_sim >= 1 && k_sim <= kMaxTopK,
-               "b200_cf_predict: bad shape");
-  B200_REQUIRE(task == 0 || task == 1, "b200_cf_predict: task %d is neither 0 (rating) nor 1 (ranking)", task);
-  if (n == 0) return 0;
-  const unsigned grid = (unsigned)ceil_div64(n, WARPS);
-  if (task == 0)
-    neighbour_predict_kernel<true><<<grid, THREADS, 0, (cudaStream_t)stream>>>(
-        ptr, idx, labels, n_rows, nbr_ids, nbr_scores, nbr_count, n_queries, k_sim, rows, queries, n, default_pred,
-        out);
-  else
-    neighbour_predict_kernel<false><<<grid, THREADS, 0, (cudaStream_t)stream>>>(
-        ptr, idx, labels, n_rows, nbr_ids, nbr_scores, nbr_count, n_queries, k_sim, rows, queries, n, default_pred,
-        out);
-  count_launch();
-  return check_cuda(cudaGetLastError(), "neighbour_predict_kernel");
+        s, m, sq, n_x, min_common, k_sim, p.sort_cap, p.smem_acc ? 1 : 0, W.tasks, n_tasks, W.counter, W.acc, W.tl,
+        W.split_rows, W.split_tl, W.split_n, nbr_ids, nbr_scores, nbr_count);
+  };
+  auto finalize = [&](unsigned n_slots) {
+    cf_split_finalize_kernel<<<n_slots, THREADS, (size_t)p.sort_cap * 8, stream>>>(
+        W.slot_item, sq, min_common, k_sim, p.sort_cap, n_x, W.split_rows, W.split_tl, W.split_n, nbr_ids,
+        nbr_scores, nbr_count);
+  };
+  return run_rounds(sptr, work, kMinPieceWork, p, W, stream, cut, scores, finalize);
 }

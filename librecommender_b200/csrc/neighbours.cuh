@@ -1,6 +1,7 @@
-// Device code shared by the neighbourhood engines (swing.cu, cf.cu): per-target accumulator rows with a first-touch
-// list, heavy targets split over CTAs into global split rows, the exact radix select of a row's top k, and the
-// serving pieces (candidate accumulation of recommend, predict over a neighbour table).
+// What the scoring of the neighbourhood engines (swing.cu, cf.cu) shares: per-target accumulator rows with a
+// first-touch list, heavy targets split over CTAs into global split rows, the exact radix select of a row's top k, and
+// on the host the plan, the workspace and the rounds of tasks that drive a scores kernel.  Serving a neighbour table
+// (recommend, predict) is neighbours.cu.
 //
 // Accumulator rows.  A persistent CTA owns one row of n_targets entries, in shared memory when it fits and otherwise
 // one global row per resident CTA.  The add that finds an entry untouched appends its id to the CTA's touched list,
@@ -9,6 +10,9 @@
 // target's split slot, with its own touched list, and a finalize kernel selects from that row.
 #pragma once
 #include "common.cuh"
+
+#include <algorithm>
+#include <vector>
 
 namespace b200 {
 namespace nbr {
@@ -19,7 +23,6 @@ constexpr int kMaxTopK = 4096;
 constexpr int kSlots = 64;                    // split targets in flight per round
 constexpr int kMaxPieces = 1024;              // pieces per split target
 constexpr int kMaxGlobalCtasPerSm = 4;        // global accumulator rows: bound their number
-constexpr uint32_t kFiltered = 0xfffffffeu;   // recommend: a consumed item while filtering (restored to REMOVED)
 
 // target row `item`, its entry / outer position range [pb, pe), and its split slot (-1: the whole target)
 struct Task { int32_t item, pb, pe, slot; };
@@ -115,113 +118,134 @@ __device__ void select_topk(ValueOf value_of, const int32_t* tl, int64_t T, int 
   __syncthreads();
 }
 
-// recommend: row[j] += v in a dense score row whose untouched entries hold kRemovedBits and whose filtered entries
-// hold kFiltered.  The add that finds kRemovedBits stores v itself and counts one more candidate in *cand.
-__device__ __forceinline__ void add_candidate(uint32_t* row, int32_t j, float v, unsigned long long* cand) {
-  uint32_t old = row[j];
-  for (;;) {
-    if (old == kFiltered) return;
-    const float nv = old == kRemovedBits ? v : __fadd_rn(__uint_as_float(old), v);
-    const uint32_t prev = atomicCAS(&row[j], old, __float_as_uint(nv));
-    if (prev == old) {
-      if (old == kRemovedBits) atomicAdd(cand, 1ull);
-      return;
-    }
-    old = prev;
-  }
+// ---- host: the plan, the workspace and the rounds of a scores kernel ------------------------------------------------
+
+struct Plan {
+  bool smem_acc;     // the accumulator rows are in shared memory, else one global row per resident CTA
+  int ctas;          // resident CTAs of the scores kernel; 0 when its shared memory cannot fit
+  size_t smem;       // its dynamic shared memory
+  int sort_cap;      // power of two >= top_k
+};
+
+// The plan of `kernel` over rows of n accumulator entries of entry_bytes each.  Dynamic shared memory:
+// [sort keys u64 sort_cap][extra_smem bytes of the engine's][acc entry_bytes * n (shared path)].
+template <typename Kernel>
+Plan make_plan(Kernel kernel, int64_t n, int top_k, size_t entry_bytes, size_t extra_smem) {
+  Plan p;
+  p.sort_cap = pow2_ceil(top_k);
+  int dev = 0, optin = 0;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
+  const size_t reserve = 2048;     // the kernel's static shared memory
+  const size_t base = (size_t)p.sort_cap * 8 + extra_smem, acc = (size_t)n * entry_bytes;
+  p.smem_acc = base + acc + reserve <= (size_t)optin;
+  p.smem = base + (p.smem_acc ? acc : 0);
+  p.ctas = 0;
+  if (p.smem + reserve > (size_t)optin) return p;     // extra_smem alone does not fit (Swing's bitmap)
+  if (cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem) != cudaSuccess) return p;
+  int per_sm = 0;
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, THREADS, p.smem) != cudaSuccess) return p;
+  if (!p.smem_acc) per_sm = std::min(per_sm, kMaxGlobalCtasPerSm);
+  p.ctas = per_sm * num_sms();
+  return p;
 }
 
-// recommend: fill row r (user u) of scores [B, ld] with kRemovedBits, mark u's consumed items kFiltered when
-// filtering, let `accumulate(row, &cand)` add the user's terms through add_candidate, restore the filtered entries
-// to kRemovedBits and write the number of candidates (entries that got a term) to *count.  A user outside
-// [0, n_users) gets an all-REMOVED row and count 0.  Every thread of the CTA calls it.
-template <typename Accumulate>
-__device__ void recommend_row(int64_t u, int64_t n_users, int64_t n_items, const int64_t* cons_ptr,
-                              const int32_t* cons_idx, int filter, float* scores_row, int64_t* count,
-                              Accumulate accumulate) {
-  __shared__ unsigned long long s_cand;
-  uint32_t* row = reinterpret_cast<uint32_t*>(scores_row);
-  for (int64_t n = threadIdx.x; n < n_items; n += blockDim.x) row[n] = kRemovedBits;
-  if (threadIdx.x == 0) s_cand = 0;
-  const bool known = u >= 0 && u < n_users;
-  const bool filt = known && filter && cons_ptr != nullptr;
-  __syncthreads();
-  if (filt) {
-    for (int64_t e = cons_ptr[u] + threadIdx.x; e < cons_ptr[u + 1]; e += blockDim.x) {
-      const int32_t c = cons_idx[e];
-      if (c >= 0 && c < n_items) row[c] = kFiltered;
-    }
-    __syncthreads();
-  }
-  if (known) accumulate(row, &s_cand);
-  __syncthreads();
-  if (filt) {
-    for (int64_t e = cons_ptr[u] + threadIdx.x; e < cons_ptr[u + 1]; e += blockDim.x) {
-      const int32_t c = cons_idx[e];
-      if (c >= 0 && c < n_items) row[c] = kRemovedBits;
-    }
-  }
-  if (threadIdx.x == 0) *count = (int64_t)s_cand;
-}
+inline size_t round256(size_t bytes) { return (bytes + 255) & ~(size_t)255; }
 
-// One warp per (row r, query q): the first min(top_k, nbr_count[q]) neighbours of q, intersected with row r of a
-// sorted CSR (ptr / idx, and labels for kRating), recfarm's compute_pred (inference.rs:48-71):
-//   ranking: sum of the intersected neighbours' scores / their number;
-//   rating:  sum over them of label * sim / (sum of their sims), each term as written (a zero sum gives NaN or inf).
-// default_pred for an id outside range or an empty intersection.
-template <bool kRating>
-__global__ void __launch_bounds__(THREADS) neighbour_predict_kernel(
-    const int64_t* __restrict__ ptr, const int32_t* __restrict__ idx, const float* __restrict__ labels,
-    int64_t n_rows, const int32_t* __restrict__ nbr_ids, const float* __restrict__ nbr_scores,
-    const int64_t* __restrict__ nbr_count, int64_t n_queries, int top_k, const int64_t* __restrict__ rows,
-    const int64_t* __restrict__ queries, int64_t n, float default_pred, float* __restrict__ out) {
-  const int64_t r = ((int64_t)blockIdx.x * THREADS + threadIdx.x) >> 5;
-  const int lane = threadIdx.x & 31;
-  if (r >= n) return;
-  const int64_t u = rows[r], i = queries[r];
-  if (u < 0 || u >= n_rows || i < 0 || i >= n_queries) {
-    if (lane == 0) out[r] = default_pred;
-    return;
+// A scores call's workspace: the engine's own arrays (`prefix` bytes at its start), then the scheduler's pieces, each
+// rounded to 256 B on its own.  Entry is the accumulator entry.  With ws == nullptr only `bytes` is meaningful.
+template <typename Entry>
+struct Workspace {
+  unsigned* counter;                  // the task counter of a round
+  Task* tasks;                        // a round's tasks
+  int32_t* slot_item;                 // the target of each split slot in use
+  int32_t* tl;                        // one touched list of n per resident CTA
+  Entry* acc;                         // one accumulator row of n per resident CTA; nullptr on the shared path
+  Entry* split_rows;                  // per split slot: a row of n, its touched list and its touched count
+  int32_t* split_tl;
+  unsigned long long* split_n;
+  size_t bytes;                       // the whole workspace, prefix included
+
+  Workspace(unsigned char* ws, size_t prefix, int64_t n, const Plan& p) {
+    size_t off = prefix;
+    auto take = [&](size_t b) {
+      const size_t at = off;
+      off += round256(b);
+      return ws ? static_cast<void*>(ws + at) : nullptr;
+    };
+    counter = static_cast<unsigned*>(take(4));
+    tasks = static_cast<Task*>(take(((size_t)n + (size_t)kSlots * kMaxPieces) * sizeof(Task)));
+    slot_item = static_cast<int32_t*>(take((size_t)kSlots * 4));
+    tl = static_cast<int32_t*>(take((size_t)p.ctas * n * 4));
+    acc = static_cast<Entry*>(take(p.smem_acc ? 0 : (size_t)p.ctas * n * sizeof(Entry)));
+    if (p.smem_acc) acc = nullptr;
+    split_rows = static_cast<Entry*>(take((size_t)kSlots * n * sizeof(Entry)));
+    split_tl = static_cast<int32_t*>(take((size_t)kSlots * n * 4));
+    split_n = static_cast<unsigned long long*>(take((size_t)kSlots * 8));
+    bytes = off;
   }
-  const int kk = (int)min((int64_t)top_k, nbr_count[i]);
-  const int64_t a0 = ptr[u], a1 = ptr[u + 1];
-  float sum = 0.f;
-  int hits = 0;
-  for (int s = lane; s < kk && a1 > a0; s += 32) {
-    const int32_t j = nbr_ids[i * top_k + s];
-    int64_t lo = a0, hi = a1;          // row u is sorted: lower bound of j
-    while (lo < hi) {
-      const int64_t mid = (lo + hi) >> 1;
-      if (idx[mid] < j) lo = mid + 1; else hi = mid;
+};
+
+// Runs the scores kernel over the n targets with weight[x] > 0 (row x of the host row pointers ptr holds
+// ptr[x + 1] - ptr[x] entries), heaviest first, ties to the smaller id.  A target of more than one entry whose
+// weight exceeds the piece size max(min_piece, total weight / (8 resident CTAs)) is split:
+// cut(x, entries, n_pieces, slot, tasks) appends its pieces, n_pieces = min(kMaxPieces, ceil(weight / piece)).
+// Each round gives up to kSlots split targets a slot, split targets first, then takes an even, strided share of the
+// whole targets; a round without tasks is skipped.  scores(n_tasks) launches the scores kernel on the round's
+// uploaded tasks, finalize(n_slots) the split finalize kernel over its slots.  Synchronises `stream` once at the end.
+template <typename Entry, typename Cut, typename Scores, typename Finalize>
+int run_rounds(const std::vector<int64_t>& ptr, const std::vector<int64_t>& weight, int64_t min_piece,
+               const Plan& p, const Workspace<Entry>& w, cudaStream_t stream, Cut cut, Scores scores,
+               Finalize finalize) {
+  const int64_t n = (int64_t)weight.size();
+  int64_t total = 0;
+  for (int64_t x = 0; x < n; ++x) total += weight[x];
+  if (total == 0) return 0;
+  const int64_t piece = std::max(min_piece, total / ((int64_t)p.ctas * 8));
+  std::vector<int32_t> whole, split;
+  for (int64_t x = 0; x < n; ++x) {
+    if (weight[x] == 0) continue;
+    (weight[x] > piece && ptr[x + 1] - ptr[x] > 1 ? split : whole).push_back((int32_t)x);
+  }
+  auto heavier = [&](int32_t a, int32_t b) { return weight[a] != weight[b] ? weight[a] > weight[b] : a < b; };
+  std::sort(whole.begin(), whole.end(), heavier);
+  std::sort(split.begin(), split.end(), heavier);
+
+  if (!p.smem_acc) B200_CUDA_OK(cudaMemsetAsync(w.acc, 0, (size_t)p.ctas * n * sizeof(Entry), stream));
+  B200_CUDA_OK(cudaMemsetAsync(w.split_rows, 0, (size_t)kSlots * n * sizeof(Entry), stream));
+  B200_CUDA_OK(cudaMemsetAsync(w.split_n, 0, (size_t)kSlots * 8, stream));
+
+  const int64_t rounds = std::max<int64_t>(1, ceil_div64((int64_t)split.size(), kSlots));
+  std::vector<Task> tasks;
+  std::vector<int32_t> slot_item;
+  for (int64_t r = 0; r < rounds; ++r) {
+    tasks.clear();
+    slot_item.clear();
+    for (int64_t s = r * kSlots; s < (int64_t)split.size() && s < (r + 1) * kSlots; ++s) {
+      const int32_t x = split[s];
+      cut(x, ptr[x + 1] - ptr[x], std::min<int64_t>(kMaxPieces, ceil_div64(weight[x], piece)),
+          (int32_t)slot_item.size(), tasks);
+      slot_item.push_back(x);
     }
-    if (lo < a1 && idx[lo] == j) {
-      sum += nbr_scores[i * top_k + s];
-      ++hits;
+    for (size_t t = (size_t)r; t < whole.size(); t += (size_t)rounds)
+      tasks.push_back(Task{whole[t], 0, (int32_t)(ptr[whole[t] + 1] - ptr[whole[t]]), -1});
+    if (tasks.empty()) continue;
+    B200_CUDA_OK(cudaMemcpyAsync(w.tasks, tasks.data(), tasks.size() * sizeof(Task), cudaMemcpyHostToDevice, stream));
+    B200_CUDA_OK(cudaMemsetAsync(w.counter, 0, 4, stream));
+    scores((int)tasks.size());
+    count_launch();
+    B200_CUDA_OK(cudaGetLastError());
+    if (!slot_item.empty()) {
+      B200_CUDA_OK(cudaMemcpyAsync(w.slot_item, slot_item.data(), slot_item.size() * 4, cudaMemcpyHostToDevice,
+                                   stream));
+      finalize((unsigned)slot_item.size());
+      count_launch();
+      B200_CUDA_OK(cudaGetLastError());
     }
   }
-  sum = warp_sum(sum);
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) hits += __shfl_xor_sync(0xffffffffu, hits, o);
-  if (!kRating) {
-    if (lane == 0) out[r] = hits ? __fdiv_rn(sum, (float)hits) : default_pred;
-    return;
-  }
-  if (!hits) {
-    if (lane == 0) out[r] = default_pred;
-    return;
-  }
-  float acc = 0.f;                   // rating: a second pass over the hits, once their sum of sims is known
-  for (int s = lane; s < kk; s += 32) {
-    const int32_t j = nbr_ids[i * top_k + s];
-    int64_t lo = a0, hi = a1;
-    while (lo < hi) {
-      const int64_t mid = (lo + hi) >> 1;
-      if (idx[mid] < j) lo = mid + 1; else hi = mid;
-    }
-    if (lo < a1 && idx[lo] == j) acc += __fdiv_rn(__fmul_rn(labels[lo], nbr_scores[i * top_k + s]), sum);
-  }
-  acc = warp_sum(acc);
-  if (lane == 0) out[r] = acc;
+  // the host task vectors are released on return: wait for the last upload to have been read
+  B200_CUDA_OK(cudaStreamSynchronize(stream));
+  return 0;
 }
 
 }  // namespace nbr

@@ -1,5 +1,5 @@
-// Swing — the item-item swing scores of recfarm (rust/src/graph.rs:147-234) and the neighbourhood recommend /
-// predict of rust/src/swing.rs:153-240 and rust/src/inference.rs:11-96, on the device.
+// Swing — the item-item swing scores of recfarm (rust/src/graph.rs:147-234) on the device.  The neighbourhood
+// recommend / predict of rust/src/swing.rs:153-240 over the resulting table is neighbours.cu's.
 //
 // Scores.  R is the user x item interaction CSR (rows sorted, duplicate-free), R^T its item x user CSR.
 // w_u = 1 / sqrt(|I_u|) in fp32 (IEEE sqrt, correctly rounded reciprocal).  For a target item i and every pair of its
@@ -25,10 +25,8 @@
 // neighbours.cuh's exact radix select on (score bits << 32 | ~id) (scores are positive, so their bits order as floats).
 #include "common.cuh"
 #include "neighbours.cuh"
-#include "philox.cuh"
 #include "../../include/b200reco.h"
 
-#include <algorithm>
 #include <vector>
 
 namespace b200 {
@@ -42,20 +40,6 @@ struct Graph {
   const int64_t* user_ptr; const int32_t* user_items;
   const int64_t* item_ptr; const int32_t* item_users;
 };
-
-struct Plan {
-  bool smem_acc;
-  int ctas;
-  size_t smem;       // dynamic shared memory of the scores kernel
-  int sort_cap;      // power of two >= top_k
-  int64_t bm_words;
-};
-
-// shared memory: [sort keys u64 sort_cap][bitmap u32 bm_words][acc f32 n_items (smem path)]
-__host__ inline size_t smem_bytes(int64_t n_items, int sort_cap, bool smem_acc) {
-  const int64_t bm_words = (n_items + 31) / 32;
-  return (size_t)sort_cap * 8 + (size_t)bm_words * 4 + (smem_acc ? (size_t)n_items * 4 : 0);
-}
 
 __device__ __forceinline__ float pair_term(float wu, float wv, float alpha, int cnt) {
   // graph.rs:185-186: user_weights[u] * user_weights[v] * (alpha + k).recip(), k = |C| - 1, all fp32
@@ -184,90 +168,15 @@ __global__ void __launch_bounds__(THREADS) swing_split_finalize_kernel(
   if (threadIdx.x == 0) split_n[s] = 0;
 }
 
-__global__ void __launch_bounds__(THREADS) swing_recommend_kernel(
-    const int64_t* __restrict__ user_ptr, const int32_t* __restrict__ user_items, const float* __restrict__ labels,
-    int64_t n_users, const int32_t* __restrict__ nbr_ids, const float* __restrict__ nbr_scores,
-    const int64_t* __restrict__ nbr_count, int64_t n_items, int top_k, const int64_t* __restrict__ cons_ptr,
-    const int32_t* __restrict__ cons_idx, int filter, const int64_t* __restrict__ users, float* __restrict__ scores,
-    int64_t ld, int64_t* __restrict__ counts) {
-  const int64_t r = blockIdx.x;
-  const int64_t u = users[r];
-  recommend_row(u, n_users, n_items, cons_ptr, cons_idx, filter, scores + r * ld, counts + r,
-                [&](uint32_t* row, unsigned long long* cand) {
-    const int64_t a0 = user_ptr[u], len = user_ptr[u + 1] - a0;
-    for (int64_t t = threadIdx.x; t < len * top_k; t += THREADS) {
-      const int64_t e = a0 + t / top_k;
-      const int s = (int)(t % top_k);
-      const int32_t i = user_items[e];
-      if (s >= nbr_count[i]) continue;
-      const int32_t j = nbr_ids[(int64_t)i * top_k + s];
-      // swing.rs:213-218: item_scores[j] += i_j_swing_score * i_label
-      add_candidate(row, j, __fmul_rn(nbr_scores[(int64_t)i * top_k + s], labels[e]), cand);
-    }
-  });
-}
-
-// random_rec: a row with more than n_rec candidates gets a uniform key in [1, 2) per candidate, keyed by
-// (seed, user, item), so its top n_rec by key is a uniform draw of n_rec distinct candidates
-__global__ void __launch_bounds__(THREADS) swing_random_keys_kernel(float* __restrict__ scores, int64_t ld,
-                                                                    int64_t n_items, const int64_t* __restrict__ users,
-                                                                    const int64_t* __restrict__ counts, int n_rec,
-                                                                    uint32_t k0, uint32_t k1) {
-  const int64_t r = blockIdx.x;
-  if (counts[r] <= n_rec) return;
-  uint32_t* row = reinterpret_cast<uint32_t*>(scores + r * ld);
-  const uint64_t u = (uint64_t)users[r];
-  for (int64_t n = threadIdx.x; n < n_items; n += THREADS) {
-    if (row[n] == kRemovedBits) continue;
-    U4 c;
-    c.x = (uint32_t)n; c.y = (uint32_t)u; c.z = (uint32_t)(u >> 32); c.w = 0x53574e47u;
-    row[n] = 0x3f800000u | (philox4x32_10(c, k0, k1).x >> 9);
-  }
-}
-
 // ---------------------------------------------------------------------------------------------------------------
+// shared memory: [sort keys u64 sort_cap][bitmap u32 (n_items + 31) / 32][acc f32 n_items (shared path)]
 Plan make_plan(int64_t n_items, int top_k) {
-  Plan p;
-  p.sort_cap = pow2_ceil(top_k);
-  p.bm_words = (n_items + 31) / 32;
-  int dev = 0, optin = 0;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
-  const size_t reserve = 2048;     // the kernel's static shared memory
-  p.smem_acc = smem_bytes(n_items, p.sort_cap, true) + reserve <= (size_t)optin;
-  p.smem = smem_bytes(n_items, p.sort_cap, p.smem_acc);
-  p.ctas = 0;
-  if (p.smem + reserve > (size_t)optin) return p;
-  if (cudaFuncSetAttribute(swing_scores_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem) !=
-      cudaSuccess)
-    return p;
-  int per_sm = 0;
-  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, swing_scores_kernel, THREADS, p.smem) != cudaSuccess)
-    return p;
-  if (!p.smem_acc) per_sm = std::min(per_sm, kMaxGlobalCtasPerSm);
-  p.ctas = per_sm * num_sms();
-  return p;
+  return nbr::make_plan(swing_scores_kernel, n_items, top_k, sizeof(float), (size_t)(n_items + 31) / 32 * 4);
 }
 
-struct Layout {
-  size_t w, counter, tasks, slot_item, tl, acc, split_rows, split_tl, split_n, total;
-};
-
-Layout layout(int64_t n_users, int64_t n_items, const Plan& p) {
-  Layout L;
-  size_t off = 0;
-  auto take = [&](size_t bytes) { const size_t at = off; off += (bytes + 255) & ~(size_t)255; return at; };
-  L.w = take((size_t)n_users * 4);
-  L.counter = take(4);
-  L.tasks = take(((size_t)n_items + (size_t)kSlots * kMaxPieces) * sizeof(Task));
-  L.slot_item = take((size_t)kSlots * 4);
-  L.tl = take((size_t)p.ctas * n_items * 4);
-  L.acc = take(p.smem_acc ? 0 : (size_t)p.ctas * n_items * 4);
-  L.split_rows = take((size_t)kSlots * n_items * 4);
-  L.split_tl = take((size_t)kSlots * n_items * 4);
-  L.split_n = take((size_t)kSlots * 8);
-  L.total = off;
-  return L;
+// the workspace: the user weights, then the scheduler's pieces
+Workspace<float> carve(unsigned char* ws, int64_t n_users, int64_t n_items, const Plan& p) {
+  return Workspace<float>(ws, round256((size_t)n_users * 4), n_items, p);
 }
 
 }  // namespace swing
@@ -284,7 +193,7 @@ extern "C" int b200_swing_scores_workspace_bytes(int64_t n_users, int64_t n_item
   const Plan p = make_plan(n_items, top_k);
   B200_REQUIRE(p.ctas > 0, "b200_swing_scores: a %lld-item bitmap does not fit in shared memory",
                (long long)n_items);
-  *bytes = layout(n_users, n_items, p).total;
+  *bytes = carve(nullptr, n_users, n_items, p).bytes;
   return 0;
 }
 
@@ -300,17 +209,9 @@ extern "C" int b200_swing_scores(const int64_t* user_ptr, const int32_t* user_it
   B200_REQUIRE(alpha >= 0.f && alpha <= 3.4028235e38f, "b200_swing_scores: alpha must be finite and >= 0");
   cudaStream_t stream = (cudaStream_t)stream_;
   const Plan p = make_plan(n_items, top_k);
-  const Layout L = layout(n_users, n_items, p);
   unsigned char* ws = static_cast<unsigned char*>(workspace);
-  float* w = reinterpret_cast<float*>(ws + L.w);
-  unsigned* counter = reinterpret_cast<unsigned*>(ws + L.counter);
-  Task* tasks_d = reinterpret_cast<Task*>(ws + L.tasks);
-  int32_t* slot_item_d = reinterpret_cast<int32_t*>(ws + L.slot_item);
-  int32_t* tl = reinterpret_cast<int32_t*>(ws + L.tl);
-  float* acc = p.smem_acc ? nullptr : reinterpret_cast<float*>(ws + L.acc);
-  float* split_rows = reinterpret_cast<float*>(ws + L.split_rows);
-  int32_t* split_tl = reinterpret_cast<int32_t*>(ws + L.split_tl);
-  unsigned long long* split_n = reinterpret_cast<unsigned long long*>(ws + L.split_n);
+  const Workspace<float> W = carve(ws, n_users, n_items, p);
+  float* w = reinterpret_cast<float*>(ws);
 
   B200_CUDA_OK(cudaMemsetAsync(nbr_ids, 0xff, (size_t)n_items * top_k * 4, stream));
   B200_CUDA_OK(cudaMemsetAsync(nbr_scores, 0, (size_t)n_items * top_k * 4, stream));
@@ -322,81 +223,44 @@ extern "C" int b200_swing_scores(const int64_t* user_ptr, const int32_t* user_it
   B200_CUDA_OK(cudaStreamSynchronize(stream));
   B200_REQUIRE(iptr[0] == 0, "b200_swing_scores: item_ptr[0] != 0");
   std::vector<int64_t> pairs(n_items);
-  int64_t total = 0;
+  bool any_pair = false;
   for (int64_t i = 0; i < n_items; ++i) {
     const int64_t d = iptr[i + 1] - iptr[i];
     B200_REQUIRE(d >= 0 && d <= n_users, "b200_swing_scores: item %lld has a bad degree", (long long)i);
     pairs[i] = d * (d - 1) / 2;
-    total += pairs[i];
+    any_pair |= pairs[i] > 0;
   }
-  if (total == 0) return 0;
-  const int64_t piece = std::max(kMinPiecePairs, total / ((int64_t)p.ctas * 8));
-  std::vector<int32_t> whole, split;
-  for (int64_t i = 0; i < n_items; ++i) {
-    if (pairs[i] == 0) continue;
-    (pairs[i] > piece ? split : whole).push_back((int32_t)i);
-  }
-  auto heavier = [&](int32_t a, int32_t b) { return pairs[a] != pairs[b] ? pairs[a] > pairs[b] : a < b; };
-  std::sort(whole.begin(), whole.end(), heavier);
-  std::sort(split.begin(), split.end(), heavier);
+  if (!any_pair) return 0;
 
   B200_REQUIRE(n_users > 0, "b200_swing_scores: no users");
   user_weights_kernel<<<(unsigned)ceil_div64(n_users, 256), 256, 0, stream>>>(user_ptr, n_users, w);
   count_launch();
   B200_CUDA_OK(cudaGetLastError());
-  if (!p.smem_acc) B200_CUDA_OK(cudaMemsetAsync(acc, 0, (size_t)p.ctas * n_items * 4, stream));
-  B200_CUDA_OK(cudaMemsetAsync(split_rows, 0, (size_t)kSlots * n_items * 4, stream));
-  B200_CUDA_OK(cudaMemsetAsync(split_n, 0, (size_t)kSlots * 8, stream));
 
   const Graph g{user_ptr, user_items, item_ptr, item_users};
-  const int64_t rounds = std::max<int64_t>(1, ceil_div64((int64_t)split.size(), kSlots));
-  std::vector<Task> tasks;
-  std::vector<int32_t> slot_item;
-  for (int64_t r = 0; r < rounds; ++r) {
-    tasks.clear();
-    slot_item.clear();
-    for (int64_t s = r * kSlots; s < (int64_t)split.size() && s < (r + 1) * kSlots; ++s) {
-      const int32_t i = split[s];
-      const int d = (int)(iptr[i + 1] - iptr[i]);
-      const int64_t n_pieces = std::min<int64_t>(kMaxPieces, ceil_div64(pairs[i], piece));
-      const int32_t slot = (int32_t)slot_item.size();
-      slot_item.push_back(i);
-      // contiguous outer ranges of about pairs / n_pieces pairs each (position p pairs with d - 1 - p users)
-      int64_t acc_pairs = 0, k = 1;
-      int pb = 0;
-      for (int q = 0; q < d - 1; ++q) {
-        acc_pairs += d - 1 - q;
-        if (acc_pairs * n_pieces >= k * pairs[i] || q == d - 2) {
-          tasks.push_back(Task{i, pb, q + 1, slot});
-          pb = q + 1;
-          ++k;
-        }
+  // contiguous outer ranges of about pairs / n_pieces pairs each (position q pairs with d - 1 - q users)
+  auto cut = [&](int32_t i, int64_t d, int64_t n_pieces, int32_t slot, std::vector<Task>& tasks) {
+    int64_t acc_pairs = 0, k = 1;
+    int pb = 0;
+    for (int q = 0; q < d - 1; ++q) {
+      acc_pairs += d - 1 - q;
+      if (acc_pairs * n_pieces >= k * pairs[i] || q == d - 2) {
+        tasks.push_back(Task{i, pb, q + 1, slot});
+        pb = q + 1;
+        ++k;
       }
     }
-    for (size_t t = (size_t)r; t < whole.size(); t += (size_t)rounds) tasks.push_back(Task{whole[t], 0, (int32_t)(iptr[whole[t] + 1] - iptr[whole[t]]), -1});
-    if (tasks.empty()) continue;
-    B200_CUDA_OK(cudaMemcpyAsync(tasks_d, tasks.data(), tasks.size() * sizeof(Task), cudaMemcpyHostToDevice, stream));
-    B200_CUDA_OK(cudaMemsetAsync(counter, 0, 4, stream));
+  };
+  auto scores = [&](int n_tasks) {
     swing_scores_kernel<<<p.ctas, THREADS, p.smem, stream>>>(
-        g, w, alpha, n_items, top_k, p.sort_cap, p.smem_acc ? 1 : 0, tasks_d, (int)tasks.size(), counter, acc, tl,
-        split_rows, split_tl, split_n, nbr_ids, nbr_scores, nbr_count);
-    count_launch();
-    B200_CUDA_OK(cudaGetLastError());
-    if (!slot_item.empty()) {
-      B200_CUDA_OK(cudaMemcpyAsync(slot_item_d, slot_item.data(), slot_item.size() * 4, cudaMemcpyHostToDevice,
-                                   stream));
-      const size_t fsmem = (size_t)p.sort_cap * 8;
-      B200_CUDA_OK(cudaFuncSetAttribute(swing_split_finalize_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                        (int)fsmem));
-      swing_split_finalize_kernel<<<(unsigned)slot_item.size(), THREADS, fsmem, stream>>>(
-          slot_item_d, top_k, p.sort_cap, n_items, split_rows, split_tl, split_n, nbr_ids, nbr_scores, nbr_count);
-      count_launch();
-      B200_CUDA_OK(cudaGetLastError());
-    }
-  }
-  // the host task vectors are released on return: wait for the last upload to have been read
-  B200_CUDA_OK(cudaStreamSynchronize(stream));
-  return 0;
+        g, w, alpha, n_items, top_k, p.sort_cap, p.smem_acc ? 1 : 0, W.tasks, n_tasks, W.counter, W.acc, W.tl,
+        W.split_rows, W.split_tl, W.split_n, nbr_ids, nbr_scores, nbr_count);
+  };
+  auto finalize = [&](unsigned n_slots) {
+    swing_split_finalize_kernel<<<n_slots, THREADS, (size_t)p.sort_cap * 8, stream>>>(
+        W.slot_item, top_k, p.sort_cap, n_items, W.split_rows, W.split_tl, W.split_n, nbr_ids, nbr_scores, nbr_count);
+  };
+  return run_rounds(iptr, pairs, kMinPiecePairs, p, W, stream, cut, scores, finalize);
 }
 
 extern "C" int b200_swing_plan(int64_t n_items, int32_t top_k, int32_t* smem_acc, int32_t* ctas) {
@@ -406,53 +270,4 @@ extern "C" int b200_swing_plan(int64_t n_items, int32_t top_k, int32_t* smem_acc
   *smem_acc = p.smem_acc ? 1 : 0;
   *ctas = p.ctas;
   return 0;
-}
-
-extern "C" int b200_swing_recommend(const int64_t* user_ptr, const int32_t* user_items, const float* user_labels,
-                                    int64_t n_users, const int32_t* nbr_ids, const float* nbr_scores,
-                                    const int64_t* nbr_count, int64_t n_items, int32_t top_k,
-                                    const int64_t* consumed_ptr, const int32_t* consumed_idx, int32_t filter_consumed,
-                                    const int64_t* users, int64_t B, float* scores, int64_t ld, int64_t* counts,
-                                    void* stream) {
-  B200_REQUIRE(user_ptr && user_items && user_labels && nbr_ids && nbr_scores && nbr_count && users && scores &&
-               counts, "b200_swing_recommend: null pointer");
-  B200_REQUIRE(!filter_consumed || consumed_ptr, "b200_swing_recommend: filtering needs the consumed CSR");
-  B200_REQUIRE(B >= 0 && B <= 0x7fffffff && n_items >= 1 && ld >= n_items && n_users >= 0,
-               "b200_swing_recommend: bad shape");
-  B200_REQUIRE(top_k >= 1 && top_k <= kMaxTopK, "b200_swing_recommend: bad top_k");
-  if (B == 0) return 0;
-  swing_recommend_kernel<<<(unsigned)B, THREADS, 0, (cudaStream_t)stream>>>(
-      user_ptr, user_items, user_labels, n_users, nbr_ids, nbr_scores, nbr_count, n_items, top_k, consumed_ptr,
-      consumed_idx, filter_consumed, users, scores, ld, counts);
-  count_launch();
-  return check_cuda(cudaGetLastError(), "swing_recommend_kernel");
-}
-
-extern "C" int b200_swing_random_keys(float* scores, int64_t ld, int64_t B, int64_t n_items, const int64_t* users,
-                                      const int64_t* counts, int32_t n_rec, uint64_t seed, void* stream) {
-  B200_REQUIRE(scores && users && counts, "b200_swing_random_keys: null pointer");
-  B200_REQUIRE(B >= 0 && B <= 0x7fffffff && n_items >= 1 && ld >= n_items && n_rec >= 1,
-               "b200_swing_random_keys: bad shape");
-  if (B == 0) return 0;
-  swing_random_keys_kernel<<<(unsigned)B, THREADS, 0, (cudaStream_t)stream>>>(
-      scores, ld, n_items, users, counts, n_rec, (uint32_t)seed, (uint32_t)(seed >> 32));
-  count_launch();
-  return check_cuda(cudaGetLastError(), "swing_random_keys_kernel");
-}
-
-extern "C" int b200_swing_predict(const int64_t* user_ptr, const int32_t* user_items, int64_t n_users,
-                                  const int32_t* nbr_ids, const float* nbr_scores, const int64_t* nbr_count,
-                                  int64_t n_items, int32_t top_k, const int64_t* users, const int64_t* items,
-                                  int64_t n, float default_pred, float* out, void* stream) {
-  B200_REQUIRE(user_ptr && nbr_ids && nbr_scores && nbr_count && users && items && out,
-               "b200_swing_predict: null pointer");
-  B200_REQUIRE(n >= 0 && n_items >= 1 && n_users >= 0 && top_k >= 1 && top_k <= kMaxTopK,
-               "b200_swing_predict: bad shape");
-  if (n == 0) return 0;
-  // the mean swing score of the item's first top_k neighbours that row u of R holds: compute_pred "ranking"
-  neighbour_predict_kernel<false><<<(unsigned)ceil_div64(n, WARPS), THREADS, 0, (cudaStream_t)stream>>>(
-      user_ptr, user_items, nullptr, n_users, nbr_ids, nbr_scores, nbr_count, n_items, top_k, users, items, n,
-      default_pred, out);
-  count_launch();
-  return check_cuda(cudaGetLastError(), "neighbour_predict_kernel");
 }

@@ -1,6 +1,6 @@
 """Time UserCF and ItemCF on the GPU (``librecommender_b200.cf``): ``compute_similarities`` (``b200_cf_cosine``),
-recommend for a set of users (ItemCF: ``b200_swing_recommend``, UserCF: ``b200_user_cf_recommend``, then
-``b200_topk_rows``) and predict (``b200_cf_predict``).
+recommend for a set of users (``b200_nbr_recommend``, item-based for ItemCF and user-based for UserCF, then
+``b200_topk_rows``) and predict (``b200_nbr_predict``).
 
     python tools/profile_cf.py [--reps 5] [--out /tmp/cf.json]
 

@@ -1,5 +1,5 @@
 """Time Swing on the GPU (``librecommender_b200.swing``): ``compute_swing`` (``b200_swing_scores``), recommend for a set
-of users (``b200_swing_recommend`` + ``b200_topk_rows``) and predict (``b200_swing_predict``).
+of users (``b200_nbr_recommend`` + ``b200_topk_rows``) and predict (``b200_nbr_predict``).
 
     python tools/profile_swing.py [--reps 5] [--out /tmp/swing.json]
 
